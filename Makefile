@@ -2,12 +2,11 @@
 PY ?= python
 
 help:
-	@echo "make build          compile the native module for sm_100a (nvcc) and import the package"
+	@echo "make build          compile the native module for sm_90a (nvcc) and import the package"
 	@echo "make test           CPU test-suite (gloo, 2 ranks)"
-	@echo "make test-gpu       GPU test-suite (needs a B200)"
+	@echo "make test-gpu       GPU test-suite (needs an H100)"
 	@echo "make template-test  render a project skeleton into /tmp and list it (reference: cookiecutter --no-input)"
 	@echo "make bench          headline benchmark JSON line (1 GPU)"
-	@echo "make sass           SASS mnemonic summary of the built kernels -> profiles/sass_summary.md"
 	@echo "make clean          remove build artefacts"
 
 build:
@@ -26,10 +25,7 @@ template-test:
 bench:
 	$(PY) bench.py --gpus 1 --steps 30 --warmup 5
 
-sass:
-	$(PY) tools/sass_summary.py
-
 clean:
 	rm -rf distributeddeeplearning_b200/csrc/build distributeddeeplearning_b200/_C.so /tmp/ddl_template_test
 
-.PHONY: help build test test-gpu template-test bench sass clean
+.PHONY: help build test test-gpu template-test bench clean

@@ -5,12 +5,13 @@ batch 256/GPU").
 
     python bench.py --gpus N --steps K --warmup W            # this repo (N>1: run under torchrun, or
                                                              #  bench.py re-launches itself with the local launcher)
-    python bench.py --impl reference --gpus N ...            # the reference's unmodified script (baseline/_ref)
+    python bench.py --impl reference --gpus N ...            # the reference's unmodified script (oracle/_ref, made by build())
+    python bench.py ... --dump-outputs DIR                   # also save what the last timed step computed (.npy)
 
 Prints ONE JSON line on rank 0.  Timed region = exactly K full training steps (forward, loss,
 backward, fused allreduce + SGD update) between barrier + cuda.synchronize on both sides, CUDA events
 on the launching stream, max over ranks.  Per-step working set (>5 GB of activations at batch 256)
-exceeds the 126 MB L2, so no explicit L2 flush is needed ("l2": "working_set_exceeds_l2").
+exceeds the 50 MB L2, so no explicit L2 flush is needed ("l2": "working_set_exceeds_l2").
 ``e2e`` repeats the measurement through the public API with, every step, a host->device copy of that
 step's inputs from pinned memory (uint8 NHWC images, the decoded-JPEG format, + int64 labels) and a
 device->host read of the step's loss.
@@ -28,7 +29,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
-REF_SCRIPT = os.path.join(HERE, "baseline", "_ref", "PyTorch_benchmark", "src", "pytorch_synthetic_benchmark.py")
+REF_SCRIPT = os.path.join(HERE, "oracle", "_ref", "PyTorch_benchmark", "src", "pytorch_synthetic_benchmark.py")
 METRIC = "resnet50_synthetic_train_images_per_sec"
 
 
@@ -44,6 +45,9 @@ def parse():
     p.add_argument("--fp16-allreduce", action="store_true")
     p.add_argument("--no-selfcheck", action="store_true",
                    help="N>1: skip the engine self-checks that run before the timed region")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write what the last one computed (loss, and a fixed seeded sample of the "
+                        "updated parameters and buffers) as float32/float64 .npy files into DIR (rank 0)")
     p.add_argument("--cuda-graph", choices=["on", "off"], default=os.environ.get("DDL_BENCH_GRAPH", "on"),
                    help="replay the whole training step from one captured CUDA graph (falls back to eager if capture fails)")
     return p.parse_args()
@@ -130,6 +134,32 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------------------
+# outputs of the last timed step
+# ------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 1 << 21          # elements of the flattened parameters + buffers kept (ResNet-50 has ~25.6 M)
+
+
+def dump_outputs(session, out_dir):
+    """Write what one training step hands back to its caller: the loss and the model state it updated.  The state is
+    the model's parameters and floating-point buffers in ``named_parameters`` / ``named_buffers`` order, flattened and
+    concatenated; a fixed seeded sample of DUMP_SAMPLE positions is stored (``state_sample.npy``, float32) with those
+    positions (``state_index.npy``, float64) so that two builds can be compared element by element."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(session.last_loss)], dtype=np.float64))
+    tensors = [p.detach() for _, p in session.model.named_parameters()]
+    tensors += [b.detach() for _, b in session.model.named_buffers() if b.is_floating_point()]
+    flat = torch.cat([t.float().flatten() for t in tensors])
+    n = flat.numel()
+    idx = np.arange(n) if n <= DUMP_SAMPLE else np.sort(np.random.default_rng(0).choice(n, DUMP_SAMPLE, replace=False))
+    sample = flat[torch.from_numpy(idx).to(flat.device)].cpu().numpy().astype(np.float32)
+    np.save(os.path.join(out_dir, "state_sample.npy"), sample)
+    np.save(os.path.join(out_dir, "state_index.npy"), idx.astype(np.float64))
+
+
+# ------------------------------------------------------------------------------------------------
 # this repo's arm
 # ------------------------------------------------------------------------------------------------
 def run_ours(a):
@@ -199,6 +229,8 @@ def run_ours(a):
     ms, launches = region(session.step, a.steps, a.warmup, on_start=sampler.mark)
     clocks = sampler.stop() if rank == 0 else {}
     loss = float(session.last_loss)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(session, a.dump_outputs)
     value = world * B * a.steps / (ms / 1e3)
 
     # ---- end to end: per-step H2D of the inputs from pinned memory + D2H of the loss --------------
@@ -270,8 +302,7 @@ def run_ours(a):
 
     dtype = "bf16"
     if _fp8.enabled():          # DDL_PRECISION=fp8 experiment runs (the headline stays bf16)
-        dtype = "fp8 operands (e4m3/e5m2%s) for forward/dgrad convs with K >= %d, bf16 elsewhere" % (
-            ", MX block scales on 1x1 forward" if _fp8.MX else "", _fp8.MIN_K)
+        dtype = "fp8 operands (e4m3) for forward convs with K >= %d, bf16 elsewhere" % _fp8.MIN_K
     if rank == 0:
         base = None
         try:
@@ -311,12 +342,7 @@ def run_reference(a):
         return 0
 
     if not os.path.isfile(REF_SCRIPT):
-        inst = os.path.join(HERE, "baseline", "install_reference.py")
-        if int(os.environ.get("RANK", "0")) == 0 and os.path.isfile(inst):
-            subprocess.run([sys.executable, inst], capture_output=True)
-        time.sleep(1.0)
-    if not os.path.isfile(REF_SCRIPT):
-        return unavailable("reference is a cookiecutter template (not pip-installable) and baseline/_ref scripts are absent")
+        return unavailable("oracle/_ref holds no reference scripts (build() copies them from a reference checkout)")
     try:
         import torch
         import torchvision  # noqa: F401

@@ -1,14 +1,14 @@
-"""b200-ddl: a Blackwell-native distributed-training benchmark harness.
+"""ddl: an H100-native distributed-training benchmark harness.
 
 Capabilities of microsoft/DistributedDeepLearning's PyTorch templates
 (PyTorch_benchmark / PyTorch_imagenet / PyTorch_hvd; the TensorFlow twins
-collapse onto them), rebuilt for one 8xB200 NVSwitch box:
+collapse onto them), rebuilt for one 8xH100 NVSwitch box:
 
 * ``cli``        local launcher + task tree (replaces cookiecutter/AzureML control plane)
 * ``workloads``  synthetic benchmark, ImageNet trainer, resume-capable trainer
 * ``parallel``   Horovod-equivalent API, static bucket plan, fused allreduce+SGD over
                  NVLink peer / NVLS multicast memory
-* ``ops``        hand-written sm_100a kernels (tcgen05/TMEM/TMA conv-GEMMs, fused BN,
+* ``ops``        hand-written sm_90a kernels (wgmma/TMA conv-GEMMs, fused BN,
                  softmax-xent, pools, Philox synthetic data) + fp32 PyTorch references
 * ``models``     ResNet-50/101/152 (+18/34), VGG, AlexNet, Inception-v3
 * ``data``       synthetic datasets, ImageFolder pipeline, samplers, ImageNet prep

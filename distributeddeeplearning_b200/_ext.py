@@ -1,7 +1,7 @@
 """In-tree build + loader of the native module ``distributeddeeplearning_b200._C``.
 
 * ``build()``  compiles every ``csrc/**/*.cu`` with
-  ``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` (cross-compiles without a GPU),
+  ``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` (cross-compiles without a GPU),
   every ``csrc/**/*.cpp`` with g++, and links ``_C.so`` next to this file (so the artefact
   travels with the source tree and shows up as an in-tree native module).
 * ``load()``   imports ``_C``; (re)builds first when the sources are newer than the artefact.
@@ -28,7 +28,7 @@ _STAMP = os.path.join(_BUILD, "sources.sha")
 _LOCK = threading.Lock()
 _MODULE = None
 
-NVCC_ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 
 
@@ -154,7 +154,7 @@ KERNEL_LAUNCHES = {
     "maxpool_fwd": 1, "maxpool_bwd": 1, "avgpool_fwd": 1, "avgpool_bwd": 1, "global_avgpool_fwd": 1,
     "global_avgpool_bwd": 1, "softmax_xent": 1, "philox_normal_nhwc": 1, "philox_labels": 1, "nchw_to_nhwc_norm": 1,
     "nhwc_u8_to_nhwc4": 1, "cast_f32_bf16": 1, "pack_stem_weight": 1, "unpack_stem_grad": 1, "bias_relu_bwd": 1,
-    "dropout": 1, "add_bf16": 1, "fp8_quantize": 1, "fp8_quantize_mx": 1, "fp8_amax": 1, "fp8_update_scales": 1, "pad_nhwc4": 1, "concat_channels": 1, "bn_relu_maxpool_fwd": 1, "bn_pool_bwd": 2,
+    "dropout": 1, "add_bf16": 1, "fp8_quantize": 1, "fp8_quantize_mx": 1, "fp8_transpose_taps": 1, "fp8_amax": 1, "fp8_update_scales": 1, "pad_nhwc4": 1, "concat_channels": 1, "bn_relu_maxpool_fwd": 1, "bn_pool_bwd": 2,
 }
 LAUNCH_COUNT = [0]          # kernels of THIS repo launched so far (bench.py reports the per-region delta)
 

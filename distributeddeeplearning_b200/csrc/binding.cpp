@@ -36,9 +36,8 @@ cudaError_t launch_conv_gemm(int mode, const ConvArgs& a, const void* w, int w_r
 cudaError_t launch_conv_wgrad(const WgradArgs& a, const void* dy, const void* x_matrix, int splits,
                               cudaStream_t stream);
 void set_conv_force_stages(int s);
-void set_conv_persistent(int on);
 void set_wgrad_swap(int on);
-void set_conv_bn256(int on);
+void set_conv_persistent(int on);
 void set_conv_cluster(int on);
 void set_conv_deep(int on);
 void set_pdl(int on);
@@ -72,7 +71,7 @@ PoolArgs pool_args(int N, int H, int W, int C, int Pq, int Q, int k, int stride,
 }  // namespace
 
 PYBIND11_MODULE(_C, m) {
-  m.doc() = "b200-ddl native runtime + sm_100a kernels";
+  m.doc() = "ddl native runtime + sm_90a kernels";
   m.attr("MAX_COMM_BLOCKS") = ddl::kMaxCommBlocks;
   m.attr("COMM_CHANNELS") = ddl::kCommChannels;
   m.attr("SIGNAL_PAD_BYTES") = ddl::kSignalPadBytes;
@@ -240,8 +239,6 @@ PYBIND11_MODULE(_C, m) {
   });
 
   // ------------------------------------------------------------------ conv / GEMM
-  m.def("set_conv_persistent", &ddl::set_conv_persistent, "tuning hook: 1 = persistent kernel for TMA-fed modes");
-  m.def("set_conv_cluster", &ddl::set_conv_cluster, "tuning hook: 1 = CTA pairs with TMA-multicast weight tiles");
   m.def("conv_timeout_info", []() {
     unsigned int v[8];
     check(ddl::conv_timeout_info(v), "conv_timeout_info");
@@ -250,8 +247,9 @@ PYBIND11_MODULE(_C, m) {
   m.def("set_conv_wait_hint", &ddl::set_conv_wait_hint, "tuning hook: suspend-time hint (ns) of the conv kernels' mbarrier waits, 0 = none");
   m.def("set_bn_reverse", &ddl::set_bn_reverse, "1 (default) = BN forward / backward-reduce walk the rows from the end (L2 reuse of the producer's tail), 0 = front to back");
   m.def("set_pdl", &ddl::set_pdl, "0 = plain stream order, 1 = conv / BN kernels allow programmatic dependent launch (default), 2 = + trigger at the last tile, 3 = + trigger at block start");
-  m.def("set_conv_deep", &ddl::set_conv_deep, "tuning hook: 0 = never the deep-ring kernel, 1 = policy, 2 = always");
-  m.def("set_conv_bn256", &ddl::set_conv_bn256, "tuning hook: 0 = no 128x256 persistent tiles");
+  m.def("set_conv_persistent", &ddl::set_conv_persistent, "tuning hook: 0 = never the persistent conv kernel, 1 = policy, 2 = always");
+  m.def("set_conv_cluster", &ddl::set_conv_cluster, "tuning hook: 1 = the persistent kernel runs as CTA pairs sharing the weight tile by TMA multicast");
+  m.def("set_conv_deep", &ddl::set_conv_deep, "tuning hook: 2 = persistent CTA pairs wherever they apply, 3/4 = persistent single CTAs");
   m.def("set_wgrad_swap", &ddl::set_wgrad_swap, "tuning hook: 0 = no operand-role swap for narrow-output wgrad tiles");
   m.def("set_conv_force_stages", &ddl::set_conv_force_stages, "tuning hook: force the pipeline depth (0 = policy)");
   m.def("conv_gemm",
@@ -444,6 +442,10 @@ PYBIND11_MODULE(_C, m) {
   }, "bf16 [rows][K] -> e4m3 [rows][K] + UE8M0 block scales (32 elements) in the tensor core's 512-byte atom order");
   m.def("fp8_amax", [](ptr_t x, int64_t n, ptr_t slot, int sms, ptr_t stream) {
     check(ddl::launch_fp8_amax(P<const __nv_bfloat16>(x), n, P<ddl::Fp8Slot>(slot), sms, S(stream)), "fp8_amax");
+  });
+  m.def("fp8_transpose_taps", [](ptr_t in, ptr_t out, int rows, int taps, int cols, ptr_t stream) {
+    check(ddl::launch_fp8_transpose_taps(P<const uint8_t>(in), P<uint8_t>(out), rows, taps, cols, S(stream)),
+          "fp8_transpose_taps");
   });
   m.def("fp8_update_scales", [](ptr_t slots, int n, ptr_t stream) {
     check(ddl::launch_fp8_update_scales(P<ddl::Fp8Slot>(slots), n, S(stream)), "fp8_update_scales");

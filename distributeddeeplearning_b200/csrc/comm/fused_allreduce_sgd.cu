@@ -1,5 +1,5 @@
-// Fused gradient allreduce + cast/scale + SGD-momentum update over NVLink-5 peer / NVLS multicast
-// memory — the B200-native replacement for the reference's Horovod path
+// Fused gradient allreduce + cast/scale + SGD-momentum update over NVLink peer / NVLS multicast
+// memory — the native replacement for the reference's Horovod path
 //   hvd.DistributedOptimizer: per-parameter allreduce_async_ -> fusion buffer -> ncclAllReduce ->
 //   div_(size) -> optimizer.step() (161 x add_/mul_/add_)           (SURVEY.md X2, K12-K16, K19)
 //

@@ -1,4 +1,4 @@
-// Shared device helpers for the b200-ddl kernels (sm_100a only).
+// Shared device helpers for the b200-ddl kernels (sm_90a).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -14,20 +14,16 @@ constexpr int kWarp = 32;
 
 // ---------------------------------------------------------------------------------------------
 // programmatic dependent launch (PDL): a kernel launched with launch_pdl() (launch.h) may become resident while its
-// predecessor in the stream is still draining; everything it does before pdl_wait() (index math, barrier init, TMEM
-// allocation, tensor-map prefetch) overlaps that tail.  RULE: pdl_wait() comes before the first access to global
+// predecessor in the stream is still draining; everything it does before pdl_wait() (index math, barrier init,
+// tensor-map prefetch) overlaps that tail.  RULE: pdl_wait() comes before the first access to global
 // memory — it returns once the predecessor grid has completed and its writes are visible (no-op without the launch
 // attribute).  pdl_trigger() lets the NEXT kernel in the stream start its own preamble early.
 // ---------------------------------------------------------------------------------------------
-// Triggering is a mode per translation unit (c_pdl_trigger, set_pdl): measured on ResNet-50 (bench.py, 1 GPU, same box)
-//   set_pdl(0) plain stream order                                   18.59 / 18.65 ms per step
-//   set_pdl(1) attribute only: dependents launch as the last blocks exit and skip the completion flush
-//                                                                    18.43 / 18.46 ms  (default)
-//   set_pdl(3) every block triggers at its start                    +0.3 ms: dependents that become resident while the
-//              predecessor drains land unevenly on the SMs, and every kernel here assigns its tiles / rows statically
-//              to a grid sized for an even spread
-//   set_pdl(2) the persistent conv kernels trigger when they start their LAST tile; everything else as (1):
-//              +0.10 / +0.21 ms against (1) on a second box (18.93 / 18.89 vs 19.03 / 19.10 ms) — also a loss
+// Triggering is a mode per translation unit (c_pdl_trigger, set_pdl): 0 plain stream order, 1 (default) the launch
+// attribute only (dependents launch as the last blocks exit), 2 the conv kernels trigger at their last tile, 3 every
+// block triggers at its start.  Every kernel here assigns its tiles / rows statically to a grid sized for an even spread,
+// so dependents that become resident early land unevenly on the SMs; the default was chosen on that ground and was not
+// re-measured on H100.
 __constant__ int c_pdl_trigger;       // 0 = never explicitly, 1 = at the last tile (conv), 2 = at block start
 DDL_DEVICE void pdl_trigger() {
   if (c_pdl_trigger == 2) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");

@@ -69,7 +69,7 @@ DDL_DEVICE bool bn_thread_map(int C, int& c0, int& row0, int& row_stride) {
 // FP8: also emit the e4m3 twin of z (z * slot scale) and fold max|z| into the slot — the quantisation pass of the fp8
 // training mode rides in this kernel's streaming pass (+1 byte written per element) instead of re-reading z.
 // BLOCK_WIDE: every thread of the block reaches this point (flat thread mapping): fold through shared memory and issue ONE
-// atomic per block — ~9.5k same-address atomics per launch (one per warp) were measured to cost ~10 us per BN kernel.
+// atomic per block instead of ~9.5k same-address atomics per launch (one per warp), which serialise on one address.
 template <bool BLOCK_WIDE>
 DDL_DEVICE void fp8_fold_amax(Fp8Slot* slot, float amax) {
   amax = warp_max(amax);
@@ -187,8 +187,8 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) 
 // accumulates S1 = sum dy and S2 = sum dy * x (raw x); dbeta = S1, dgamma = invstd * (S2 - mean * S1).
 // Mapping: a block owns ONE 64-channel chunk (blockIdx.y) and 32 row lanes (thread = 8 channels x 1 row lane),
 // so a block ends with 64 x 2 partial sums -> 128 atomics per block and only gridDim.x contributions per address.
-// (A block spanning all channels would issue C x 2 atomics per block: ~5 M contended atomics for C = 2048, a
-// ~100 us floor that was measured to dominate the small layers.)
+// (A block spanning all channels would issue C x 2 atomics per block: ~5 M contended atomics for C = 2048, enough to
+// dominate the small layers.)
 template <int MASK>
 __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdArgs a) {
   pdl_trigger();

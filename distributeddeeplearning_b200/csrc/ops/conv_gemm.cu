@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA implicit-GEMM convolution kernels for sm_100a (bf16 in, fp32 accumulate).
+// wgmma / TMA implicit-GEMM convolution kernels for sm_90a (bf16 in, fp32 accumulate).
 //
 // Replaces the cuDNN conv fwd / bwd-data / bwd-filter and cuBLAS FC calls of the reference's
 // training step (SURVEY.md K2, K3, K4, K10; N4, N5).  All three passes are GEMMs on NHWC data:
@@ -7,18 +7,18 @@
 //   dgrad  dX[m][ci] = sum_k  im2colT(dY)[m][k] * W[co][(r,s,ci)]   k = (r, s, co)   (B is MN-major)
 //   wgrad  dW[co][k] = sum_m  dY[m][co]        * im2col(X)[m][k]    (A and B are MN-major, split-K)
 //
-// One CTA = 6 warps:
-//   warps 0-3  epilogue (TMEM -> registers -> smem -> coalesced global stores; fused BN statistics /
-//              bias / ReLU / residual add).  In the gather modes (strided convs, stem) the same warps
-//              first act as im2col producers: each thread owns one 128-byte row of the operand tile and
-//              fills it with cp.async (zero-fill = padding / tails) in the 128B-swizzled image tcgen05 reads.
-//   warp 4     TMA producer: weights always; the activation operand too whenever it is a plain matrix
+// One CTA = 13 warps:
+//   warps 0-7  two consumer warpgroups: warpgroup g issues the wgmma of accumulator rows [64g, 64g+64) of the
+//              128-row tile and keeps them in registers, then runs the epilogue (registers -> smem staging ->
+//              coalesced global stores; fused BN statistics / bias / ReLU / residual add)
+//   warps 8-11 im2col producers in the gather modes (strided convs, stem): each thread owns one 128-byte row of the
+//              operand tile and fills it with cp.async (zero-fill = padding / tails) in the 128B-swizzled image wgmma
+//              reads; idle in the TMA-fed modes
+//   warp 12    TMA producer: weights always; the activation operand too whenever it is a plain matrix
 //              (2-D map) or a stride-1 convolution window (ONE 4-D box per filter tap — the hardware does
 //              the im2col, out-of-bounds coordinates supply the zero padding)
-//   warp 5     TMEM allocator + the single thread that issues tcgen05.mma and tcgen05.commit
-// Stages are handed over with mbarriers (full/empty ring + one accumulator-ready barrier).  The pipeline
-// depth is chosen per launch (short-K layers take less shared memory, so more CTAs are resident per SM
-// and one CTA's epilogue overlaps the others' loads).
+// Stages are handed over with mbarriers (full/empty ring); a consumer warp releases a stage once the wgmma group that
+// read it has retired.  The ring is as deep as shared memory allows (one CTA per SM).
 #include "conv_gemm.cuh"
 #include "tc_utils.cuh"
 #include "../launch.h"
@@ -36,24 +36,24 @@ namespace {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;                       // bf16 elements = 128 bytes = one swizzle row
 constexpr int kATileBytes = kBlockM * 128;        // 16 KB
-constexpr int kProducerThreads = 128;              // warps 0-3: gather producers (and epilogue group 0)
-constexpr int kEpiGroups = 2;                      // epilogue warp groups: group g owns columns [g*N/2, (g+1)*N/2)
-constexpr int kEpiThreads = 128 * kEpiGroups;      // warps 0-3 (+ warps 6-9)
-constexpr int kThreads = 192 + 128 * (kEpiGroups - 1);
+constexpr int kEpiThreads = 256;                  // warps 0-7: the two consumer warpgroups
+constexpr int kProducerWarp0 = 8;                 // warps 8-11: cp.async gather producers
+constexpr int kProducerThreads = 128;
+constexpr int kTmaWarp = 12;
+constexpr int kThreads = 13 * 32;
 constexpr int kLag = 2;                           // cp.async groups kept in flight per producer
-constexpr int kMaxStages = 4;
+constexpr int kMaxStages = 8;
 
 template <int BLOCK_N>
 struct FwdCfg {
   static constexpr int kBTileBytes = BLOCK_N * 128;
   static constexpr int kStageBytes = kATileBytes + kBTileBytes;
   static constexpr int kPitch = BLOCK_N * 2 + 16;                 // epilogue staging row pitch (bytes)
-  static constexpr int kEpiBytes = kBlockM * kPitch;
-  static constexpr int kMaxStagesN = (BLOCK_N <= 64) ? 4 : 3;
-  static constexpr int smem_bytes(int stages) {
-    const int pipe = stages * kStageBytes;
-    return (pipe > kEpiBytes ? pipe : kEpiBytes) + 256 /*barriers*/ + 8192 /*stats scratch*/ + 1024 /*alignment*/;
-  }
+  static constexpr int kEpiBytes = ((kBlockM * kPitch + 1023) / 1024) * 1024;
+  static constexpr int kFixed = kEpiBytes + 256 /*barriers*/ + 8192 /*stats scratch*/ + 1024 /*alignment*/;
+  static constexpr int kMaxStagesN = (232448 - kFixed) / kStageBytes > kMaxStages ? kMaxStages
+                                                                                   : (232448 - kFixed) / kStageBytes;
+  static constexpr int smem_bytes(int stages) { return stages * kStageBytes + kFixed; }
 };
 
 DDL_DEVICE void named_bar_sync(int id, int nthreads) {
@@ -86,11 +86,10 @@ constexpr bool mode_stem(int mode) { return mode == kConvStem || mode == kConvSt
 
 
 // ---------------------------------------------------------------------------------------------
-// epilogue building blocks (shared by the one-tile and the persistent kernel)
+// epilogue building blocks
 // ---------------------------------------------------------------------------------------------
 // All staging traffic uses 32-bit shared-window addresses (ld/st.shared): generic LD/ST through the aligned
-// dynamic-smem pointer cost 64-bit address arithmetic per access and showed up as ~15 % of the epilogue's
-// instruction stream in the ncu source view (profiles/ncu_summary.md).
+// dynamic-smem pointer cost 64-bit address arithmetic per access.
 DDL_DEVICE void sts128(uint32_t addr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" :: "r"(addr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
@@ -111,40 +110,35 @@ DDL_DEVICE float lds_f32(uint32_t addr) { return __uint_as_float(lds32(addr)); }
 // are then wrong by construction; production launches never set them (native.py builds variant words from bits 0-8).
 constexpr int kDbgNoStats = 1 << 12;   // no statistics pass (and no atomics)
 constexpr int kDbgNoStore = 1 << 13;   // no global stores
-constexpr int kDbgNoDrain = 1 << 14;   // no TMEM -> staging copy
+constexpr int kDbgNoDrain = 1 << 14;   // no accumulator -> staging copy
 
-// TMEM accumulator columns [c_begin, c_end) of this thread's row -> (bias, ReLU) -> bf16 -> staging row.
-// `stg_row`: shared address of the row's staging line; `zero_row`: the row lies outside the image (tile modes).
-template <bool BIAS_RELU>
-DDL_DEVICE void epi_tmem_to_stage(uint32_t taddr_row, uint32_t stg_row, int c_begin, int c_end, const ConvArgs& a,
-                                  int n0, bool zero_row, float deq = 1.0f) {
+// wgmma accumulator fragment of this thread -> (dequantise, bias, ReLU) -> bf16 -> staging rows r0 and r0 + 8.
+// `z0` / `z1`: the row lies outside the image (tile modes) and is staged as zeros.
+template <int BLOCK_N, bool BIAS_RELU>
+DDL_DEVICE void epi_acc_to_stage(const float (&acc)[BLOCK_N / 2], uint32_t stg, int r0, bool z0, bool z1,
+                                 const ConvArgs& a, int n0, float deq) {
+  constexpr int kPitch = BLOCK_N * 2 + 16;
   if (a.variant & kDbgNoDrain) return;
-#pragma unroll 1
-  for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-    uint32_t v[32];
-    tmem_ld_32x32(taddr_row + c0, v);
-    tmem_ld_wait();
-    uint32_t packed[16];
+  const uint32_t row0 = stg + r0 * kPitch, row1 = row0 + 8 * kPitch;
+  const int cq = 2 * (threadIdx.x & 3);
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      float x0 = __uint_as_float(v[2 * j]) * deq, x1 = __uint_as_float(v[2 * j + 1]) * deq;
-      if (BIAS_RELU) {
-        if (a.bias) {
-          const int cb = n0 + c0 + 2 * j;
-          if (cb < a.n_valid) x0 += a.bias[cb];
-          if (cb + 1 < a.n_valid) x1 += a.bias[cb + 1];
-        }
-        if (a.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int c = 8 * j + cq;
+    float x0 = acc[4 * j] * deq, x1 = acc[4 * j + 1] * deq, y0 = acc[4 * j + 2] * deq, y1 = acc[4 * j + 3] * deq;
+    if (BIAS_RELU) {
+      if (a.bias) {
+        const float b0 = (n0 + c < a.n_valid) ? a.bias[n0 + c] : 0.f;
+        const float b1 = (n0 + c + 1 < a.n_valid) ? a.bias[n0 + c + 1] : 0.f;
+        x0 += b0; x1 += b1; y0 += b0; y1 += b1;
       }
-      packed[j] = zero_row ? 0u : pack_bf16x2(x0, x1);
+      if (a.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
     }
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      sts128(stg_row + c0 * 2 + j * 16, packed[4 * j], packed[4 * j + 1], packed[4 * j + 2], packed[4 * j + 3]);
+    sts32(row0 + c * 2, z0 ? 0u : pack_bf16x2(x0, x1));
+    sts32(row1 + c * 2, z1 ? 0u : pack_bf16x2(y0, y1));
   }
 }
 
-// ---- packed fp32 pairs (FADD2 / FFMA2: one issue slot for two lanes of statistics math) -----------------------------
+// ---- fp32 pairs (two statistics lanes per 64-bit register pair) -------------------------------------------------
 DDL_DEVICE uint64_t f2_pack(float lo, float hi) {
   uint64_t d;
   asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(lo), "f"(hi));
@@ -158,19 +152,21 @@ DDL_DEVICE uint64_t f2_from_bf16x2(uint32_t u) {            // {bf16 lo, bf16 hi
   return d;
 }
 DDL_DEVICE uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  return f2_pack(a0 + b0, a1 + b1);
 }
 DDL_DEVICE uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  f2_unpack(c, c0, c1);
+  return f2_pack(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 
-// Per-thread partial BN statistics of 8 consecutive output channels (4 packed pairs each): they live in registers
-// ACROSS the tiles a persistent CTA walks (as long as the tiles share their first channel n0) and are flushed — warp
-// shuffles, one shared-memory fold, one atomic per channel and statistic — only when n0 changes or the CTA is done.
+// Per-thread partial BN statistics of 8 consecutive output channels (4 pairs each), flushed with warp shuffles, one
+// shared-memory fold and one atomic per channel and statistic.
 struct StatAcc {
   uint64_t s[4], q[4];
   int n0;                       // first channel of the tile column these sums belong to; -1 = empty
@@ -281,14 +277,14 @@ DDL_DEVICE void epi_stats_flush(uint32_t red, int etid, int ew, const ConvArgs& 
       const int which = c / BLOCK_N, col = c - which * BLOCK_N;
       float v = 0.f;
 #pragma unroll
-      for (int wq = 0; wq < 4 * kEpiGroups; ++wq) v += lds_f32(red + ((wq * 2 + which) * BLOCK_N + col) * 4);
+      for (int wq = 0; wq < kEpiThreads / 32; ++wq) v += lds_f32(red + ((wq * 2 + which) * BLOCK_N + col) * 4);
       if (n0 + col < a.n_valid) atomicAdd((which ? a.sumsq : a.sum) + n0 + col, v);
     }
   } else {
     for (int col = etid; col < BLOCK_N; col += kEpiThreads) {      // dbeta += S1, dgamma += invstd * (S2 - mean * S1)
       float t1 = 0.f, t2 = 0.f;
 #pragma unroll
-      for (int wq = 0; wq < 4 * kEpiGroups; ++wq) {
+      for (int wq = 0; wq < kEpiThreads / 32; ++wq) {
         t1 += lds_f32(red + ((wq * 2 + 0) * BLOCK_N + col) * 4);
         t2 += lds_f32(red + ((wq * 2 + 1) * BLOCK_N + col) * 4);
       }
@@ -371,7 +367,7 @@ DDL_DEVICE void epi_store(uint32_t stg, int etid, const ConvArgs& a, int n0, int
   }
 }
 
-// One-shot form (one tile per call: accumulate, publish, store) for the kernels that do not carry sums across tiles.
+// One tile: accumulate, publish, store.
 template <int BLOCK_N, bool STATS, bool TILE>
 DDL_DEVICE void epi_stats_store(uint32_t stg, uint32_t red, int etid, int ew, const ConvArgs& a, int n0, int m0) {
   if (STATS) {
@@ -387,68 +383,85 @@ DDL_DEVICE void epi_stats_store(uint32_t stg, uint32_t red, int etid, int ew, co
 // ---------------------------------------------------------------------------------------------
 // fwd / dgrad / plain-GEMM / stem kernel
 // ---------------------------------------------------------------------------------------------
-template <int BLOCK_N, int MODE, bool STATS>
-__global__ void __launch_bounds__(kThreads, 3)
-conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ TmaSet tmAs, ConvArgs a) {
+// One M x N tile per CTA.  fp8 operands (FP8: e4m3 x e4m3, K-major A and B) use the same 128-byte k-blocks.
+template <int N, int FP8, bool BMN>
+DDL_DEVICE void mma_kstep(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (FP8 == 2) {
+    if constexpr (N == 128) wgmma_e5m2e4m3_n128<0, 0>(d, da, db, accumulate);
+    else wgmma_e5m2e4m3_n64<0, 0>(d, da, db, accumulate);
+  } else if constexpr (FP8 == 1) {
+    if constexpr (N == 128) wgmma_e4m3_n128<0, 0>(d, da, db, accumulate);
+    else wgmma_e4m3_n64<0, 0>(d, da, db, accumulate);
+  } else {
+    if constexpr (N == 128) wgmma_bf16_n128<0, BMN ? 1 : 0>(d, da, db, accumulate);
+    else wgmma_bf16_n64<0, BMN ? 1 : 0>(d, da, db, accumulate);
+  }
+}
+
+template <int BLOCK_N, int MODE, bool STATS, int FP8, bool PERSIST, bool CL>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBh,
+                 const __grid_constant__ TmaSet tmAs, ConvArgs a, int n_tiles, int m_tiles) {
+  static_assert(!(PERSIST || CL) || mode_a_tma(MODE), "tile loops and CTA pairs need TMA-fed operands");
   const CUtensorMap& tmA = tmAs.m[0];
   using Cfg = FwdCfg<BLOCK_N>;
   constexpr bool kATma = mode_a_tma(MODE);
-  constexpr bool kBMn = mode_b_mn(MODE);
+  constexpr bool kBMn = mode_b_mn(MODE) && FP8 == 0;   // fp8 data gradients read a transposed, K-major weight copy
   constexpr bool kTile = mode_tile(MODE);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nstages = a.stages;
-  const int pipe_bytes = nstages * Cfg::kStageBytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (pipe_bytes > Cfg::kEpiBytes ? pipe_bytes : Cfg::kEpiBytes));
+  // [operand ring][epilogue staging tile][barriers (256 B)][statistics scratch]: the staging tile has its own space so
+  // that the producers can fill the ring for the next tile while the consumers drain this one
+  const uint32_t stg = smem_u32(smem) + nstages * Cfg::kStageBytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + nstages * Cfg::kStageBytes + Cfg::kEpiBytes);
   uint64_t* empty = full + kMaxStages;
-  uint64_t* acc_full = empty + kMaxStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
 
   const int warp = threadIdx.x >> 5;
-  const int n0 = blockIdx.x * BLOCK_N;
   const int KB = a.KB;
-
-  // ---- tile -> output rows ------------------------------------------------------------------------
-  int m0 = blockIdx.y * kBlockM;          // linear modes: rows [m0, m0+128)
-  int tq0 = 0, tp0 = 0, tn0 = 0;          // tile modes: box origin in the output's (w, h, n) space
-  if (kTile) {
-    int t = blockIdx.y;
-    const int wb = t % a.tiles_w; t /= a.tiles_w;
-    const int hb = t % a.tiles_h;
-    const int nb = t / a.tiles_h;
-    tq0 = wb * a.tw; tp0 = hb * a.th; tn0 = nb * a.tn;
-    m0 = 0;
-  }
+  // work items: (N tile, M tile) — or, for a CTA pair, (N tile, two consecutive M tiles), one per CTA of the pair.
+  // A CTA (pair) takes items unit, unit + units, ...; one item per CTA (pair) unless PERSIST.
+  const uint32_t rank = CL ? cluster_ctarank() : 0u;
+  const int unit = CL ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
+  const int units = CL ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  const int items = n_tiles * (CL ? (m_tiles + 1) / 2 : m_tiles);
+  int n0 = 0, m0 = 0, tq0 = 0, tp0 = 0, tn0 = 0;
+  auto decode = [&](int item) {
+    n0 = (item % n_tiles) * BLOCK_N;
+    const int mt = (item / n_tiles) * (CL ? 2 : 1) + static_cast<int>(rank);   // may be m_tiles (odd pair): all rows empty
+    m0 = mt * kBlockM;                       // linear modes: rows [m0, m0+128)
+    if (kTile) {                             // tile modes: box origin in the output's (w, h, n) space
+      int t = mt;
+      const int wb = t % a.tiles_w; t /= a.tiles_w;
+      const int hb = t % a.tiles_h;
+      const int nb = t / a.tiles_h;
+      tq0 = wb * a.tw; tp0 = hb * a.th; tn0 = nb * a.tn;
+      m0 = 0;
+    }
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < nstages; ++s) {
       mbar_init(&full[s], kATma ? 1u : (kProducerThreads + 1u));
-      mbar_init(&empty[s], 1u);
+      mbar_init(&empty[s], (kEpiThreads / 32) * (CL ? 2u : 1u));   // one arrival per consumer warp (of both CTAs)
     }
-    mbar_init(acc_full, 1u);
     fence_mbar_init();
   }
-  if (warp == 4 && elect_one()) {
+  if (warp == kTmaWarp && elect_one()) {
     tma_prefetch_desc(&tmB);
+    if (CL) tma_prefetch_desc(&tmBh);
     if (kATma) tma_prefetch_desc(&tmA);
   }
-  if (warp == 5) tmem_alloc<BLOCK_N>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (CL) cluster_sync_all();          // the peer's barriers are initialised before anything multicasts into it
   pdl_trigger();      // the next kernel in the stream may start its own preamble
   pdl_wait();         // everything above overlapped the previous kernel's tail; global memory is touched only below
 
-  if (warp < 4 || warp >= 6) {
-    const int egrp = warp < 4 ? 0 : 1;                 // epilogue group
-    const int qw = warp & 3;                           // TMEM lane quarter this warp may read (= warp % 4)
-    const int erow = qw * 32 + (threadIdx.x & 31);     // accumulator row owned in the epilogue
-    const int etid = egrp * 128 + erow;                // dense index over the epilogue threads
-    const int ew = egrp * 4 + qw;                      // dense epilogue warp index
-    // =============================== gather producers ===================================
-    if (!kATma && warp < 4) {
-      const int row = threadIdx.x;
+  if (warp >= kProducerWarp0 && warp < kTmaWarp) {
+    // =============================== gather producers (one tile) ========================
+    decode(unit);
+    if (!kATma) {
+      const int row = threadIdx.x - kEpiThreads;
       const int m = m0 + row;
       const bool row_ok = m < a.M;
       int img = 0, dh = 0, dw = 0;
@@ -527,762 +540,146 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
       fence_proxy_async_smem();
       for (int kb = (KB > kLag ? KB - kLag : 0); kb < KB; ++kb) mbar_arrive(&full[kb % nstages]);
     }
-
-    // =================================== epilogue ========================================
-    // my accumulator row -> output row
-    const int row = erow;
-    int my_m;                     // linear output row index of this thread's accumulator row, or -1
-    if (kTile) {
-      const int wl = row % a.tw;
-      const int t2 = row / a.tw;
-      const int hl = t2 % a.th;
-      const int nl = t2 / a.th;
-      const bool ok = nl < a.tn && (tn0 + nl) < a.batch && (tp0 + hl) < a.dstH && (tq0 + wl) < a.dstW;
-      my_m = ok ? ((tn0 + nl) * a.outH + (tp0 + hl) * a.out_stride + a.out_pa) * a.outW +
-                      (tq0 + wl) * a.out_stride + a.out_pb
-                : -1;
-    } else {
-      my_m = (m0 + row) < a.M ? (m0 + row) : -1;
-    }
-    mbar_wait(acc_full, 0, 20);
-    tc_fence_after();
-    // pipeline buffers are free (every MMA that read them has completed): the tile is staged over them
-    const uint32_t stg = smem_u32(smem);
-    const uint32_t stg_row = stg + row * Cfg::kPitch;
-    constexpr int kColsPerGroup = BLOCK_N / kEpiGroups;
-    const uint32_t taddr_row = tmem_base + (static_cast<uint32_t>(qw * 32) << 16);
-    const bool zero_row = kTile && my_m < 0;          // rows outside the image: exact zeros (keeps the BN sums clean)
-    if (!STATS && (a.bias != nullptr || a.relu))
-      epi_tmem_to_stage<true>(taddr_row, stg_row, egrp * kColsPerGroup, (egrp + 1) * kColsPerGroup, a, n0, zero_row);
-    else
-      epi_tmem_to_stage<false>(taddr_row, stg_row, egrp * kColsPerGroup, (egrp + 1) * kColsPerGroup, a, n0, zero_row);
-    // the row's destination index rides in the pad bytes of its staging row (pitch = 2*BLOCK_N + 16)
-    if (kTile && egrp == 0) sts32(stg_row + BLOCK_N * 2, static_cast<uint32_t>(my_m));
-    tc_fence_before();
-    named_bar_sync(1, kEpiThreads);
-    epi_stats_store<BLOCK_N, STATS, kTile>(stg, smem_u32(full) + 256, etid, ew, a, n0, m0);
-  } else if (warp == 4) {
+  } else if (warp == kTmaWarp) {
     // ================================== TMA producer =====================================
     if (elect_one()) {
-      int tap = 0, cc = 0, tap_r = 0, tap_s = 0;
       int stage = 0;
       uint32_t phase = 0;
-      const uint32_t a_bytes = kTile ? static_cast<uint32_t>(a.tw * a.th * a.tn) * 128u : kATileBytes;
-      for (int kb = 0; kb < KB; ++kb) {
-        mbar_wait(&empty[stage], phase ^ 1u, 17);
-        uint8_t* sA = smem + stage * Cfg::kStageBytes;
-        const uint32_t sB = smem_u32(sA + kATileBytes);
-        mbar_arrive_expect_tx(&full[stage], Cfg::kBTileBytes + (kATma ? a_bytes : 0u));
-        // tap of this k-block: weight tap index + (tile modes) source box offset / source map
-        int widx = tap, dh = 0, dw = 0, mapi = 0;
-        if (kTile) {
-          if (a.ntaps > 0) {
-            widx = a.tap_widx[tap]; dh = a.tap_dh[tap]; dw = a.tap_dw[tap]; mapi = a.tap_map[tap];
-          } else if (MODE == kConvTileFwd) {
-            dh = tap_r * a.dil - a.pad; dw = tap_s * a.dil - a.pad_w;
-          } else {
-            dh = a.pad - tap_r * a.dil; dw = a.pad_w - tap_s * a.dil;
+      for (int item = unit; item < items; item += units) {
+        decode(item);
+        int tap = 0, cc = 0, tap_r = 0, tap_s = 0;
+        const uint32_t a_bytes = kTile ? static_cast<uint32_t>(a.tw * a.th * a.tn) * 128u : kATileBytes;
+        for (int kb = 0; kb < KB; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1u, 17);
+          uint8_t* sA = smem + stage * Cfg::kStageBytes;
+          const uint32_t sB = smem_u32(sA + kATileBytes);
+          mbar_arrive_expect_tx(&full[stage], Cfg::kBTileBytes + (kATma ? a_bytes : 0u));
+          // tap of this k-block: weight tap index + (tile modes) source box offset / source map
+          int widx = tap, dh = 0, dw = 0, mapi = 0;
+          if (kTile) {
+            if (a.ntaps > 0) {
+              widx = a.tap_widx[tap]; dh = a.tap_dh[tap]; dw = a.tap_dw[tap]; mapi = a.tap_map[tap];
+            } else if (MODE == kConvTileFwd) {
+              dh = tap_r * a.dil - a.pad; dw = tap_s * a.dil - a.pad_w;
+            } else {
+              dh = a.pad - tap_r * a.dil; dw = a.pad_w - tap_s * a.dil;
+            }
           }
-        }
-        if (kBMn) {
-          // weights W[co][(r,s,ci)]: K rows = 64 output channels, N = input channels (contiguous)
+          const int kcol = FP8 ? 128 : kBlockK;          // elements per 128-byte k-block
+          if (CL) {
+            // each CTA of the pair loads half of the weight tile and multicasts it into both CTAs
+            if (kBMn) {
+              tma_load_2d_multicast(sB + rank * 8192u, &tmB, widx * a.ldc + n0 + static_cast<int>(rank) * 64, cc * 64,
+                                    &full[stage], 0x3);
+            } else {
+              tma_load_2d_multicast(sB + rank * (BLOCK_N / 2) * 128u, &tmBh,
+                                    mode_stem(MODE) ? kb * kBlockK : widx * a.kstride + cc * kcol,
+                                    n0 + static_cast<int>(rank) * (BLOCK_N / 2), &full[stage], 0x3);
+            }
+          } else if (kBMn) {
+            // weights W[co][(r,s,ci)]: K rows = 64 output channels, N = input channels (contiguous)
 #pragma unroll
-          for (int j = 0; j < BLOCK_N / 64; ++j)
-            tma_load_2d(sB + j * 8192, &tmB, widx * a.ldc + n0 + j * 64, cc * 64, &full[stage]);
-        } else {
-          tma_load_2d(sB, &tmB, mode_stem(MODE) ? kb * kBlockK : widx * a.kstride + cc * kBlockK, n0, &full[stage]);
+            for (int j = 0; j < BLOCK_N / 64; ++j)
+              tma_load_2d(sB + j * 8192, &tmB, widx * a.ldc + n0 + j * 64, cc * 64, &full[stage]);
+          } else {
+            tma_load_2d(sB, &tmB, mode_stem(MODE) ? kb * kBlockK : widx * a.kstride + cc * kcol, n0, &full[stage]);
+          }
+          if (MODE == kConvGemm || MODE == kConvGemmDgrad) {
+            tma_load_2d(smem_u32(sA), &tmA, kb * kcol, m0, &full[stage]);
+          } else if (MODE == kConvStemTma) {
+            tma_load_5d(smem_u32(sA), &tmA, 0, kb, tq0, tp0, tn0, &full[stage]);
+          } else if (kTile) {
+            tma_load_4d(smem_u32(sA), &tmAs.m[mapi], cc * kcol, tq0 + dw, tp0 + dh, tn0, &full[stage]);
+          }
+          if (++cc == a.cchunks) { cc = 0; ++tap; if (++tap_s == a.S) { tap_s = 0; ++tap_r; } }
+          if (++stage == nstages) { stage = 0; phase ^= 1u; }
         }
-        if (MODE == kConvGemm || MODE == kConvGemmDgrad) {
-          tma_load_2d(smem_u32(sA), &tmA, kb * kBlockK, m0, &full[stage]);
-        } else if (MODE == kConvStemTma) {
-          tma_load_5d(smem_u32(sA), &tmA, 0, kb, tq0, tp0, tn0, &full[stage]);
-        } else if (kTile) {
-          tma_load_4d(smem_u32(sA), &tmAs.m[mapi], cc * 64, tq0 + dw, tp0 + dh, tn0, &full[stage]);
-        }
-        if (++cc == a.cchunks) { cc = 0; ++tap; if (++tap_s == a.S) { tap_s = 0; ++tap_r; } }
-        if (++stage == nstages) { stage = 0; phase ^= 1u; }
       }
     }
+    __syncwarp();
   } else {
-    // =================================== MMA issuer =======================================
-    constexpr uint32_t idesc = idesc_bf16(kBlockM, BLOCK_N, 0, kBMn ? 1 : 0);
-    const uint64_t odA0 = smem_desc_sw128(smem_u32(smem), 0, 1024);
+    // ============================ consumers: wgmma + epilogue =============================
+    // warpgroup g = warps 4g..4g+3 owns accumulator rows [64g, 64g + 64) of the tile
+    const int wg = warp >> 2;
+    const int lane = threadIdx.x & 31;
+    const uint64_t odA0 = smem_desc_sw128(smem_u32(smem) + wg * (kATileBytes / 2), 0, 1024);
     const uint64_t odB0 = kBMn ? smem_desc_sw128(smem_u32(smem) + kATileBytes, 8192, 1024)
                                : smem_desc_sw128(smem_u32(smem) + kATileBytes, 0, 1024);
     const uint32_t oa_lo = static_cast<uint32_t>(odA0), oa_hi = static_cast<uint32_t>(odA0 >> 32);
     const uint32_t ob_lo = static_cast<uint32_t>(odB0), ob_hi = static_cast<uint32_t>(odB0 >> 32);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int kb = 0; kb < KB; ++kb) {
-      mbar_wait(&full[stage], phase, 18);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t so = static_cast<uint32_t>(stage) * (Cfg::kStageBytes >> 4);
-#pragma unroll
-        for (int k = 0; k < kBlockK / 16; ++k) {
-          const uint64_t da = desc_join(oa_lo + so + 2u * k, oa_hi);
-          const uint64_t db = desc_join(ob_lo + so + (kBMn ? 128u : 2u) * k, ob_hi);
-          umma_bf16(tmem_base, da, db, idesc, (kb | k) != 0);
-        }
-        umma_commit(&empty[stage]);
-        if (kb == KB - 1) umma_commit(acc_full);
-      }
+    // hand a stage back to the producers (of both CTAs of a pair: either may multicast into it next)
+    auto release = [&](int s) {
       __syncwarp();
-      if (++stage == nstages) { stage = 0; phase ^= 1u; }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<BLOCK_N>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// persistent variant for the TMA-fed modes (GEMM, TILE_FWD, TILE_DGRAD, GEMM_DGRAD)
-// ---------------------------------------------------------------------------------------------
-// One CTA per resident slot (2 per SM) walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...  The operand ring
-// keeps streaming across tile boundaries, the accumulator is double-buffered in TMEM (2 x BLOCK_N columns) and the
-// 8 epilogue warps drain tile i while the MMA thread already accumulates tile i+1: the per-tile fixed latency
-// (TMEM alloc, barrier init, first TMA round trip, epilogue) that bounds the one-tile-per-CTA kernel on short-K
-// layers is paid once per CTA instead of once per tile.
-template <int BLOCK_N>
-struct PersistCfg {
-  static constexpr int kBTileBytes = BLOCK_N * 128;
-  static constexpr int kStageBytes = kATileBytes + kBTileBytes;
-  static constexpr int kPitch = BLOCK_N * 2 + 16;
-  static constexpr int kEpiBytes = ((kBlockM * kPitch + 1023) / 1024) * 1024;
-  // BLOCK_N = 256: one CTA per SM (its two accumulators fill the 512 TMEM columns); a 128 x 256 tile re-uses every
-  // activation k-block for twice the output columns, i.e. 25 % less L2 -> shared traffic per FLOP than 128 x 128
-  static constexpr int kStages = (BLOCK_N <= 64) ? 3 : 2;
-  static constexpr int kRedBytes = 4 * kEpiGroups * 2 * BLOCK_N * 4;      // [epi warps][2][BLOCK_N] floats
-  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 256 + kRedBytes + 1024;
-};
-
-// CLUSTER = launched as thread-block clusters of 2 CTAs that work on the SAME N tile and adjacent M tiles: each CTA
-// fetches half of the weight tile and TMA-multicasts it into both CTAs' shared memory, so the B operand crosses
-// L2 -> SM once per pair (operand traffic per 128 x 128 tile: 32 KB -> 24 KB).  A stage may be refilled only when
-// BOTH CTAs' MMAs have consumed it: `empty` counts two arrivals, delivered by a multicast tcgen05.commit.
-// CL: 0 = independent CTAs, 1 = the multicast pairs described above, 2 = CTA pairs sharing ONE MMA (cta_group::2,
-// M = 256): each CTA loads its 128 rows of A and only HALF of the weight tile; the leader CTA issues the MMAs, which
-// read both SMs' shared memory and write both SMs' TMEM.  Bytes entering each SM per 128 x 128 outputs: 32 KB -> 24 KB.
-//   barriers (CL = 2): leader.full[s] = expect_tx of BOTH CTAs' operand bytes (the peer's TMA loads complete on the
-//   leader's barrier: cp.async.bulk.tensor.cta_group::2); empty[s] / acc_full[b] in both CTAs = the leader's multicast
-//   commit; leader.acc_empty[b] = both epilogues (the peer arrives remotely).
-template <int BLOCK_N, int MODE, bool STATS, int CL>
-__global__ void __launch_bounds__(kThreads, 2)
-conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBh,
-                            const __grid_constant__ TmaSet tmAs, ConvArgs a, int n_tiles, int m_tiles) {
-  using Cfg = PersistCfg<BLOCK_N>;
-  constexpr bool kBMn = mode_b_mn(MODE);
-  constexpr bool kTile = mode_tile(MODE);
-  constexpr int kStages = Cfg::kStages;
-  constexpr bool CLUSTER = CL != 0;
-  constexpr bool PAIR = CL == 2;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stg = smem + kStages * Cfg::kStageBytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(stg + Cfg::kEpiBytes);
-  uint64_t* empty = full + kMaxStages;
-  uint64_t* acc_full = empty + kMaxStages;      // [2]
-  uint64_t* acc_empty = acc_full + 2;           // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* red = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);
-
-  const int warp = threadIdx.x >> 5;
-  const int KB = a.KB;
-  // work items: tiles (t -> n tile fastest), or with CLUSTER pairs of M tiles: item -> (n tile, M tiles 2j and 2j+1)
-  const int crank = CLUSTER ? static_cast<int>(cluster_ctarank()) : 0;
-  const int m_items = CLUSTER ? (m_tiles + 1) / 2 : m_tiles;
-  const int total = n_tiles * m_items;
-  const int item0 = CLUSTER ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int item_step = CLUSTER ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full[s], 1u);
-      mbar_init(&empty[s], CL == 1 ? 2u : 1u);
-    }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1u); mbar_init(&acc_empty[b], PAIR ? 2u : 1u); }
-    fence_mbar_init();
-  }
-  if (warp == 4 && elect_one()) {
-    tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmAs.m[0]);
-  }
-  if (warp == 5) {
-    if (PAIR) tmem_alloc_pair<2 * BLOCK_N>(tmem_slot);
-    else tmem_alloc<2 * BLOCK_N>(tmem_slot);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (CLUSTER) cluster_sync_all();      // the peer's mbarriers exist before any multicast can signal them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_trigger();
-  pdl_wait();         // preamble done; from here on the kernel reads and writes global memory
-
-  // returns false for the padding tile of an odd M-tile count (its CTA still runs loads and MMAs in lock-step with
-  // the peer, on the clamped last tile, but writes nothing)
-  auto tile_origin = [&](int t, int& n0, int& m0, int& tq0, int& tp0, int& tn0) -> bool {
-    const int nt = t % n_tiles;
-    int mt = t / n_tiles;
-    bool valid = true;
-    if (CLUSTER) {
-      mt = 2 * mt + crank;
-      valid = mt < m_tiles;
-      if (!valid) mt = m_tiles - 1;
-    }
-    n0 = nt * BLOCK_N;
-    m0 = mt * kBlockM;
-    tq0 = tp0 = tn0 = 0;
-    if (kTile) {
-      const int wb = mt % a.tiles_w; mt /= a.tiles_w;
-      const int hb = mt % a.tiles_h;
-      const int nb = mt / a.tiles_h;
-      tq0 = wb * a.tw; tp0 = hb * a.th; tn0 = nb * a.tn;
-      m0 = 0;
-    }
-    return valid;
-  };
-
-  if (warp < 4 || warp >= 6) {
-    // =================================== epilogue warps =======================================
-    const int egrp = warp < 4 ? 0 : 1;
-    const int qw = warp & 3;
-    const int row = qw * 32 + (threadIdx.x & 31);
-    const int etid = egrp * 128 + row;
-    const int ew = egrp * 4 + qw;
-    constexpr int kColsPerGroup = BLOCK_N / kEpiGroups;
-    const uint32_t stg_u32 = smem_u32(stg);
-    const uint32_t red_u32 = smem_u32(red);
-    int it = 0;
-    // BN statistics ride in registers across tiles: t advances by gridDim.x, so whenever the grid is a multiple of the
-    // number of N tiles (2 x 148 CTAs: 1, 2, 4 or 8 tiles) a CTA stays in ONE tile column and publishes its sums once
-    StatAcc acc;
-    acc.clear();
-    for (int t = item0; t < total; t += item_step, ++it) {
-      int n0, m0, tq0, tp0, tn0;
-      const bool valid = tile_origin(t, n0, m0, tq0, tp0, tn0);
-      if (CLUSTER && !valid) {          // padding tile: keep the accumulator hand-shake going, write nothing
-        const int pbuf = it & 1;
-        mbar_wait(&acc_full[pbuf], (it >> 1) & 1, 36);
-        tc_fence_after();
-        tc_fence_before();
-        named_bar_sync(1, kEpiThreads);
-        if (etid == 0) {
-          if (PAIR && crank != 0) mbar_arrive_cluster(mapa_shared(smem_u32(&acc_empty[pbuf]), 0));
-          else mbar_arrive(&acc_empty[pbuf]);
+      if (lane == 0) {
+        if (CL) {
+          const uint32_t local = smem_u32(&empty[s]);
+          mbar_arrive_cluster(mapa_shared(local, 0));
+          mbar_arrive_cluster(mapa_shared(local, 1));
+        } else {
+          mbar_arrive(&empty[s]);
         }
-        continue;
-      }
-      int my_m;
-      if (kTile) {
-        const int wl = row % a.tw;
-        const int t2 = row / a.tw;
-        const int hl = t2 % a.th;
-        const int nl = t2 / a.th;
-        const bool ok = nl < a.tn && (tn0 + nl) < a.batch && (tp0 + hl) < a.dstH && (tq0 + wl) < a.dstW;
-        my_m = ok ? ((tn0 + nl) * a.outH + (tp0 + hl) * a.out_stride + a.out_pa) * a.outW +
-                        (tq0 + wl) * a.out_stride + a.out_pb
-                  : -1;
-      } else {
-        my_m = (m0 + row) < a.M ? (m0 + row) : -1;
-      }
-      const int buf = it & 1;
-      mbar_wait(&acc_full[buf], (it >> 1) & 1, 36);
-      tc_fence_after();
-      const uint32_t stg_row = stg_u32 + row * Cfg::kPitch;
-      const uint32_t taddr_row = tmem_base + (static_cast<uint32_t>(qw * 32) << 16) + buf * BLOCK_N;
-      const bool zero_row = kTile && my_m < 0;
-      if (!STATS && (a.bias != nullptr || a.relu))
-        epi_tmem_to_stage<true>(taddr_row, stg_row, egrp * kColsPerGroup, (egrp + 1) * kColsPerGroup, a, n0, zero_row);
-      else
-        epi_tmem_to_stage<false>(taddr_row, stg_row, egrp * kColsPerGroup, (egrp + 1) * kColsPerGroup, a, n0, zero_row);
-      if (kTile && egrp == 0) sts32(stg_row + BLOCK_N * 2, static_cast<uint32_t>(my_m));
-      tc_fence_before();
-      named_bar_sync(1, kEpiThreads);
-      if (etid == 0) {                                  // every epilogue thread has finished reading this TMEM buffer
-        if (PAIR && crank != 0) mbar_arrive_cluster(mapa_shared(smem_u32(&acc_empty[buf]), 0));   // the leader issues the MMAs
-        else mbar_arrive(&acc_empty[buf]);
-      }
-      if (STATS) {
-        if (acc.n0 >= 0 && acc.n0 != n0) epi_stats_flush<BLOCK_N>(red_u32, etid, ew, a, acc);   // CTA-uniform branch
-        epi_stats_accum<BLOCK_N, kTile>(stg_u32, etid, a, n0, m0, acc);
-      }
-      epi_store<BLOCK_N, kTile>(stg_u32, etid, a, n0, m0);
-      named_bar_sync(1, kEpiThreads);      // staging may be overwritten by the next tile
-    }
-    if (STATS && acc.n0 >= 0) epi_stats_flush<BLOCK_N>(red_u32, etid, ew, a, acc);
-  } else if (warp == 4) {
-    // ===================================== TMA producer =======================================
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t a_bytes = kTile ? static_cast<uint32_t>(a.tw * a.th * a.tn) * 128u : kATileBytes;
-      for (int t = item0; t < total; t += item_step) {
-        int n0, m0, tq0, tp0, tn0;
-        tile_origin(t, n0, m0, tq0, tp0, tn0);
-        if (t + item_step >= total) pdl_trigger_last_tile();
-        int tap = 0, cc = 0, tap_r = 0, tap_s = 0;
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1u, 33);
-          uint8_t* sA = smem + stage * Cfg::kStageBytes;
-          const uint32_t sB = smem_u32(sA + kATileBytes);
-          // CTA pair: every load of BOTH CTAs completes on the LEADER's barrier (it alone waits for operands), which
-          // therefore expects the bytes of the whole pair; the peer CTA arrives nowhere.
-          const uint32_t pair_bar = PAIR ? mapa_shared(smem_u32(&full[stage]), 0) : 0u;
-          if (!PAIR) mbar_arrive_expect_tx(&full[stage], Cfg::kBTileBytes + a_bytes);
-          else if (crank == 0) mbar_arrive_expect_tx(&full[stage], 2u * (Cfg::kBTileBytes / 2 + a_bytes));
-          int widx = tap, dh = 0, dw = 0, mapi = 0;
-          if (kTile) {
-            if (a.ntaps > 0) {
-              widx = a.tap_widx[tap]; dh = a.tap_dh[tap]; dw = a.tap_dw[tap]; mapi = a.tap_map[tap];
-            } else if (MODE == kConvTileFwd) {
-              dh = tap_r * a.dil - a.pad; dw = tap_s * a.dil - a.pad_w;
-            } else {
-              dh = a.pad - tap_r * a.dil; dw = a.pad_w - tap_s * a.dil;
-            }
-          }
-          if (PAIR) {
-            // my half of the weight tile into MY shared memory only: the pair MMA reads the other half from the peer
-            if (kBMn) tma_load_2d_pair(sB, &tmB, widx * a.ldc + n0 + crank * (BLOCK_N / 2), cc * 64, pair_bar);
-            else tma_load_2d_pair(sB, &tmBh, mode_stem(MODE) ? kb * kBlockK : widx * a.kstride + cc * kBlockK,
-                                  n0 + crank * (BLOCK_N / 2), pair_bar);
-            if (MODE == kConvStemTma) tma_load_5d_pair(smem_u32(sA), &tmAs.m[0], 0, kb, tq0, tp0, tn0, pair_bar);
-            else if (kTile) tma_load_4d_pair(smem_u32(sA), &tmAs.m[mapi], cc * 64, tq0 + dw, tp0 + dh, tn0, pair_bar);
-            else tma_load_2d_pair(smem_u32(sA), &tmAs.m[0], kb * kBlockK, m0, pair_bar);
-          } else {
-            if (CLUSTER) {
-              // my half of the weight tile, delivered to both CTAs of the pair (each CTA's `full` barrier sees both halves)
-              if (kBMn) {       // BLOCK_N = 128: the two 64-column boxes are the halves
-                tma_load_2d_multicast(sB + crank * 8192, &tmB, widx * a.ldc + n0 + crank * 64, cc * 64, &full[stage], 0x3);
-              } else {          // K-major: rows [crank * BLOCK_N/2, +BLOCK_N/2) through the half-height box map
-                tma_load_2d_multicast(sB + crank * (BLOCK_N / 2) * 128, &tmBh,
-                                      mode_stem(MODE) ? kb * kBlockK : widx * a.kstride + cc * kBlockK,
-                                      n0 + crank * (BLOCK_N / 2), &full[stage], 0x3);
-              }
-            } else if (kBMn) {
-#pragma unroll
-              for (int j = 0; j < BLOCK_N / 64; ++j)
-                tma_load_2d(sB + j * 8192, &tmB, widx * a.ldc + n0 + j * 64, cc * 64, &full[stage]);
-            } else {
-              // the weight map's box holds min(BLOCK_N, 128) rows
-              constexpr int kBoxRows = BLOCK_N < 128 ? BLOCK_N : 128;
-#pragma unroll
-              for (int h = 0; h < BLOCK_N / kBoxRows; ++h)
-                tma_load_2d(sB + h * kBoxRows * 128, &tmB, mode_stem(MODE) ? kb * kBlockK : widx * a.kstride + cc * kBlockK,
-                            n0 + h * kBoxRows, &full[stage]);
-            }
-            if (MODE == kConvStemTma) tma_load_5d(smem_u32(sA), &tmAs.m[0], 0, kb, tq0, tp0, tn0, &full[stage]);
-            else if (kTile) tma_load_4d(smem_u32(sA), &tmAs.m[mapi], cc * 64, tq0 + dw, tp0 + dh, tn0, &full[stage]);
-            else tma_load_2d(smem_u32(sA), &tmAs.m[0], kb * kBlockK, m0, &full[stage]);
-          }
-          if (++cc == a.cchunks) { cc = 0; ++tap; if (++tap_s == a.S) { tap_s = 0; ++tap_r; } }
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    // ====================================== MMA issuer ========================================
-    constexpr uint32_t idesc = idesc_bf16(PAIR ? 2 * kBlockM : kBlockM, BLOCK_N, 0, kBMn ? 1 : 0);
-    // stage-0 descriptors built once; stage / K-slice steps are 32-bit adds on the low word (see desc_join)
-    const uint64_t pdA0 = smem_desc_sw128(smem_u32(smem), 0, 1024);
-    const uint64_t pdB0 = kBMn ? smem_desc_sw128(smem_u32(smem) + kATileBytes, 8192, 1024)
-                               : smem_desc_sw128(smem_u32(smem) + kATileBytes, 0, 1024);
-    const uint32_t pa_lo = static_cast<uint32_t>(pdA0), pa_hi = static_cast<uint32_t>(pdA0 >> 32);
-    const uint32_t pb_lo = static_cast<uint32_t>(pdB0), pb_hi = static_cast<uint32_t>(pdB0 >> 32);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    if (PAIR && crank != 0) {
-      // peer CTA of a pair: the leader issues the MMAs for both (its operands' arrival is signalled to the leader directly)
-    } else {
-      for (int t = item0; t < total; t += item_step, ++it) {
-        const int buf = it & 1;
-        mbar_wait(&acc_empty[buf], ((it >> 1) & 1) ^ 1u, 35);     // epilogue(s) have drained this TMEM buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * BLOCK_N;
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(&full[stage], phase, 34);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t so = static_cast<uint32_t>(stage) * (Cfg::kStageBytes >> 4);
-#pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) {
-              const uint64_t da = desc_join(pa_lo + so + 2u * k, pa_hi);
-              const uint64_t db = desc_join(pb_lo + so + (kBMn ? 128u : 2u) * k, pb_hi);
-              if (PAIR) umma_bf16_pair(d_tmem, da, db, idesc, (kb | k) != 0);
-              else umma_bf16(d_tmem, da, db, idesc, (kb | k) != 0);
-            }
-            if (PAIR) {
-              umma_commit_pair_multicast(&empty[stage], 0x3);          // frees the stage in both CTAs
-              if (kb == KB - 1) umma_commit_pair_multicast(&acc_full[buf], 0x3);
-            } else {
-              if (CLUSTER) umma_commit_multicast(&empty[stage], 0x3);  // frees the stage in BOTH CTAs of the pair
-              else umma_commit(&empty[stage]);
-              if (kb == KB - 1) umma_commit(&acc_full[buf]);
-            }
-          }
-          __syncwarp();
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (CLUSTER) cluster_sync_all();      // no CTA leaves while its peer may still multicast into it / signal its barriers
-  if (warp == 5) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair<2 * BLOCK_N>(tmem_base);
-    else tmem_dealloc<2 * BLOCK_N>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// deep-ring persistent kernel: ONE CTA per SM (or one cta_group::2 CTA pair per SM pair)
-// ---------------------------------------------------------------------------------------------
-// What bounds the long-K layers is operand delivery, L2 -> shared memory: a 128 x 128 x 64 step needs 32 KB per 256
-// tensor-pipe cycles = 128 B/cycle/SM, while the chip sustains ~45 B/cycle/SM out of L2 (cuBLAS's own bf16 peak with
-// 256 x 256 pair tiles sits right at that limit).  This variant therefore
-//   * spends the whole SM on one CTA: the ring is as deep as 227 KB allow (5 x 32 KB for 128 x 128, 3 x 48 KB for
-//     128 x 256, 5 x 32 KB for a 256 x 256 pair tile), so TMA round trips (~1-1.5 k cycles under load) stay covered;
-//   * supports 256-wide tiles (A is re-used for twice the columns: 96 B/cycle) and CTA pairs with ONE M = 256 MMA
-//     (tcgen05.mma.cta_group::2: each SM loads its 128 rows of A and HALF of the weight tile: 64 B/cycle at N = 256);
-//   * drains the accumulator in 64-column chunks through two small staging buffers (2 x 18 KB instead of one
-//     34-68 KB tile image), which is what frees the shared memory for the ring.
-// TMEM: 2 x BLOCK_N columns (double-buffered accumulator; N = 256 uses all 512 columns — fine with one CTA per SM).
-template <int BLOCK_N, bool PAIR>
-struct DeepCfg {
-  static constexpr int kBLoadRows = PAIR ? BLOCK_N / 2 : BLOCK_N;   // weight rows (K-major) / columns (MN-major) per CTA
-  static constexpr int kBTileBytes = kBLoadRows * 128;
-  static constexpr int kSfBytes = 1024;                              // MX scale atoms of a stage: SFA 512 B + SFB 512 B
-  static constexpr int kStageBytes = kATileBytes + kBTileBytes + kSfBytes;
-  static constexpr int kChunk = 64;                                  // accumulator columns drained per epilogue pass
-  static constexpr int kChunkPitch = kChunk * 2 + 16;
-  static constexpr int kChunkBytes = kBlockM * kChunkPitch;          // 18,432
-  static constexpr int kRedBytes = 4 * kEpiGroups * 2 * kChunk * 4;  // [epi warps][2][64] floats
-  static constexpr int kFixed = 256 /*barriers*/ + kRedBytes + 1024 /*alignment*/;
-  static constexpr int kStagesFit = (232448 - kFixed - 2 * kChunkBytes) / kStageBytes;
-  static constexpr int kStages = kStagesFit > 8 ? 8 : kStagesFit;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kChunkBytes + kFixed;
-};
-constexpr int kDeepMaxStages = 8;
-
-template <int BLOCK_N, int MODE, bool STATS, bool PAIR>
-__global__ void __launch_bounds__(kThreads, 1)
-conv_gemm_deep_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBh,
-                      const __grid_constant__ TmaSet tmAs, ConvArgs a, int n_tiles, int m_tiles) {
-  using Cfg = DeepCfg<BLOCK_N, PAIR>;
-  constexpr bool kBMn = mode_b_mn(MODE);
-  constexpr bool kTile = mode_tile(MODE);
-  constexpr int kStages = Cfg::kStages;
-  static_assert(!(PAIR && kBMn && BLOCK_N < 128), "MN-major pair tiles need 64-column halves");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stg = smem + kStages * Cfg::kStageBytes;                   // two chunk staging buffers
-  uint64_t* full = reinterpret_cast<uint64_t*>(stg + 2 * Cfg::kChunkBytes);
-  uint64_t* empty = full + kDeepMaxStages;
-  uint64_t* acc_full = empty + kDeepMaxStages;  // [2]
-  uint64_t* acc_empty = acc_full + 2;           // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* red = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);
-
-  const int warp = threadIdx.x >> 5;
-  const int KB = a.KB;
-  const int crank = PAIR ? static_cast<int>(cluster_ctarank()) : 0;
-  const int m_items = PAIR ? (m_tiles + 1) / 2 : m_tiles;
-  const int total = n_tiles * m_items;
-  const int item0 = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int item_step = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full[s], 1u);
-      mbar_init(&empty[s], 1u);
-    }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1u); mbar_init(&acc_empty[b], PAIR ? 2u : 1u); }
-    fence_mbar_init();
-  }
-  if (warp == 4 && elect_one()) {
-    tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmBh);
-    tma_prefetch_desc(&tmAs.m[0]);
-  }
-  // single-CTA 128-wide tiles may run MX block-scaled operands: 8 more TMEM columns for the scale factors (the CTA owns
-  // the SM, so rounding the allocation up to the next power of two costs nothing)
-  constexpr int kTmemCols = (!PAIR && BLOCK_N == 128) ? 512 : 2 * BLOCK_N;
-  if (warp == 5) {
-    if (PAIR) tmem_alloc_pair<kTmemCols>(tmem_slot);
-    else tmem_alloc<kTmemCols>(tmem_slot);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR) cluster_sync_all();         // the peer's mbarriers exist before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_trigger();
-  pdl_wait();         // preamble done; from here on the kernel reads and writes global memory
-
-  auto tile_origin = [&](int t, int& n0, int& m0, int& tq0, int& tp0, int& tn0) -> bool {
-    const int nt = t % n_tiles;
-    int mt = t / n_tiles;
-    bool valid = true;
-    if (PAIR) {
-      mt = 2 * mt + crank;
-      valid = mt < m_tiles;
-      if (!valid) mt = m_tiles - 1;     // padding tile of an odd M-tile count: loads + MMAs in lock-step, no stores
-    }
-    n0 = nt * BLOCK_N;
-    m0 = mt * kBlockM;
-    tq0 = tp0 = tn0 = 0;
-    if (kTile) {
-      const int wb = mt % a.tiles_w; mt /= a.tiles_w;
-      const int hb = mt % a.tiles_h;
-      const int nb = mt / a.tiles_h;
-      tq0 = wb * a.tw; tp0 = hb * a.th; tn0 = nb * a.tn;
-      m0 = 0;
-    }
-    return valid;
-  };
-
-  if (warp < 4 || warp >= 6) {
-    // =================================== epilogue warps =======================================
-    const int egrp = warp < 4 ? 0 : 1;
-    const int qw = warp & 3;
-    const int row = qw * 32 + (threadIdx.x & 31);
-    const int etid = egrp * 128 + row;
-    const int ew = egrp * 4 + qw;
-    const uint32_t stg_u32 = smem_u32(stg);
-    const uint32_t red_u32 = smem_u32(red);
-    const bool bias_relu = !STATS && (a.bias != nullptr || a.relu);
-    const float deq = (a.fp8 == 1 || a.fp8 == 2) ? (*a.deq_a) * (*a.deq_b) : 1.0f;   // per-tensor fp8: undo both scales
-    int it = 0;
-    uint32_t chunk_ctr = 0;             // staging buffer = chunk_ctr & 1 (identical sequence in every epilogue thread)
-    constexpr int kChunks = BLOCK_N / Cfg::kChunk;
-    // BN statistics stay in registers across the tiles of one tile column (see the persistent kernel); one accumulator
-    // set per 64-column chunk, published together when the column changes and at the end
-    StatAcc acc[kChunks];
-#pragma unroll
-    for (int ch = 0; ch < kChunks; ++ch) acc[ch].clear();
-    auto flush_all = [&]() {
-#pragma unroll
-      for (int ch = 0; ch < kChunks; ++ch) {
-        if (acc[ch].n0 >= 0) epi_stats_flush<Cfg::kChunk>(red_u32, etid, ew, a, acc[ch]);
-        named_bar_sync(1, kEpiThreads);          // the next flush rewrites the scratch the fold above reads
       }
     };
-    for (int t = item0; t < total; t += item_step, ++it) {
-      int n0, m0, tq0, tp0, tn0;
-      const bool valid = tile_origin(t, n0, m0, tq0, tp0, tn0);
-      const int buf = it & 1;
-      mbar_wait(&acc_full[buf], (it >> 1) & 1, 52);
-      tc_fence_after();
-      if (PAIR && !valid) {             // padding tile: keep the accumulator hand-shake going, write nothing
-        tc_fence_before();
-        named_bar_sync(1, kEpiThreads);
-        if (etid == 0) {
-          if (crank != 0) mbar_arrive_cluster(mapa_shared(smem_u32(&acc_empty[buf]), 0));
-          else mbar_arrive(&acc_empty[buf]);
-        }
-        continue;
-      }
-      int my_m;
-      if (kTile) {
-        const int wl = row % a.tw;
-        const int t2 = row / a.tw;
-        const int hl = t2 % a.th;
-        const int nl = t2 / a.th;
-        const bool ok = nl < a.tn && (tn0 + nl) < a.batch && (tp0 + hl) < a.dstH && (tq0 + wl) < a.dstW;
-        my_m = ok ? ((tn0 + nl) * a.outH + (tp0 + hl) * a.out_stride + a.out_pa) * a.outW +
-                        (tq0 + wl) * a.out_stride + a.out_pb
-                  : -1;
-      } else {
-        my_m = (m0 + row) < a.M ? (m0 + row) : -1;
-      }
-      const bool zero_row = kTile && my_m < 0;
-      const uint32_t taddr_row = tmem_base + (static_cast<uint32_t>(qw * 32) << 16) + buf * BLOCK_N;
-      if (STATS && acc[0].n0 >= 0 && acc[0].n0 != n0) flush_all();      // CTA-uniform branch
-#pragma unroll
-      for (int ch = 0; ch < kChunks; ++ch, ++chunk_ctr) {
-        const uint32_t sbuf = stg_u32 + (chunk_ctr & 1u) * Cfg::kChunkBytes;
-        const uint32_t stg_row = sbuf + row * Cfg::kChunkPitch;
-        // my 32 of the chunk's 64 columns: TMEM -> (bias, ReLU) -> bf16 -> staging row
-        if (bias_relu)
-          epi_tmem_to_stage<true>(taddr_row + ch * Cfg::kChunk, stg_row, egrp * 32, egrp * 32 + 32, a,
-                                  n0 + ch * Cfg::kChunk, zero_row, deq);
-        else
-          epi_tmem_to_stage<false>(taddr_row + ch * Cfg::kChunk, stg_row, egrp * 32, egrp * 32 + 32, a,
-                                   n0 + ch * Cfg::kChunk, zero_row, deq);
-        if (kTile && egrp == 0) sts32(stg_row + Cfg::kChunk * 2, static_cast<uint32_t>(my_m));
-        if (ch == kChunks - 1) tc_fence_before();
-        // all 256 threads: the chunk is staged; everybody has also left the buffer written two chunks ago
-        named_bar_sync(1, kEpiThreads);
-        if (ch == kChunks - 1 && etid == 0) {           // every epilogue thread has finished reading this TMEM buffer
-          if (PAIR && crank != 0) mbar_arrive_cluster(mapa_shared(smem_u32(&acc_empty[buf]), 0));
-          else mbar_arrive(&acc_empty[buf]);
-        }
-        // (no trailing barrier: the next chunk stages into the OTHER buffer, and nobody rewrites the stats scratch or
-        //  this buffer before passing the next chunk's barrier, which everyone reaches only after leaving this call)
-        if (STATS) epi_stats_accum<Cfg::kChunk, kTile>(sbuf, etid, a, n0 + ch * Cfg::kChunk, m0, acc[ch]);
-        epi_store<Cfg::kChunk, kTile>(sbuf, etid, a, n0 + ch * Cfg::kChunk, m0);
-      }
-    }
-    if (STATS) flush_all();
-  } else if (warp == 4) {
-    // ===================================== TMA producer =======================================
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t a_bytes = kTile ? static_cast<uint32_t>(a.tw * a.th * a.tn) * 128u : kATileBytes;
-      const int kElems = a.fp8 ? 128 : 64;            // elements in one 128-byte operand row = K extent of a k-block
-      const int mnBoxes = Cfg::kBLoadRows / kElems;   // MN-major B: boxes of kElems columns x kElems K-rows (128 B rows)
-      const uint32_t mnBoxBytes = 128u * static_cast<uint32_t>(kElems);
-      for (int t = item0; t < total; t += item_step) {
-        int n0, m0, tq0, tp0, tn0;
-        tile_origin(t, n0, m0, tq0, tp0, tn0);
-        if (t + item_step >= total) pdl_trigger_last_tile();
-        int tap = 0, cc = 0, tap_r = 0, tap_s = 0;
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1u, 49);
-          uint8_t* sA = smem + stage * Cfg::kStageBytes;
-          const uint32_t sB = smem_u32(sA + kATileBytes);
-          const uint32_t pair_bar = PAIR ? mapa_shared(smem_u32(&full[stage]), 0) : 0u;
-          const bool mx = !PAIR && a.fp8 == 3;
-          if (!PAIR) mbar_arrive_expect_tx(&full[stage], Cfg::kBTileBytes + a_bytes + (mx ? 1024u : 0u));
-          else if (crank == 0) mbar_arrive_expect_tx(&full[stage], 2u * (Cfg::kBTileBytes + a_bytes));
-          if (mx) {      // this k-block's scale atoms (GEMM mode: tile = row block m0/128, weight block n0/128)
-            const uint32_t sSF = sB + Cfg::kBTileBytes;
-            bulk_load(sSF, a.sfa + (static_cast<size_t>(m0 / kBlockM) * KB + kb) * 512, 512, &full[stage]);
-            bulk_load(sSF + 512, a.sfb + (static_cast<size_t>(n0 / 128) * KB + kb) * 512, 512, &full[stage]);
-          }
-          int widx = tap, dh = 0, dw = 0, mapi = 0;
-          if (kTile) {
-            if (a.ntaps > 0) {
-              widx = a.tap_widx[tap]; dh = a.tap_dh[tap]; dw = a.tap_dw[tap]; mapi = a.tap_map[tap];
-            } else if (MODE == kConvTileFwd) {
-              dh = tap_r * a.dil - a.pad; dw = tap_s * a.dil - a.pad_w;
-            } else {
-              dh = a.pad - tap_r * a.dil; dw = a.pad_w - tap_s * a.dil;
-            }
-          }
-          const int kcoord = widx * a.kstride + cc * kElems;
-          const int nb0 = n0 + crank * Cfg::kBLoadRows;        // first weight row / column this CTA fetches
-          if (PAIR) {
-            if (kBMn) {
-              for (int j = 0; j < mnBoxes; ++j)
-                tma_load_2d_pair(sB + j * mnBoxBytes, &tmB, widx * a.ldc + nb0 + j * kElems, cc * kElems, pair_bar);
-            } else if (Cfg::kBLoadRows == 128) {
-              tma_load_2d_pair(sB, &tmB, kcoord, nb0, pair_bar);           // the full map's box is 128 rows
-            } else {
-              tma_load_2d_pair(sB, &tmBh, kcoord, nb0, pair_bar);          // half-height box map
-            }
-            if (kTile) tma_load_4d_pair(smem_u32(sA), &tmAs.m[mapi], cc * kElems, tq0 + dw, tp0 + dh, tn0, pair_bar);
-            else tma_load_2d_pair(smem_u32(sA), &tmAs.m[0], kb * kElems, m0, pair_bar);
-          } else {
-            if (kBMn) {
-              for (int j = 0; j < mnBoxes; ++j)
-                tma_load_2d(sB + j * mnBoxBytes, &tmB, widx * a.ldc + n0 + j * kElems, cc * kElems, &full[stage]);
-            } else {
-              constexpr int kBoxRows = BLOCK_N < 128 ? BLOCK_N : 128;      // the weight map's box height
-#pragma unroll
-              for (int h = 0; h < BLOCK_N / kBoxRows; ++h)
-                tma_load_2d(sB + h * kBoxRows * 128, &tmB, kcoord, n0 + h * kBoxRows, &full[stage]);
-            }
-            if (kTile) tma_load_4d(smem_u32(sA), &tmAs.m[mapi], cc * kElems, tq0 + dw, tp0 + dh, tn0, &full[stage]);
-            else tma_load_2d(smem_u32(sA), &tmAs.m[0], kb * kElems, m0, &full[stage]);
-          }
-          if (++cc == a.cchunks) { cc = 0; ++tap; if (++tap_s == a.S) { tap_s = 0; ++tap_r; } }
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    // ====================================== MMA issuer ========================================
-    constexpr int kMmaM = PAIR ? 2 * kBlockM : kBlockM;
-    const bool f8 = a.fp8 != 0;
-    const bool mxk = !PAIR && BLOCK_N == 128 && !kBMn && a.fp8 == 3;      // MX block-scaled operands (K-major GEMM only)
-    const uint32_t idesc = f8 ? idesc_f8(kMmaM, BLOCK_N, a.fp8 == 2 ? 1 : 0, 0, 0, kBMn ? 1 : 0)
-                              : idesc_bf16(kMmaM, BLOCK_N, 0, kBMn ? 1 : 0);
-    // MN-major B: K rows of 128 bytes; one MMA consumes 16 (bf16) / 32 (fp8) K rows, chunks of 64 / 128 columns
-    const uint32_t mnKStep = f8 ? 4096u : 2048u, mnLbo = f8 ? 16384u : 8192u;
-    // descriptors of stage 0 / K slice 0, built once; stages and K slices are 32-bit adds on the low word
-    const uint32_t sA0 = smem_u32(smem), sB0 = sA0 + kATileBytes;
-    const uint64_t dA0 = smem_desc_sw128(sA0, 0, 1024);
-    const uint64_t dB0 = kBMn ? smem_desc_sw128(sB0, mnLbo, 1024) : smem_desc_sw128(sB0, 0, 1024);
-    const uint32_t a_lo = static_cast<uint32_t>(dA0), a_hi = static_cast<uint32_t>(dA0 >> 32);
-    const uint32_t b_lo = static_cast<uint32_t>(dB0), b_hi = static_cast<uint32_t>(dB0 >> 32);
-    constexpr uint32_t kStageStep = Cfg::kStageBytes >> 4;
-    const uint32_t bStep = kBMn ? (mnKStep >> 4) : 2u;         // K slice of one MMA in 16-byte units (A: always 2)
+    const int etid = threadIdx.x;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    float acc[BLOCK_N / 2];
     int stage = 0;
     uint32_t phase = 0;
-    int it = 0;
-    if (!(PAIR && crank != 0)) {        // the leader issues the MMAs of a pair
-      for (int t = item0; t < total; t += item_step, ++it) {
-        const int buf = it & 1;
-        mbar_wait(&acc_empty[buf], ((it >> 1) & 1) ^ 1u, 51);     // epilogue(s) have drained this TMEM buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * BLOCK_N;
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(&full[stage], phase, 50);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t so = static_cast<uint32_t>(stage) * kStageStep;
-            if (mxk) {
-              // scale atoms of this k-block: shared memory -> TMEM (4 columns each), in order with the MMAs that use them
-              const uint32_t sSF = sB0 + Cfg::kBTileBytes + static_cast<uint32_t>(stage) * Cfg::kStageBytes;
-              tmem_cp_32x128b_warpx4(tmem_base + 2 * BLOCK_N, smem_desc_nosw(sSF, 0, 128));
-              tmem_cp_32x128b_warpx4(tmem_base + 2 * BLOCK_N + 4, smem_desc_nosw(sSF + 512, 0, 128));
-            }
+    for (int item = unit; item < items; item += units) {
+      decode(item);
+      int prev = -1;
+      for (int kb = 0; kb < KB; ++kb) {
+        mbar_wait(&full[stage], phase, 18);
+        const uint32_t so = static_cast<uint32_t>(stage) * (Cfg::kStageBytes >> 4);
+        wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {                      // 4 x 32 bytes of K per 128-byte row
-              const uint64_t da = desc_join(a_lo + so + 2u * k, a_hi);
-              const uint64_t db = desc_join(b_lo + so + bStep * k, b_hi);
-              const bool acc = (kb | k) != 0;
-              if (mxk) {
-                umma_mxf8(d_tmem, da, db, idesc_mxf8(kBlockM, BLOCK_N, 0, 0, k, k), acc, tmem_base + 2 * BLOCK_N,
-                          tmem_base + 2 * BLOCK_N + 4);
-              } else if (f8) {
-                if (PAIR) umma_f8_pair(d_tmem, da, db, idesc, acc);
-                else umma_f8(d_tmem, da, db, idesc, acc);
-              } else {
-                if (PAIR) umma_bf16_pair(d_tmem, da, db, idesc, acc);
-                else umma_bf16(d_tmem, da, db, idesc, acc);
-              }
-            }
-            if (PAIR) {
-              umma_commit_pair_multicast(&empty[stage], 0x3);          // frees the stage in both CTAs
-              if (kb == KB - 1) umma_commit_pair_multicast(&acc_full[buf], 0x3);
-            } else {
-              umma_commit(&empty[stage]);
-              if (kb == KB - 1) umma_commit(&acc_full[buf]);
-            }
-          }
-          __syncwarp();
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t da = desc_join(oa_lo + so + 2u * k, oa_hi);
+          const uint64_t db = desc_join(ob_lo + so + (kBMn ? 128u : 2u) * k, ob_hi);
+          mma_kstep<BLOCK_N, FP8, kBMn>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
         }
+        wgmma_commit();
+        wgmma_wait<1>();               // the previous k-block's MMAs are done: hand its stage back to the producers
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == nstages) { stage = 0; phase ^= 1u; }
       }
+      wgmma_wait<0>();
+      acc_fence(acc);
+      release(prev);
+      // every consumer is past the previous tile's stores: the staging tile may be rewritten
+      named_bar_sync(1, kEpiThreads);
+      auto dest_row = [&](int row) -> int {     // output row of accumulator row `row`, or -1
+        if (kTile) {
+          const int wl = row % a.tw;
+          const int t2 = row / a.tw;
+          const int hl = t2 % a.th;
+          const int nl = t2 / a.th;
+          const bool ok = nl < a.tn && (tn0 + nl) < a.batch && (tp0 + hl) < a.dstH && (tq0 + wl) < a.dstW;
+          return ok ? ((tn0 + nl) * a.outH + (tp0 + hl) * a.out_stride + a.out_pa) * a.outW + (tq0 + wl) * a.out_stride +
+                          a.out_pb
+                    : -1;
+        }
+        return (m0 + row) < a.M ? (m0 + row) : -1;
+      };
+      // rows outside the image: exact zeros (keeps the BN sums clean)
+      const bool z0 = kTile && dest_row(r0) < 0, z1 = kTile && dest_row(r0 + 8) < 0;
+      const float deq = FP8 ? *a.deq_a * *a.deq_b : 1.0f;
+      if (!STATS && (a.bias != nullptr || a.relu)) epi_acc_to_stage<BLOCK_N, true>(acc, stg, r0, z0, z1, a, n0, deq);
+      else epi_acc_to_stage<BLOCK_N, false>(acc, stg, r0, z0, z1, a, n0, deq);
+      // the row's destination index rides in the pad bytes of its staging row (pitch = 2*BLOCK_N + 16)
+      if (kTile && etid < kBlockM) sts32(stg + etid * Cfg::kPitch + BLOCK_N * 2, static_cast<uint32_t>(dest_row(etid)));
+      named_bar_sync(1, kEpiThreads);
+      epi_stats_store<BLOCK_N, STATS, kTile>(stg, smem_u32(full) + 256, etid, warp, a, n0, m0);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR) cluster_sync_all();         // no CTA leaves while its peer may still signal its barriers / read its smem
-  if (warp == 5) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair<kTmemCols>(tmem_base);
-    else tmem_dealloc<kTmemCols>(tmem_base);
-  }
+  if (CL) cluster_sync_all();          // no CTA leaves while its peer may still multicast into it or arrive on it
 }
 
 // ---------------------------------------------------------------------------------------------
 // wgrad kernel: dW[co][k] += sum over a pixel range of dY[m][co] * im2col(X)[m][k]
 // ---------------------------------------------------------------------------------------------
-constexpr int kWgMaxStages = 3;
+constexpr int kWgMaxStages = 4;
 constexpr int kWgStageBytes = 32768;           // A: 2 x [64 pix][64 co], B: 2 x [64 pix][64 k]
 constexpr int kWgPitch = 132;                  // fp32 staging pitch (floats)
 constexpr int kWgEpiBytes = kBlockM * kWgPitch * 4;
@@ -1291,11 +688,10 @@ constexpr int wg_smem_bytes(int stages) {
 }
 
 // SWAP = operand roles exchanged for narrow outputs (Cout tile of 64): the 128-row MMA dimension carries the k
-// columns and N = 64 output channels, so no half of the tensor-core tile multiplies zero rows (ncu: the Cout = 64
-// layers kept the pipe ~49 % busy doing 50 % useful work).  The accumulator comes out transposed ([k col][co]) and
-// is staged transposed so the global reductions stay row-contiguous.
+// columns and N = 64 output channels, so no half of the tensor-core tile multiplies zero rows.  The accumulator comes
+// out transposed ([k col][co]) and is staged transposed so the global reductions stay row-contiguous.
 template <int MODE, bool SWAP>
-__global__ void __launch_bounds__(kThreads, 3)
+__global__ void __launch_bounds__(kThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ TmaSet tmXs, WgradArgs a) {
   const CUtensorMap& tmX = tmXs.m[0];
   constexpr bool kXTma = (MODE == kConvGemm || MODE == kConvTileFwd || MODE == kConvStemTma);
@@ -1306,8 +702,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   const int pipe_bytes = nstages * kWgStageBytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (pipe_bytes > kWgEpiBytes ? pipe_bytes : kWgEpiBytes));
   uint64_t* empty = full + kWgMaxStages;
-  uint64_t* acc_full = empty + kWgMaxStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
 
   const int warp = threadIdx.x >> 5;
   const int col0 = blockIdx.x * 128;          // first k column of this tile
@@ -1321,16 +715,14 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   if (threadIdx.x == 0) {
     for (int s = 0; s < nstages; ++s) {
       mbar_init(&full[s], kXTma ? 1u : (kProducerThreads + 1u));
-      mbar_init(&empty[s], 1u);
+      mbar_init(&empty[s], kEpiThreads / 32);
     }
-    mbar_init(acc_full, 1u);
     fence_mbar_init();
   }
-  if (warp == 4 && elect_one()) {
+  if (warp == kTmaWarp && elect_one()) {
     tma_prefetch_desc(&tmDy);
     if (kXTma) tma_prefetch_desc(&tmX);
   }
-  if (warp == 5) tmem_alloc<128>(tmem_slot);
   if (kTile) {
     // pixel boxes may hold fewer than 64 rows: the unused K rows of EVERY operand chunk must read as zero
     const int rows = a.tw * a.th * a.tn;
@@ -1342,18 +734,13 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
       }
     fence_proxy_async_smem();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < 4 || warp >= 6) {
-    const int egrp = warp < 4 ? 0 : 1;
-    const int qw = warp & 3;
-    const int ew = egrp * 4 + qw;
-    if (!kXTma && warp < 4) {
-      const int chunk = threadIdx.x >> 6;      // which 64-column half of the B tile
-      const int row = threadIdx.x & 63;        // pixel row inside the k-block
+  if (warp >= kProducerWarp0 && warp < kTmaWarp) {
+    if (!kXTma) {
+      const int t = threadIdx.x - kEpiThreads;
+      const int chunk = t >> 6;                // which 64-column half of the B tile
+      const int row = t & 63;                  // pixel row inside the k-block
       const int colc = col0 + chunk * 64;      // first k column of my chunk
       const bool col_ok = colc < a.ncols;
       int tap_r = 0, tap_s = 0, c_off = 0;
@@ -1420,47 +807,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
       fence_proxy_async_smem();
       for (int i = (KB > kLag ? KB - kLag : 0); i < KB; ++i) mbar_arrive(&full[i % nstages]);
     }
-
-    // epilogue: TMEM -> fp32 staging -> coalesced vector reductions into the gradient arena
-    mbar_wait(acc_full, 0, 68);
-    tc_fence_after();
-    float* stg = reinterpret_cast<float*>(smem);
-    const int row = qw * 32 + (threadIdx.x & 31);
-    constexpr int kAccCols = SWAP ? 64 : 128;
-#pragma unroll 1
-    for (int c0 = egrp * (kAccCols / kEpiGroups); c0 < (egrp + 1) * (kAccCols / kEpiGroups); c0 += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(qw * 32) << 16) + c0, v);
-      tmem_ld_wait();
-      if (SWAP) {
-        // accumulator row = k column, accumulator column = output channel: stage as [co][k col]
-#pragma unroll
-        for (int j = 0; j < 32; ++j) stg[(c0 + j) * kWgPitch + row] = __uint_as_float(v[j]);
-      } else {
-        float4* d = reinterpret_cast<float4*>(stg + row * kWgPitch + c0);
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          d[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                             __uint_as_float(v[4 * j + 3]));
-      }
-    }
-    tc_fence_before();
-    named_bar_sync(1, kEpiThreads);
-    const int lane = threadIdx.x & 31;
-    const int vc = col0 + lane * 4;                    // column in the padded (tap, Cpad) space
-    const int vtap = vc / a.Cpad;
-    const int vch = vc - vtap * a.Cpad;
-    if (vc < a.ncols && vch < a.Cw) {                  // channel padding of a tap has no dw column
-      const int c = vtap * a.Cw + vch;
-      for (int r = ew; r < kCoTile; r += 4 * kEpiGroups) {
-        const int co = co0 + r;
-        if (co < a.Cout) {
-          const float4 val = *reinterpret_cast<const float4*>(stg + r * kWgPitch + lane * 4);
-          red_add_f32x4(a.dw + static_cast<size_t>(co) * a.ldw + c, val.x, val.y, val.z, val.w);
-        }
-      }
-    }
-  } else if (warp == 4) {
+  } else if (warp == kTmaWarp) {
     if (elect_one()) {
       // taps / channel offsets of the two 64-column chunks of the B tile (tile mode)
       int tdh[2] = {0, 0}, tdw[2] = {0, 0}, tmap[2] = {0, 0}, tc0[2] = {0, 0};
@@ -1520,35 +867,72 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
       }
     }
   } else {
-    constexpr uint32_t idesc = idesc_bf16(128, SWAP ? 64 : 128, 1, 1);
-    int stage = 0;
+    // consumers: warpgroup g multiplies the g-th 64-wide chunk of the M operand (both operands MN-major)
+    constexpr int kN = SWAP ? 64 : 128;
+    const int wg = warp >> 2;
+    const int lane = threadIdx.x & 31;
+    float acc[kN / 2];
+#pragma unroll
+    for (int i = 0; i < kN / 2; ++i) acc[i] = 0.f;
+    int stage = 0, prev = -1;
     uint32_t phase = 0;
     for (int i = 0; i < KB; ++i) {
       mbar_wait(&full[stage], phase, 66);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sDy = smem_u32(smem + stage * kWgStageBytes);
-        const uint32_t sX = sDy + 16384;
-        const uint32_t sA = SWAP ? sX : sDy;      // M operand: 128 rows = two 64-wide MN-major chunks 8 KB apart
-        const uint32_t sB = SWAP ? sDy : sX;      // N operand (SWAP: one 64-channel chunk of dY)
+      const uint32_t sDy = smem_u32(smem + stage * kWgStageBytes);
+      const uint32_t sX = sDy + 16384;
+      const uint32_t sA = (SWAP ? sX : sDy) + wg * 8192;   // M operand: 128 rows = two 64-wide MN-major chunks 8 KB apart
+      const uint32_t sB = SWAP ? sDy : sX;                 // N operand (SWAP: one 64-channel chunk of dY)
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t da = smem_desc_sw128(sA + k * 2048, 8192, 1024);
-          const uint64_t db = smem_desc_sw128(sB + k * 2048, 8192, 1024);
-          umma_bf16(tmem_base, da, db, idesc, (i | k) != 0);
-        }
-        umma_commit(&empty[stage]);
-        if (i == KB - 1) umma_commit(acc_full);
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t da = smem_desc_sw128(sA + k * 2048, 8192, 1024);
+        const uint64_t db = smem_desc_sw128(sB + k * 2048, 8192, 1024);
+        if constexpr (SWAP) wgmma_bf16_n64<1, 1>(acc, da, db, (i | k) != 0 ? 1u : 0u);
+        else wgmma_bf16_n128<1, 1>(acc, da, db, (i | k) != 0 ? 1u : 0u);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = stage;
       if (++stage == nstages) { stage = 0; phase ^= 1u; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<128>(tmem_base);
+    wgmma_wait<0>();
+    acc_fence(acc);
+    named_bar_sync(1, kEpiThreads);
+    // epilogue: registers -> fp32 staging -> coalesced vector reductions into the gradient arena
+    float* stg = reinterpret_cast<float*>(smem);
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < kN / 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      if (SWAP) {
+        // accumulator row = k column, accumulator column = output channel: stage as [co][k col]
+        stg[c * kWgPitch + r0] = acc[4 * j];
+        stg[(c + 1) * kWgPitch + r0] = acc[4 * j + 1];
+        stg[c * kWgPitch + r0 + 8] = acc[4 * j + 2];
+        stg[(c + 1) * kWgPitch + r0 + 8] = acc[4 * j + 3];
+      } else {
+        *reinterpret_cast<float2*>(stg + r0 * kWgPitch + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(stg + (r0 + 8) * kWgPitch + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+    }
+    named_bar_sync(1, kEpiThreads);
+    const int vc = col0 + lane * 4;                    // column in the padded (tap, Cpad) space
+    const int vtap = vc / a.Cpad;
+    const int vch = vc - vtap * a.Cpad;
+    if (vc < a.ncols && vch < a.Cw) {                  // channel padding of a tap has no dw column
+      const int c = vtap * a.Cw + vch;
+      for (int r = warp; r < kCoTile; r += kEpiThreads / 32) {
+        const int co = co0 + r;
+        if (co < a.Cout) {
+          const float4 val = *reinterpret_cast<const float4*>(stg + r * kWgPitch + lane * 4);
+          red_add_f32x4(a.dw + static_cast<size_t>(co) * a.ldw + c, val.x, val.y, val.z, val.w);
+        }
+      }
+    }
   }
 }
 
@@ -1651,247 +1035,135 @@ inline int stem_sp(int S) { return S <= 4 ? 4 : (S <= 8 ? 8 : 16); }
 
 inline int floor_div(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 
-template <int BLOCK_N, int MODE, bool STATS>
-cudaError_t launch_fwd_t(const CUtensorMap& tmB, const TmaSet& tmA, const ConvArgs& a, int n_total, int m_tiles,
-                         cudaStream_t stream) {
+int g_num_sms = 0;
+
+int num_sms() {
+  if (g_num_sms == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
+    if (g_num_sms <= 0) g_num_sms = 132;
+  }
+  return g_num_sms;
+}
+
+template <int BLOCK_N, int MODE, bool STATS, int FP8, bool PERSIST, bool CL>
+cudaError_t launch_fwd_t(const CUtensorMap& tmB, const CUtensorMap& tmBh, const TmaSet& tmA, const ConvArgs& a,
+                         int n_total, int m_tiles, cudaStream_t stream) {
   using Cfg = FwdCfg<BLOCK_N>;
-  auto kern = conv_gemm_kernel<BLOCK_N, MODE, STATS>;
-  static int configured = 0;
-  const int smem = Cfg::smem_bytes(a.stages);
-  if (configured < smem) {
+  auto kern = conv_gemm_kernel<BLOCK_N, MODE, STATS, FP8, PERSIST, CL>;
+  static bool configured = false;
+  if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::smem_bytes(Cfg::kMaxStagesN));
     if (e != cudaSuccess) return e;
-    configured = Cfg::smem_bytes(Cfg::kMaxStagesN);
-  }
-  dim3 grid(n_total / BLOCK_N, m_tiles);
-  return launch_pdl(kern, grid, dim3(kThreads), smem, stream, 1, tmB, tmA, a);
-}
-
-int g_persistent = 1;        // TMA-fed modes use the persistent kernel (tuning hook: set_conv_persistent)
-int g_num_sms = 0;
-
-template <int BLOCK_N, int MODE, bool STATS, int CL>
-cudaError_t launch_persistent_t(const CUtensorMap& tmB, const CUtensorMap& tmBh, const TmaSet& tmA, const ConvArgs& a,
-                                int n_total, int m_tiles, cudaStream_t stream) {
-  using Cfg = PersistCfg<BLOCK_N>;
-  constexpr bool CLUSTER = CL != 0;
-  auto kern = conv_gemm_persistent_kernel<BLOCK_N, MODE, STATS, CL>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    if (e != cudaSuccess) return e;
+    if (CL) {
+      e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
+      if (e != cudaSuccess) return e;
+    }
     configured = true;
   }
-  if (g_num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
-  }
   const int n_tiles = n_total / BLOCK_N;
-  const long long items = static_cast<long long>(n_tiles) * (CLUSTER ? (m_tiles + 1) / 2 : m_tiles);
-  long long grid = (BLOCK_N > 128 ? 1LL : 2LL) * g_num_sms;      // BLOCK_N = 256 owns the SM's whole TMEM
-  if (CLUSTER) {
-    if (grid > 2 * items) grid = 2 * items;
-    grid &= ~1LL;
-    return launch_pdl(kern, dim3(static_cast<unsigned>(grid)), dim3(kThreads), Cfg::kSmemBytes, stream, 2, tmB, tmBh, tmA, a,
-                      n_tiles, m_tiles);
+  const long long items = static_cast<long long>(n_tiles) * (CL ? (m_tiles + 1) / 2 : m_tiles);
+  long long units = items;
+  if (PERSIST) {                                   // one CTA (pair) per SM (pair), each walking several tiles
+    const long long slots = CL ? num_sms() / 2 : num_sms();
+    if (units > slots) units = slots;
   }
-  if (grid > items) grid = items;
-  return launch_pdl(kern, dim3(static_cast<unsigned>(grid)), dim3(kThreads), Cfg::kSmemBytes, stream, 1, tmB, tmBh, tmA, a,
-                    n_tiles, m_tiles);
-}
-
-template <int BLOCK_N, int MODE, bool STATS, bool PAIR>
-cudaError_t launch_deep_t(const CUtensorMap& tmB, const CUtensorMap& tmBh, const TmaSet& tmA, const ConvArgs& a,
-                          int n_total, int m_tiles, cudaStream_t stream) {
-  using Cfg = DeepCfg<BLOCK_N, PAIR>;
-  auto kern = conv_gemm_deep_kernel<BLOCK_N, MODE, STATS, PAIR>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  if (g_num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
-  }
-  const int n_tiles = n_total / BLOCK_N;
-  const long long items = static_cast<long long>(n_tiles) * (PAIR ? (m_tiles + 1) / 2 : m_tiles);
-  long long grid = g_num_sms;                      // one CTA per SM
-  if (PAIR) {
-    if (grid > 2 * items) grid = 2 * items;
-    grid &= ~1LL;
-  } else if (grid > items) {
-    grid = items;
-  }
-  return launch_pdl(kern, dim3(static_cast<unsigned>(grid)), dim3(kThreads), Cfg::kSmemBytes, stream, PAIR ? 2 : 1, tmB, tmBh,
-                    tmA, a, n_tiles, m_tiles);
+  const long long grid = units * (CL ? 2 : 1);
+  if (grid > 0x7fffffffLL) return cudaErrorInvalidValue;
+  return launch_pdl(kern, dim3(static_cast<unsigned>(grid)), dim3(kThreads), Cfg::smem_bytes(a.stages), stream,
+                    CL ? 2 : 1, tmB, tmBh, tmA, a, n_tiles, m_tiles);
 }
 
 // Variant word (ConvArgs::variant; 0 = built-in policy).  The Python layer autotunes it per layer shape on first use
 // (ops/native.py: the analogue of the reference's `cudnn.benchmark = True`, pytorch_synthetic_benchmark.py:57).
-//   bits 0-3  kernel: 1 = one tile per CTA, 2 = persistent (2 CTAs/SM, 2-3 stage ring), 3 = deep ring (1 CTA/SM)
-//   bits 4-7  tile width: 0 = widest that divides Cout, 1 = 64, 2 = 128, 3 = 256 (deep only)
-//   bit  8    deep only: CTA pairs sharing one M = 256 MMA (cta_group::2)
-constexpr int kVarOneTile = 1, kVarPersistent = 2, kVarDeep = 3;
+//   bits 0-3  kernel: 1 = one tile per CTA, 2 = persistent (one CTA per SM walking tiles)
+//   bit  8    CTA pairs (clusters of two along M) that share the weight tile by TMA multicast
+// (3 = the deep-ring kernel of tensor-memory GPUs has no sm_90 form and is rejected)
+constexpr int kVarOneTile = 1, kVarPersistent = 2;
 
-template <int MODE>
-constexpr bool mode_deep(){ return MODE == kConvGemm || MODE == kConvTileFwd || MODE == kConvTileDgrad || MODE == kConvGemmDgrad; }
-
-template <int MODE>
-cudaError_t launch_deep_mode(const CUtensorMap& tmB, const CUtensorMap& tmBh, const TmaSet& tmA, const ConvArgs& a,
-                             int n_total, int m_tiles, bool stats, int bn, bool pair, cudaStream_t stream) {
-  if constexpr (!mode_deep<MODE>()) {
-    return cudaErrorInvalidValue;
-  } else {
-#define DDL_DEEP(BN, PR)                                                                                     \
-  return stats ? launch_deep_t<BN, MODE, true, PR>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)              \
-               : launch_deep_t<BN, MODE, false, PR>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
-    if (bn == 256) { if (pair) { DDL_DEEP(256, true); } else { DDL_DEEP(256, false); } }
-    if (bn == 128) { if (pair) { DDL_DEEP(128, true); } else { DDL_DEEP(128, false); } }
-    if (bn == 64) {
-      if constexpr (!mode_b_mn(MODE)) { if (pair) { DDL_DEEP(64, true); } }
-      DDL_DEEP(64, false);
-    }
-#undef DDL_DEEP
-    return cudaErrorInvalidValue;
-  }
-}
-
-// Pipeline-depth policy.  Short-K tiles are dominated by per-CTA fixed latency (TMEM alloc, first TMA
-// round trip, epilogue), so they get a shallow ring -> small shared-memory footprint -> 3-4 CTAs per SM whose
-// prologues/epilogues overlap.  Long-K tiles get the deep ring.  g_force_stages (tuning hook) overrides.
+// Pipeline-depth policy: one CTA per SM, so the ring is as deep as the shared memory allows (TMA round trips stay
+// covered on long-K layers).  g_force_stages (tuning hook) overrides.
 int g_force_stages = 0;
-int g_cluster = 0;          // tuning hook: 1 = CTA pairs with TMA-multicast weight tiles, 2 = cta_group::2 pair MMAs
-int g_bn256 = 0;            // tuning hook: 1 lets long-K layers use 128 x 256 persistent tiles (measured 1.7 % SLOWER on
-                            // ResNet-50: one CTA per SM leaves the epilogue half the warps; kept for A/B runs)
-int g_deep = 1;             // tuning hook: 0 = never use the deep-ring kernel, 1 = policy, 2-4 = wherever it applies
 int g_wgrad_swap = 1;       // tuning hook: 0 disables the operand-role swap of narrow-output wgrad tiles
+int g_persistent = 1;       // tuning hook: 0 = never the persistent kernel, 1 = policy (variant word), 2 = always
+int g_cluster = 0;          // tuning hook: != 0 = the persistent kernel runs as CTA pairs wherever they apply
+int g_deep = 1;             // tuning hook: 0 = never, 1 = policy, 2 = persistent CTA pairs wherever they apply,
+                            //   3 / 4 = persistent single CTAs (one CTA per SM with the deepest ring, as the deep-ring
+                            //   kernel of tensor-memory GPUs; tiles are at most 128 wide on sm_90)
 
 template <int BLOCK_N, int MODE>
 int pick_stages(int KB) {
   const int max_s = FwdCfg<BLOCK_N>::kMaxStagesN;
-  int s;
-  if (g_force_stages > 0) s = g_force_stages;
-  else if (!mode_a_tma(MODE)) s = max_s;          // cp.async gather: needs depth > kLag whenever it wraps
-  else s = (KB <= 18) ? 2 : max_s;
+  int s = g_force_stages > 0 ? g_force_stages : max_s;
   if (s > max_s) s = max_s;
   if (s > KB) s = KB;
-  if (!mode_a_tma(MODE) && KB > s && s <= kLag) s = kLag + 1;
+  // a consumer releases a stage only after issuing the next k-block's MMAs, and a gather producer completes a stage
+  // only kLag k-blocks after filling it: a ring that wraps needs 2 (TMA) / kLag + 2 (gather) stages not to dead-lock
+  const int min_s = mode_a_tma(MODE) ? 2 : kLag + 2;
+  if (KB > s && s < min_s) s = min_s;
   return s < 1 ? 1 : s;
 }
 
-struct WeightDesc {       // what the B tensor maps are built from (their box height depends on the tile width chosen)
-  const void* w;
-  int rows, cols, esize;
-};
-
-// B-operand maps for a kernel whose N tile is `bn` wide: full box (min(bn, 128) weight rows) and half box (bn / 2 rows: one
-// CTA's share of a pair tile).  MN-major weights (data gradient) use square boxes of one swizzle row x as many K rows.
-bool make_b_maps(int mode, const WeightDesc& wd, int bn, CUtensorMap* full, CUtensorMap* half) {
-  const uint32_t kcols = 128u / wd.esize;
-  if (mode_b_mn(mode)) {
-    if (!make_map_2d(full, wd.w, wd.rows, wd.cols, wd.cols, kcols, kcols, wd.esize)) return false;
-    *half = *full;
-    return true;
-  }
-  if (!make_map_2d(full, wd.w, wd.rows, wd.cols, wd.cols, kcols, bn < 128 ? bn : 128, wd.esize)) return false;
-  if (!make_map_2d(half, wd.w, wd.rows, wd.cols, wd.cols, kcols, bn / 2 < 128 ? bn / 2 : 128, wd.esize)) *half = *full;
-  return true;
+template <int MODE>
+constexpr bool mode_persist() {
+  return MODE == kConvGemm || MODE == kConvTileFwd || MODE == kConvTileDgrad || MODE == kConvGemmDgrad;
 }
 
-template <int MODE>
-cudaError_t launch_fwd_mode(const WeightDesc& wd, const CUtensorMap& tmB, const CUtensorMap& tmBh, bool have_half_map,
-                            const TmaSet& tmA, ConvArgs a, int n_total, int m_tiles, bool stats, cudaStream_t stream) {
-  const int var_kind = a.variant & 0xf, var_bn = (a.variant >> 4) & 0xf, var_pair = (a.variant >> 8) & 1;
-  if (g_num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
-  }
-  const long long tiles128 = static_cast<long long>(n_total / ((n_total % 128 == 0) ? 128 : 64)) * m_tiles;
-  // ---- deep-ring kernel (one CTA / CTA pair per SM): long-K layers with at least a couple of waves of tiles -------
-  if (mode_deep<MODE>() && g_deep &&
-      (var_kind == kVarDeep || (var_kind == 0 && (g_deep >= 2 || (a.KB >= 8 && tiles128 >= 2LL * g_num_sms))))) {
-    int bn = (n_total % 256 == 0) ? 256 : ((n_total % 128 == 0) ? 128 : 64);
-    if (var_kind == kVarDeep && var_bn != 0) {
-      const int want = var_bn == 1 ? 64 : (var_bn == 2 ? 128 : 256);
-      if (n_total % want != 0) return cudaErrorInvalidValue;
-      bn = want;
-    }
-    // test hooks: g_deep = 2 forces the deep kernel with pairs wherever possible, 3 = without pairs, 4 = without pairs
-    // and without 256-wide tiles
-    bool pair = var_kind == kVarDeep ? var_pair != 0 : (g_deep != 3 && g_deep != 4);
-    if (var_kind != kVarDeep && g_deep == 4 && bn == 256) bn = 128;
-    // pairs need two M tiles, 64-column halves of an MN-major weight tile, and a loadable half of a K-major one
-    // (bn = 256: the full map's 128-row box; narrower: the half-height box map)
-    if (m_tiles < 2 || (mode_b_mn(MODE) && bn < (a.fp8 ? 256 : 128))) pair = false;
-    if (a.fp8 && mode_b_mn(MODE) && bn < 128) return cudaErrorInvalidValue;
-    // the weight maps' box heights follow THIS kernel's tile width (not the widest tile Cout would allow)
-    CUtensorMap dB, dBh;
-    if (!make_b_maps(MODE, wd, bn, &dB, &dBh)) return cudaErrorUnknown;
-    return launch_deep_mode<MODE>(dB, dBh, tmA, a, n_total, m_tiles, stats, bn, pair, stream);
-  }
-  if (var_kind == kVarDeep) return cudaErrorInvalidValue;
-  bool persistent = false;
-  if (mode_a_tma(MODE) && g_persistent) {
-    // persistence pays when every CTA gets several tiles (measured crossover ~3.5 tiles per resident CTA);
-    // below that the one-tile-per-CTA kernel with 3 CTAs/SM wins.  g_persistent == 2 forces it (tuning).
-    persistent = g_persistent == 2 || tiles128 * 2 >= 7LL * 2 * g_num_sms;
-  }
-  if (mode_a_tma(MODE) && var_kind == kVarPersistent) persistent = true;
-  if (var_kind == kVarOneTile) persistent = false;
-  // 128 x 256 tiles: only where the main loop (operand traffic) matters (K >= 256) — with one CTA per SM the epilogue
-  // has half the warps to hide its latency, which would cost the short-K, store-bound layers
-  if (persistent && g_bn256 && n_total % 256 == 0 && a.KB >= 4 &&
-      static_cast<long long>(n_total / 256) * m_tiles >= 4LL * g_num_sms) {
-    return stats ? launch_persistent_t<256, MODE, true, 0>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
-                 : launch_persistent_t<256, MODE, false, 0>(tmB, tmBh, tmA, a, n_total, m_tiles, stream);
-  }
-  if (persistent) {
-    // CTA pairs sharing the weight tile through TMA multicast: where operand traffic matters (K >= 128) and the half
-    // tile is loadable (K-major: half-height box map; MN-major: the two 64-column boxes of a 128-wide tile)
-    const bool pair = g_cluster && m_tiles >= 2 && a.KB >= 2 &&
-                      (mode_b_mn(MODE) ? (n_total % 128 == 0) : have_half_map);
-    if (n_total % 128 == 0) {
-      if (pair && g_cluster == 2)
-        return stats ? launch_persistent_t<128, MODE, true, 2>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
-                     : launch_persistent_t<128, MODE, false, 2>(tmB, tmBh, tmA, a, n_total, m_tiles, stream);
-      if (pair)
-        return stats ? launch_persistent_t<128, MODE, true, 1>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
-                     : launch_persistent_t<128, MODE, false, 1>(tmB, tmBh, tmA, a, n_total, m_tiles, stream);
-      return stats ? launch_persistent_t<128, MODE, true, 0>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
-                   : launch_persistent_t<128, MODE, false, 0>(tmB, tmBh, tmA, a, n_total, m_tiles, stream);
-    }
-    if (n_total % 64 == 0) {
-      if (pair && !mode_b_mn(MODE) && g_cluster == 2)
-        return stats ? launch_persistent_t<64, MODE, true, 2>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
-                     : launch_persistent_t<64, MODE, false, 2>(tmB, tmBh, tmA, a, n_total, m_tiles, stream);
-      if (pair && !mode_b_mn(MODE))
-        return stats ? launch_persistent_t<64, MODE, true, 1>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
-                     : launch_persistent_t<64, MODE, false, 1>(tmB, tmBh, tmA, a, n_total, m_tiles, stream);
-      return stats ? launch_persistent_t<64, MODE, true, 0>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
-                   : launch_persistent_t<64, MODE, false, 0>(tmB, tmBh, tmA, a, n_total, m_tiles, stream);
+template <int BLOCK_N, int MODE>
+cudaError_t launch_bn(const CUtensorMap& tmB, const CUtensorMap& tmBh, const TmaSet& tmA, ConvArgs a, int n_total,
+                      int m_tiles, bool stats, bool persistent, bool pair, cudaStream_t stream) {
+  a.stages = pick_stages<BLOCK_N, MODE>(a.KB);
+#define DDL_FWD(FP8, PER, CLU)                                                                                    \
+  return stats ? launch_fwd_t<BLOCK_N, MODE, true, FP8, PER, CLU>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)   \
+               : launch_fwd_t<BLOCK_N, MODE, false, FP8, PER, CLU>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)
+  if (a.fp8) {
+    // fp8 wgmma reads K-major operands only: e4m3 x e4m3 forward GEMM / tile modes, e5m2 x e4m3 data gradients on the
+    // transposed weight copy; one tile per CTA
+    if constexpr (MODE == kConvGemm || MODE == kConvTileFwd) {
+      if (a.fp8 == 1) { DDL_FWD(1, false, false); }
+    } else if constexpr (MODE == kConvGemmDgrad || MODE == kConvTileDgrad) {
+      if (a.fp8 == 2) { DDL_FWD(2, false, false); }
     }
     return cudaErrorInvalidValue;
   }
-  if (n_total % 128 == 0) {
-    a.stages = pick_stages<128, MODE>(a.KB);
-    return stats ? launch_fwd_t<128, MODE, true>(tmB, tmA, a, n_total, m_tiles, stream)
-                 : launch_fwd_t<128, MODE, false>(tmB, tmA, a, n_total, m_tiles, stream);
+  if constexpr (mode_persist<MODE>()) {
+    if (persistent && pair) { DDL_FWD(0, true, true); }
+    if (persistent) { DDL_FWD(0, true, false); }
   }
-  if (n_total % 64 == 0) {
-    a.stages = pick_stages<64, MODE>(a.KB);
-    return stats ? launch_fwd_t<64, MODE, true>(tmB, tmA, a, n_total, m_tiles, stream)
-                 : launch_fwd_t<64, MODE, false>(tmB, tmA, a, n_total, m_tiles, stream);
+  DDL_FWD(0, false, false);
+#undef DDL_FWD
+}
+
+template <int MODE>
+cudaError_t launch_fwd_mode(const CUtensorMap& tmB, const CUtensorMap& tmBh, const TmaSet& tmA, const ConvArgs& a,
+                            int n_total, int m_tiles, bool stats, cudaStream_t stream) {
+  const int var_kind = a.variant & 0xf;
+  const bool var_pair = ((a.variant >> 8) & 1) != 0;
+  if (var_kind != 0 && var_kind != kVarOneTile && var_kind != kVarPersistent) return cudaErrorInvalidValue;
+  const int bn = (n_total % 128 == 0) ? 128 : 64;
+  if (n_total % 64 != 0) return cudaErrorInvalidValue;
+  // pairs need two M tiles and a weight tile that splits into two loadable halves (MN-major: two 64-column boxes)
+  const bool pair_ok = m_tiles >= 2 && (!mode_b_mn(MODE) || bn == 128);
+  bool persistent = false, pair = false;
+  if (var_kind == kVarPersistent) {
+    if (!mode_persist<MODE>() || a.fp8 || (var_pair && !pair_ok)) return cudaErrorInvalidValue;
+    persistent = true;
+    pair = var_pair;
+  } else if (var_kind == 0 && mode_persist<MODE>() && !a.fp8) {
+    if (g_deep >= 2) {
+      persistent = true;
+      pair = g_deep == 2 && pair_ok;
+    } else if (g_persistent == 2) {
+      persistent = true;
+      pair = g_cluster != 0 && pair_ok;
+    }
+  } else if (var_pair) {
+    return cudaErrorInvalidValue;
   }
-  return cudaErrorInvalidValue;
+  if (bn == 128) return launch_bn<128, MODE>(tmB, tmBh, tmA, a, n_total, m_tiles, stats, persistent, pair, stream);
+  return launch_bn<64, MODE>(tmB, tmBh, tmA, a, n_total, m_tiles, stats, persistent, pair, stream);
 }
 
 }  // namespace
@@ -1908,9 +1180,8 @@ cudaError_t conv_timeout_info(unsigned int out[8]) {
 }
 
 void set_conv_force_stages(int s) { g_force_stages = s; }
-void set_conv_persistent(int on) { g_persistent = on; }
 void set_wgrad_swap(int on) { g_wgrad_swap = on; }
-void set_conv_bn256(int on) { g_bn256 = on; }
+void set_conv_persistent(int on) { g_persistent = on; }
 void set_conv_cluster(int on) { g_cluster = on; }
 void set_conv_deep(int on) { g_deep = on; }
 void set_conv_wait_hint(int ns) {
@@ -1937,29 +1208,20 @@ cudaError_t launch_conv_gemm(int mode, const ConvArgs& a_in, const void* w, int 
   const int es = a.fp8 ? 1 : 2;                   // operand element size (bytes)
   const uint32_t kcols = 128u / es;               // elements in a 128-byte swizzle row
   if (a.fp8) {
-    // fp8 operands run on the deep-ring kernel only (GEMM / stride-1-or-2 tile modes), with 128-element k-blocks
-    if (!(mode == kConvGemm || mode == kConvTileFwd || mode == kConvTileDgrad || mode == kConvGemmDgrad))
+    // fp8 operands, K-major, 128-element k-blocks: e4m3 x e4m3 forward (GEMM / tile modes) or e5m2 x e4m3 data
+    // gradient (GEMM / tile modes; `w` is then the transposed weight copy [Cin][R*S*Cout], a.kstride = Cout)
+    const bool fwd = a.fp8 == 1 && (mode == kConvGemm || mode == kConvTileFwd);
+    const bool dgrad = a.fp8 == 2 && (mode == kConvGemmDgrad || mode == kConvTileDgrad);
+    if (!(fwd || dgrad) || a.deq_a == nullptr || a.deq_b == nullptr || (dgrad && n_total % 128 != 0))
       return cudaErrorInvalidValue;
-    if (a.fp8 == 3) {
-      // MX block-scaled operands: K-major GEMM, one 128-wide single-CTA tile per row block (scale atoms are per 128 rows)
-      if (mode != kConvGemm || n_total % 128 != 0 || a.sfa == nullptr || a.sfb == nullptr) return cudaErrorInvalidValue;
-      a.variant = kVarDeep | (2 << 4);
-    } else if (a.deq_a == nullptr || a.deq_b == nullptr) {
-      return cudaErrorInvalidValue;
-    }
-    if (mode_b_mn(mode) && n_total % 128 != 0) return cudaErrorInvalidValue;    // MN-major boxes are 128 columns wide
-    if ((a.variant & 0xf) == 0) a.variant = kVarDeep;
-    if ((a.variant & 0xf) != kVarDeep) return cudaErrorInvalidValue;
   }
-  CUtensorMap tmBh;                 // K-major weights: half-height box (one CTA's share of a multicast pair)
-  bool have_half = false;
-  if (mode_b_mn(mode)) {
+  CUtensorMap tmBh;                 // K-major weights: half-height box (one CTA's share of a CTA-pair tile)
+  if (mode_b_mn(mode) && !a.fp8) {
     if (!make_map_2d(&tmB, w, w_rows, w_cols, w_cols, kcols, kcols, es)) return cudaErrorUnknown;
     tmBh = tmB;
   } else {
     if (!make_map_2d(&tmB, w, w_rows, w_cols, w_cols, kcols, bn, es)) return cudaErrorUnknown;
-    have_half = make_map_2d(&tmBh, w, w_rows, w_cols, w_cols, kcols, bn / 2, es);     // pair tiles / multicast halves
-    if (!have_half) tmBh = tmB;
+    if (!make_map_2d(&tmBh, w, w_rows, w_cols, w_cols, kcols, bn / 2, es)) return cudaErrorUnknown;
   }
   a.ntaps = 0;
   a.outH = a.dstH; a.outW = a.dstW; a.out_stride = 1; a.out_pa = 0; a.out_pb = 0;
@@ -1967,17 +1229,16 @@ cudaError_t launch_conv_gemm(int mode, const ConvArgs& a_in, const void* w, int 
   a.zfill = 0;
   int m_tiles = (a.M + kBlockM - 1) / kBlockM;
   const bool stats = a.sum != nullptr;
-  const WeightDesc wd{w, w_rows, w_cols, es};
   auto dispatch = [&](const ConvArgs& args, int tiles) -> cudaError_t {
     switch (mode) {
-      case kConvFwd: return launch_fwd_mode<kConvFwd>(wd, tmB, tmBh, have_half, tmA, args, n_total, tiles, stats, stream);
-      case kConvDgrad: return launch_fwd_mode<kConvDgrad>(wd, tmB, tmBh, have_half, tmA, args, n_total, tiles, stats, stream);
-      case kConvGemm: return launch_fwd_mode<kConvGemm>(wd, tmB, tmBh, have_half, tmA, args, n_total, tiles, stats, stream);
-      case kConvStem: return launch_fwd_mode<kConvStem>(wd, tmB, tmBh, have_half, tmA, args, n_total, tiles, stats, stream);
-      case kConvTileFwd: return launch_fwd_mode<kConvTileFwd>(wd, tmB, tmBh, have_half, tmA, args, n_total, tiles, stats, stream);
-      case kConvTileDgrad: return launch_fwd_mode<kConvTileDgrad>(wd, tmB, tmBh, have_half, tmA, args, n_total, tiles, stats, stream);
-      case kConvGemmDgrad: return launch_fwd_mode<kConvGemmDgrad>(wd, tmB, tmBh, have_half, tmA, args, n_total, tiles, stats, stream);
-      case kConvStemTma: return launch_fwd_mode<kConvStemTma>(wd, tmB, tmBh, have_half, tmA, args, n_total, tiles, stats, stream);
+      case kConvFwd: return launch_fwd_mode<kConvFwd>(tmB, tmBh, tmA, args, n_total, tiles, stats, stream);
+      case kConvDgrad: return launch_fwd_mode<kConvDgrad>(tmB, tmBh, tmA, args, n_total, tiles, stats, stream);
+      case kConvGemm: return launch_fwd_mode<kConvGemm>(tmB, tmBh, tmA, args, n_total, tiles, stats, stream);
+      case kConvStem: return launch_fwd_mode<kConvStem>(tmB, tmBh, tmA, args, n_total, tiles, stats, stream);
+      case kConvTileFwd: return launch_fwd_mode<kConvTileFwd>(tmB, tmBh, tmA, args, n_total, tiles, stats, stream);
+      case kConvTileDgrad: return launch_fwd_mode<kConvTileDgrad>(tmB, tmBh, tmA, args, n_total, tiles, stats, stream);
+      case kConvGemmDgrad: return launch_fwd_mode<kConvGemmDgrad>(tmB, tmBh, tmA, args, n_total, tiles, stats, stream);
+      case kConvStemTma: return launch_fwd_mode<kConvStemTma>(tmB, tmBh, tmA, args, n_total, tiles, stats, stream);
       default: return cudaErrorInvalidValue;
     }
   };
@@ -2115,12 +1376,12 @@ cudaError_t launch_conv_wgrad(const WgradArgs& a_in, const void* dy, const void*
   if (splits > a.total_kb) splits = a.total_kb;
   a.kb_per_split = (a.total_kb + splits - 1) / splits;
   splits = (a.total_kb + a.kb_per_split - 1) / a.kb_per_split;
-  // TMA-fed wgrad tiles run best with a 2-deep ring (measured: 3 CTAs/SM beat a deeper pipeline); the cp.async
-  // gather modes need depth > kLag
+  // one CTA per SM: the deepest ring that fits (the cp.async gather modes need depth > kLag)
   const bool tma_fed = (a.mode == kConvGemm || a.mode == kConvTileFwd || a.mode == kConvStemTma);
-  a.stages = tma_fed ? 2 : kWgMaxStages;
+  a.stages = kWgMaxStages;
   if (g_force_stages > 0 && g_force_stages <= kWgMaxStages && tma_fed) a.stages = g_force_stages;
   if (a.stages > a.kb_per_split) a.stages = a.kb_per_split;
+  if (a.kb_per_split > a.stages && a.stages < (tma_fed ? 2 : kLag + 2)) a.stages = tma_fed ? 2 : kLag + 2;   // see pick_stages
   if (a.stages < 1) a.stages = 1;
   const int smem = wg_smem_bytes(a.stages);
   // narrow outputs (the last 128-channel tile would be at most half full): swap operand roles, 64-channel tiles

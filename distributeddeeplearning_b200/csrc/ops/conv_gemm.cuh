@@ -1,4 +1,4 @@
-// Host/device shared argument structs for the tcgen05 implicit-GEMM convolution kernels.
+// Host/device shared argument structs for the wgmma implicit-GEMM convolution kernels.
 #pragma once
 
 #include <cuda.h>
@@ -63,14 +63,10 @@ struct ConvArgs {
   // A k-block is still 128 BYTES per row (128 fp8 elements), so shared-memory images, swizzle and descriptors keep
   // their geometry; tensor maps are built over bytes.  The epilogue multiplies the accumulator by *deq_a * *deq_b
   // (the operands' inverse quantisation scales, device-resident: ops.h Fp8Slot::inv_scale).
-  int fp8;                    // 3 = MX block-scaled e4m3 x e4m3 (kind::mxf8f6f4.block_scale): one UE8M0 scale per 32 K elements
-                              //   of every A row / B row, delivered as 512-byte atoms (see sfa / sfb); GEMM mode,
-                              //   128-wide single-CTA deep-ring tiles only
+  int fp8;
   const float* deq_a;
   const float* deq_b;
-  // MX scale factors in the tensor core's atom order: atom (row block of 128, k-block of 128 elements) is 512 bytes,
-  // byte (r % 32) * 16 + (r / 32) * 4 + s holds the scale of row r, K sub-block s (32 elements): exactly the image one
-  // tcgen05.cp 32x128b.warpx4 moves into 4 TMEM columns.  sfa: [ceil(M/128)][KB][512], sfb: [n_total/128][KB][512].
+  // MX block scales (unused by the sm_90a kernels, which have no block-scaled MMA; the launcher rejects fp8 = 3)
   const uint8_t* sfa;
   const uint8_t* sfb;
   int variant;                // kernel variant word chosen by the caller's autotuner (0 = built-in policy); see

@@ -1,4 +1,4 @@
-// FP8 (e4m3 / e5m2) operand preparation for the tcgen05 `kind::f8f6f4` conv / GEMM path (BASELINE config #3:
+// FP8 (e4m3 / e5m2) operand preparation for the fp8 wgmma conv / GEMM path (BASELINE config #3:
 // ResNet-50 with 8-bit tensor-core operands; the reference's only reduced-precision switch is the TF benchmark's
 // `--use_fp16`, TensorFlow_benchmark/tensorflow_benchmark.py:51,77).
 //
@@ -144,6 +144,31 @@ cudaError_t launch_fp8_quantize_mx(const __nv_bfloat16* x, uint8_t* out, uint8_t
   int64_t blocks = (total + 255) / 256;
   if (blocks > 8LL * sms) blocks = 8LL * sms;
   quantize_mx_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, out, sf, rows, K);
+  return cudaGetLastError();
+}
+
+// fp8 codes [rows][taps][cols] -> [cols][taps][rows]: the data gradient's K-major copy of a quantised weight matrix.
+// 32 x 32 byte tiles through shared memory (coalesced reads and writes), one grid z slice per filter tap.
+__global__ void transpose_taps_u8_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, int rows, int taps,
+                                         int cols) {
+  __shared__ uint8_t t[32][33];
+  const int tap = blockIdx.z;
+  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int r = r0 + i, c = c0 + threadIdx.x;
+    if (r < rows && c < cols) t[i][threadIdx.x] = in[(static_cast<size_t>(r) * taps + tap) * cols + c];
+  }
+  __syncthreads();
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int c = c0 + i, r = r0 + threadIdx.x;
+    if (c < cols && r < rows) out[(static_cast<size_t>(c) * taps + tap) * rows + r] = t[threadIdx.x][i];
+  }
+}
+
+cudaError_t launch_fp8_transpose_taps(const uint8_t* in, uint8_t* out, int rows, int taps, int cols, cudaStream_t stream) {
+  if (rows <= 0 || taps <= 0 || cols <= 0 || taps > 65535) return cudaErrorInvalidValue;
+  const dim3 grid((cols + 31) / 32, (rows + 31) / 32, taps);
+  transpose_taps_u8_kernel<<<grid, dim3(32, 8), 0, stream>>>(in, out, rows, taps, cols);
   return cudaGetLastError();
 }
 

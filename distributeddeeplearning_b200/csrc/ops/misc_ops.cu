@@ -107,8 +107,8 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const __nv_bfloat16* _
 
 // gather formulation: each INPUT pixel sums the dy of the windows whose arg-max it is (no atomics)
 // 3x3 / stride 2 / pad 1 forward (the ResNet / DenseNet stem pool): all nine 16-byte window loads of a thread are issued
-// before the first compare (the generic kernel's tap loop exposed one L2 round trip per tap: 236 us for the 565 MB this
-// layer moves at batch 256, i.e. 2.4 TB/s).  Out-of-image taps load nothing and can never win.
+// before the first compare (the generic kernel's tap loop exposes one L2 round trip per tap on the ~565 MB this layer
+// moves at batch 256).  Out-of-image taps load nothing and can never win.
 __global__ void __launch_bounds__(256) maxpool_fwd_k3s2_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* y,
                                                                uint8_t* argmax, PoolArgs p) {
   const int groups = p.C / 8;
@@ -638,7 +638,7 @@ __global__ void __launch_bounds__(256) add_bf16_kernel(const __nv_bfloat16* __re
   }
 }
 
-inline int grid_for(int64_t work, int per_block = 256, int cap = 148 * 16) {
+inline int grid_for(int64_t work, int per_block = 256, int cap = 132 * 16) {     // 16 blocks per SM of an H100 SXM
   int64_t b = (work + per_block - 1) / per_block;
   if (b > cap) b = cap;
   if (b < 1) b = 1;

@@ -1,4 +1,4 @@
-// Host-visible launchers of the memory-bound sm_100a kernels (NHWC bf16 activations).
+// Host-visible launchers of the memory-bound sm_90a kernels (NHWC bf16 activations).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -156,8 +156,10 @@ cudaError_t launch_fp8_quantize(const __nv_bfloat16* x, uint8_t* out, int64_t n,
                                 cudaStream_t stream);
 cudaError_t launch_fp8_amax(const __nv_bfloat16* x, int64_t n, Fp8Slot* slot, int sms, cudaStream_t stream);
 cudaError_t launch_fp8_update_scales(Fp8Slot* slots, int n, cudaStream_t stream);
+// codes [rows][taps][cols] -> [cols][taps][rows] (the data gradient's K-major copy of quantised weights)
+cudaError_t launch_fp8_transpose_taps(const uint8_t* in, uint8_t* out, int rows, int taps, int cols, cudaStream_t stream);
 // MX (OCP microscaling) quantisation of a row-major bf16 matrix [rows][K], K % 128 == 0: e4m3 codes + one UE8M0 scale per
-// 32 consecutive K elements of a row, written in the 512-byte atom order of tcgen05 (ConvArgs::sfa): sf must hold
+// 32 consecutive K elements of a row, written in 512-byte atoms (ConvArgs::sfa): sf must hold
 // ceil(rows/128) * (K/128) * 512 bytes and be zero-initialised (rows beyond `rows` keep scale byte 0).
 cudaError_t launch_fp8_quantize_mx(const __nv_bfloat16* x, uint8_t* out, uint8_t* sf, int64_t rows, int64_t K, int sms,
                                    cudaStream_t stream);

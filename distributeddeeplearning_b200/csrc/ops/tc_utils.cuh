@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA / mbarrier PTX wrappers for sm_100a (no CUTLASS dependency).
+// wgmma / TMA / mbarrier PTX wrappers for sm_90a (no CUTLASS dependency).
 //
 // Conventions used by every GEMM-shaped kernel in this repo
 //   * operand tiles live in shared memory as rows of 128 bytes (64 bf16) with the 128B swizzle:
@@ -9,7 +9,8 @@
 //   * MN-major operand : row = K index, the 128 B row = 64 consecutive M/N elements.
 //                        descriptor: SBO = 1024 (8 K-rows), LBO = bytes between 64-wide M/N chunks,
 //                        K-advance of 16 elements = +2048 B.
-//   * accumulators: fp32 in TMEM, D row i -> TMEM lane i, D column j -> TMEM column j.
+//   * accumulators: fp32 registers of the issuing warpgroup (wgmma m64nNk16 fragment layout): warp w of the group,
+//     lane l holds rows 16w + l/4 and 16w + l/4 + 8, columns 8j + 2(l%4) + {0, 1} of every 8-column block j.
 #pragma once
 
 #include <cuda.h>
@@ -47,7 +48,7 @@ DDL_DEVICE void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
 }
 // c_wait_hint_ns != 0: pass that suspend-time hint to try_wait (the thread sleeps in hardware until the phase completes
 // or the time is up, instead of returning after the short system default and re-issuing the poll loop) — tuning hook
-// set_conv_wait_hint, A/B-measured in BASELINE.md
+// set_conv_wait_hint
 __constant__ unsigned int c_wait_hint_ns;
 DDL_DEVICE bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -71,11 +72,9 @@ DDL_DEVICE bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 // the first waiter that exceeds the bound records WHERE it was stuck (site id, block, thread, parity) in a device-side
 // diagnostic block and raises an abort flag; every other waiter of this and later kernels then drains immediately, so
 // the launch terminates (with garbage results) and the host can read the record (conv_timeout_info) and raise.
-// `site` = 16 * kernel family (1 one-tile, 2 persistent, 3 deep-ring, 4 wgrad) + role (1 producer waits for a free
-// stage, 2 MMA waits for operands, 3 MMA waits for a drained accumulator, 4 epilogue waits for the accumulator).
-// The bound is an iteration count (each failed try_wait already suspends the thread for a hardware-defined window),
-// which keeps the spin loop short: the ncu source view showed the former clock64()-based loop of the TMA / MMA warps
-// taking ~25 % of all issued instructions in short-K kernels.
+// `site` = 16 * kernel family (1 conv, 4 wgrad) + role (1 producer waits for a free stage, 2 MMA waits for
+// operands).  The bound is an iteration count (each failed try_wait already suspends the thread for a hardware-defined
+// window), which keeps the spin loop short.
 __device__ unsigned int g_mbar_diag[8];     // [0] abort flag, [1] site, [2] blockIdx.x, [3] threadIdx.x, [4] parity
 
 DDL_DEVICE void mbar_wait(uint64_t* bar, uint32_t parity, uint32_t site = 0) {
@@ -117,63 +116,11 @@ DDL_DEVICE void tma_load_2d_multicast(uint32_t dst_smem, const CUtensorMap* m, i
       :: "r"(dst_smem), "l"(reinterpret_cast<uint64_t>(m)), "r"(x), "r"(y), "r"(smem_u32(bar)), "h"(cta_mask)
       : "memory");
 }
-// tcgen05.commit arriving on the mbarrier at the same offset in every CTA of `cta_mask`
-DDL_DEVICE void umma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               :: "r"(smem_u32(bar)), "h"(cta_mask) : "memory");
-}
-
-// ---- CTA pair (cta_group::2): one MMA spans two SMs, each SM holding its 128 rows of A and HALF of B ---------------
-template <int COLS>
-DDL_DEVICE void tmem_alloc_pair(uint32_t* slot_in_smem) {      // one whole warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(slot_in_smem)), "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-DDL_DEVICE void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" :: "r"(taddr), "n"(COLS) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 rows: 128 per CTA] * B[N columns: N/2 per CTA]; issued by ONE thread of the leader CTA
-DDL_DEVICE void umma_bf16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-  const uint32_t acc = accumulate ? 1u : 0u;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
-}
-DDL_DEVICE void umma_commit_pair_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               :: "r"(smem_u32(bar)), "h"(cta_mask) : "memory");
-}
 // address of `local` (a shared::cta address) in CTA `rank` of this cluster
 DDL_DEVICE uint32_t mapa_shared(uint32_t local, uint32_t rank) {
   uint32_t r;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local), "r"(rank));
   return r;
-}
-// TMA loads of a CTA pair: data lands in the ISSUING CTA's shared memory, the complete_tx goes to `bar_cluster_addr`,
-// which may be the peer (leader) CTA's mbarrier (shared::cluster address from mapa_shared).
-DDL_DEVICE void tma_load_2d_pair(uint32_t dst_smem, const CUtensorMap* m, int x, int y, uint32_t bar_cluster_addr) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-      :: "r"(dst_smem), "l"(reinterpret_cast<uint64_t>(m)), "r"(x), "r"(y), "r"(bar_cluster_addr) : "memory");
-}
-DDL_DEVICE void tma_load_4d_pair(uint32_t dst_smem, const CUtensorMap* m, int c0, int c1, int c2, int c3,
-                                 uint32_t bar_cluster_addr) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      :: "r"(dst_smem), "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar_cluster_addr)
-      : "memory");
-}
-DDL_DEVICE void tma_load_5d_pair(uint32_t dst_smem, const CUtensorMap* m, int c0, int c1, int c2, int c3, int c4,
-                                 uint32_t bar_cluster_addr) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-      :: "r"(dst_smem), "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4),
-         "r"(bar_cluster_addr)
-      : "memory");
 }
 DDL_DEVICE void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" :: "r"(cluster_addr) : "memory");
@@ -204,132 +151,108 @@ DDL_DEVICE void tma_load_2d(uint32_t dst_smem, const CUtensorMap* m, int x, int 
       :: "r"(dst_smem), "l"(reinterpret_cast<uint64_t>(m)), "r"(x), "r"(y), "r"(smem_u32(bar)) : "memory");
 }
 
-// ---- TMEM ------------------------------------------------------------------------------------
-template <int COLS>
-DDL_DEVICE void tmem_alloc(uint32_t* slot_in_smem) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-               :: "r"(smem_u32(slot_in_smem)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-DDL_DEVICE void tmem_dealloc(uint32_t taddr) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "n"(COLS) : "memory");
-}
-DDL_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-DDL_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 32 columns of fp32: thread i of the warp receives lane (base_lane + i), 32 columns.
-DDL_DEVICE void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
-DDL_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- UMMA descriptors ----------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128B swizzle (layout_type = 2), version 1 (Blackwell).
+// ---- wgmma ----------------------------------------------------------------------------------
+// Shared-memory matrix descriptor, 128B swizzle (sm_90 layout type 1 in bits [62,64)).
 DDL_DEVICE uint64_t smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);              // start address  [0,14)
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;         // leading offset [16,30)
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;         // stride offset  [32,46)
-  d |= 1ull << 46;                                                      // version = 1
-  d |= 2ull << 61;                                                      // SWIZZLE_128B
+  d |= 1ull << 62;                                                      // SWIZZLE_128B
   return d;
 }
 // The start-address field (16-byte units, bits [0,14)) sits in the descriptor's low word and never carries out of it for
-// addresses below 256 KB, so stepping through stages / K slices is ONE 32-bit add on a pre-built descriptor.  The MMA
-// thread issues 4 MMAs per k-block on its own: rebuilding two 64-bit descriptors per MMA (~25 dependent integer
-// instructions each) made that single thread, not the tensor core, the pacing resource of a one-CTA-per-SM kernel.
+// addresses below 256 KB, so stepping through stages / K slices is ONE 32-bit add on a pre-built descriptor.
 DDL_DEVICE uint64_t desc_join(uint32_t lo, uint32_t hi) {
   uint64_t d;
   asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
   return d;
 }
-// Instruction descriptor: bf16 x bf16 -> fp32, M x N tile, operand major-ness (0 = K, 1 = MN).
-__host__ __device__ constexpr uint32_t idesc_bf16(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
+DDL_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+DDL_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+DDL_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across a wgmma fence or wait
+template <int R>
+DDL_DEVICE void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i]) :: "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-DDL_DEVICE void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-  const uint32_t acc = accumulate ? 1u : 0u;
+// D(64 x N) (+)= A(64 x K) * B(K x N) for one warpgroup.  TA / TB: operand is MN-major (1) or K-major (0); the fp8
+// forms (K = 32 per instruction, e4m3 x e4m3 and e5m2 x e4m3) take K-major operands only.
+template <int TA, int TB>
+DDL_DEVICE void wgmma_bf16_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
 }
-// fp8 operands (kind::f8f6f4, dense, fp32 accumulate): format codes 0 = e4m3, 1 = e5m2; K = 32 elements (32 bytes) per MMA
-__host__ __device__ constexpr uint32_t idesc_f8(int m, int n, int a_fmt, int b_fmt, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (static_cast<uint32_t>(a_fmt) << 7) | (static_cast<uint32_t>(b_fmt) << 10) |
-         (static_cast<uint32_t>(a_mn_major) << 15) | (static_cast<uint32_t>(b_mn_major) << 16) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-DDL_DEVICE void umma_f8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-  const uint32_t acc = accumulate ? 1u : 0u;
+template <int TA, int TB>
+DDL_DEVICE void wgmma_e4m3_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d)
+      : "memory");
 }
-DDL_DEVICE void umma_f8_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-  const uint32_t acc = accumulate ? 1u : 0u;
+template <int TA, int TB>
+DDL_DEVICE void wgmma_bf16_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
 }
-// ---- MX block-scaled fp8 (kind::mxf8f6f4.block_scale, scale vector = 32 elements, UE8M0 scales in TMEM) ------------
-// instruction descriptor of the block-scaled kinds: no C format field; scale format bit 23 (1 = E8M0); a_sf_id / b_sf_id
-// select WHICH of the 4 bytes of a scale column this MMA's K sub-block uses.
-__host__ __device__ constexpr uint32_t idesc_mxf8(int m, int n, int a_fmt, int b_fmt, int a_sf_id, int b_sf_id) {
-  return (static_cast<uint32_t>(b_sf_id) << 4) | (static_cast<uint32_t>(a_fmt) << 7) | (static_cast<uint32_t>(b_fmt) << 10) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (1u << 23) | (static_cast<uint32_t>(m >> 4) << 24) |
-         (static_cast<uint32_t>(a_sf_id) << 29);
-}
-DDL_DEVICE void umma_mxf8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate,
-                          uint32_t tmem_sfa, uint32_t tmem_sfb) {
-  const uint32_t acc = accumulate ? 1u : 0u;
+template <int TA, int TB>
+DDL_DEVICE void wgmma_e4m3_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}"
-      :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc), "r"(tmem_sfa), "r"(tmem_sfb) : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d)
+      : "memory");
 }
-// shared memory -> TMEM copy of one 512-byte scale atom: 32 rows x 16 bytes, broadcast to the four 32-lane quarters
-DDL_DEVICE void tmem_cp_32x128b_warpx4(uint32_t dst_tmem, uint64_t src_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" :: "r"(dst_tmem), "l"(src_desc) : "memory");
+
+template <int TA, int TB>
+DDL_DEVICE void wgmma_e5m2e4m3_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e5m2.e4m3 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d)
+      : "memory");
 }
-// un-swizzled (interleave) K-major descriptor of a dense [rows][16 B] block: 8-row core matrices 128 bytes apart
-DDL_DEVICE uint64_t smem_desc_nosw(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
-  return d;
-}
-// plain (non-tensor) bulk copy global -> shared, completing on an mbarrier
-DDL_DEVICE void bulk_load(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               :: "r"(dst_smem), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-// Arrive on `bar` when all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-DDL_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-               :: "r"(smem_u32(bar)) : "memory");
+template <int TA, int TB>
+DDL_DEVICE void wgmma_e5m2e4m3_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e5m2.e4m3 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d)
+      : "memory");
 }
 
 // vectorised fp32 reduction into global memory (wgrad split-K)

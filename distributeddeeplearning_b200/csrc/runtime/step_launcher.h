@@ -36,7 +36,7 @@ struct StepLauncherConfig {
   float* M = nullptr;
   void* Wb = nullptr;                        // bf16 compute copy of the weights
   const SgdHyper* hyper_dev = nullptr;
-  int comm_blocks = 32, sms = 148;
+  int comm_blocks = 32, sms = 132;         // callers pass the device's SM count; 132 = H100 SXM
   bool use_mc = false, wire_bf16 = false;
   int64_t oneshot_bytes = 0;
   uint64_t scalars_off = 0;

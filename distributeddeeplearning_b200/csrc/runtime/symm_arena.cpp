@@ -1,9 +1,9 @@
 // Symmetric (peer-mapped) device arena with optional NVLS multicast alias.
 //
-// This is the B200-native replacement for the transport setup the reference inherits from
+// This is the native replacement for the transport setup the reference inherits from
 // NCCL/MPI (SURVEY.md 2.4, N3): every rank allocates the same-sized physical arena with the
 // CUDA VMM API, exports it as a POSIX fd, imports the 7 peers' arenas and maps them into its
-// own address space.  Kernels then address `peer_ptrs[r] + offset` directly over NVLink 5.
+// own address space.  Kernels then address `peer_ptrs[r] + offset` directly over NVLink.
 // When the fabric supports it, one multicast object is bound over all arenas; stores to /
 // reductions from `mc_ptr + offset` are replicated / reduced inside the NVSwitch
 // (multimem.st / multimem.ld_reduce).

@@ -5,7 +5,7 @@ The reference's benchmark resolves ``--model`` against every torchvision constru
 0.2.1 (SURVEY.md 2.7).  A dense layer is pre-activation — ``norm1 -> relu -> conv1(1x1) -> norm2 -> relu ->
 conv2(3x3)`` — so it maps onto: one standalone BN+ReLU kernel (``ops.batch_norm_act``), one fused conv+BN+ReLU unit
 and one plain conv; the growing feature map is assembled by the native channel-concat kernel.  All widths are
-multiples of 16, which the tcgen05 conv kernels accept (partial 64-channel k-blocks are zero-filled by TMA).
+multiples of 16, which the wgmma conv kernels accept (partial 64-channel k-blocks are zero-filled by TMA).
 """
 from __future__ import annotations
 

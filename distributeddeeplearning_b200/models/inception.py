@@ -5,7 +5,7 @@ Keys match ``torchvision.models.inception_v3``.  The reference cannot actually r
 SURVEY.md Q2); here the workloads size the input from ``model.input_size`` and add the 0.4-weighted
 auxiliary loss.
 
-Every layer runs on the tcgen05 conv kernels: Inception's widths (32/48/80/96/192/288/320/448 ...) are multiples
+Every layer runs on the wgmma conv kernels: Inception's widths (32/48/80/96/192/288/320/448 ...) are multiples
 of 8, which is all the kernels need (partial 64-channel k-blocks are zero-filled by TMA, partial N tiles masked), and
 the 1x7 / 7x1 kernels use per-axis padding.  Branch outputs are concatenated by ``ops.concat_channels`` (one native
 gather kernel forward, one scatter kernel backward).

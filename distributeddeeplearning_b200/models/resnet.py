@@ -4,7 +4,7 @@ Architecture and state_dict keys match ``torchvision.models.resnet*`` — the mo
 instantiates by name (``PyTorch_benchmark/src/pytorch_synthetic_benchmark.py:60``,
 ``PyTorch_imagenet/src/imagenet_pytorch_horovod.py:383``, ``PyTorch_hvd/...:115``; the TF twin
 builds the same v1.5 variant, ``TensorFlow_imagenet/src/resnet_model.py:193-195,237-320``).
-Every conv+BN(+ReLU)(+residual) is ONE fused op (``ops.conv_bn_act``): tcgen05 implicit GEMM with
+Every conv+BN(+ReLU)(+residual) is ONE fused op (``ops.conv_bn_act``): wgmma implicit GEMM with
 BN statistics in its epilogue, then a single BN-apply/ReLU/add pass.
 """
 from __future__ import annotations

@@ -1,7 +1,7 @@
 """VGG-11/13/16/19 (+BN variants) — the large-gradient allreduce stress model (527.8 MiB fp32 for
 VGG-16, one 392 MiB FC tensor; SURVEY.md 2.7).  Keys match ``torchvision.models.vgg*``.
 
-conv+bias+ReLU is one tcgen05 kernel (bias/ReLU in the epilogue, SURVEY.md K20); the three FC
+conv+bias+ReLU is one wgmma kernel (bias/ReLU in the epilogue, SURVEY.md K20); the three FC
 layers are the same GEMM kernel; dropout recomputes its Philox mask in backward.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Fused ops: hand-written sm_100a kernels on CUDA, PyTorch composites on CPU (see functional.py)."""
+"""Fused ops: hand-written sm_90a kernels on CUDA, PyTorch composites on CPU (see functional.py)."""
 from .functional import (  # noqa: F401
     advance_dropout_step,
     avg_pool2d,

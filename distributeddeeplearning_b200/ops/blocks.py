@@ -27,9 +27,9 @@ from . import native
 from .functional import CL, grad_buffer, notify_ready, run_wgrad, weight_bf16
 
 
-# Measured on B200 (ResNet-50, batch 256): folding the BN-backward reduction into the producing dgrad's epilogue removes
-# 32 launches and one read of each inner gradient tensor but makes those (already epilogue-bound) dgrads slower: net
-# +0.4 ms/step.  Off unless DDL_FUSE_BN_REDUCE=1.
+# Folding the BN-backward reduction into the producing dgrad's epilogue removes 32 launches and one read of each inner
+# gradient tensor but makes those (already epilogue-bound) dgrads slower.  Off unless DDL_FUSE_BN_REDUCE=1 (not
+# re-measured on H100).
 FUSE_BN_REDUCE = os.environ.get("DDL_FUSE_BN_REDUCE", "0") != "0"
 
 

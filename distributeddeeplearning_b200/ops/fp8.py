@@ -1,9 +1,11 @@
 """FP8 training mode: e4m3 activations / weights and e5m2 gradients as tensor-core operands of the forward and
-data-gradient convolutions (``tcgen05.mma.kind::f8f6f4``), everything else unchanged (bf16 activations in memory, fp32
-accumulation, bf16 weight-gradient GEMMs, fp32 BN / softmax / master weights / optimizer).
+data-gradient convolutions (``wgmma ... .e4m3.e4m3`` / ``.e5m2.e4m3``), everything else unchanged (bf16 activations in
+memory, fp32 accumulation, bf16 weight-gradient GEMMs, fp32 BN / softmax / master weights / optimizer).  fp8 wgmma reads
+K-major operands only, so the data gradient takes its weights from a per-step transposed e4m3 copy
+``[Cin][R*S*Cout]`` (``quantize_weight_t``) instead of reading the forward's copy MN-major.
 
 Reference parity: the only reduced-precision switch the reference has is ``--use_fp16`` of its TensorFlow benchmark
-tasks (``TensorFlow_benchmark/tensorflow_benchmark.py:51,77``); on Blackwell the equivalent "use the fast tensor-core
+tasks (``TensorFlow_benchmark/tensorflow_benchmark.py:51,77``); on Hopper the equivalent "use the fast tensor-core
 format" switch is FP8 (BASELINE config #3).  Enabled with ``--precision fp8`` on the trainers / ``DDL_PRECISION=fp8``.
 
 Recipe = delayed per-tensor scaling (csrc/ops/fp8.cu): each quantised tensor role owns a slot {amax, scale,
@@ -21,7 +23,7 @@ import torch
 
 from .. import _ext
 
-_STATE = {"mx_launches": 0, "enabled": os.environ.get("DDL_PRECISION", "bf16").lower() == "fp8", "table": None, "n": 0, "slots": {},
+_STATE = {"enabled": os.environ.get("DDL_PRECISION", "bf16").lower() == "fp8", "table": None, "n": 0, "slots": {},
           "calibrated": set(), "step": 0, "wcache": {}, "stats": {"fwd": 0, "dgrad": 0}}
 _MAX_SLOTS = 4096
 
@@ -142,34 +144,6 @@ def twin_of(t: torch.Tensor):
     return e[1], e[2]
 
 
-# ---- MX (OCP microscaling) block-scaled operands: one UE8M0 scale per 32 K elements of every row -----------------------
-MX = os.environ.get("DDL_FP8_MX", "0") == "1"      # 1x1 convolutions / GEMMs use kind::mxf8f6f4.block_scale
-
-
-def quantize_mx(x2d_bf16: torch.Tensor, rows: int, K: int):
-    """bf16 row-major [rows][K] (K % 128 == 0) -> (e4m3 codes uint8 [rows][K], scale atoms uint8): the scales are laid out
-    in the 512-byte atoms tcgen05 copies into TMEM (row block of 128 x K block of 128)."""
-    from . import native
-
-    C = _ext.load()
-    dev = x2d_bf16.device
-    out = torch.empty(rows * K, dtype=torch.uint8, device=dev)
-    sf = torch.zeros(((rows + 127) // 128) * (K // 128) * 512, dtype=torch.uint8, device=dev)
-    C.fp8_quantize_mx(x2d_bf16.data_ptr(), out.data_ptr(), sf.data_ptr(), rows, K, native.sm_count(dev.index or 0),
-                      torch.cuda.current_stream(dev).cuda_stream)
-    return out, sf
-
-
-def quantize_weight_mx(w_bf16: torch.Tensor):
-    key = ("wmx", w_bf16.data_ptr(), tuple(w_bf16.shape))
-    hit = _STATE["wcache"].get(key)
-    if hit is not None and hit[0] == _STATE["step"]:
-        return hit[1], hit[2]
-    q, sf = quantize_mx(w_bf16, w_bf16.shape[0], w_bf16.shape[1])
-    _STATE["wcache"][key] = (_STATE["step"], q, sf)
-    return q, sf
-
-
 def quantize_weight(w_bf16: torch.Tensor) -> Tuple[torch.Tensor, int]:
     """e4m3 copy of a bf16 weight matrix, quantised once per step and shared by forward and dgrad."""
     key = ("w", w_bf16.data_ptr(), tuple(w_bf16.shape))
@@ -179,6 +153,22 @@ def quantize_weight(w_bf16: torch.Tensor) -> Tuple[torch.Tensor, int]:
     q, idx = quantize(w_bf16, key)
     _STATE["wcache"][key] = (_STATE["step"], q, idx)
     return q, idx
+
+
+def quantize_weight_t(w_bf16: torch.Tensor, taps: int, cin: int) -> Tuple[torch.Tensor, int]:
+    """The data gradient's K-major e4m3 weights: this step's copy of ``w_bf16`` [Cout][taps*Cin] transposed to
+    [Cin][taps*Cout] (same codes, same scale slot), made once per step."""
+    q, idx = quantize_weight(w_bf16)
+    key = ("wt", w_bf16.data_ptr(), tuple(w_bf16.shape))
+    hit = _STATE["wcache"].get(key)
+    if hit is not None and hit[0] == _STATE["step"]:
+        return hit[1], hit[2]
+    cout = w_bf16.shape[0]
+    qt = torch.empty((cin, taps * cout), dtype=torch.uint8, device=w_bf16.device)
+    _ext.load().fp8_transpose_taps(q.data_ptr(), qt.data_ptr(), cout, taps, cin,
+                                   torch.cuda.current_stream(w_bf16.device).cuda_stream)
+    _STATE["wcache"][key] = (_STATE["step"], qt, idx)
+    return qt, idx
 
 
 def end_of_step(device=None) -> None:
@@ -193,9 +183,8 @@ def end_of_step(device=None) -> None:
     _STATE["step"] += 1          # next step quantises its weights again (a captured step never reuses an eager copy)
 
 
-# fp8 pays where the main loop dominates: measured per layer (profiles/layer_bench_fp8.md), reductions of >= 512
-# elements run 1.5-1.9x faster than bf16, shorter ones are epilogue-bound and lose (the fp8 path exists on the
-# one-CTA-per-SM deep-ring kernel only, which trails the two-CTA persistent kernel on short-K layers).
+# fp8 pays where the main loop dominates (long reductions); short ones are epilogue-bound.  The 512-element threshold
+# was not re-measured on H100.
 MIN_K = int(os.environ.get("DDL_FP8_MIN_K", "512"))
 
 
@@ -204,7 +193,7 @@ def fwd_eligible(cin: int, cout: int, taps: int = 1) -> bool:
 
 
 def dgrad_eligible(cin: int, cout: int, taps: int = 1) -> bool:
-    # reduction dim = Cout (k-blocks of 128), MN-major weight boxes are 128 input channels wide
+    # reduction dim = Cout (k-blocks of 128), transposed weight rows = input channels (N tiles of 128)
     return _STATE["enabled"] and cout % 128 == 0 and cin % 128 == 0 and cout * taps >= MIN_K
 
 

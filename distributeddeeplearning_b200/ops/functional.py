@@ -1,4 +1,4 @@
-"""Differentiable fused ops: native sm_100a kernels on CUDA, plain PyTorch composites on CPU.
+"""Differentiable fused ops: native sm_90a kernels on CUDA, plain PyTorch composites on CPU.
 
 Each public function has ONE GPU implementation (the hand-written kernels; there is no
 cuDNN/cuBLAS/ATen alternative behind a switch on the flagship path) and a CPU implementation built
@@ -259,8 +259,8 @@ class _ConvBnActPool(torch.autograd.Function):
         return (dx,) + (None,) * 13
 
 
-# Measured on B200 (ResNet-50, batch 256): the fused stem trades ~1.2 GB of HBM traffic for ~5 GB of L2 gathers and is
-# 0.25 ms/step SLOWER than BN-apply + max-pool as separate streaming kernels, so it is off unless DDL_FUSE_STEM_POOL=1.
+# The fused stem trades ~1.2 GB of HBM traffic for ~5 GB of L2 gathers; it is off unless DDL_FUSE_STEM_POOL=1 (which of
+# the two is faster on H100 was not measured).
 FUSE_STEM_POOL = os.environ.get("DDL_FUSE_STEM_POOL", "0") != "0"
 
 

@@ -1,9 +1,9 @@
-"""Checked Python wrappers over the sm_100a kernels in ``_C`` (GPU only).
+"""Checked Python wrappers over the sm_90a kernels in ``_C`` (GPU only).
 
 Activations are ``torch.bfloat16`` tensors with logical shape ``[N, C, H, W]`` and
 ``channels_last`` memory (physically NHWC).  Convolution weights are logical
 ``[Cout, Cin, R, S]`` ``channels_last`` (physically KRSC), which is exactly the row-major
-``[Cout][R*S*Cin]`` GEMM operand the tcgen05 kernels consume — the bf16 compute copy is a flat
+``[Cout][R*S*Cin]`` GEMM operand the wgmma kernels consume — the bf16 compute copy is a flat
 cast of the fp32 master, and wgrad writes the fp32 gradient in the same layout.
 """
 from __future__ import annotations
@@ -26,18 +26,16 @@ def _C():
         C.set_wgrad_swap(0)
     if os.environ.get("DDL_CONV_PERSISTENT", "") in ("0", "2"):    # tuning hook: 0 = never, 2 = always persistent
         C.set_conv_persistent(int(os.environ["DDL_CONV_PERSISTENT"]))
-    if os.environ.get("DDL_CONV_CLUSTER", "0") in ("1", "2"):     # tuning hook: 1 = CTA pairs + TMA multicast of the
-        C.set_conv_cluster(int(os.environ["DDL_CONV_CLUSTER"]))       #   weights, 2 = cta_group::2 pair MMAs
-    if os.environ.get("DDL_CONV_BN256", "0") == "1":       # tuning hook (A/B runs): 128 x 256 persistent tiles
-        C.set_conv_bn256(1)
+    if os.environ.get("DDL_CONV_CLUSTER", "0") in ("1", "2"):     # tuning hook: the persistent kernel as CTA pairs that
+        C.set_conv_cluster(int(os.environ["DDL_CONV_CLUSTER"]))       #   share the weight tile by TMA multicast
     if os.environ.get("DDL_BN_REVERSE", "") in ("0", "1"):             # BN row traversal order (A/B runs)
         C.set_bn_reverse(int(os.environ["DDL_BN_REVERSE"]))
     if os.environ.get("DDL_CONV_WAIT_HINT", ""):                       # ns; suspend-time hint of the mbarrier waits (A/B runs)
         C.set_conv_wait_hint(int(os.environ["DDL_CONV_WAIT_HINT"]))
     if os.environ.get("DDL_PDL", "") in ("0", "1", "2", "3"):         # programmatic dependent launch (A/B runs, launch.h)
         C.set_pdl(int(os.environ["DDL_PDL"]))
-    if os.environ.get("DDL_CONV_DEEP", "") in ("0", "2", "3", "4"):   # 0 = never the deep-ring kernel; 2-4 = force it
-        C.set_conv_deep(int(os.environ["DDL_CONV_DEEP"]))            #   (with pairs / without / without + N <= 128)
+    if os.environ.get("DDL_CONV_DEEP", "") in ("0", "2", "3", "4"):   # 2 = persistent CTA pairs wherever they apply,
+        C.set_conv_deep(int(os.environ["DDL_CONV_DEEP"]))            #   3 / 4 = persistent single CTAs
     return C
 
 
@@ -45,26 +43,25 @@ def _C():
 # per-shape kernel autotuning — the analogue of the reference's ``torch.backends.cudnn.benchmark = True``
 # (``PyTorch_benchmark/src/pytorch_synthetic_benchmark.py:57``, ``PyTorch_imagenet/src/imagenet_pytorch_horovod.py:378``)
 # ------------------------------------------------------------------------------------------------
-# The tcgen05 conv/GEMM launcher has several kernels for the same maths (one tile per CTA; persistent with two CTAs per
-# SM; deep-ring with one CTA or one cta_group::2 pair per SM, 64/128/256-wide tiles).  Which one wins depends on K, the
-# number of tiles and how memory-bound the epilogue is, so the first (eager) call of every distinct layer shape times
-# the applicable variants on the real operands and remembers the winner; CUDA-graph capture and all later calls use
-# the table.  ``DDL_CONV_AUTOTUNE=0`` keeps the launcher's built-in policy.
-VAR_ONE_TILE, VAR_PERSISTENT, VAR_DEEP = 1, 2, 3
+# The launcher (csrc/ops/conv_gemm.cu) has several kernels for the same maths (one tile per CTA; persistent with one
+# CTA per SM walking tiles; the persistent kernel as CTA pairs sharing the weight tile by TMA multicast).  Which one wins
+# depends on K, the number of tiles and how memory-bound the epilogue is, so the first (eager) call of every distinct
+# layer shape times the applicable variants on the real operands and remembers the winner; CUDA-graph capture and all
+# later calls use the table.  ``DDL_CONV_AUTOTUNE=0`` keeps the launcher's built-in policy.
+VAR_ONE_TILE, VAR_PERSISTENT = 1, 2
+VAR_PAIR = 1 << 8
 _TUNE = {"enabled": os.environ.get("DDL_CONV_AUTOTUNE", "1") == "1", "table": {}, "timings": {}}
 
 
-def conv_variants(n_total: int, m_rows: int, kb: int, b_mn_major: bool):
-    """Variant words worth timing for an ``m_rows`` x ``n_total`` x ``kb*64`` problem (see launch_fwd_mode)."""
-    out = [VAR_ONE_TILE, VAR_PERSISTENT]
-    if m_rows < 128 * 148:            # less than one wave of 128-row tiles: the persistent kernels cannot pay
-        return out[:1]
-    widths = [w for w in (256, 128, 64) if n_total % w == 0][:2]
-    for w in widths:
-        code = {64: 1, 128: 2, 256: 3}[w]
-        out.append(VAR_DEEP | (code << 4))
-        if not (b_mn_major and w < 128):
-            out.append(VAR_DEEP | (code << 4) | (1 << 8))
+def conv_variants(n_total: int, m_rows: int, kb: int, b_mn_major: bool, fp8: bool = False):
+    """Variant words worth timing for an ``m_rows`` x ``n_total`` x ``kb*64`` problem (see launch_fwd_mode).  fp8
+    operands run on the one-tile kernel only."""
+    out = [VAR_ONE_TILE]
+    if fp8 or m_rows < 128 * 132:     # less than one wave of 128-row tiles: the persistent kernels cannot pay
+        return out
+    out.append(VAR_PERSISTENT)
+    if not (b_mn_major and n_total % 128 != 0):       # MN-major weight tiles split into two 64-column boxes
+        out.append(VAR_PERSISTENT | VAR_PAIR)
     return out
 
 
@@ -74,10 +71,7 @@ def force_variant(v: Optional[int]) -> None:
 
 
 def variant_name(v: int) -> str:
-    kind = {0: "policy", 1: "one-tile", 2: "persistent", 3: "deep"}[v & 0xf]
-    if (v & 0xf) == 3:
-        kind += "-N%d" % {0: 0, 1: 64, 2: 128, 3: 256}[(v >> 4) & 0xf] + ("-pair" if (v >> 8) & 1 else "")
-    return kind
+    return {0: "policy", 1: "one-tile", 2: "persistent"}[v & 0xf] + ("-pair" if v & VAR_PAIR else "")
 
 
 def autotune_table():
@@ -86,19 +80,18 @@ def autotune_table():
             for k, v in _TUNE["table"].items()}
 
 
-_SITES = {1: "producer waits for a free stage", 2: "MMA waits for operands", 3: "MMA waits for a drained accumulator",
-          4: "epilogue waits for the accumulator"}
-_FAMILIES = {1: "one-tile", 2: "persistent", 3: "deep-ring", 4: "wgrad"}
+_SITES = {1: "producer waits for a free stage", 2: "MMA waits for operands"}
+_FAMILIES = {1: "conv", 4: "wgrad"}
 
 
 def conv_timeouts(raise_error: bool = True):
-    """Post-mortem of the tcgen05 kernels' bounded mbarrier waits (tc_utils.cuh): None, or a description of the first
+    """Post-mortem of the conv kernels' bounded mbarrier waits (tc_utils.cuh): None, or a description of the first
     wait that timed out since the last call (the kernels drain instead of hanging / trapping; results are garbage)."""
     info = _C().conv_timeout_info()
     if not info[0]:
         return None
     site = int(info[1])
-    msg = (f"tcgen05 pipeline timeout in the {_FAMILIES.get(site >> 4, '?')} kernel: "
+    msg = (f"conv pipeline timeout in the {_FAMILIES.get(site >> 4, '?')} kernel: "
            f"{_SITES.get(site & 15, 'site %d' % site)} (block {info[2]}, thread {info[3]}, parity {info[4]})")
     if raise_error:
         raise RuntimeError(msg)
@@ -115,7 +108,7 @@ def _tuned(key, candidates, launch, accumulators=()):
     if v is not None:
         return launch(v)
     if torch.cuda.is_current_stream_capturing() or len(candidates) < 2:
-        return launch(candidates[0] if len(candidates) == 1 else 0)
+        return launch(0)                               # nothing to choose: the launcher's policy (and its tuning hooks)
     times = {}
     for c in candidates:
         try:
@@ -341,7 +334,7 @@ def stem_prepare(x4: torch.Tensor, kernel: Tuple[int, int], stride: int, pad, di
 
 
 def supports_conv(cin: int, cout: int) -> bool:
-    """Shapes the tcgen05 implicit-GEMM kernels handle natively: channel counts that are multiples of 8 (one 16-byte
+    """Shapes the wgmma implicit-GEMM kernels handle natively: channel counts that are multiples of 8 (one 16-byte
     vector; partial 64-channel k-blocks / N tiles are zero-filled or masked in the kernels) or an NHWC4 stem."""
     return cout % 8 == 0 and (cin % 8 == 0 or cin <= 4)
 
@@ -397,19 +390,6 @@ def conv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, kernel: Tuple[int, int], str
 
     one_by_one = R == 1 and S == 1 and stride == 1 and ph == 0 and pw == 0
     tile_ok = USE_TILE_TMA and (stride == 1 or (stride == 2 and R * S <= 16 and USE_TILE_S2))
-    if _fp8.enabled() and _fp8.MX and one_by_one and Cin % 128 == 0 and Cout % 128 == 0 and M >= 2048 and bias is None \
-            and Cin >= _fp8.MIN_K:
-        # MX block-scaled e4m3 operands (kind::mxf8f6f4.block_scale): one UE8M0 scale per 32 channels of every pixel and
-        # of every filter, applied by the tensor core itself — no per-tensor scale, nothing to undo in the epilogue
-        xq, sfa = _fp8.quantize_mx(x, M, Cin)
-        wq, sfb = _fp8.quantize_weight_mx(w_bf16)
-        cch8 = Cin // 128
-        _fp8.count("fwd")
-        _fp8._STATE["mx_launches"] += 1
-        C.conv_gemm(C.CONV_GEMM, 0, y.data_ptr(), 0, 0, s_ptr, ss_ptr, M, cch8, Cout, H, W, Cin, P, Q, 1, 1, 1, 0, 1, cch8,
-                    int(relu), Cout, wq.data_ptr(), wr, wc, n_total, xq.data_ptr(), Cin, N, 0, 0, 0, 0, _stream(), 0, Cin,
-                    fp8=3, sfa=sfa.data_ptr(), sfb=sfb.data_ptr())
-        return (y, st) if stats else y
     if _fp8.fwd_eligible(Cin, Cout, R * S) and (one_by_one or tile_ok) and M >= 2048:
         # e4m3 operands: quantise x (delayed per-tensor scale) and take this step's e4m3 weights; a k-block is 128
         # channels (128 bytes), the epilogue multiplies by inv_scale(x) * inv_scale(w)
@@ -420,7 +400,7 @@ def conv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, kernel: Tuple[int, int], str
         wq, sw = _fp8.quantize_weight(w_bf16)
         cch8 = Cin // 128
         fp8kw = dict(fp8=1, deq_a=_fp8.inv_scale_ptr(sx, x.device), deq_b=_fp8.inv_scale_ptr(sw, x.device))
-        cands = [v for v in conv_variants(n_total, M, R * S * cch8, False) if (v & 0xf) == VAR_DEEP]
+        cands = conv_variants(n_total, M, R * S * cch8, False, fp8=True)
         _fp8.count("fwd")
         if one_by_one:
             _tuned(("fwd1x1_f8", N, H, W, Cin, Cout, stats, bias is not None, relu), cands,
@@ -515,39 +495,41 @@ def conv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, kernel: Tuple[in
     if _fp8.dgrad_eligible(Cin, Cout, R * S if stride == 1 else max(1, (R * S) // 4)) and bn_reduce is None \
             and N * H * W >= 2048 and \
             (one_by_one or (stride == 1 and USE_TILE_TMA) or s2_tile):
-        # e5m2 output gradients x e4m3 weights (the forward's quantised copy, consumed MN-major): k-blocks of 128
-        # output channels; the epilogue (incl. the shortcut-gradient add) runs on the de-quantised fp32 accumulator
+        # e5m2 output gradients x e4m3 weights, both K-major: the weights come as this step's transposed e4m3 copy
+        # [Cin][R*S*Cout] (same scale as the forward's copy); k-blocks of 128 output channels; the epilogue (incl. the
+        # shortcut-gradient add) runs on the de-quantised fp32 accumulator
         tw_ = _fp8.twin_of(dy)                      # produced by the BN-backward kernel that wrote dy, if any
         if tw_ is None:
             _fp8.request_twin(dy)
         dyq, sd = tw_ if tw_ is not None else _fp8.quantize(dy, ("dy", wp, N, P, Q), e5m2=True)
-        wq, sw = _fp8.quantize_weight(w_bf16)
+        wt, sw = _fp8.quantize_weight_t(w_bf16, R * S, Cin)
+        wtp, wtr, wtc = wt.data_ptr(), Cin, R * S * Cout
         cch8 = Cout // 128
         fp8kw = dict(fp8=2, deq_a=_fp8.inv_scale_ptr(sd, dy.device), deq_b=_fp8.inv_scale_ptr(sw, dy.device))
         _fp8.count("dgrad")
         if one_by_one:
-            cands = [v for v in conv_variants(n_total, N * H * W, cch8, True) if (v & 0xf) == VAR_DEEP]
+            cands = conv_variants(n_total, N * H * W, cch8, True, fp8=True)
             _tuned(("dgrad1x1_f8", N, H, W, Cin, Cout, add is not None, add_mask is not None), cands,
                    lambda v: C.conv_gemm(C.CONV_GEMM_DGRAD, 0, dx.data_ptr(), _ptr(add), 0, 0, 0, N * H * W, cch8, Cin, P,
-                                         Q, Cout, H, W, 1, 1, 1, 0, 1, cch8, 0, Cin, wq.data_ptr(), wr, wc, n_total,
-                                         dyq.data_ptr(), Cout, N, 0, 0, 0, 0, _stream(), 0, 0, _ptr(add_mask), variant=v,
+                                         Q, Cout, H, W, 1, 1, 1, 0, 1, cch8, 0, Cin, wtp, wtr, wtc, n_total,
+                                         dyq.data_ptr(), Cout, N, 0, 0, 0, 0, _stream(), 0, Cout, _ptr(add_mask), variant=v,
                                          **fp8kw))
         elif stride == 1:
             tw, th, tn = tile_geometry(H, W, N, 128)
-            cands = [v for v in conv_variants(n_total, N * H * W, R * S * cch8, True) if (v & 0xf) == VAR_DEEP]
+            cands = conv_variants(n_total, N * H * W, R * S * cch8, True, fp8=True)
             _tuned(("dgrad_f8", N, H, W, Cin, Cout, R, S, ph, pw, dil, add is not None, add_mask is not None), cands,
                    lambda v: C.conv_gemm(C.CONV_TILE_DGRAD, 0, dx.data_ptr(), _ptr(add), 0, 0, 0, N * H * W,
                                          R * S * cch8, Cin, P, Q, Cout, H, W, R, S, 1, ph, dil, cch8, 0, Cin,
-                                         wq.data_ptr(), wr, wc, n_total, dyq.data_ptr(), Cout, N, tw, th, tn, 0,
-                                         _stream(), pw, 0, _ptr(add_mask), variant=v, **fp8kw))
+                                         wtp, wtr, wtc, n_total, dyq.data_ptr(), Cout, N, tw, th, tn, 0,
+                                         _stream(), pw, Cout, _ptr(add_mask), variant=v, **fp8kw))
         else:
             tw, th, tn = tile_geometry((H + 1) // 2, (W + 1) // 2, N, 128)
-            cands = [v for v in conv_variants(n_total, N * ((H + 1) // 2) * ((W + 1) // 2),
-                                              max(1, (R * S * cch8) // 4), True) if (v & 0xf) == VAR_DEEP]
+            cands = conv_variants(n_total, N * ((H + 1) // 2) * ((W + 1) // 2),
+                                              max(1, (R * S * cch8) // 4), True, fp8=True)
             _tuned(("dgrad_s2_f8", N, H, W, Cin, Cout, R, S, ph, pw, dil, zfill), cands,
                    lambda v: C.conv_gemm(C.CONV_TILE_DGRAD, 0, dx.data_ptr(), 0, 0, 0, 0, N * H * W, R * S * cch8, Cin, P,
-                                         Q, Cout, H, W, R, S, 2, ph, dil, cch8, 0, Cin, wq.data_ptr(), wr, wc, n_total,
-                                         dyq.data_ptr(), Cout, N, tw, th, tn, zfill, _stream(), pw, 0, 0, variant=v,
+                                         Q, Cout, H, W, R, S, 2, ph, dil, cch8, 0, Cin, wtp, wtr, wtc, n_total,
+                                         dyq.data_ptr(), Cout, N, tw, th, tn, zfill, _stream(), pw, Cout, 0, variant=v,
                                          **fp8kw))
         return dx
     if R == 1 and S == 1 and stride == 1 and ph == 0 and pw == 0:

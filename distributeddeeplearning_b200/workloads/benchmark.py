@@ -12,7 +12,7 @@
 
 What differs underneath (SURVEY.md 3.2): the step is device-timed with CUDA events and reduced
 with max over ranks (the reference host-times rank 0 with ``timeit`` and no synchronize); the model
-runs the hand-written sm_100a kernels in bf16 with fp32 master weights; ``DistributedOptimizer``
+runs the hand-written sm_90a kernels in bf16 with fp32 master weights; ``DistributedOptimizer``
 is the fused NVLink allreduce+SGD engine; the fixed batch is generated on the device.
 """
 from __future__ import annotations
@@ -48,7 +48,7 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--momentum", type=float, default=0.0)
     p.add_argument("--json", type=str, default=None, help="also write a JSON summary to this path ('-' = stdout)")
     p.add_argument("--profile", action="store_true", help="wrap phases in NVTX ranges")
-    p.add_argument("--precision", choices=["bf16", "fp8", "mxfp8"], default="bf16",
+    p.add_argument("--precision", choices=["bf16", "fp8"], default="bf16",
                    help="tensor-core operand format of the forward / data-gradient convolutions")
     p.add_argument("--phase-times", action="store_true",
                    help="after the benchmark, device-time forward / backward / optimizer join of a few eager steps and "
@@ -241,13 +241,12 @@ def run(args) -> Dict:
 
         os.environ["DDL_NO_CUDA"] = "1"
     dist.init()
-    if getattr(args, "precision", "bf16") in ("fp8", "mxfp8"):
+    if getattr(args, "precision", "bf16") == "fp8":
         if not cuda:
             raise SystemExit("--precision fp8 needs a CUDA device")
         from ..ops import fp8
 
         fp8.enable(True)
-        fp8.MX = args.precision == "mxfp8"
     session = BenchmarkSession(args.model, args.batch_size, cuda, args.fp16_allreduce, args.lr, args.momentum,
                                profile=args.profile)
     device = "GPU" if cuda else "CPU"

@@ -2,7 +2,7 @@
 
 A training step of this framework is ~340 kernel launches on three streams (main, weight-gradient side stream,
 bucket/comm stream) plus the Python autograd walk; at the reference's default batch of 64 images per GPU the host
-cannot issue them as fast as one B200 retires them.  ``GraphedStep`` captures ``fn(*static_inputs)`` once (after
+cannot issue them as fast as one H100 retires them.  ``GraphedStep`` captures ``fn(*static_inputs)`` once (after
 warm-up) and replays it: per step the host copies the new inputs into the static buffers, refreshes the pinned
 hyper-parameter blob (so LR schedules keep working — the upload is a memcpy node of the graph) and issues a single
 ``cudaGraphLaunch``.

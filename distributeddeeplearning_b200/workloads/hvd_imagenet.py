@@ -48,7 +48,7 @@ def build_parser():
     p.add_argument("--model", default="resnet50")
     p.add_argument("--synthetic-length", type=int, default=int(os.getenv("FAKE_DATA_LENGTH", 1281167)))
     p.add_argument("--num-workers", type=int, default=4)
-    p.add_argument("--precision", choices=["bf16", "fp8", "mxfp8"], default="bf16",
+    p.add_argument("--precision", choices=["bf16", "fp8"], default="bf16",
                    help="tensor-core operand format of the forward / data-gradient convolutions (ops/fp8.py)")
     p.add_argument("--no-cuda-graph", action="store_true", default=False,
                    help="launch every kernel of the training step eagerly instead of replaying a captured CUDA graph")
@@ -71,13 +71,12 @@ def _progress(total, desc, disable):
 
 def main(argv=None) -> int:
     args = build_parser().parse_args(argv)
-    if args.precision in ("fp8", "mxfp8"):
+    if args.precision == "fp8":
         if args.no_cuda:
             raise SystemExit("--precision fp8 needs CUDA")
         from ..ops import fp8
 
         fp8.enable(True)
-        fp8.MX = args.precision == "mxfp8"
     args.cuda = not args.no_cuda and torch.cuda.is_available()
     if not args.cuda:
         os.environ["DDL_NO_CUDA"] = "1"

@@ -185,17 +185,15 @@ def main(training_data_path=None, validation_data_path=None, use_gpu=False, save
         torch.cuda.manual_seed(_SEED)
     logger.info("PyTorch version {}".format(torch.__version__))
     precision = str(precision).lower()
-    if precision not in ("bf16", "fp8", "mxfp8"):
-        raise ValueError(f"precision must be bf16, fp8 or mxfp8, got {precision!r}")
-    if precision in ("fp8", "mxfp8"):
+    if precision not in ("bf16", "fp8"):
+        raise ValueError(f"precision must be bf16 or fp8, got {precision!r}")
+    if precision == "fp8":
         if not use_gpu:
-            raise ValueError("--precision fp8 needs --use_gpu True (tcgen05 fp8 tensor cores)")
+            raise ValueError("--precision fp8 needs --use_gpu True (fp8 tensor cores)")
         from ..ops import fp8
 
         fp8.enable(True)
-        fp8.MX = precision == "mxfp8"         # 1x1 forward convolutions with MX block-scaled operands (kind::mxf8f6f4)
-        logger.info("Precision: fp8 operands (e4m3 activations/weights, e5m2 gradients), fp32 accumulate"
-                    + ("; MX block scales (UE8M0 per 32 channels) for the 1x1 forward convolutions" if fp8.MX else ""))
+        logger.info("Precision: fp8 operands (e4m3 activations/weights) for the forward convolutions, fp32 accumulate")
 
     run = writer = None
     if rank == 0:

@@ -11,7 +11,7 @@ os.environ.setdefault("OMP_NUM_THREADS", "2")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on a B200 box with `pytest -m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 box with `pytest -m gpu`)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -100,7 +100,7 @@ def test_launch_accounting_table_matches_module(C):
 
     missing = [k for k in _ext.KERNEL_LAUNCHES if not hasattr(C, k)]
     assert not missing, missing
-    for hook in ("set_conv_persistent", "set_conv_cluster", "set_conv_bn256", "set_wgrad_swap", "set_conv_force_stages"):
+    for hook in ("set_conv_persistent", "set_conv_cluster", "set_wgrad_swap", "set_conv_force_stages", "set_conv_wait_hint"):
         assert hasattr(C, hook), hook
     n0 = _ext.launch_count()
     _ext.add_launches(7)
@@ -171,30 +171,30 @@ def test_step_launcher_accounting_without_a_gpu(C):
 
 def test_conv_variant_words_are_well_formed():
     """The autotuner's candidate list (ops/native.py) only produces variant words the launcher understands
-    (conv_gemm.cu: bits 0-3 kernel, 4-7 tile width, 8 pair) — never the epilogue debug bits 12-14 of tools/epi_probe.py."""
+    (conv_gemm.cu: bits 0-3 kernel 1 = one tile / 2 = persistent, bit 8 CTA pair, only with the persistent kernel) —
+    never the epilogue debug bits 12-14 of tools/epi_probe.py — and the fp8 forward convolutions only the one-tile kernel."""
     from distributeddeeplearning_b200.ops import native
 
     seen = set()
     for n_total in (64, 128, 192, 256, 512, 1024, 2048):
-        for m_rows in (128, 128 * 148 - 1, 128 * 148, 802816):
+        for m_rows in (128, 128 * 132 - 1, 128 * 132, 802816):
             for kb in (1, 4, 18, 36):
                 for mn in (False, True):
                     cands = native.conv_variants(n_total, m_rows, kb, mn)
                     assert cands[0] == native.VAR_ONE_TILE and len(set(cands)) == len(cands)
-                    if m_rows < 128 * 148:
+                    if m_rows < 128 * 132:
                         assert cands == [native.VAR_ONE_TILE]
                     for v in cands:
                         assert v >> 9 == 0, hex(v)                       # nothing above the pair bit
                         kind, width, pair = v & 0xf, (v >> 4) & 0xf, (v >> 8) & 1
-                        assert kind in (1, 2, 3) and width in (0, 1, 2, 3)
-                        if kind != 3:
-                            assert width == 0 and pair == 0
-                        else:
-                            assert n_total % {1: 64, 2: 128, 3: 256}[width] == 0
+                        assert kind in (1, 2) and width == 0
+                        if pair:
+                            assert kind == 2 and (not mn or n_total % 128 == 0)   # MN-major halves: 64-column boxes
                         name = native.variant_name(v)
-                        assert name.startswith(("one-tile", "persistent", "deep"))
+                        assert name.startswith(("one-tile", "persistent"))
                         seen.add(name)
-    assert {"one-tile", "persistent", "deep-N256-pair", "deep-N64"} <= seen
+                    assert native.conv_variants(n_total, m_rows, kb, mn, fp8=True) == [native.VAR_ONE_TILE]
+    assert {"one-tile", "persistent", "persistent-pair"} <= seen
 
 
 def test_fp8_eligibility_rules():

@@ -6,7 +6,7 @@
    multicast (NVLS) and peer-to-peer transports; replicas must stay bit-identical; broadcast kernel.
 2. sweep: in-place allreduce 64 KiB .. 1 GiB (fp32 / bf16; one-shot / two-shot; NVLS / P2P), device-timed
    with CUDA events, max over ranks, busbw = algbw * 2(N-1)/N, next to NCCL's all_reduce on the same sizes.
-Writes gpurun_out/comm_sweep_N{world}.json.
+With COMM_JSON=PATH the sweep is also written there as JSON.
 """
 import json
 import os
@@ -146,10 +146,9 @@ def main():
         oks.append(eq["ok"])
     max_bytes = int(os.environ.get("SWEEP_MAX", 1 << 30))
     res = [] if "--no-sweep" in sys.argv else sweep(max_bytes)
-    if dist.rank() == 0 and res:
-        os.makedirs("gpurun_out", exist_ok=True)
+    if dist.rank() == 0 and res and os.environ.get("COMM_JSON"):
         json.dump({"world": world, "multicast": had_mc, "results": res, "engine_checks_ok": all(oks)},
-                  open(f"gpurun_out/comm_sweep_N{world}.json", "w"), indent=1)
+                  open(os.environ["COMM_JSON"], "w"), indent=1)
     log("ENGINE CHECKS:", "all ok" if all(oks) else "FAILURES")
     dist.shutdown()
     return 0 if all(oks) else 1

@@ -5,9 +5,9 @@ For each gradient bucket of ResNet-50 (or --model) at batch --batch-size, in EAG
 between the launches): when the bucket became ready relative to the start of backward, how long its kernel ran on the
 comm stream (barrier-in wait + data phase [+ closing barrier on the last bucket]), and how much of the step was exposed
 after the last weight-gradient kernel (= what data parallelism costs on top of the single-GPU step).  Also reports the
-achieved fraction of the per-bucket roofline S*(1 + 1/N) bytes / 900 GB/s (NVLS two-shot: each rank pulls its
+achieved fraction of the per-bucket roofline S*(1 + 1/N) bytes / 450 GB/s (NVLink 4 per direction on H100; NVLS two-shot: each rank pulls its
 1/N slice through the switch and pushes S/N fp32 weights + S/N/2 bf16 copies + S/N zeros to every replica).
-Writes gpurun_out/comm_timeline_N{world}.json; max over ranks per bucket.
+Max over ranks per bucket; --json PATH also writes the timeline as JSON.
 """
 import argparse
 import json
@@ -27,6 +27,7 @@ def main():
     ap.add_argument("--batch-size", type=int, default=256)
     ap.add_argument("--steps", type=int, default=6)
     ap.add_argument("--fp16-allreduce", action="store_true")
+    ap.add_argument("--json", default=None)
     a = ap.parse_args()
     dist.init()
     rank, world = dist.rank(), dist.size()
@@ -94,16 +95,16 @@ def main():
         for bk in last["buckets"]:
             S = bk["mbytes"] * 1e6
             # NVLS two-shot wire per GPU: the reduce phase delivers this rank's S/N slice, the broadcast phase pushes
-            # S/N of results to the switch and every replica receives S: ~S * (1 + 1/N) bytes at 900 GB/s per direction
+            # S/N of results to the switch and every replica receives S: ~S * (1 + 1/N) bytes at 450 GB/s per direction (NVLink 4)
             Sw = S * wire / 4
-            roof = Sw * (1.0 + 1.0 / world) / 900e9 * 1e3 if world > 1 else 0.0
+            roof = Sw * (1.0 + 1.0 / world) / 450e9 * 1e3 if world > 1 else 0.0
             bk["roofline_ms"] = roof
             bk["achieved"] = roof / bk["kernel_ms"] if bk["kernel_ms"] > 0 else 0
             print(f"| {bk['bucket']} | {bk['mbytes']:.2f} | {bk['ready_at_ms']:.2f} | {bk['start_at_ms']:.2f} | "
                   f"{bk['kernel_ms']:.3f} | {roof:.3f} | {bk['achieved']:.2f} |")
-        os.makedirs("gpurun_out", exist_ok=True)
-        json.dump({"world": world, "model": a.model, "batch": a.batch_size, "steps": out_steps},
-                  open(f"gpurun_out/comm_timeline_N{world}.json", "w"), indent=1)
+        if a.json:
+            json.dump({"world": world, "model": a.model, "batch": a.batch_size, "steps": out_steps}, open(a.json, "w"),
+                      indent=1)
     dist.shutdown()
 
 

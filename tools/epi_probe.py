@@ -29,8 +29,7 @@ for (ci, hw, co, k, s, p) in SHAPES:
     mb = y.numel() * 2 / 1e6
     print(f"== {ci}x{hw}->{co} k{k}: out {mb:.0f} MB, in {x.numel() * 2 / 1e6:.0f} MB; memset {t_set:.1f} us "
           f"({mb / t_set * 1e3:.0f} GB/s), copy {t_cpy:.1f} us ({2 * mb / t_cpy * 1e3:.0f} GB/s r+w)", flush=True)
-    for base, name in ((2, "persistent"), (1, "one-tile"), (3 | (3 << 4), "deep-N256"), (3 | (2 << 4), "deep-N128"),
-                       (3 | (1 << 4), "deep-N64")):
+    for base, name in ((2, "persistent"), (1, "one-tile"), (2 | (1 << 8), "persistent-pair")):
         row = []
         for d, dn in DBG:
             nv.force_variant(base | (d << 12))

@@ -65,7 +65,7 @@ def report_abs(name, got, ref, rtol, atol):
 
 def g_fp8():
     """FP8 operand path: quantisation kernels vs torch.float8 casts; e4m3 x e4m3 forward and e5m2 x e4m3 data-gradient
-    convolutions (tcgen05 kind::f8f6f4, deep-ring kernel) vs an fp32 convolution of the DE-QUANTISED operands (isolates
+    convolutions (fp8 wgmma, one-tile kernel) vs an fp32 convolution of the DE-QUANTISED operands (isolates
     the kernel from the quantisation error) and vs the unquantised fp32 result (bounds the quantisation error)."""
     import torch
     import torch.nn.functional as F
@@ -138,39 +138,6 @@ def g_fp8():
         ref = torch.nn.grad.conv2d_input(xs, w.float(), dy.float(), s, p)
         report("  vs unquantised fp32", dx, ref, 1.5e-1)
         fp8.end_of_step()
-    # ---- MX block-scaled operands (kind::mxf8f6f4.block_scale): 1x1 convolutions = plain GEMMs
-    fp8.MX = True
-    for (n, ci, hw, co) in [(32, 128, 28, 256), (64, 512, 14, 128), (32, 1024, 14, 256), (33, 256, 15, 384)]:
-        x = cl(bf(torch.randn(n, ci, hw, hw, device=dev) * torch.rand(1, ci, 1, 1, device=dev) * 4))   # uneven channel scales
-        w = bf(torch.randn(co, ci, 1, 1, device=dev) * (1.0 / ci ** 0.5))
-        wb = _w_bf16(w)
-        before = fp8._STATE["mx_launches"]
-        y, st = nv.conv_fwd(x, wb, (1, 1), 1, 0, stats=True)
-        torch.cuda.synchronize()
-        assert fp8._STATE["mx_launches"] == before + 1, "MX path not taken"
-        M = n * hw * hw
-
-        def deq(codes, sf, rows, K):
-            v = codes.view(torch.float8_e4m3fn).float().view(rows, K)
-            kb = K // 128
-            sfv = sf.view((rows + 127) // 128, kb, 32, 4, 4).float()          # [mblk][kblk][m0][m1][s]
-            r = torch.arange(rows, device=dev)
-            blk, m0, m1 = r // 128, r % 32, (r % 128) // 32
-            e = sfv[blk, :, m0, m1, :]                                         # [rows][kb][4]
-            scale = torch.pow(2.0, e - 127.0).reshape(rows, kb * 4).repeat_interleave(32, dim=1)
-            return v * scale
-
-        xq, sfa = fp8.quantize_mx(x, M, ci)
-        wq, sfb = fp8.quantize_weight_mx(wb)
-        xd = deq(xq, sfa, M, ci)
-        wd = deq(wq, sfb, co, ci)
-        xm = x.permute(0, 2, 3, 1).reshape(M, ci).float()
-        report(f"MX quantise x n{n} c{ci}: de-quantised vs bf16", xd, xm, 0.07)
-        ref_q = (xd @ wd.t()).view(n, hw, hw, co).permute(0, 3, 1, 2)
-        report(f"MX conv 1x1 n{n} c{ci} {hw}x{hw}->{co} vs de-quantised fp32 GEMM", y, ref_q, 1e-2)
-        report("  vs unquantised fp32", y, _conv_ref(x, w, 1, 0), 6e-2)
-        fp8.end_of_step()
-    fp8.MX = False
     # ---- producer-side twins: BN-apply forward (e4m3) and BN backward (e5m2) emit the fp8 copy in their own pass
     ch, n, hw = 256, 16, 14
     yb = cl(bf(torch.randn(n, ch, hw, hw, device=dev) * 2 + 0.3))
