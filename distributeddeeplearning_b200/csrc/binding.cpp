@@ -258,14 +258,14 @@ PYBIND11_MODULE(_C, m) {
            int cchunks, int relu, int n_valid, ptr_t w, int w_rows, int w_cols, int n_total, ptr_t a_matrix, int a_cols,
            int batch, int tw, int th, int tn, int zfill, ptr_t stream, int pad_w, int kstride, ptr_t add_mask,
            ptr_t bnr_y, ptr_t bnr_gamma, ptr_t bnr_beta, ptr_t bnr_mean, ptr_t bnr_invstd, int variant, int fp8,
-           ptr_t deq_a, ptr_t deq_b, ptr_t sfa, ptr_t sfb) {
+           ptr_t deq_a, ptr_t deq_b, ptr_t sfa, ptr_t sfb, ptr_t bnr_mask) {
           ConvArgs a;
           a.variant = variant;
           a.fp8 = fp8; a.deq_a = P<const float>(deq_a); a.deq_b = P<const float>(deq_b);
           a.sfa = P<const uint8_t>(sfa); a.sfb = P<const uint8_t>(sfb);
           a.bnr_y = P<const __nv_bfloat16>(bnr_y); a.bnr_gamma = P<const float>(bnr_gamma);
           a.bnr_beta = P<const float>(bnr_beta); a.bnr_mean = P<const float>(bnr_mean);
-          a.bnr_invstd = P<const float>(bnr_invstd);
+          a.bnr_invstd = P<const float>(bnr_invstd); a.bnr_mask = P<const uint8_t>(bnr_mask);
           a.add_mask = P<const uint8_t>(add_mask);
           a.zfill = zfill;
           a.pad_w = pad_w < 0 ? pad : pad_w;
@@ -286,7 +286,7 @@ PYBIND11_MODULE(_C, m) {
         py::arg("zfill"), py::arg("stream"), py::arg("pad_w") = -1, py::arg("kstride") = 0, py::arg("add_mask") = 0,
         py::arg("bnr_y") = 0, py::arg("bnr_gamma") = 0, py::arg("bnr_beta") = 0, py::arg("bnr_mean") = 0,
         py::arg("bnr_invstd") = 0, py::arg("variant") = 0, py::arg("fp8") = 0, py::arg("deq_a") = 0,
-        py::arg("deq_b") = 0, py::arg("sfa") = 0, py::arg("sfb") = 0);
+        py::arg("deq_b") = 0, py::arg("sfa") = 0, py::arg("sfb") = 0, py::arg("bnr_mask") = 0);
   m.def("conv_wgrad",
         [](int mode, ptr_t x, ptr_t dy, ptr_t dw, int M, int Cout, int dy_ld, int ldw, int ncols, int H, int W, int C, int Pq,
            int Q, int R, int Sx, int stride, int pad, int dil, int cchunks, int splits, int batch, int tw, int th, int tn,

@@ -51,9 +51,17 @@ struct FwdCfg {
   static constexpr int kPitch = BLOCK_N * 2 + 16;                 // epilogue staging row pitch (bytes)
   static constexpr int kEpiBytes = ((kBlockM * kPitch + 1023) / 1024) * 1024;
   static constexpr int kFixed = kEpiBytes + 256 /*barriers*/ + 8192 /*stats scratch*/ + 1024 /*alignment*/;
-  static constexpr int kMaxStagesN = (232448 - kFixed) / kStageBytes > kMaxStages ? kMaxStages
-                                                                                   : (232448 - kFixed) / kStageBytes;
-  static constexpr int smem_bytes(int stages) { return stages * kStageBytes + kFixed; }
+  static constexpr int kYBytes = kBlockM * BLOCK_N * 2;           // BN input tile of the fused BN-backward reduction
+  static constexpr int max_stages(int fixed) {
+    return (232448 - fixed) / kStageBytes > kMaxStages ? kMaxStages : (232448 - fixed) / kStageBytes;
+  }
+  static constexpr int kMaxStagesN = max_stages(kFixed);
+  static constexpr int kMaxStagesBnr = max_stages(kFixed + kYBytes);   // the y tile takes its space from the ring
+  static constexpr int smem_bytes(int stages, bool bnr = false) {
+    return stages * kStageBytes + kFixed + (bnr ? kYBytes : 0);
+  }
+  static constexpr int kSmemMax = smem_bytes(kMaxStagesN) > smem_bytes(kMaxStagesBnr, true)
+                                      ? smem_bytes(kMaxStagesN) : smem_bytes(kMaxStagesBnr, true);
 };
 
 DDL_DEVICE void named_bar_sync(int id, int nthreads) {
@@ -177,14 +185,56 @@ struct StatAcc {
   }
 };
 
-// Fold the staged bf16 tile (row pitch BLOCK_N*2+16) into `acc`.  Thread = (column group of 8, row slice); invalid rows
-// hold zeros.  Entered by all kEpiThreads epilogue threads after the staging writes were made visible (named barrier 1).
+// val + (add gated by the 8 bits of `bits`), in the rounding of the stores: bf16 -> fp32 sum -> bf16.
+DDL_DEVICE uint4 add_gated_bf16x8(uint4 val, uint4 o, uint32_t bits) {
+  o.x &= ((bits & 1u) ? 0x0000ffffu : 0u) | ((bits & 2u) ? 0xffff0000u : 0u);
+  o.y &= ((bits & 4u) ? 0x0000ffffu : 0u) | ((bits & 8u) ? 0xffff0000u : 0u);
+  o.z &= ((bits & 16u) ? 0x0000ffffu : 0u) | ((bits & 32u) ? 0xffff0000u : 0u);
+  o.w &= ((bits & 64u) ? 0x0000ffffu : 0u) | ((bits & 128u) ? 0xffff0000u : 0u);
+  float2 p, q;
+  p = unpack_bf16x2(val.x); q = unpack_bf16x2(o.x); val.x = pack_bf16x2(p.x + q.x, p.y + q.y);
+  p = unpack_bf16x2(val.y); q = unpack_bf16x2(o.y); val.y = pack_bf16x2(p.x + q.x, p.y + q.y);
+  p = unpack_bf16x2(val.z); q = unpack_bf16x2(o.z); val.z = pack_bf16x2(p.x + q.x, p.y + q.y);
+  p = unpack_bf16x2(val.w); q = unpack_bf16x2(o.w); val.w = pack_bf16x2(p.x + q.x, p.y + q.y);
+  return val;
+}
+
+// Thread mapping of the statistics pass: thread = (column group of 8 channels, slice of kRowsPer consecutive rows).
+template <int BLOCK_N>
+struct StatMap {
+  static constexpr int kColGroups = BLOCK_N / 8;                 // 16 (N=128) or 8 (N=64)
+  static constexpr int kSlices = kEpiThreads / kColGroups;       // row slices
+  static constexpr int kRowsPer = kBlockM / kSlices;             // rows per thread
+};
+
+// Fused BN-backward reduction: copy the BN input rows this thread's statistics pass will pair with the gradient tile
+// into `ybuf` (dense rows of BLOCK_N*2 bytes) with cp.async, so that the loads run under the tile's MMAs instead of in
+// the epilogue.  Issued and later read by the same thread, so cp.async.wait_group is the only synchronisation needed.
+// Rows with no destination (`dest_row` < 0) and channels past n_valid are zero-filled and drop out of the sums.
+template <int BLOCK_N, typename DestRow>
+DDL_DEVICE void epi_bnr_prefetch(uint32_t ybuf, int etid, const ConvArgs& a, int n0, DestRow dest_row) {
+  using Map = StatMap<BLOCK_N>;
+  const int cg = etid % Map::kColGroups;
+  const int sl = etid / Map::kColGroups;
+  const int c0 = n0 + cg * 8;
+#pragma unroll 1
+  for (int r = 0; r < Map::kRowsPer; ++r) {
+    const int row = sl * Map::kRowsPer + r;
+    const int m = c0 < a.n_valid ? dest_row(row) : -1;
+    cp_async_16(ybuf + row * (BLOCK_N * 2) + cg * 16, m >= 0 ? a.bnr_y + static_cast<size_t>(m) * a.ldc + c0 : a.bnr_y,
+                m >= 0);
+  }
+  cp_async_commit();
+}
+
+// Fold the staged bf16 tile (row pitch BLOCK_N*2+16) into `acc`.  Thread = StatMap; invalid rows hold zeros.  Entered by
+// all kEpiThreads epilogue threads after the staging writes were made visible (named barrier 1).
 template <int BLOCK_N, bool TILE>
-DDL_DEVICE void epi_stats_accum(uint32_t stg, int etid, const ConvArgs& a, int n0, int m0, StatAcc& acc) {
+DDL_DEVICE void epi_stats_accum(uint32_t stg, uint32_t ybuf, int etid, const ConvArgs& a, int n0, int m0, StatAcc& acc) {
   constexpr int kPitch = BLOCK_N * 2 + 16;
-  constexpr int kColGroups = BLOCK_N / 8;                 // 16 (N=128) or 8 (N=64)
-  constexpr int kSlices = kEpiThreads / kColGroups;       // row slices
-  constexpr int kRowsPer = kBlockM / kSlices;             // rows per thread
+  constexpr int kColGroups = StatMap<BLOCK_N>::kColGroups;
+  constexpr int kRowsPer = StatMap<BLOCK_N>::kRowsPer;
+  if (a.bnr_y != nullptr) cp_async_wait<0>();            // this thread's y rows (epi_bnr_prefetch) have landed
   if (a.variant & kDbgNoStats) return;
   const int cg = etid % kColGroups;
   const int sl = etid / kColGroups;
@@ -203,9 +253,24 @@ DDL_DEVICE void epi_stats_accum(uint32_t stg, int etid, const ConvArgs& a, int n
     return;
   }
   // fused BN-backward reduction (see ConvArgs::bnr_y): S1 = sum dm, S2 = sum dm * y with the ReLU mask of the BN
-  // recomputed from y.  The y tile is read with the same coalesced 16-byte accesses the stores use.
+  // recomputed from y or read from its bit mask.  The y rows come from `ybuf` (zeros where the gradient row is zero as
+  // well).
   const int c0 = n0 + cg * 8;
   if (c0 >= a.n_valid) return;
+  const uint32_t y0 = ybuf + (sl * kRowsPer) * (BLOCK_N * 2) + cg * 16;
+  // linear rows: the shortcut gradient is added to the staged tile here, before the sums, so that the sums and the
+  // stores see the same value; the loads of all rows (add, its gate bits, the BN's mask bits) are issued together
+  uint4 addv[kRowsPer];
+  uint32_t gate[kRowsPer], zbits[kRowsPer];
+#pragma unroll
+  for (int r = 0; r < kRowsPer; ++r) {
+    const int m = m0 + sl * kRowsPer + r;
+    const bool ok = !TILE && m < a.M;
+    const size_t off = static_cast<size_t>(ok ? m : 0) * a.ldc + c0;
+    addv[r] = (ok && a.add) ? *reinterpret_cast<const uint4*>(a.add + off) : make_uint4(0, 0, 0, 0);
+    gate[r] = (ok && a.add && a.add_mask) ? a.add_mask[off >> 3] : 0xffu;
+    zbits[r] = (ok && a.bnr_mask) ? a.bnr_mask[off >> 3] : 0u;
+  }
   uint64_t sc[4], sh[4];
 #pragma unroll
   for (int qd = 0; qd < 2; ++qd) {
@@ -217,21 +282,21 @@ DDL_DEVICE void epi_stats_accum(uint32_t stg, int etid, const ConvArgs& a, int n
     sc[2 * qd] = f2_pack(s0, s1); sh[2 * qd] = f2_pack(b4.x - m4.x * s0, b4.y - m4.y * s1);
     sc[2 * qd + 1] = f2_pack(s2, s3); sh[2 * qd + 1] = f2_pack(b4.z - m4.z * s2, b4.w - m4.w * s3);
   }
-#pragma unroll 2
+#pragma unroll
   for (int r = 0; r < kRowsPer; ++r) {
-    const int row = sl * kRowsPer + r;
-    int m;
-    if (TILE) m = static_cast<int>(lds32(stg + row * kPitch + BLOCK_N * 2));
-    else m = (m0 + row) < a.M ? (m0 + row) : -1;
-    if (m < 0) continue;
-    const uint4 u = lds128(p0 + r * kPitch);
-    const uint4 yv = *reinterpret_cast<const uint4*>(a.bnr_y + static_cast<size_t>(m) * a.ldc + c0);
+    uint4 u = lds128(p0 + r * kPitch);
+    if (!TILE && a.add) {
+      u = add_gated_bf16x8(u, addv[r], gate[r]);
+      sts128(p0 + r * kPitch, u.x, u.y, u.z, u.w);      // published to epi_store by the barrier in epi_stats_flush
+    }
+    const uint4 yv = lds128(y0 + r * (BLOCK_N * 2));
     const uint32_t du[4] = {u.x, u.y, u.z, u.w}, yu[4] = {yv.x, yv.y, yv.z, yv.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const uint64_t y2 = f2_from_bf16x2(yu[j]);
       float z0, z1, d0, d1;
       f2_unpack(f2_fma(y2, sc[j], sh[j]), z0, z1);
+      if (a.bnr_mask) { z0 = (zbits[r] >> (2 * j)) & 1u ? 1.f : 0.f; z1 = (zbits[r] >> (2 * j + 1)) & 1u ? 1.f : 0.f; }
       f2_unpack(f2_from_bf16x2(du[j]), d0, d1);
       const uint64_t dm = f2_pack(z0 > 0.f ? d0 : 0.f, z1 > 0.f ? d1 : 0.f);
       acc.s[j] = f2_add(acc.s[j], dm);
@@ -311,7 +376,8 @@ DDL_DEVICE void epi_store(uint32_t stg, int etid, const ConvArgs& a, int n0, int
   if (a.variant & kDbgNoStore) return;
   uint32_t sp = stg + r0 * kPitch + ch * 16;
   const size_t coff = static_cast<size_t>(n0 + ch * 8);
-  if (a.add == nullptr && !(TILE && a.zfill)) {
+  const __nv_bfloat16* add = a.bnr_y == nullptr ? a.add : nullptr;     // else: added in epi_stats_accum
+  if (add == nullptr && !(TILE && a.zfill)) {
     // plain stores (every forward launch): nothing but the shared load, the row's address and the store
     if (!TILE) {
       const int rows = a.M - m0;                            // valid rows of this tile (>= kBlockM except in the last one)
@@ -342,20 +408,8 @@ DDL_DEVICE void epi_store(uint32_t stg, int etid, const ConvArgs& a, int n0, int
     if (m < 0) continue;
     uint4 val = lds128(sp);
     const size_t off = static_cast<size_t>(m) * a.ldc + coff;
-    if (a.add) {
-      uint4 o = *reinterpret_cast<const uint4*>(a.add + off);
-      if (a.add_mask) {
-        const uint32_t bits = a.add_mask[off >> 3];
-        o.x &= ((bits & 1u) ? 0x0000ffffu : 0u) | ((bits & 2u) ? 0xffff0000u : 0u);
-        o.y &= ((bits & 4u) ? 0x0000ffffu : 0u) | ((bits & 8u) ? 0xffff0000u : 0u);
-        o.z &= ((bits & 16u) ? 0x0000ffffu : 0u) | ((bits & 32u) ? 0xffff0000u : 0u);
-        o.w &= ((bits & 64u) ? 0x0000ffffu : 0u) | ((bits & 128u) ? 0xffff0000u : 0u);
-      }
-      float2 p, q;
-      p = unpack_bf16x2(val.x); q = unpack_bf16x2(o.x); val.x = pack_bf16x2(p.x + q.x, p.y + q.y);
-      p = unpack_bf16x2(val.y); q = unpack_bf16x2(o.y); val.y = pack_bf16x2(p.x + q.x, p.y + q.y);
-      p = unpack_bf16x2(val.z); q = unpack_bf16x2(o.z); val.z = pack_bf16x2(p.x + q.x, p.y + q.y);
-      p = unpack_bf16x2(val.w); q = unpack_bf16x2(o.w); val.w = pack_bf16x2(p.x + q.x, p.y + q.y);
+    if (add) {
+      val = add_gated_bf16x8(val, *reinterpret_cast<const uint4*>(add + off), a.add_mask ? a.add_mask[off >> 3] : 0xffu);
     }
     *reinterpret_cast<uint4*>(a.out + off) = val;
     if (TILE && a.zfill) {      // even outH/outW guaranteed by the host: all three siblings exist
@@ -369,11 +423,12 @@ DDL_DEVICE void epi_store(uint32_t stg, int etid, const ConvArgs& a, int n0, int
 
 // One tile: accumulate, publish, store.
 template <int BLOCK_N, bool STATS, bool TILE>
-DDL_DEVICE void epi_stats_store(uint32_t stg, uint32_t red, int etid, int ew, const ConvArgs& a, int n0, int m0) {
+DDL_DEVICE void epi_stats_store(uint32_t stg, uint32_t red, uint32_t ybuf, int etid, int ew, const ConvArgs& a, int n0,
+                                int m0) {
   if (STATS) {
     StatAcc acc;
     acc.clear();
-    epi_stats_accum<BLOCK_N, TILE>(stg, etid, a, n0, m0, acc);
+    epi_stats_accum<BLOCK_N, TILE>(stg, ybuf, etid, a, n0, m0, acc);
     acc.n0 = n0;
     epi_stats_flush<BLOCK_N>(red, etid, ew, a, acc);
   }
@@ -411,11 +466,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nstages = a.stages;
-  // [operand ring][epilogue staging tile][barriers (256 B)][statistics scratch]: the staging tile has its own space so
-  // that the producers can fill the ring for the next tile while the consumers drain this one
+  // [operand ring][epilogue staging tile][barriers (256 B)][statistics scratch][BN input tile (bnr_y only)]: the staging
+  // tile has its own space so that the producers can fill the ring for the next tile while the consumers drain this one
   const uint32_t stg = smem_u32(smem) + nstages * Cfg::kStageBytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + nstages * Cfg::kStageBytes + Cfg::kEpiBytes);
   uint64_t* empty = full + kMaxStages;
+  const uint32_t ybuf = smem_u32(full) + 256 + 8192;
 
   const int warp = threadIdx.x >> 5;
   const int KB = a.KB;
@@ -627,6 +683,24 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
     uint32_t phase = 0;
     for (int item = unit; item < items; item += units) {
       decode(item);
+      auto dest_row = [&](int row) -> int {     // output row of accumulator row `row`, or -1
+        if (kTile) {
+          const int wl = row % a.tw;
+          const int t2 = row / a.tw;
+          const int hl = t2 % a.th;
+          const int nl = t2 / a.th;
+          const bool ok = nl < a.tn && (tn0 + nl) < a.batch && (tp0 + hl) < a.dstH && (tq0 + wl) < a.dstW;
+          return ok ? ((tn0 + nl) * a.outH + (tp0 + hl) * a.out_stride + a.out_pa) * a.outW + (tq0 + wl) * a.out_stride +
+                          a.out_pb
+                    : -1;
+        }
+        return (m0 + row) < a.M ? (m0 + row) : -1;
+      };
+      if (STATS && a.bnr_y != nullptr) epi_bnr_prefetch<BLOCK_N>(ybuf, etid, a, n0, dest_row);
+      // the first wgmma of the tile overwrites acc (scale-d = 0), but only at run time: clearing it here tells the
+      // compiler that acc is dead between the drain and the next tile, which frees its 64 registers for the epilogue
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
       int prev = -1;
       for (int kb = 0; kb < KB; ++kb) {
         mbar_wait(&full[stage], phase, 18);
@@ -649,19 +723,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
       release(prev);
       // every consumer is past the previous tile's stores: the staging tile may be rewritten
       named_bar_sync(1, kEpiThreads);
-      auto dest_row = [&](int row) -> int {     // output row of accumulator row `row`, or -1
-        if (kTile) {
-          const int wl = row % a.tw;
-          const int t2 = row / a.tw;
-          const int hl = t2 % a.th;
-          const int nl = t2 / a.th;
-          const bool ok = nl < a.tn && (tn0 + nl) < a.batch && (tp0 + hl) < a.dstH && (tq0 + wl) < a.dstW;
-          return ok ? ((tn0 + nl) * a.outH + (tp0 + hl) * a.out_stride + a.out_pa) * a.outW + (tq0 + wl) * a.out_stride +
-                          a.out_pb
-                    : -1;
-        }
-        return (m0 + row) < a.M ? (m0 + row) : -1;
-      };
       // rows outside the image: exact zeros (keeps the BN sums clean)
       const bool z0 = kTile && dest_row(r0) < 0, z1 = kTile && dest_row(r0 + 8) < 0;
       const float deq = FP8 ? *a.deq_a * *a.deq_b : 1.0f;
@@ -670,7 +731,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
       // the row's destination index rides in the pad bytes of its staging row (pitch = 2*BLOCK_N + 16)
       if (kTile && etid < kBlockM) sts32(stg + etid * Cfg::kPitch + BLOCK_N * 2, static_cast<uint32_t>(dest_row(etid)));
       named_bar_sync(1, kEpiThreads);
-      epi_stats_store<BLOCK_N, STATS, kTile>(stg, smem_u32(full) + 256, etid, warp, a, n0, m0);
+      epi_stats_store<BLOCK_N, STATS, kTile>(stg, smem_u32(full) + 256, ybuf, etid, warp, a, n0, m0);
     }
   }
   if (CL) cluster_sync_all();          // no CTA leaves while its peer may still multicast into it or arrive on it
@@ -1054,8 +1115,7 @@ cudaError_t launch_fwd_t(const CUtensorMap& tmB, const CUtensorMap& tmBh, const 
   auto kern = conv_gemm_kernel<BLOCK_N, MODE, STATS, FP8, PERSIST, CL>;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::smem_bytes(Cfg::kMaxStagesN));
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemMax);
     if (e != cudaSuccess) return e;
     if (CL) {
       e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
@@ -1072,7 +1132,8 @@ cudaError_t launch_fwd_t(const CUtensorMap& tmB, const CUtensorMap& tmBh, const 
   }
   const long long grid = units * (CL ? 2 : 1);
   if (grid > 0x7fffffffLL) return cudaErrorInvalidValue;
-  return launch_pdl(kern, dim3(static_cast<unsigned>(grid)), dim3(kThreads), Cfg::smem_bytes(a.stages), stream,
+  return launch_pdl(kern, dim3(static_cast<unsigned>(grid)), dim3(kThreads),
+                    Cfg::smem_bytes(a.stages, STATS && a.bnr_y != nullptr), stream,
                     CL ? 2 : 1, tmB, tmBh, tmA, a, n_tiles, m_tiles);
 }
 
@@ -1094,8 +1155,8 @@ int g_deep = 1;             // tuning hook: 0 = never, 1 = policy, 2 = persisten
                             //   kernel of tensor-memory GPUs; tiles are at most 128 wide on sm_90)
 
 template <int BLOCK_N, int MODE>
-int pick_stages(int KB) {
-  const int max_s = FwdCfg<BLOCK_N>::kMaxStagesN;
+int pick_stages(int KB, bool bnr) {
+  const int max_s = bnr ? FwdCfg<BLOCK_N>::kMaxStagesBnr : FwdCfg<BLOCK_N>::kMaxStagesN;
   int s = g_force_stages > 0 ? g_force_stages : max_s;
   if (s > max_s) s = max_s;
   if (s > KB) s = KB;
@@ -1114,7 +1175,7 @@ constexpr bool mode_persist() {
 template <int BLOCK_N, int MODE>
 cudaError_t launch_bn(const CUtensorMap& tmB, const CUtensorMap& tmBh, const TmaSet& tmA, ConvArgs a, int n_total,
                       int m_tiles, bool stats, bool persistent, bool pair, cudaStream_t stream) {
-  a.stages = pick_stages<BLOCK_N, MODE>(a.KB);
+  a.stages = pick_stages<BLOCK_N, MODE>(a.KB, stats && a.bnr_y != nullptr);
 #define DDL_FWD(FP8, PER, CLU)                                                                                    \
   return stats ? launch_fwd_t<BLOCK_N, MODE, true, FP8, PER, CLU>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)   \
                : launch_fwd_t<BLOCK_N, MODE, false, FP8, PER, CLU>(tmB, tmBh, tmA, a, n_total, m_tiles, stream)

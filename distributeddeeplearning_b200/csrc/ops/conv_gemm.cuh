@@ -39,7 +39,10 @@ struct ConvArgs {
   //   sum[c] += S1 = sum_m dm,   sumsq[c] += invstd[c] * (S2 - mean[c] * S1),  S2 = sum_m dm * y[m][c]
   // where dm = out[m][c] * [gamma*invstd*(y - mean) + beta > 0] — i.e. dbeta and dgamma of that BN (ReLU mask
   // recomputed from its saved input y), so the separate reduce pass over (d, y) is not needed.
+  // With `bnr_mask` the ReLU mask comes from that BN's forward bit mask instead (a residual layer: its output includes
+  // the shortcut); with `add` (linear rows only) the sums are taken over the stored value acc + gated add.
   const __nv_bfloat16* bnr_y;
+  const uint8_t* bnr_mask;
   const float* bnr_gamma;
   const float* bnr_beta;
   const float* bnr_mean;

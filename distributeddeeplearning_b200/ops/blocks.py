@@ -12,13 +12,13 @@ produced exactly once.  It also trims Python/autograd overhead (1 node instead o
     backward  (dy_L, dres) = bn_bwd(dout; mask from out)      d_{L-1} = dgrad_L(dy_L)      wgrad_L
               dy_i = bn_bwd(d_i; mask recomputed from y_i)    d_{i-1} = dgrad_i(dy_i)      wgrad_i
               dx = dgrad_1(dy_1) + (dres | dgrad_d(bn_bwd(dres)))          <- the '+' is the dgrad epilogue
+    where dgrad_1 is a 1x1 conv, its epilogue also takes the previous block's bn_L sums over dx (``_Bn3Handoff``)
 
 Reference parity: the maths is exactly torchvision's BasicBlock/Bottleneck (SURVEY.md 2.7); this only changes how
 the backward is scheduled.
 """
 from __future__ import annotations
 
-import os
 from typing import Sequence
 
 import torch
@@ -27,10 +27,27 @@ from . import native
 from .functional import CL, grad_buffer, notify_ready, run_wgrad, weight_bf16
 
 
-# Folding the BN-backward reduction into the producing dgrad's epilogue removes 32 launches and one read of each inner
-# gradient tensor but makes those (already epilogue-bound) dgrads slower.  Off unless DDL_FUSE_BN_REDUCE=1 (not
-# re-measured on H100).
-FUSE_BN_REDUCE = os.environ.get("DDL_FUSE_BN_REDUCE", "0") != "0"
+class _Bn3Handoff:
+    """Lets the next block's first dgrad take the block-output BN's dbeta / dgamma sums.
+
+    The block's forward fills in what that BN's backward reduction reads (its input y, saved mean / invstd, gamma,
+    beta and the output's ReLU bit mask).  The next block's backward computes the gradient of that output with a 1x1
+    dgrad that also accumulates the sums (``conv_dgrad(..., bn_reduce=...)``) and records the tensor it returned.  This
+    block's backward uses the sums only if the gradient it receives is that very tensor, unmodified: had autograd added
+    another consumer's gradient, the sums would not describe it, and the stand-alone reduction runs instead."""
+
+    def __init__(self):
+        self.bn = None          # (y, save, gamma, beta, zmask) of the block-output BN
+        self.sums = None        # fp32 [2, C] scratch in bn_act_bwd layout
+        self.dx = None
+        self.version = -1
+
+    def pre_reduced(self, dout):
+        d, sums = self.dx, self.sums
+        self.bn = self.sums = self.dx = None
+        if d is None or dout.data_ptr() != d.data_ptr() or dout.shape != d.shape or dout._version != self.version:
+            return None
+        return sums
 
 
 class _ResidualBlock(torch.autograd.Function):
@@ -59,6 +76,7 @@ class _ResidualBlock(torch.autograd.Function):
             last = i == n_main - 1
             if last:      # residual layer: backward masks with 1 bit per element instead of re-reading the block output
                 z, save, zmask = native.bn_act_fwd(y, stats, g, b, rm, rv, eps, mom, True, identity, True, want_mask=True)
+                cfg["bn3_out"].bn = (y, save, g, b, zmask)
             else:
                 z, save = native.bn_act_fwd(y, stats, g, b, rm, rv, eps, mom, True, None, True)
             saved += [h, y, save]
@@ -84,7 +102,7 @@ class _ResidualBlock(torch.autograd.Function):
         dres = None
         dx = None
         gated_add = None
-        pre = None
+        pre = cfg["bn3_out"].pre_reduced(dout)          # block-output BN sums taken by the next block's dgrad, if any
         for i in range(n_main - 1, -1, -1):
             w, g, b, _, _ = layers[i]
             st, pad, dil, _, _ = cfg["layers"][i]
@@ -107,13 +125,15 @@ class _ResidualBlock(torch.autograd.Function):
                 dres = dr
             pre = None
             if i > 0:
-                # the dgrad that produces d_{i-1} also reduces dbeta / dgamma of BN_{i-1} in its epilogue (it holds the
-                # gradient tile anyway and only has to read the y tile): BN_{i-1}'s backward is then one pass, not two
+                # where it pays (1x1 dgrads), the dgrad that produces d_{i-1} also reduces dbeta / dgamma of BN_{i-1}
+                # in its epilogue (it holds the gradient tile anyway and only has to read the y tile, which it fetches
+                # while its MMAs run): BN_{i-1}'s backward is then one pass over (d_{i-1}, y) instead of two
                 gp, bp = layers[i - 1][1], layers[i - 1][2]
-                pre = native.zeros_f32((2, h_in.shape[1]), h_in.device) if FUSE_BN_REDUCE else None
+                fuse = native.dgrad_fuses_bn_reduce(kernel, st, pad)
+                pre = native.zeros_f32((2, h_in.shape[1]), h_in.device) if fuse else None
                 d = native.conv_dgrad(dy, ctx.wbs[i], h_in.shape, kernel, st, pad, dil,
                                       bn_reduce=(saved[3 * (i - 1) + 1], gp, bp, saved[3 * (i - 1) + 2], pre)
-                                      if pre is not None else None)
+                                      if fuse else None)
             elif need_dx:
                 add = dres
                 if has_ds:
@@ -131,13 +151,23 @@ class _ResidualBlock(torch.autograd.Function):
                     for p in (gd, bd, wd):
                         if p.requires_grad:
                             notify_ready(p)
+                # x is the previous block's output: where this dgrad can, it also takes that block's BN3 sums
+                prev = cfg["bn3_in"]
+                bnr = None
+                if prev is not None and prev.bn is not None and native.dgrad_fuses_bn_reduce(kernel, st, pad):
+                    py, psave, pg, pb, pmask = prev.bn
+                    prev.sums = native.zeros_f32((2, x.shape[1]), x.device)
+                    bnr = (py, pg, pb, psave, prev.sums, pmask)
                 if gated_add is not None:
                     dx = native.conv_dgrad(dy, ctx.wbs[0], x.shape, kernel, st, pad, dil, add=gated_add[0],
-                                           add_mask=gated_add[1])
+                                           add_mask=gated_add[1], bn_reduce=bnr)
                 elif native.dgrad_supports_add(kernel, st):
-                    dx = native.conv_dgrad(dy, ctx.wbs[0], x.shape, kernel, st, pad, dil, add=add)
+                    dx = native.conv_dgrad(dy, ctx.wbs[0], x.shape, kernel, st, pad, dil, add=add, bn_reduce=bnr)
                 else:
+                    bnr = None
                     dx = native.add(native.conv_dgrad(dy, ctx.wbs[0], x.shape, kernel, st, pad, dil), add)
+                if bnr is not None:
+                    prev.dx, prev.version = dx, dx._version
             if w.requires_grad:
                 gw = grad_buffer(w)
                 run_wgrad(w, lambda h_in=h_in, dy=dy, gw=gw, kernel=kernel, st=st, pad=pad, dil=dil:
@@ -179,9 +209,14 @@ def residual_block(x: torch.Tensor, convs: Sequence, bns: Sequence, downsample=N
     """convs/bns: the main-path layer containers (``models.layers.Conv2d`` / ``BatchNorm2d``) in order;
     downsample: optional (conv, bn) pair of the projection shortcut."""
     mods = list(zip(convs, bns)) + ([tuple(downsample)] if downsample is not None else [])
+    # a block output carries its BN3 handoff; the first block to consume it takes it (a second consumer finds none)
+    prev = x.__dict__.pop("_ddl_bn3", None)
     cfg = {"n_main": len(convs), "has_ds": downsample is not None,
-           "layers": [(c.stride, c.padding, c.dilation, b.eps, b.momentum) for c, b in mods]}
+           "layers": [(c.stride, c.padding, c.dilation, b.eps, b.momentum) for c, b in mods],
+           "bn3_in": prev, "bn3_out": _Bn3Handoff()}
     params = []
     for c, b in mods:
         params += [c.weight, b.weight, b.bias, b.running_mean, b.running_var]
-    return _ResidualBlock.apply(x, cfg, *params)
+    out = _ResidualBlock.apply(x, cfg, *params)
+    out._ddl_bn3 = cfg["bn3_out"]
+    return out

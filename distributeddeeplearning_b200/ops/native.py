@@ -446,9 +446,11 @@ def conv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, kernel: Tuple[in
     """dx = conv_transpose(dy, w) (+ add [gated by the bit mask ``add_mask``: uint8 [M, Cin/8]]).
     ``w_bf16`` is the forward matrix [Cout, R*S*Cin].
 
-    ``bn_reduce = (y, gamma, beta, save, scratch)``: dx is the output gradient of a BN+ReLU layer whose saved input is
-    ``y``; the kernel's epilogue then also accumulates that BN's dbeta / dgamma sums into ``scratch`` (fp32 [2, Cin],
-    zeroed), so ``bn_act_bwd(..., pre_reduced=scratch)`` can skip its reduction pass over (dx, y)."""
+    ``bn_reduce = (y, gamma, beta, save, scratch[, zmask])``: dx is the output gradient of a BN+ReLU layer whose saved
+    input is ``y``; the kernel's epilogue then also accumulates that BN's dbeta / dgamma sums into ``scratch`` (fp32
+    [2, Cin], zeroed), so ``bn_act_bwd(..., pre_reduced=scratch)`` can skip its reduction pass over (dx, y).  The ReLU
+    mask is recomputed from ``y``, or, with ``zmask`` (the layer's forward bit mask, for a residual layer), read from it.
+    With ``add`` (1x1 stride-1 only) the sums are over the stored value, the product plus the gated ``add``."""
     C = _C()
     _check_act(dy, "dy")
     N, Cin, H, W = x_shape
@@ -479,19 +481,22 @@ def conv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, kernel: Tuple[in
     wp, wr, wc = w_bf16.data_ptr(), w_bf16.shape[0], w_bf16.shape[1]
     bnr = {}
     s1 = s2 = 0
+    one_by_one = R == 1 and S == 1 and stride == 1 and ph == 0 and pw == 0
     if bn_reduce is not None:
-        by, bgam, bbeta, bsave, bscr = bn_reduce
-        if add is not None:
-            raise ValueError("bn_reduce cannot be combined with add (the sums are taken before the epilogue add)")
+        by, bgam, bbeta, bsave, bscr = bn_reduce[:5]
+        bmask = bn_reduce[5] if len(bn_reduce) > 5 else None
+        if (add is not None or bmask is not None) and not one_by_one:
+            raise ValueError("bn_reduce with add or a bit mask needs a 1x1 stride-1 data gradient (linear rows)")
         if tuple(by.shape) != (N, Cin, H, W) or bscr.shape != (2, Cin):
             raise ValueError("bn_reduce: y / scratch do not match dx")
+        if bmask is not None and (bmask.dtype != torch.uint8 or bmask.numel() != N * H * W * (Cin // 8)):
+            raise ValueError("bn_reduce: expected a uint8 [N*H*W, Cin/8] bit mask")
         _check_act(by, "bn_reduce.y")
         bnr = dict(bnr_y=by.data_ptr(), bnr_gamma=bgam.data_ptr(), bnr_beta=bbeta.data_ptr(),
-                   bnr_mean=bsave[0].data_ptr(), bnr_invstd=bsave[1].data_ptr())
+                   bnr_mean=bsave[0].data_ptr(), bnr_invstd=bsave[1].data_ptr(), bnr_mask=_ptr(bmask))
         s1, s2 = bscr[1].data_ptr(), bscr[0].data_ptr()      # scratch layout of bn_act_bwd: [0] = dgamma, [1] = dbeta
     from . import fp8 as _fp8
 
-    one_by_one = R == 1 and S == 1 and stride == 1 and ph == 0 and pw == 0
     if _fp8.dgrad_eligible(Cin, Cout, R * S if stride == 1 else max(1, (R * S) // 4)) and bn_reduce is None \
             and N * H * W >= 2048 and \
             (one_by_one or (stride == 1 and USE_TILE_TMA) or s2_tile):
@@ -533,7 +538,8 @@ def conv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, kernel: Tuple[in
                                          **fp8kw))
         return dx
     if R == 1 and S == 1 and stride == 1 and ph == 0 and pw == 0:
-        _tuned(("dgrad1x1", N, H, W, Cin, Cout, add is not None, add_mask is not None, bn_reduce is not None),
+        _tuned(("dgrad1x1", N, H, W, Cin, Cout, add is not None, add_mask is not None,
+                0 if bn_reduce is None else len(bn_reduce)),
                conv_variants(n_total, N * H * W, cch, True),
                lambda v: C.conv_gemm(C.CONV_GEMM_DGRAD, 0, dx.data_ptr(), _ptr(add), 0, s1, s2, N * H * W, cch, Cin, P, Q,
                                      Cout, H, W, 1, 1, 1, 0, 1, cch, 0, Cin, wp, wr, wc, n_total, dy.data_ptr(), Cout, N,
@@ -738,8 +744,8 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
     dres = torch.empty_like(y) if want_dres else None
     scratch = pre_reduced if pre_reduced is not None else zeros_f32((2, Ch), y.device)
     mask_from_x = bool(relu and beta is not None and not had_residual)     # z is not read at all in that case
-    if pre_reduced is not None and not mask_from_x:
-        raise ValueError("pre_reduced sums are only defined for BN+ReLU layers without residual")
+    if pre_reduced is not None and not (mask_from_x or (relu and zmask is not None)):
+        raise ValueError("pre_reduced sums are only defined for BN+ReLU layers (mask from y or from the bit mask)")
     if relu and not mask_from_x and zmask is None and z is None:
         raise ValueError("bn_act_bwd: need z or zmask for the ReLU mask of a residual layer")
     from . import fp8 as _fp8
@@ -971,6 +977,14 @@ def dgrad_supports_add(kernel: Tuple[int, int], stride: int) -> bool:
     """Whether conv_dgrad can fold ``+ add`` into its epilogue for this geometry without leaving the fast path
     (the stride-2 phase decomposition writes each output phase from a different launch, so it cannot)."""
     return not (stride == 2 and USE_TILE_TMA and USE_TILE_S2 and kernel[0] * kernel[1] <= 16)
+
+
+def dgrad_fuses_bn_reduce(kernel: Tuple[int, int], stride: int, pad) -> bool:
+    """Whether ``conv_dgrad(..., bn_reduce=...)`` costs less than the plain dgrad plus the stand-alone BN-backward
+    reduction pass.  Measured on H100 at the ResNet-50 shapes: yes for 1x1 stride-1 data gradients (bandwidth-bound
+    GEMMs; the y tile is fetched under the MMAs), no for window convolutions, where the statistics epilogue of their many
+    short tiles costs more than the reduction pass it replaces."""
+    return tuple(kernel) == (1, 1) and stride == 1 and _pad2(pad) == (0, 0)
 
 
 # ------------------------------------------------------------------------------------------------

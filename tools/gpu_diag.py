@@ -447,8 +447,12 @@ def g_conv_dgrad():
     dx = nv.conv_dgrad(dy, _w_bf16(w), x.shape, (3, 3), 1, 1, add=add)
     report("conv_dgrad + add", dx, x.grad + add.float(), 2e-2)
     # BN-backward reduction fused into the dgrad epilogue: dbeta / dgamma sums equal the stand-alone reduce kernel's
+    # (1x1 linear rows, 3x3 stride-1 tiles, 3x3 stride-2 phase tiles on even and odd images, 1x1 stride 2 with
+    # zero-filled siblings, the gather kernel for a 5x5 stride-2 window, odd M tails, 64-wide channel tiles)
     for (n, ci, h, co, k, s_, p_) in [(2, 64, 12, 128, 3, 1, 1), (3, 128, 9, 256, 1, 1, 0), (2, 64, 16, 64, 3, 2, 1),
-                                      (2, 96, 10, 160, 1, 1, 0), (4, 256, 14, 64, 1, 1, 0)]:
+                                      (2, 96, 10, 160, 1, 1, 0), (4, 256, 14, 64, 1, 1, 0), (3, 64, 7, 64, 1, 1, 0),
+                                      (2, 128, 14, 256, 1, 2, 0), (2, 64, 13, 128, 3, 2, 1), (2, 64, 12, 64, 5, 2, 2),
+                                      (3, 128, 7, 128, 3, 1, 1)]:
         xs = (n, ci, h, h)
         w_ = bf(torch.randn(co, ci, k, k, device=dev) * (1.0 / (co * k * k) ** 0.5))
         ho = (h + 2 * p_ - k) // s_ + 1
@@ -467,6 +471,35 @@ def g_conv_dgrad():
         dy_b, _, _ = nv.bn_act_bwd(d_plain, zdummy, ybn, save, gam, True, False, None, None, beta=bet, had_residual=False,
                                    pre_reduced=pre)
         report("   bn apply from fused sums", dy_b, dy_a, 2e-3)
+    # the same with the shortcut add (gated or not) and the ReLU mask of a residual BN taken from its bit mask: the sums
+    # are over the stored value acc + add
+    def bitmask(pos):
+        b8 = cl(pos.to(torch.uint8)).permute(0, 2, 3, 1).reshape(-1, pos.shape[1] // 8, 8)
+        return (b8.to(torch.int32) << torch.arange(8, device=dev, dtype=torch.int32)).sum(-1).to(torch.uint8).contiguous()
+
+    for (n, ci, h, co, gated) in [(3, 256, 7, 64, True), (2, 512, 10, 128, False), (2, 128, 9, 64, True)]:
+        xs = (n, ci, h, h)
+        w_ = bf(torch.randn(co, ci, 1, 1, device=dev) * (1.0 / co ** 0.5))
+        dyv = cl(bf(torch.randn(n, co, h, h, device=dev)))
+        addv = cl(bf(torch.randn(*xs, device=dev)))
+        amask = bitmask(torch.rand(*xs, device=dev) > 0.4) if gated else None
+        ybn = cl(bf(torch.randn(*xs, device=dev) * 1.5 + 0.3))
+        zmask_ = bitmask(torch.rand(*xs, device=dev) > 0.5)
+        gam, bet = torch.rand(ci, device=dev) + 0.5, torch.randn(ci, device=dev) * 0.3
+        save = torch.stack([ybn.float().mean((0, 2, 3)), 1.0 / (ybn.float().var((0, 2, 3), unbiased=False) + 1e-5).sqrt()]).contiguous()
+        pre = torch.zeros(2, ci, device=dev)
+        d_fused = nv.conv_dgrad(dyv, _w_bf16(w_), xs, (1, 1), 1, 0, add=addv, add_mask=amask,
+                                bn_reduce=(ybn, gam, bet, save, pre, zmask_))
+        d_plain = nv.conv_dgrad(dyv, _w_bf16(w_), xs, (1, 1), 1, 0, add=addv, add_mask=amask)
+        report(f"dgrad+add{'+mask' if gated else ''}+bn-reduce(bits) c{ci}<-{co}: dx unchanged", d_fused, d_plain, 1e-6)
+        dy_a, dr_a, scr = nv.bn_act_bwd(d_plain, None, ybn, save, gam, True, True, None, None, beta=bet, had_residual=True,
+                                        zmask=zmask_)
+        report("   dgamma", pre[0], scr[0], 2e-3, atol=2e-3)
+        report("   dbeta", pre[1], scr[1], 2e-3, atol=2e-3)
+        dy_b, dr_b, _ = nv.bn_act_bwd(d_plain, None, ybn, save, gam, True, True, None, None, beta=bet, had_residual=True,
+                                      zmask=zmask_, pre_reduced=pre)
+        report("   bn apply from fused sums", dy_b, dy_a, 2e-3)
+        report("   dres from fused sums", dr_b, dr_a, 1e-6)
     # epilogue add gated by a ReLU bit mask (shortcut gradient of an identity residual block)
     zpos = torch.rand(2, 64, 8, 8, device=dev) > 0.5
     bits = cl(zpos.to(torch.uint8)).permute(0, 2, 3, 1).reshape(-1, 8, 8)       # [M, C/8, 8]
