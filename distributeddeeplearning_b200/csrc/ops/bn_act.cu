@@ -297,11 +297,14 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_apply_kernel(BnBwdAr
     Vec8 mean = load8_f32(a.mean + c0), invstd = load8_f32(a.invstd + c0), gam = load8_f32(a.gamma + c0);
     Vec8 db = load8_f32(a.dbeta + c0), dg = load8_f32(a.dgamma + c0);
     const float inv_n = 1.f / static_cast<float>(a.M);
-    if (row0 == 0 && a.gamma_grad) {   // exactly one thread per channel group: accumulate parameter grads
+    if (row0 == 0) {   // exactly one thread per channel group: accumulate parameter grads (each one only if it trains)
+      if (a.gamma_grad) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        a.gamma_grad[c0 + i] += dg.v[i];
-        a.beta_grad[c0 + i] += db.v[i];
+        for (int i = 0; i < 8; ++i) a.gamma_grad[c0 + i] += dg.v[i];
+      }
+      if (a.beta_grad) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) a.beta_grad[c0 + i] += db.v[i];
       }
     }
 #pragma unroll
@@ -526,11 +529,14 @@ bn_pool_bwd_apply_kernel(BnBwdArgs a, PoolArgs p, const __nv_bfloat16* __restric
     Vec8 mean = load8_f32(a.mean + c0), invstd = load8_f32(a.invstd + c0), gam = load8_f32(a.gamma + c0);
     Vec8 db = load8_f32(a.dbeta + c0), dg = load8_f32(a.dgamma + c0), bet = load8_f32(a.beta + c0);
     const float inv_n = 1.f / static_cast<float>(a.M);
-    if (row0 == 0 && a.gamma_grad) {
+    if (row0 == 0) {
+      if (a.gamma_grad) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        a.gamma_grad[c0 + i] += dg.v[i];
-        a.beta_grad[c0 + i] += db.v[i];
+        for (int i = 0; i < 8; ++i) a.gamma_grad[c0 + i] += dg.v[i];
+      }
+      if (a.beta_grad) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) a.beta_grad[c0 + i] += db.v[i];
       }
     }
 #pragma unroll

@@ -175,15 +175,19 @@ class _ResidualBlock(torch.autograd.Function):
             for p in (g, b, w):
                 if p.requires_grad:
                     notify_ready(p)
-        if not need_dx and has_ds:
-            # block input needs no gradient but the downsample parameters still do
+        if not need_dx and has_ds and any(p.requires_grad for p in layers[n_main][:3]):
+            # block input needs no gradient but (some of) the downsample parameters still do
             wd, gd, bd, _, _ = layers[n_main]
             std, padd, dild, _, _ = cfg["layers"][n_main]
             yd, save_d, wbd = ctx.ds_pack
-            dyd, _, _ = native.bn_act_bwd(dres, yd, yd, save_d, gd, False, False, grad_buffer(gd), grad_buffer(bd))
-            native.conv_wgrad(x, dyd, grad_buffer(wd), (wd.shape[2], wd.shape[3]), std, padd, dild)
+            dyd, _, _ = native.bn_act_bwd(dres, yd, yd, save_d, gd, False, False,
+                                          grad_buffer(gd) if gd.requires_grad else None,
+                                          grad_buffer(bd) if bd.requires_grad else None)
+            if wd.requires_grad:
+                native.conv_wgrad(x, dyd, grad_buffer(wd), (wd.shape[2], wd.shape[3]), std, padd, dild)
             for p in (gd, bd, wd):
-                notify_ready(p)
+                if p.requires_grad:
+                    notify_ready(p)
         return (dx, None) + (None,) * (5 * len(layers))
 
 

@@ -196,11 +196,9 @@ class _ConvBnAct(torch.autograd.Function):
                       *((xp,) if xp is not None else ()))
         # LAST: a ready bucket may launch its allreduce+update kernel on the side stream now; everything
         # this layer still needed from the weight arenas (gamma, wb) has been enqueued before the event
-        if gamma.requires_grad:
-            notify_ready(gamma)
-            notify_ready(beta)
-        if weight.requires_grad:
-            notify_ready(weight)
+        for p in (gamma, beta, weight):
+            if p.requires_grad:
+                notify_ready(p)
         return (dx, dres) + (None,) * 12
 
 
@@ -251,11 +249,9 @@ class _ConvBnActPool(torch.autograd.Function):
         if weight.requires_grad:
             gw = grad_buffer(weight)
             run_wgrad(weight, lambda: native.conv_wgrad(x, dy, gw, kernel, stride, pad, dil), x, dy)
-        if gamma.requires_grad:
-            notify_ready(gamma)
-            notify_ready(beta)
-        if weight.requires_grad:
-            notify_ready(weight)
+        for p in (gamma, beta, weight):
+            if p.requires_grad:
+                notify_ready(p)
         return (dx,) + (None,) * 13
 
 
@@ -299,9 +295,9 @@ class _BnAct(torch.autograd.Function):
         gg = grad_buffer(gamma) if gamma.requires_grad else None
         bg = grad_buffer(beta) if beta.requires_grad else None
         dx, _, _ = native.bn_act_bwd(dz, z, x, save, gamma, ctx.relu, False, gg, bg, beta=beta, had_residual=False)
-        if gamma.requires_grad:
-            notify_ready(gamma)
-            notify_ready(beta)
+        for p in (gamma, beta):
+            if p.requires_grad:
+                notify_ready(p)
         return (dx if ctx.needs_input_grad[0] else None,) + (None,) * 8
 
 

@@ -23,7 +23,7 @@ def _group(name, timeout=600, env=None):
     assert "FAIL" not in r.stdout, tail
 
 
-@pytest.mark.parametrize("group", ["elementwise", "gemm", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "zoo", "zoograd", "conv_generic", "graph", "fp8", "benchshape"])
+@pytest.mark.parametrize("group", ["elementwise", "gemm", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "zoo", "zoograd", "conv_generic", "graph", "fp8", "benchshape", "block"])
 def test_kernel_group(group):
     """Default configuration: the per-shape autotuner picks among the kernel variants (a variant that dead-locks on a
     shape makes the group fail: gpu_diag reports the tuner's rejections and any pipeline timeout).  `benchshape` runs
@@ -38,7 +38,7 @@ def test_deep_ring_kernel_forced(mode):
     (clusters sharing the weight tile by TMA multicast) wherever possible, 3 / 4 = single CTAs.  On sm_90 tiles are at
     most 128 wide, so 3 and 4 select the same kernel (and the one test_persistent_kernel_forced runs); every value of the
     hook stays covered because every value is accepted and has to keep working."""
-    for group in ("gemm", "conv_fwd", "conv_dgrad", "conv_generic"):
+    for group in ("gemm", "conv_fwd", "conv_dgrad", "conv_generic", "block"):
         _group(group, timeout=300, env={"DDL_CONV_DEEP": mode, "DDL_CONV_AUTOTUNE": "0"})
 
 
@@ -46,7 +46,7 @@ def test_persistent_kernel_forced():
     """The persistent kernel (one CTA per SM walking tiles; the producers fill the ring for the next tile while the
     consumers drain this one) forced onto every TMA-fed shape — the autotuner offers it only for layers with at least a
     wave of tiles, which the small test shapes never reach."""
-    for group in ("gemm", "conv_fwd", "conv_dgrad", "conv_generic"):
+    for group in ("gemm", "conv_fwd", "conv_dgrad", "conv_generic", "block"):
         _group(group, timeout=300, env={"DDL_CONV_PERSISTENT": "2", "DDL_CONV_DEEP": "0", "DDL_CONV_AUTOTUNE": "0"})
 
 
@@ -55,7 +55,7 @@ def test_cluster_pair_kernels(mode):
     """Thread-block-cluster variant of the persistent conv kernel (CTA pairs that TMA-multicast the weight tile), forced
     onto every TMA-fed shape with either hook value: sm_90 has no pair MMA, so 1 and 2 select the same kernel, and both
     stay covered because both values are accepted and have to keep working."""
-    for group in ("gemm", "conv_dgrad"):
+    for group in ("gemm", "conv_dgrad", "block"):
         _group(group, timeout=300, env={"DDL_CONV_CLUSTER": mode, "DDL_CONV_PERSISTENT": "2"})
 
 

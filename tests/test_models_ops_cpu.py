@@ -163,3 +163,29 @@ def test_batch_norm_act_composite_matches_torch():
     z = ops.batch_norm_act(x, g, b, rm, rv, 1e-5, 0.1, True, True)
     ref = torch.relu(torch.nn.functional.batch_norm(x, torch.zeros(8), torch.ones(8), g, b, True, 0.1, 1e-5))
     assert torch.allclose(z, ref, atol=1e-5)
+
+
+def test_bn3_handoff_hands_sums_only_to_the_unmodified_gradient():
+    """A block takes the BN3 sums of the next block's dgrad only for the very tensor that dgrad returned, unmodified,
+    and only once."""
+    from distributeddeeplearning_b200.ops.blocks import _Bn3Handoff
+
+    d = torch.randn(2, 16, 3, 3).contiguous(memory_format=torch.channels_last)
+
+    def armed():
+        h = _Bn3Handoff()
+        h.bn, h.sums, h.dx, h.version = ("y", "save", "gamma", "beta", "mask"), torch.randn(2, 16), d, d._version
+        return h
+
+    h = armed()
+    sums = h.sums
+    assert h.pre_reduced(d) is sums
+    assert h.bn is None and h.sums is None and h.dx is None       # cleared: the next call finds nothing
+    assert h.pre_reduced(d) is None
+    assert armed().pre_reduced(d.clone()) is None                   # same values, different storage
+    assert armed().pre_reduced(d[:1]) is None                       # same storage start, different shape
+    h = armed()
+    d.mul_(2.0)                                                     # modified in place: the version moved on
+    assert h.pre_reduced(d) is None
+    assert armed().pre_reduced(d) is not None                       # re-armed at the current version
+    assert _Bn3Handoff().pre_reduced(d) is None                     # never armed

@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 
 
@@ -46,21 +46,32 @@ def bf(t):
     return t.to(torch.bfloat16)
 
 
-def report_abs(name, got, ref, rtol, atol):
-    """allclose-style check: |got - ref| <= atol + rtol * |ref| ELEMENT-WISE (small-magnitude errors are not hidden
-    behind max|ref| the way `report` normalises)."""
+def _bound_ratio(got, ref, rtol, atol, arms):
+    """(violations, worst err / bound, finite) of |got - ref| <= atol + arms * rms(ref) + rtol * |ref|."""
     import torch
 
-    got, ref = got.float(), ref.float()
+    got, ref = got.double(), ref.double()
     err = (got - ref).abs()
-    bound = atol + rtol * ref.abs()
-    bad = int((err > bound).sum().item())
-    worst = float((err / bound).max().item())
-    ok = bad == 0 and bool(torch.isfinite(got).all().item())
-    print(f"[{'ok' if ok else 'FAIL'}] {name:58s} violations={bad}/{err.numel()} worst={worst:.3f}x of (atol {atol:g} + rtol {rtol:g}*|ref|)",
+    bound = atol + arms * ref.pow(2).mean().sqrt() + rtol * ref.abs()
+    bound = torch.where(bound > 0, bound, torch.full_like(bound, 1e-300))
+    return int((err > bound).sum().item()), float((err / bound).max().item()), bool(torch.isfinite(got).all().item())
+
+
+def report_abs(name, got, ref, rtol, atol, arms=0.0, also=None):
+    """allclose-style check: |got - ref| <= atol + arms * rms(ref) + rtol * |ref| ELEMENT-WISE (small-magnitude errors
+    are not hidden behind max|ref| the way `report` normalises).  ``also = (got2, ref2)``: a second implementation of
+    the same tensor (not checked) whose worst ratio to the same bound is printed alongside.  Returns the worst ratio."""
+    bad, worst, finite = _bound_ratio(got, ref, rtol, atol, arms)
+    ok = bad == 0 and finite
+    desc = f"atol {atol:g} + " if atol else ""
+    desc += f"{arms:g}*rms(ref) + " if arms else ""
+    other = ""
+    if also is not None:
+        other = f" (bf16 composite {_bound_ratio(also[0], also[1], rtol, atol, arms)[1]:.3f}x)"
+    print(f"[{'ok' if ok else 'FAIL'}] {name:58s} violations={bad}/{got.numel()} worst={worst:.3f}x{other} of ({desc}rtol {rtol:g}*|ref|)",
           flush=True)
     RESULTS.append(ok)
-    return ok
+    return worst
 
 
 def g_fp8():
@@ -675,6 +686,470 @@ def g_bn():
         dy2, dres2, _ = nv.bn_act_bwd(dz, None, y, save2, gamma, True, True, g2, b2, zmask=zmask)
         report_abs(f"  bitmask C={c} dy", dy2, dy, 2.0 ** -7, 1e-6)      # one bf16 ulp: see the atomics note above
         report(f"  bitmask C={c} dres", dres2, dres, 1e-6)
+
+
+# ---- whole residual blocks (ops/blocks.py) against a float64 torch.nn twin ---------------------------------------------
+# Element-wise budgets |got - ref| <= a * rms(ref) + r * |ref| per tensor kind, (a, r).  The native block stores every
+# activation and activation gradient in bf16 (relative rounding <= 2^-9 per store) and multiplies bf16 weights; the
+# float64 twin rounds nothing.  r is one or two bf16 roundings of the tensor itself.  a covers what the stores upstream
+# of it leave behind: a conv output y stored in bf16 before its BN carries 2^-9 * |y|, i.e. up to 2^-9 * 4 sigma * gamma
+# / sigma after normalisation, and three such layers forward plus three backward put the largest of 10^4..10^7 output
+# elements at a few % of rms; batch reductions (weight gradients of 1x1 convs in particular) collect that tail over many
+# rows.  The values of a are set with about 2x margin over the worst ratio the repo's bf16 composite (same storage
+# points, stock cuDNN kernels) reaches on these cases, which the group prints next to native's.
+# A ReLU whose float64 input lies within that forward error of zero may switch either way, and one switched element moves
+# a whole gradient element into or out of a BN backward over a few hundred rows: so wherever |relu input| <= BLOCK_TIE *
+# rms, the twin takes the side the tested implementation took (its output / saved activations), and checks the ReLU
+# decision everywhere else.
+BLOCK_BUDGET = {"out": (2.0 ** -3, 2.0 ** -8), "running_mean": (2.0 ** -8, 2.0 ** -8),
+                "running_var": (2.0 ** -10, 2.0 ** -8), "dx": (2.0 ** -4, 2.0 ** -7), "conv weight grad": (2.0 ** -2, 2.0 ** -7),
+                "gamma grad": (2.0 ** -4, 2.0 ** -7), "beta grad": (2.0 ** -4, 2.0 ** -7)}
+BLOCK_TIE = 2.0 ** -3          # |relu input| <= BLOCK_TIE * rms: the twin takes the tested implementation's side
+BLOCK_WORST = {}               # tensor kind -> [worst native ratio, worst composite ratio]
+
+
+def _bn_twin(b):
+    import torch
+
+    t = torch.nn.BatchNorm2d(b.num_features, eps=b.eps, momentum=b.momentum)
+    with torch.no_grad():
+        for n in ("weight", "bias"):
+            getattr(t, n).copy_(getattr(b, n))
+            getattr(t, n).requires_grad_(getattr(b, n).requires_grad)
+        t.running_mean.copy_(b.running_mean)
+        t.running_var.copy_(b.running_var)
+    return t.to(device=b.weight.device, dtype=torch.float64).train()
+
+
+def _conv_twin(c):
+    import torch
+
+    t = torch.nn.Conv2d(c.in_channels, c.out_channels, c.kernel_size, c.stride, c.padding, c.dilation, bias=False)
+    with torch.no_grad():
+        t.weight.copy_(c.weight)
+    t.weight.requires_grad_(c.weight.requires_grad)
+    return t.to(device=c.weight.device, dtype=torch.float64)
+
+
+def _tie_relu(v, tie):
+    """relu(v) whose gradient passes where v > 0, except where |v| is within the bf16 forward error of zero: there the
+    tested implementation's output sign ``tie`` decides (None: plain ReLU)."""
+    import torch
+
+    mask = v > 0
+    if tie is not None:
+        mask = torch.where(v.abs() <= BLOCK_TIE * v.pow(2).mean().sqrt(), tie, mask)
+    return torch.relu(v).detach() + (v - v.detach()) * mask
+
+
+class _BlockTwin:
+    """float64 torch.nn copy of a ``models.resnet`` BasicBlock / Bottleneck (training-mode BN, same eps / momentum,
+    same weights and running statistics, same trainable parameters)."""
+
+    def __init__(self, blk):
+        self.convs = [_conv_twin(getattr(blk, f"conv{i}")) for i in (1, 2, 3) if hasattr(blk, f"conv{i}")]
+        self.bns = [_bn_twin(getattr(blk, f"bn{i}")) for i in (1, 2, 3) if hasattr(blk, f"bn{i}")]
+        ds = blk.downsample
+        self.ds = (_conv_twin(ds[0]), _bn_twin(ds[1])) if ds is not None else None
+        self.tie = self.inner_ties = None        # the tested implementation's outputs / inner activations > 0
+
+    def __call__(self, x):
+        import torch
+
+        h = x
+        for i, (c, b) in enumerate(zip(self.convs, self.bns)):
+            h = b(c(h))
+            if i < len(self.convs) - 1:
+                h = _tie_relu(h, self.inner_ties[i] if self.inner_ties is not None else None)
+        idn = x if self.ds is None else self.ds[1](self.ds[0](x))
+        return _tie_relu(h + idn, self.tie)
+
+    def named(self):
+        """(name, module) in the same order as ``_block_named``."""
+        out = []
+        for i, (c, b) in enumerate(zip(self.convs, self.bns)):
+            out += [(f"conv{i + 1}", c), (f"bn{i + 1}", b)]
+        if self.ds is not None:
+            out += [("downsample.0", self.ds[0]), ("downsample.1", self.ds[1])]
+        return out
+
+
+def _block_named(blk):
+    out = []
+    for i in (1, 2, 3):
+        if hasattr(blk, f"conv{i}"):
+            out += [(f"conv{i}", getattr(blk, f"conv{i}")), (f"bn{i}", getattr(blk, f"bn{i}"))]
+    if blk.downsample is not None:
+        out += [("downsample.0", blk.downsample[0]), ("downsample.1", blk.downsample[1])]
+    return out
+
+
+def _chain(mods, x):
+    """x -> block 0 -> block 1 -> ...; the loss reads the last output."""
+    h = x
+    for m in mods:
+        h = m(h)
+    return [h]
+
+
+def _bneck(inp, planes, stride=1, proj=False):
+    import torch
+
+    from distributeddeeplearning_b200.models.layers import BatchNorm2d, Conv2d
+    from distributeddeeplearning_b200.models.resnet import Bottleneck
+
+    ds = torch.nn.Sequential(Conv2d(inp, planes * 4, 1, stride), BatchNorm2d(planes * 4)) if proj else None
+    return Bottleneck(inp, planes, stride, ds)
+
+
+def _basic(inp, planes, stride=1, proj=False):
+    import torch
+
+    from distributeddeeplearning_b200.models.layers import BatchNorm2d, Conv2d
+    from distributeddeeplearning_b200.models.resnet import BasicBlock
+
+    ds = torch.nn.Sequential(Conv2d(inp, planes, 1, stride), BatchNorm2d(planes)) if proj else None
+    return BasicBlock(inp, planes, stride, ds)
+
+
+def _randomize_bn(mods):
+    """Non-trivial BN parameters and running statistics (gamma = 1, beta = 0 would hide a swapped or dropped term)."""
+    import torch
+
+    with torch.no_grad():
+        for m in mods:
+            for mod in m.modules():
+                if type(mod).__name__ == "BatchNorm2d":
+                    c = mod.num_features
+                    mod.weight.copy_(torch.rand(c) + 0.5)
+                    mod.bias.copy_(torch.randn(c) * 0.3)
+                    mod.running_mean.copy_(torch.randn(c) * 0.1)
+                    mod.running_var.copy_(torch.rand(c) + 0.5)
+
+
+def _check_block_tensor(name, kind, got, ref, got_c, ref_c):
+    a, r = BLOCK_BUDGET[kind]
+    w_n = report_abs(f"   {name} ({kind})", got, ref, r, 0.0, arms=a, also=(got_c, ref_c))
+    w_c = _bound_ratio(got_c, ref_c, r, 0.0, a)[1]
+    prev = BLOCK_WORST.setdefault(kind, [0.0, 0.0])
+    prev[0], prev[1] = max(prev[0], w_n), max(prev[1], w_c)
+
+
+def _run_blocks(impl, mods, fwd, x, grads, need_dx, record):
+    """One forward + backward of ``fwd(mods, x)`` with upstream gradients ``grads`` (None: drawn here, bf16) on
+    implementation ``impl`` ('native', 'torch' = the repo's bf16 composite, 'f64' = the twin).  ``record[i]`` receives
+    (block i's output, its BN3 handoff) (native / composite) so that the twin can follow its ReLU ties."""
+    import torch
+
+    if impl == "f64":
+        xin = x.double().requires_grad_(need_dx)
+        outs = fwd(mods, xin)
+        torch.autograd.backward(outs, [g.double() for g in grads])
+        return xin, outs, grads
+    from distributeddeeplearning_b200 import ops
+
+    os.environ["DDL_B200_IMPL"] = impl
+    # the composite runs a block as conv_bn_act calls: their ReLU outputs without residual are the inner activations
+    calls, conv_bn_act = [], ops.conv_bn_act
+
+    def recording(*a, **k):
+        z = conv_bn_act(*a, **k)
+        calls.append(z if a[11] and k.get("residual", a[12] if len(a) > 12 else None) is None else None)
+        return z
+
+    def post(mod, inp, out, i):
+        # the native block saved (x, mask, then per conv its input, y, stats): the inputs of conv 2.. are the inner
+        # activations.  The handoff is read here: the consuming block takes it off the tensor
+        if type(out.grad_fn).__name__ == "_ResidualBlockBackward":
+            saved = out.grad_fn.saved_tensors
+            inner = [saved[2 + 3 * k] for k in range(1, (len(saved) - 2) // 3)]
+        else:
+            inner = [t for t in calls if t is not None]
+        calls.clear()
+        record[i] = (out, out.__dict__.get("_ddl_bn3"), inner)
+
+    hooks = [m.register_forward_hook(lambda mod, inp, out, i=i: post(mod, inp, out, i)) for i, m in enumerate(mods)]
+    ops.conv_bn_act = recording
+    try:
+        xin = x.clone().requires_grad_(need_dx)
+        outs = fwd(mods, xin)
+        if grads is None:
+            grads = [cl(bf(torch.randn(o.shape, device=o.device))) for o in outs]
+        torch.autograd.backward(outs, [g.to(o.dtype) for o, g in zip(outs, grads)])
+    finally:
+        for h in hooks:
+            h.remove()
+        ops.conv_bn_act = conv_bn_act
+        os.environ["DDL_B200_IMPL"] = "native"
+    return xin, outs, grads
+
+
+def _block_case(label, mods, xshape, fwd=_chain, frozen=(), need_dx=True, passes=1, handoff=None):
+    """Compare a block graph (``fwd`` over the ``models.resnet`` blocks ``mods``) on the native path with its float64
+    twin: outputs, running statistics, dx and every parameter gradient; frozen parameters must keep ``grad is None``.
+    ``handoff``: per pass, whether block i's BN3 sums must come from the next block's dgrad (True) or not (False).
+    Returns the native modules (for differential checks)."""
+    import copy
+
+    import torch
+
+    from distributeddeeplearning_b200.ops import blocks
+
+    print(f"-- block: {label}", flush=True)
+    mods = [m.cuda().train() for m in mods]
+    _randomize_bn(mods)
+    for i, m in enumerate(mods):
+        for n, p in m.named_parameters():
+            if f"{i}.{n}" in frozen:
+                p.requires_grad_(False)
+    comp = copy.deepcopy(mods)
+    tw_n, tw_c = [_BlockTwin(m) for m in mods], [_BlockTwin(m) for m in mods]
+    used = {}
+    orig = blocks._Bn3Handoff.pre_reduced
+
+    def spy(self, dout):
+        sums = orig(self, dout)
+        used[id(self)] = sums is not None
+        return sums
+
+    res = None
+    for p in range(passes):
+        x = cl(bf(torch.randn(*xshape, device="cuda")))
+        rec_n, rec_c = {}, {}
+        blocks._Bn3Handoff.pre_reduced = spy
+        try:
+            xn, on, grads = _run_blocks("native", mods, fwd, x, None, need_dx, rec_n)
+        finally:
+            blocks._Bn3Handoff.pre_reduced = orig
+        paths = {type(rec_n[i][0].grad_fn).__name__ for i in rec_n}
+        RESULTS.append(paths == {"_ResidualBlockBackward"})
+        print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] native residual_block path taken by every block: {sorted(paths)}",
+              flush=True)
+        if handoff is not None:
+            got = [used.get(id(rec_n[i][1]), False) for i in range(len(mods))]
+            RESULTS.append(got == list(handoff))
+            print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] pass {p}: BN3 sums from the next block's dgrad per block "
+                  f"{got} (expected {list(handoff)})", flush=True)
+        xc, oc, _ = _run_blocks("torch", comp, fwd, x, grads, need_dx, rec_c)
+        for i in range(len(mods)):
+            for tw, rec in ((tw_n[i], rec_n[i]), (tw_c[i], rec_c[i])):
+                tw.tie, tw.inner_ties = rec[0].detach() > 0, [t.detach() > 0 for t in rec[2]]
+                RESULTS.append(len(tw.inner_ties) == len(tw.convs) - 1)
+        xr, orf, _ = _run_blocks("f64", tw_n, fwd, x, grads, need_dx, None)
+        xrc, orc, _ = _run_blocks("f64", tw_c, fwd, x, grads, need_dx, None)
+        res = (xn, on, xc, oc, xr, orf, xrc, orc)
+    xn, on, xc, oc, xr, orf, xrc, orc = res
+    for k, (a, b, c, d) in enumerate(zip(on, orf, oc, orc)):
+        _check_block_tensor(f"output {k}", "out", a, b, c, d)
+    if need_dx:
+        _check_block_tensor("input", "dx", xn.grad, xr.grad, xc.grad, xrc.grad)
+    for i in range(len(mods)):
+        for (name, mn), (_, mr), (_, mc), (_, mrc) in zip(_block_named(mods[i]), tw_n[i].named(), _block_named(comp[i]),
+                                                          tw_c[i].named()):
+            tag = f"b{i}.{name}"
+            if hasattr(mn, "running_mean"):
+                _check_block_tensor(tag, "running_mean", mn.running_mean, mr.running_mean, mc.running_mean, mrc.running_mean)
+                _check_block_tensor(tag, "running_var", mn.running_var, mr.running_var, mc.running_var, mrc.running_var)
+                pairs = [("weight", "gamma grad"), ("bias", "beta grad")]
+            else:
+                pairs = [("weight", "conv weight grad")]
+            for pn, kind in pairs:
+                pn_, pr, pc, prc = (getattr(m_, pn) for m_ in (mn, mr, mc, mrc))
+                if not pn_.requires_grad:
+                    RESULTS.append(pn_.grad is None and pc.grad is None)
+                    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}]    {tag}.{pn} frozen: grad stays None", flush=True)
+                    continue
+                _check_block_tensor(f"{tag}.{pn}", kind, pn_.grad, pr.grad, pc.grad, prc.grad)
+    return mods, xn.grad
+
+
+def _pool_picks(o, h, w):
+    """Flat (row * W + col) conv-output index each 3x3/2 (pad 1) max-pool output took, from the autograd node: the fused
+    stem's arg-max codes (row * 3 + col within the window) or the composite max_pool2d's indices."""
+    import torch
+
+    node = o.grad_fn
+    if type(node).__name__ == "_ConvBnActPoolBackward":
+        arg = node.saved_tensors[2].permute(0, 3, 1, 2).long()                  # [N, P, Q, C] codes -> [N, C, P, Q]
+        hc, wc = (h + 2 * 3 - 7) // 2 + 1, (w + 2 * 3 - 7) // 2 + 1            # conv output size of the 7x7/2 stem
+        p = torch.arange(arg.shape[2], device=arg.device).view(1, 1, -1, 1)
+        q = torch.arange(arg.shape[3], device=arg.device).view(1, 1, 1, -1)
+        return (p * 2 - 1 + arg // 3) * wc + (q * 2 - 1 + arg % 3)
+    while type(node).__name__ != "MaxPool2DWithIndicesBackward0":
+        node = node.next_functions[0][0]
+    return node._saved_result1
+
+
+def _layer_case(label, stem, frozen):
+    """conv_bn (3x3 conv + BN + ReLU) or the fused stem conv_bn_pool (7x7/2 conv + BN + ReLU + 3x3/2 max-pool) with
+    gamma or beta frozen, against float64: the frozen one keeps ``grad is None``, the other one and the conv weight
+    gradient match."""
+    import copy
+
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.models.layers import BatchNorm2d, Conv2d, conv_bn, conv_bn_pool, prepare_input
+    from distributeddeeplearning_b200.ops import functional
+
+    print(f"-- layer: {label}", flush=True)
+    conv = Conv2d(3, 64, 7, 2, 3) if stem else Conv2d(64, 96, 3, 1, 1)
+    bn = BatchNorm2d(conv.out_channels)
+    conv, bn = conv.cuda(), bn.cuda()
+    _randomize_bn([bn])
+    getattr(bn, frozen).requires_grad_(False)
+    impls = {"native": (conv, bn), "torch": copy.deepcopy((conv, bn))}
+    twins = {k: (_conv_twin(c), _bn_twin(b)) for k, (c, b) in impls.items()}
+    x = bf(torch.randn(2, 3, 30, 30, device="cuda")) if stem else cl(bf(torch.randn(3, 64, 11, 11, device="cuda")))
+    outs, picks, g = {}, {}, None
+    fuse = functional.FUSE_STEM_POOL
+    functional.FUSE_STEM_POOL = True          # the fused stem is opt-in (DDL_FUSE_STEM_POOL=1)
+    try:
+        for impl, (c, b) in impls.items():
+            os.environ["DDL_B200_IMPL"] = impl
+            xin = prepare_input(x) if stem else x
+            o = conv_bn_pool(xin, c, b) if stem else conv_bn(xin, c, b, relu=True)
+            if impl == "native":
+                want = "_ConvBnActPoolBackward" if stem else "_ConvBnActBackward"
+                RESULTS.append(type(o.grad_fn).__name__ == want)
+                print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] native path {type(o.grad_fn).__name__}", flush=True)
+                g = cl(bf(torch.randn(o.shape, device="cuda")))
+            if stem:
+                picks[impl] = _pool_picks(o, x.shape[2], x.shape[3])
+            o.backward(g.to(o.dtype))
+            outs[impl] = o.detach()
+    finally:
+        functional.FUSE_STEM_POOL = fuse
+        os.environ["DDL_B200_IMPL"] = "native"
+    refs = {}
+    for impl, (c, b) in twins.items():
+        v = b(c(x.double()[:, :3] if stem else x.double()))
+        if stem:
+            # the max-pool picks the implementation's arg-max (which element of a window wins is decided among values
+            # that may round to the same bf16); the pick is checked to be a window maximum to within bf16 rounding
+            z = _tie_relu(v, None)
+            idx = picks[impl]
+            o = z.flatten(2).gather(2, idx.flatten(2)).view(idx.shape)
+            best = F.max_pool2d(z.detach(), 3, 2, 1)
+            report_abs(f"   {impl} max-pool pick is a window maximum", o.detach(), best, 2.0 ** -7, 0.0,
+                       arms=2.0 ** -7)
+        else:
+            o = _tie_relu(v, outs[impl] > 0)
+        o.backward(g.double())
+        refs[impl] = o.detach()
+    _check_block_tensor("output", "out", outs["native"], refs["native"], outs["torch"], refs["torch"])
+    (cn, bnn), (cc, bnc), (cr, bnr), (crc, bnrc) = impls["native"], impls["torch"], twins["native"], twins["torch"]
+    _check_block_tensor("bn", "running_mean", bnn.running_mean, bnr.running_mean, bnc.running_mean, bnrc.running_mean)
+    _check_block_tensor("bn", "running_var", bnn.running_var, bnr.running_var, bnc.running_var, bnrc.running_var)
+    _check_block_tensor("conv.weight", "conv weight grad", cn.weight.grad, cr.weight.grad, cc.weight.grad, crc.weight.grad)
+    for pn, kind in (("weight", "gamma grad"), ("bias", "beta grad")):
+        if pn == frozen:
+            RESULTS.append(getattr(bnn, pn).grad is None and getattr(bnc, pn).grad is None)
+            print(f"[{'ok' if RESULTS[-1] else 'FAIL'}]    bn.{pn} frozen: grad stays None", flush=True)
+        else:
+            _check_block_tensor(f"bn.{pn}", kind, getattr(bnn, pn).grad, getattr(bnr, pn).grad, getattr(bnc, pn).grad,
+                                getattr(bnrc, pn).grad)
+
+
+def g_block():
+    """ops/blocks.py: every branch of the hand-written BasicBlock / Bottleneck backward (identity or projection
+    shortcut; shortcut gradient gated into, added in, or added after the conv1 dgrad; need_dx; frozen parameters), the
+    BN3 handoff between consecutive bottlenecks (used, and refused whenever the gradient is not the next block's
+    untouched dgrad output), gradient accumulation and the autotuner's trial launches inside a block, each against a
+    float64 torch.nn twin.  The same ratios of the repo's bf16 composite (DDL_B200_IMPL=torch) are printed alongside."""
+    import copy
+
+    import torch
+
+    torch.manual_seed(0)
+    B, b = _bneck, _basic
+    # single blocks: every shortcut / dgrad-epilogue path (M = 243, 392, 98, 200, 242, 72: none a multiple of 128)
+    _block_case("bottleneck, identity (gated shortcut gradient, 1x1 conv1)", [B(256, 64)], (3, 256, 9, 9))
+    _block_case("bottleneck, projection stride 1 (layer1.0)", [B(64, 64, 1, True)], (2, 64, 14, 14))
+    _block_case("bottleneck, projection stride 2 on the 3x3, 13x13 -> 7x7", [B(256, 128, 2, True)], (2, 256, 13, 13))
+    _block_case("bottleneck, layer4 width 512 -> 2048 at 7x7", [B(2048, 512)], (2, 2048, 7, 7))
+    _block_case("bottleneck, width 40 (multiple of 8, not of 64)", [B(160, 40)], (2, 160, 10, 10))
+    _block_case("basic block, identity (3x3 conv1)", [b(64, 64)], (2, 64, 11, 11))
+    _block_case("basic block, projection stride 2 (shortcut added by native.add)", [b(64, 128, 2, True)], (2, 64, 12, 12))
+    # autotuner inside blocks: M = 25,088 >= 128 x 132 rows, so the first sight of every layer shape times the variants
+    # (trial launches re-zero the BN statistics and the fused bn-reduce sums); the BN3 sums cross the boundary
+    _block_case("layer1.0 -> layer1.1 at batch 8, 56x56 (autotuned)", [B(64, 64, 1, True), B(256, 64)], (8, 64, 56, 56),
+                handoff=[True, False])
+    # the handoff is used
+    _block_case("handoff: identity -> identity", [B(256, 64), B(256, 64)], (2, 256, 9, 9), handoff=[True, False])
+    _block_case("handoff: identity -> projection consumer (sums include the downsample add)",
+                [B(256, 64), B(256, 128, 2, True)], (2, 256, 10, 10), handoff=[True, False])
+    _block_case("handoff: projection -> identity -> identity", [B(64, 64, 1, True), B(256, 64), B(256, 64)],
+                (3, 64, 8, 8), handoff=[True, True, False])
+
+    # ... and refused
+    def also_in_loss(m, x):
+        h = m[0](x)
+        return [m[1](h), h]
+
+    def hooked(fn):
+        def f(m, x):
+            h = m[0](x)
+            h.register_hook(fn)
+            return [m[1](h)]
+        return f
+
+    def fork(m, x):
+        h = m[0](x)
+        return [m[1](h), m[2](h)]
+
+    _block_case("refused: the intermediate output also enters the loss", [B(256, 64), B(256, 64)], (2, 256, 9, 9),
+                fwd=also_in_loss, handoff=[False, False])
+    _block_case("refused: a hook returns a scaled gradient", [B(256, 64), B(256, 64)], (2, 256, 9, 9),
+                fwd=hooked(lambda g: g * 0.5), handoff=[False, False])
+    _block_case("refused: a hook scales the gradient in place", [B(256, 64), B(256, 64)], (2, 256, 9, 9),
+                fwd=hooked(lambda g: g.mul_(0.5)), handoff=[False, False])
+    _block_case("refused: one output feeds two blocks", [B(256, 64), B(256, 64), B(256, 64)], (2, 256, 9, 9), fwd=fork,
+                handoff=[False, False, False])
+    _block_case("refused: the gradient arrives non-channels-last", [B(256, 64), B(256, 64)], (2, 256, 9, 9),
+                fwd=hooked(lambda g: g.contiguous()), handoff=[False, False])
+    _block_case("refused: the consumer is a basic block (3x3 conv1)", [B(128, 32), b(128, 128)], (2, 128, 9, 9),
+                handoff=[False, False])
+    # a hook returning g.clone() refuses the handoff without changing a value: BN3 gradients of block 0 with and without
+    # the handoff agree to fp32 summation order (the fused sums are taken over the same stored bf16 values), everything
+    # downstream of them to one bf16 rounding (a last-bit change of a sum may move a bf16 gradient across a rounding
+    # boundary; the forward statistics are atomics in run-dependent order as well)
+    pair = [B(256, 64), B(256, 64)]
+    torch.manual_seed(8)
+    (m_used, dx_used) = _block_case("handoff used (differential pair, part 1)", copy.deepcopy(pair), (2, 256, 9, 9),
+                                    handoff=[True, False])
+    torch.manual_seed(8)
+    (m_ref, dx_ref) = _block_case("refused: a hook returns g.clone() (differential pair, part 2)", copy.deepcopy(pair),
+                                  (2, 256, 9, 9), fwd=hooked(lambda g: g.clone()), handoff=[False, False])
+    for n, p in m_used[0].named_parameters():
+        fp32_sums = n.startswith("bn3")
+        report_abs(f"   with vs without handoff: b0.{n} grad", p.grad, m_ref[0].get_parameter(n).grad,
+                   2.0 ** -14 if fp32_sums else 2.0 ** -7, 0.0, arms=2.0 ** -14 if fp32_sums else 2.0 ** -9)
+    report_abs("   with vs without handoff: dx", dx_used, dx_ref, 2.0 ** -7, 0.0, arms=2.0 ** -9)
+    # need_dx = False: the block input does not require grad
+    _block_case("need_dx=False, identity", [B(256, 64)], (2, 256, 9, 9), need_dx=False)
+    _block_case("need_dx=False, projection", [B(64, 64, 1, True)], (2, 64, 10, 10), need_dx=False)
+    _block_case("need_dx=False, projection, downsample gamma frozen", [B(64, 64, 1, True)], (2, 64, 10, 10),
+                need_dx=False, frozen=("0.downsample.1.weight",))
+    # frozen parameters: a conv weight alone, gamma alone, beta alone, one BN with both (incl. BN3 across the handoff)
+    _block_case("frozen: conv2.weight, bn1 gamma, bn2 beta, downsample BN both", [B(64, 64, 1, True)], (2, 64, 10, 10),
+                frozen=("0.conv2.weight", "0.bn1.weight", "0.bn2.bias", "0.downsample.1.weight", "0.downsample.1.bias"))
+    _block_case("frozen: bn3 gamma / bn3 beta across the handoff, conv1.weight, downsample conv",
+                [B(64, 64, 1, True), B(256, 64)], (2, 64, 9, 9), handoff=[True, False],
+                frozen=("0.bn3.weight", "1.bn3.bias", "1.conv1.weight", "0.downsample.0.weight", "1.bn1.bias"))
+    _block_case("frozen: basic block bn1 beta, bn2 gamma, downsample gamma", [b(64, 128, 2, True)], (2, 64, 12, 12),
+                frozen=("0.bn1.bias", "0.bn2.weight", "0.downsample.1.weight"))
+    for stem in (False, True):
+        for frozen in ("weight", "bias"):
+            _layer_case(f"{'stem conv_bn_pool' if stem else 'conv_bn'}, bn {'gamma' if frozen == 'weight' else 'beta'} "
+                        "frozen", stem, frozen)
+    # gradient accumulation: two passes without zeroing sum up, the handoff used in both
+    _block_case("two passes accumulate", [B(64, 64, 1, True), B(256, 64)], (2, 64, 9, 9), passes=2,
+                handoff=[True, False])
+    print("worst element-wise ratio to the budget per tensor kind (native / bf16 composite):", flush=True)
+    for kind, (wn, wc) in BLOCK_WORST.items():
+        a, r = BLOCK_BUDGET[kind]
+        print(f"   {kind:18s} {a:g}*rms + {r:g}*|ref|: native {wn:.3f}  composite {wc:.3f}", flush=True)
 
 
 def g_sgd():
