@@ -35,6 +35,7 @@ cudaError_t launch_conv_gemm(int mode, const ConvArgs& a, const void* w, int w_r
                              const void* a_matrix, int a_cols, cudaStream_t stream);
 cudaError_t launch_conv_wgrad(const WgradArgs& a, const void* dy, const void* x_matrix, int splits,
                               cudaStream_t stream);
+cudaError_t launch_expand_grouped_weight(const void* w, void* out, int cout, int taps, int gw, cudaStream_t stream);
 void set_conv_force_stages(int s);
 void set_wgrad_swap(int on);
 void set_conv_persistent(int on);
@@ -258,8 +259,9 @@ PYBIND11_MODULE(_C, m) {
            int cchunks, int relu, int n_valid, ptr_t w, int w_rows, int w_cols, int n_total, ptr_t a_matrix, int a_cols,
            int batch, int tw, int th, int tn, int zfill, ptr_t stream, int pad_w, int kstride, ptr_t add_mask,
            ptr_t bnr_y, ptr_t bnr_gamma, ptr_t bnr_beta, ptr_t bnr_mean, ptr_t bnr_invstd, int variant, int fp8,
-           ptr_t deq_a, ptr_t deq_b, ptr_t sfa, ptr_t sfb, ptr_t bnr_mask) {
+           ptr_t deq_a, ptr_t deq_b, ptr_t sfa, ptr_t sfb, ptr_t bnr_mask, int grouped) {
           ConvArgs a;
+          a.grouped = grouped;
           a.variant = variant;
           a.fp8 = fp8; a.deq_a = P<const float>(deq_a); a.deq_b = P<const float>(deq_b);
           a.sfa = P<const uint8_t>(sfa); a.sfb = P<const uint8_t>(sfb);
@@ -286,12 +288,13 @@ PYBIND11_MODULE(_C, m) {
         py::arg("zfill"), py::arg("stream"), py::arg("pad_w") = -1, py::arg("kstride") = 0, py::arg("add_mask") = 0,
         py::arg("bnr_y") = 0, py::arg("bnr_gamma") = 0, py::arg("bnr_beta") = 0, py::arg("bnr_mean") = 0,
         py::arg("bnr_invstd") = 0, py::arg("variant") = 0, py::arg("fp8") = 0, py::arg("deq_a") = 0,
-        py::arg("deq_b") = 0, py::arg("sfa") = 0, py::arg("sfb") = 0, py::arg("bnr_mask") = 0);
+        py::arg("deq_b") = 0, py::arg("sfa") = 0, py::arg("sfb") = 0, py::arg("bnr_mask") = 0, py::arg("grouped") = 0);
   m.def("conv_wgrad",
         [](int mode, ptr_t x, ptr_t dy, ptr_t dw, int M, int Cout, int dy_ld, int ldw, int ncols, int H, int W, int C, int Pq,
            int Q, int R, int Sx, int stride, int pad, int dil, int cchunks, int splits, int batch, int tw, int th, int tn,
-           ptr_t stream, int pad_w, int Cpad, int Cw) {
+           ptr_t stream, int pad_w, int Cpad, int Cw, int group_width) {
           WgradArgs a;
+          a.group_width = group_width;
           a.pad_w = pad_w < 0 ? pad : pad_w;
           a.Cpad = Cpad > 0 ? Cpad : ncols;      // default: one tap spanning every column (stem scratch, GEMM)
           a.Cw = Cw > 0 ? Cw : ncols;
@@ -305,7 +308,11 @@ PYBIND11_MODULE(_C, m) {
         py::arg("ldw"), py::arg("ncols"), py::arg("H"), py::arg("W"), py::arg("C"), py::arg("P"), py::arg("Q"), py::arg("R"),
         py::arg("S"), py::arg("stride"), py::arg("pad"), py::arg("dil"), py::arg("cchunks"), py::arg("splits"),
         py::arg("batch"), py::arg("tw"), py::arg("th"), py::arg("tn"), py::arg("stream"), py::arg("pad_w") = -1,
-        py::arg("Cpad") = 0, py::arg("Cw") = 0);
+        py::arg("Cpad") = 0, py::arg("Cw") = 0, py::arg("group_width") = 0);
+  m.def("expand_grouped_weight", [](ptr_t w, ptr_t out, int cout, int taps, int gw, ptr_t stream) {
+    check(ddl::launch_expand_grouped_weight(P<const void>(w), P<void>(out), cout, taps, gw, S(stream)),
+          "expand_grouped_weight");
+  }, "compact grouped conv weights [Cout][taps*gw] bf16 -> block-diagonal [Cout][taps*64] (zeros off the group)");
 
   // ------------------------------------------------------------------ BN / activation
   m.def("bn_act_fwd", [](ptr_t x, ptr_t residual, ptr_t z, ptr_t sum, ptr_t sumsq, ptr_t gamma, ptr_t beta,

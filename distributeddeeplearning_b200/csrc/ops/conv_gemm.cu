@@ -574,9 +574,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
             sh = hb + tap_r * a.dil; swd = wb + tap_s * a.dil;
             ok = row_ok && sh >= 0 && sh < a.srcH && swd >= 0 && swd < a.srcW;
           }
+          const int c0 = (a.grouped ? n0 : 0) + cc * 64;     // grouped: the tile's own 64 source channels
           const __nv_bfloat16* src =
-              ok ? img_base + (static_cast<size_t>(sh) * a.srcW + swd) * a.srcC + cc * 64 : a.src;
-          const int crem = a.srcC - cc * 64;      // channels left in this tap (last k-block of a tap may be partial)
+              ok ? img_base + (static_cast<size_t>(sh) * a.srcW + swd) * a.srcC + c0 : a.src;
+          const int crem = a.srcC - c0;           // channels left in this tap (last k-block of a tap may be partial)
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const bool okj = ok && j * 8 < crem;
@@ -633,10 +634,15 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
                                     n0 + static_cast<int>(rank) * (BLOCK_N / 2), &full[stage], 0x3);
             }
           } else if (kBMn) {
-            // weights W[co][(r,s,ci)]: K rows = 64 output channels, N = input channels (contiguous)
+            if (a.grouped) {
+              // expanded grouped weights [Cout][(tap, 64)]: K rows = output channels [n0, n0 + 64), N = tap's columns
+              tma_load_2d(sB, &tmB, widx * 64, n0, &full[stage]);
+            } else {
+              // weights W[co][(r,s,ci)]: K rows = 64 output channels, N = input channels (contiguous)
 #pragma unroll
-            for (int j = 0; j < BLOCK_N / 64; ++j)
-              tma_load_2d(sB + j * 8192, &tmB, widx * a.ldc + n0 + j * 64, cc * 64, &full[stage]);
+              for (int j = 0; j < BLOCK_N / 64; ++j)
+                tma_load_2d(sB + j * 8192, &tmB, widx * a.ldc + n0 + j * 64, cc * 64, &full[stage]);
+            }
           } else {
             tma_load_2d(sB, &tmB, mode_stem(MODE) ? kb * kBlockK : widx * a.kstride + cc * kcol, n0, &full[stage]);
           }
@@ -645,7 +651,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
           } else if (MODE == kConvStemTma) {
             tma_load_5d(smem_u32(sA), &tmA, 0, kb, tq0, tp0, tn0, &full[stage]);
           } else if (kTile) {
-            tma_load_4d(smem_u32(sA), &tmAs.m[mapi], cc * kcol, tq0 + dw, tp0 + dh, tn0, &full[stage]);
+            tma_load_4d(smem_u32(sA), &tmAs.m[mapi], (a.grouped ? n0 : 0) + cc * kcol, tq0 + dw, tp0 + dh, tn0,
+                        &full[stage]);
           }
           if (++cc == a.cchunks) { cc = 0; ++tap; if (++tap_s == a.S) { tap_s = 0; ++tap_r; } }
           if (++stage == nstages) { stage = 0; phase ^= 1u; }
@@ -810,6 +817,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
         c_off = colc - tap * a.Cpad;
         tap_r = tap / a.S;
         tap_s = tap - tap_r * a.S;
+        if (a.group_width) c_off += co0;        // grouped: the input channels of this tile's 64 output channels
       }
       const int crem = a.C - c_off;             // real channels left in this tap
       const uint32_t row_off = 16384u + chunk * 8192u + row * 128u;
@@ -877,7 +885,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
         for (int j = 0; j < 2; ++j) {
           const int colc = col0 + j * 64;
           const int tap = colc / a.Cpad;
-          tc0[j] = colc - tap * a.Cpad;
+          tc0[j] = colc - tap * a.Cpad + (a.group_width ? co0 : 0);
           const int r = tap / a.S, sx = tap - r * a.S;
           const int oh = r * a.dil - a.pad, ow = sx * a.dil - a.pad_w;
           if (a.stride == 1) {
@@ -984,7 +992,21 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     const int vc = col0 + lane * 4;                    // column in the padded (tap, Cpad) space
     const int vtap = vc / a.Cpad;
     const int vch = vc - vtap * a.Cpad;
-    if (vc < a.ncols && vch < a.Cw) {                  // channel padding of a tap has no dw column
+    if (a.group_width) {
+      // grouped (SWAP, Cpad = 64): row r pairs with input channel co0 + vch; only the diagonal group x group blocks
+      // exist.  group_width % 4 == 0, so this lane's 4 columns lie in one group and land as one 16-byte vector
+      const int gw = a.group_width;
+      if (vc < a.ncols) {
+        const int c = vtap * gw + vch % gw;
+        for (int r = warp; r < kCoTile; r += kEpiThreads / 32) {
+          const int co = co0 + r;
+          if (co < a.Cout && r / gw == vch / gw) {
+            const float4 val = *reinterpret_cast<const float4*>(stg + r * kWgPitch + lane * 4);
+            red_add_f32x4(a.dw + static_cast<size_t>(co) * a.ldw + c, val.x, val.y, val.z, val.w);
+          }
+        }
+      }
+    } else if (vc < a.ncols && vch < a.Cw) {           // channel padding of a tap has no dw column
       const int c = vtap * a.Cw + vch;
       for (int r = warp; r < kCoTile; r += kEpiThreads / 32) {
         const int co = co0 + r;
@@ -1203,7 +1225,7 @@ cudaError_t launch_fwd_mode(const CUtensorMap& tmB, const CUtensorMap& tmBh, con
   const int var_kind = a.variant & 0xf;
   const bool var_pair = ((a.variant >> 8) & 1) != 0;
   if (var_kind != 0 && var_kind != kVarOneTile && var_kind != kVarPersistent) return cudaErrorInvalidValue;
-  const int bn = (n_total % 128 == 0) ? 128 : 64;
+  const int bn = (n_total % 128 == 0 && !a.grouped) ? 128 : 64;      // grouped tiles are 64 wide (block-diagonal)
   if (n_total % 64 != 0) return cudaErrorInvalidValue;
   // pairs need two M tiles and a weight tile that splits into two loadable halves (MN-major: two 64-column boxes)
   const bool pair_ok = m_tiles >= 2 && (!mode_b_mn(MODE) || bn == 128);
@@ -1264,8 +1286,16 @@ cudaError_t launch_conv_gemm(int mode, const ConvArgs& a_in, const void* w, int 
   ConvArgs a = a_in;
   CUtensorMap tmB;
   TmaSet tmA;
-  const int bn = (n_total % 128 == 0) ? 128 : 64;
+  const int bn = (n_total % 128 == 0 && !a.grouped) ? 128 : 64;
   if (n_total % 64 != 0) return cudaErrorInvalidValue;
+  if (a.grouped) {
+    // block-diagonal tiles: bf16 window convolutions (forward or data gradient, tile or gather modes) on the expanded
+    // weights, one k-block per tap; the shortcut add and the fused BN-backward reduction are not offered
+    const bool ok_mode = mode == kConvFwd || mode == kConvTileFwd || mode == kConvDgrad || mode == kConvTileDgrad;
+    if (!ok_mode || a.fp8 || a.add != nullptr || a.add_mask != nullptr || a.bnr_y != nullptr || a.cchunks != 1 ||
+        a.kstride != 64 || w_cols != a.R * a.S * 64 || w_rows != n_total || a.srcC != n_total || a.ldc != n_total)
+      return cudaErrorInvalidValue;
+  }
   const int es = a.fp8 ? 1 : 2;                   // operand element size (bytes)
   const uint32_t kcols = 128u / es;               // elements in a 128-byte swizzle row
   if (a.fp8) {
@@ -1398,6 +1428,13 @@ cudaError_t launch_conv_wgrad(const WgradArgs& a_in, const void* dy, const void*
   WgradArgs a = a_in;
   CUtensorMap tmDy;
   TmaSet tmX;
+  if (a.group_width) {
+    // grouped: window modes only, 64-channel tiles in the (tap, 64) column space, 16-byte in-group vectors
+    const int gw = a.group_width;
+    if ((a.mode != kConvFwd && a.mode != kConvTileFwd) || gw % 4 != 0 || 64 % gw != 0 || a.Cout % 64 != 0 ||
+        a.C != a.Cout || a.Cpad != 64 || a.ncols != a.R * a.S * 64 || a.ldw != a.R * a.S * gw)
+      return cudaErrorInvalidValue;
+  }
   if (a.mode == kConvTileFwd || a.mode == kConvStemTma) {
     if (a.tw * a.th * a.tn > 64 || a.tw < 1 || a.th < 1 || a.tn < 1) return cudaErrorInvalidValue;
     if (!make_map_nhwc(&tmDy, dy, a.batch, a.P, a.Q, a.dy_ld, a.tw, a.th, a.tn)) return cudaErrorUnknown;
@@ -1447,7 +1484,7 @@ cudaError_t launch_conv_wgrad(const WgradArgs& a_in, const void* dy, const void*
   const int smem = wg_smem_bytes(a.stages);
   // narrow outputs (the last 128-channel tile would be at most half full): swap operand roles, 64-channel tiles
   const int co_rem = a.Cout % 128;
-  const bool swap = g_wgrad_swap && co_rem > 0 && co_rem <= 64;
+  const bool swap = a.group_width != 0 || (g_wgrad_swap && co_rem > 0 && co_rem <= 64);   // grouped: 64-wide tiles
   dim3 grid((a.ncols + 127) / 128, swap ? (a.Cout + 63) / 64 : (a.Cout + 127) / 128, splits);
   static bool configured[16] = {};
 #define DDL_WG(MODE)                                                                                          \
@@ -1470,6 +1507,36 @@ cudaError_t launch_conv_wgrad(const WgradArgs& a_in, const void* dy, const void*
     default: return cudaErrorInvalidValue;
   }
 #undef DDL_WG
+  return cudaGetLastError();
+}
+
+// Expanded grouped weights: compact w[co][tap * gw + j] (KRSC of a [Cout, gw, R, S] weight) -> [Cout][taps * 64] with
+// row co holding its gw input channels of each tap at columns tap * 64 + (co % 64 - co % gw) + j and zeros elsewhere:
+// the B operand of the block-diagonal 64-channel tiles.  One thread per 8 output columns (one 16-byte store).
+__global__ void expand_grouped_weight_kernel(const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ out,
+                                             int cout, int taps, int gw) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int vec_per_row = taps * 8;
+  if (i >= static_cast<long long>(cout) * vec_per_row) return;
+  const int co = static_cast<int>(i / vec_per_row);
+  const int v = static_cast<int>(i - static_cast<long long>(co) * vec_per_row);
+  const int tap = v >> 3, c0 = (v & 7) * 8;             // first of the 8 columns inside the tap's 64
+  const int g0 = (co & 63) - (co & 63) % gw;             // first column of co's group inside the tap
+  __align__(16) __nv_bfloat16 vals[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = c0 + j - g0;
+    vals[j] = (c >= 0 && c < gw) ? w[static_cast<size_t>(co) * taps * gw + tap * gw + c] : __float2bfloat16(0.f);
+  }
+  *reinterpret_cast<uint4*>(out + static_cast<size_t>(co) * taps * 64 + tap * 64 + c0) =
+      *reinterpret_cast<const uint4*>(vals);
+}
+
+cudaError_t launch_expand_grouped_weight(const void* w, void* out, int cout, int taps, int gw, cudaStream_t stream) {
+  if (cout <= 0 || taps <= 0 || gw <= 0 || 64 % gw != 0) return cudaErrorInvalidValue;
+  const long long n = static_cast<long long>(cout) * taps * 8;
+  expand_grouped_weight_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
+      static_cast<const __nv_bfloat16*>(w), static_cast<__nv_bfloat16*>(out), cout, taps, gw);
   return cudaGetLastError();
 }
 

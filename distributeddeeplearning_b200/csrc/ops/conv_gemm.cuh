@@ -84,6 +84,11 @@ struct ConvArgs {
   // in the source map, which of the 4 source maps to read, and the weight tap index r*S+s
   int ntaps;
   signed char tap_dh[16], tap_dw[16], tap_map[16], tap_widx[16];
+  // grouped convolution (Cin = Cout, group width dividing 64): N tiles are 64 wide and block-diagonal.  The tile of
+  // channels [n0, n0 + 64) reads only source channels [n0, n0 + 64), one k-block per filter tap (KB = R*S taps,
+  // cchunks = 1), and the weights are the expanded matrix [Cout][R*S*64] (expand_grouped_weight): K-major with
+  // kstride = 64 in the forward, MN-major rows [n0, n0 + 64) x columns tap*64 in the data gradient.
+  int grouped;
 };
 
 struct TmaSet {          // up to 4 activation maps (the 2x2 phase sub-images of a stride-2 source)
@@ -110,6 +115,9 @@ struct WgradArgs {
   int mode;                   // kConvFwd (gather), kConvGemm (x via 2-D TMA), kConvStem, kConvTileFwd (4-D TMA)
   int stages;
   int batch, tw, th, tn, tiles_w, tiles_h;   // tile mode: a pixel block is a tw x th x tn box (<= 64 pixels)
+  int group_width;            // grouped convolution: input channels per group (0 = dense).  Tiles are 64 output
+                              //   channels x (tap, the same 64 input channels) (Cpad = 64); only the in-group entries
+                              //   are added, to dw column tap * group_width + ci % group_width
 };
 
 }  // namespace ddl

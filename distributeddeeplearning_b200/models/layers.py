@@ -23,20 +23,24 @@ CL = torch.channels_last
 class Conv2d(nn.Module):
     """Weight (and optional bias) holder for a convolution."""
 
-    def __init__(self, cin, cout, kernel_size, stride=1, padding=0, dilation=1, bias=False):
+    def __init__(self, cin, cout, kernel_size, stride=1, padding=0, dilation=1, bias=False, groups=1):
         super().__init__()
         ks = (kernel_size, kernel_size) if isinstance(kernel_size, int) else tuple(kernel_size)
+        if cin % groups != 0 or cout % groups != 0:
+            raise ValueError("in_channels and out_channels must be divisible by groups")
         self.in_channels, self.out_channels = cin, cout
         self.kernel_size, self.stride, self.padding, self.dilation = ks, stride, padding, dilation
-        w = torch.empty(cout, cin, *ks).contiguous(memory_format=CL)
+        self.groups = groups
+        w = torch.empty(cout, cin // groups, *ks).contiguous(memory_format=CL)
         self.weight = nn.Parameter(w)
+        self.weight._ddl_groups = groups     # a grouped [Cout, Cin/groups, R, S] weight is never a stem weight
         self.bias = nn.Parameter(torch.zeros(cout)) if bias else None
         self.reset_parameters()
 
     def reset_parameters(self):
         nn.init.kaiming_uniform_(self.weight, a=math.sqrt(5))
         if self.bias is not None:
-            fan_in = self.in_channels * self.kernel_size[0] * self.kernel_size[1]
+            fan_in = self.weight.shape[1] * self.kernel_size[0] * self.kernel_size[1]
             bound = 1 / math.sqrt(fan_in)
             nn.init.uniform_(self.bias, -bound, bound)
 
@@ -48,10 +52,11 @@ class Conv2d(nn.Module):
 
     def forward(self, x, relu=False):
         """Standalone conv (+bias, +ReLU) — VGG / AlexNet style layers."""
-        return ops.conv_bias_act(x, self.weight, self.bias, self.stride, self.padding, self.dilation, relu)
+        return ops.conv_bias_act(x, self.weight, self.bias, self.stride, self.padding, self.dilation, relu, self.groups)
 
     def extra_repr(self):
-        return f"{self.in_channels}, {self.out_channels}, kernel_size={self.kernel_size}, stride={self.stride}, padding={self.padding}"
+        return f"{self.in_channels}, {self.out_channels}, kernel_size={self.kernel_size}, stride={self.stride}, padding={self.padding}" + \
+            (f", groups={self.groups}" if self.groups != 1 else "")
 
 
 class BatchNorm2d(nn.Module):
@@ -74,7 +79,8 @@ def conv_bn(x, conv: Conv2d, bn: BatchNorm2d, relu=True, residual=None):
     """act(BN(conv(x)) [+ residual]) through the fused op."""
     return ops.conv_bn_act(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.stride,
                            conv.padding,
-                           conv.dilation, bn.eps, bn.momentum, relu, residual, bn.training)
+                           conv.dilation, bn.eps, bn.momentum, relu, residual, bn.training,
+                           **({"groups": conv.groups} if conv.groups != 1 else {}))
 
 
 def conv_bn_pool(x, conv: Conv2d, bn: BatchNorm2d, kernel=3, stride=2, padding=1):

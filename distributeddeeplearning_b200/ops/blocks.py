@@ -71,8 +71,12 @@ class _ResidualBlock(torch.autograd.Function):
         for i in range(n_main):
             w, g, b, rm, rv = layers[i]
             st, pad, dil, eps, mom = cfg["layers"][i]
-            wb = weight_bf16(w)
-            y, stats = native.conv_fwd(h, wb, (w.shape[2], w.shape[3]), st, pad, dil, stats=True, cout=w.shape[0])
+            groups = cfg["groups"][i]
+            wb = weight_bf16(w, groups=groups)
+            if groups > 1:      # this step's block-diagonal operand (grouped conv), kept for the data gradient
+                wb = native.expand_grouped_weight(wb, w.shape[2] * w.shape[3], groups)
+            y, stats = native.conv_fwd(h, wb, (w.shape[2], w.shape[3]), st, pad, dil, stats=True, cout=w.shape[0],
+                                       groups=groups)
             last = i == n_main - 1
             if last:      # residual layer: backward masks with 1 bit per element instead of re-reading the block output
                 z, save, zmask = native.bn_act_fwd(y, stats, g, b, rm, rv, eps, mom, True, identity, True, want_mask=True)
@@ -108,6 +112,7 @@ class _ResidualBlock(torch.autograd.Function):
             st, pad, dil, _, _ = cfg["layers"][i]
             h_in, y, save = saved[3 * i], saved[3 * i + 1], saved[3 * i + 2]
             kernel = (w.shape[2], w.shape[3])
+            groups = cfg["groups"][i]
             last = i == n_main - 1
             gg = grad_buffer(g) if g.requires_grad else None
             bg = grad_buffer(b) if b.requires_grad else None
@@ -115,7 +120,7 @@ class _ResidualBlock(torch.autograd.Function):
             #                                                    mask is recomputed from y; last layer: bit mask)
             # identity shortcut + a dgrad that can add in its epilogue: the shortcut gradient dout * (out > 0) is
             # formed there from dout and the bit mask, so the BN-backward kernel need not write (and dgrad re-read) it
-            gate = last and not has_ds and need_dx and native.dgrad_supports_add(
+            gate = last and not has_ds and need_dx and cfg["groups"][0] == 1 and native.dgrad_supports_add(
                 (layers[0][0].shape[2], layers[0][0].shape[3]), cfg["layers"][0][0])
             dy, dr, _ = native.bn_act_bwd(d, z, y, save, g, True, last and not gate, gg, bg, beta=b, had_residual=last,
                                           zmask=zmask if last else None, pre_reduced=pre)
@@ -129,11 +134,11 @@ class _ResidualBlock(torch.autograd.Function):
                 # in its epilogue (it holds the gradient tile anyway and only has to read the y tile, which it fetches
                 # while its MMAs run): BN_{i-1}'s backward is then one pass over (d_{i-1}, y) instead of two
                 gp, bp = layers[i - 1][1], layers[i - 1][2]
-                fuse = native.dgrad_fuses_bn_reduce(kernel, st, pad)
+                fuse = groups == 1 and native.dgrad_fuses_bn_reduce(kernel, st, pad)
                 pre = native.zeros_f32((2, h_in.shape[1]), h_in.device) if fuse else None
                 d = native.conv_dgrad(dy, ctx.wbs[i], h_in.shape, kernel, st, pad, dil,
                                       bn_reduce=(saved[3 * (i - 1) + 1], gp, bp, saved[3 * (i - 1) + 2], pre)
-                                      if fuse else None)
+                                      if fuse else None, groups=groups)
             elif need_dx:
                 add = dres
                 if has_ds:
@@ -154,24 +159,26 @@ class _ResidualBlock(torch.autograd.Function):
                 # x is the previous block's output: where this dgrad can, it also takes that block's BN3 sums
                 prev = cfg["bn3_in"]
                 bnr = None
-                if prev is not None and prev.bn is not None and native.dgrad_fuses_bn_reduce(kernel, st, pad):
+                if prev is not None and prev.bn is not None and groups == 1 and \
+                        native.dgrad_fuses_bn_reduce(kernel, st, pad):
                     py, psave, pg, pb, pmask = prev.bn
                     prev.sums = native.zeros_f32((2, x.shape[1]), x.device)
                     bnr = (py, pg, pb, psave, prev.sums, pmask)
                 if gated_add is not None:
                     dx = native.conv_dgrad(dy, ctx.wbs[0], x.shape, kernel, st, pad, dil, add=gated_add[0],
                                            add_mask=gated_add[1], bn_reduce=bnr)
-                elif native.dgrad_supports_add(kernel, st):
+                elif groups == 1 and native.dgrad_supports_add(kernel, st):
                     dx = native.conv_dgrad(dy, ctx.wbs[0], x.shape, kernel, st, pad, dil, add=add, bn_reduce=bnr)
                 else:
                     bnr = None
-                    dx = native.add(native.conv_dgrad(dy, ctx.wbs[0], x.shape, kernel, st, pad, dil), add)
+                    dx = native.add(native.conv_dgrad(dy, ctx.wbs[0], x.shape, kernel, st, pad, dil, groups=groups),
+                                    add)
                 if bnr is not None:
                     prev.dx, prev.version = dx, dx._version
             if w.requires_grad:
                 gw = grad_buffer(w)
-                run_wgrad(w, lambda h_in=h_in, dy=dy, gw=gw, kernel=kernel, st=st, pad=pad, dil=dil:
-                          native.conv_wgrad(h_in, dy, gw, kernel, st, pad, dil), h_in, dy)
+                run_wgrad(w, lambda h_in=h_in, dy=dy, gw=gw, kernel=kernel, st=st, pad=pad, dil=dil, groups=groups:
+                          native.conv_wgrad(h_in, dy, gw, kernel, st, pad, dil, groups=groups), h_in, dy)
             for p in (g, b, w):
                 if p.requires_grad:
                     notify_ready(p)
@@ -203,6 +210,10 @@ def residual_block_supported(x: torch.Tensor, convs: Sequence, bns: Sequence, do
             return False
         if not native.supports_conv(conv.in_channels, conv.out_channels) or not native.bn_supported(conv.out_channels):
             return False
+        groups = getattr(conv, "groups", 1)
+        if groups > 1 and (not native.supports_grouped(conv.in_channels, conv.out_channels, groups) or
+                           (downsample is not None and conv is downsample[0])):     # main-path convs only
+            return False
         if conv.in_channels <= 4 or not conv.weight.is_contiguous(memory_format=CL) and conv.weight.dim() == 4 and \
                 conv.weight.shape[2] * conv.weight.shape[3] > 1:
             return False
@@ -217,6 +228,7 @@ def residual_block(x: torch.Tensor, convs: Sequence, bns: Sequence, downsample=N
     prev = x.__dict__.pop("_ddl_bn3", None)
     cfg = {"n_main": len(convs), "has_ds": downsample is not None,
            "layers": [(c.stride, c.padding, c.dilation, b.eps, b.momentum) for c, b in mods],
+           "groups": [getattr(c, "groups", 1) for c, _ in mods],
            "bn3_in": prev, "bn3_out": _Bn3Handoff()}
     params = []
     for c, b in mods:

@@ -188,13 +188,14 @@ def end_of_step(device=None) -> None:
 MIN_K = int(os.environ.get("DDL_FP8_MIN_K", "512"))
 
 
-def fwd_eligible(cin: int, cout: int, taps: int = 1) -> bool:
-    return _STATE["enabled"] and cin % 128 == 0 and cout % 64 == 0 and cin * taps >= MIN_K
+def fwd_eligible(cin: int, cout: int, taps: int = 1, groups: int = 1) -> bool:
+    # grouped convolutions stay bf16 (their block-diagonal tiles have no fp8 form)
+    return _STATE["enabled"] and groups == 1 and cin % 128 == 0 and cout % 64 == 0 and cin * taps >= MIN_K
 
 
-def dgrad_eligible(cin: int, cout: int, taps: int = 1) -> bool:
+def dgrad_eligible(cin: int, cout: int, taps: int = 1, groups: int = 1) -> bool:
     # reduction dim = Cout (k-blocks of 128), transposed weight rows = input channels (N tiles of 128)
-    return _STATE["enabled"] and cout % 128 == 0 and cin % 128 == 0 and cout * taps >= MIN_K
+    return _STATE["enabled"] and groups == 1 and cout % 128 == 0 and cin % 128 == 0 and cout * taps >= MIN_K
 
 
 def count(kind: str) -> None:

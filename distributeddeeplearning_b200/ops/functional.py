@@ -102,15 +102,24 @@ def notify_ready(p: torch.Tensor) -> None:
         cb()
 
 
-def weight_bf16(p: torch.Tensor, kernel: Optional[Tuple[int, int]] = None) -> torch.Tensor:
+def is_stem_weight(p: torch.Tensor, groups: Optional[int] = None) -> bool:
+    """A first-layer conv weight on an NHWC4 image (Cin <= 4), which the stem kernels take re-packed.  A grouped weight
+    ``[Cout, Cin/groups, R, S]`` can have as few input channels per group (ResNeXt-50's ``[128, 4, 3, 3]``) and is not
+    one: ``groups`` defaults to the ``_ddl_groups`` attribute ``models.layers.Conv2d`` puts on its weight."""
+    g = groups if groups is not None else getattr(p, "_ddl_groups", 1)
+    return p.dim() == 4 and p.shape[1] <= 4 and g == 1
+
+
+def weight_bf16(p: torch.Tensor, kernel: Optional[Tuple[int, int]] = None, groups: Optional[int] = None) -> torch.Tensor:
     """bf16 GEMM operand of a parameter.
 
     With a fused engine attached the copy is a view into the bf16 weight arena that the
     allreduce+SGD kernel refreshes every step (no per-step cast).  Otherwise it is cast on
     demand and cached against the parameter's version counter.  Stem weights (Cin <= 4) are
-    re-packed to the padded [Cout, KB*64] matrix.
+    re-packed to the padded [Cout, KB*64] matrix.  Grouped weights come as the compact
+    [Cout, R*S*Cin/groups] matrix (``native.expand_grouped_weight`` derives the kernels' operand from it).
     """
-    stem = p.dim() == 4 and p.shape[1] <= 4
+    stem = is_stem_weight(p, groups)
     view = getattr(p, "_ddl_bf16", None)
     if view is not None and not stem:
         return view
@@ -146,13 +155,16 @@ def _krsc(p: torch.Tensor) -> bool:
 class _ConvBnAct(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, weight, gamma, beta, running_mean, running_var, stride, pad, dil, eps, momentum,
-                relu, train):
+                relu, train, groups):
         R, S = weight.shape[2], weight.shape[3]
-        wb = weight_bf16(weight)
+        wb = weight_bf16(weight, groups=groups)
+        if groups > 1:      # this step's block-diagonal operand, shared by the forward and the data gradient
+            wb = native.expand_grouped_weight(wb, R * S, groups)
         # stem: the padded / row-interleaved image the TMA kernels read is built once and shared with the wgrad kernel
-        xp = native.stem_prepare(x, (R, S), stride, pad, dil) if (train and x.shape[1] == 4) else None
-        y, stats = native.conv_fwd(x, wb, (R, S), stride, pad, dil, stats=train, cout=weight.shape[0], prepadded=xp) \
-            if train else (native.conv_fwd(x, wb, (R, S), stride, pad, dil, cout=weight.shape[0]), None)
+        xp = native.stem_prepare(x, (R, S), stride, pad, dil) if (train and x.shape[1] == 4 and groups == 1) else None
+        y, stats = native.conv_fwd(x, wb, (R, S), stride, pad, dil, stats=train, cout=weight.shape[0], prepadded=xp,
+                                   groups=groups) \
+            if train else (native.conv_fwd(x, wb, (R, S), stride, pad, dil, cout=weight.shape[0], groups=groups), None)
         use_bits = train and relu and residual is not None
         if use_bits:      # residual layer: 1-bit ReLU mask for backward instead of re-reading z
             z, save, zmask = native.bn_act_fwd(y, stats, gamma, beta, running_mean, running_var, eps, momentum, relu,
@@ -161,7 +173,7 @@ class _ConvBnAct(torch.autograd.Function):
             z, save = native.bn_act_fwd(y, stats, gamma, beta, running_mean, running_var, eps, momentum, relu, residual,
                                         train)
             zmask = None
-        ctx.cfg = (stride, pad, dil, relu, residual is not None, (R, S))
+        ctx.cfg = (stride, pad, dil, relu, residual is not None, (R, S), groups)
         ctx.params = (weight, gamma, beta)
         if train:
             # wb is a view of the engine's bf16 weight arena: kept as a plain attribute (no autograd
@@ -174,7 +186,7 @@ class _ConvBnAct(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dz):
-        stride, pad, dil, relu, has_res, kernel = ctx.cfg
+        stride, pad, dil, relu, has_res, kernel, groups = ctx.cfg
         weight, gamma, beta = ctx.params
         x, y, z, save = ctx.saved_tensors
         zmask = z if (z is not None and z.dtype == torch.uint8) else None     # residual layers saved the bit mask
@@ -188,30 +200,33 @@ class _ConvBnAct(torch.autograd.Function):
                                         zmask=zmask)
         dx = None
         if ctx.needs_input_grad[0]:
-            dx = native.conv_dgrad(dy, wb, x.shape, kernel, stride, pad, dil)
+            dx = native.conv_dgrad(dy, wb, x.shape, kernel, stride, pad, dil, groups=groups)
         if weight.requires_grad:
             gw = grad_buffer(weight)
             xp = ctx.xp
-            run_wgrad(weight, lambda: native.conv_wgrad(x, dy, gw, kernel, stride, pad, dil, prepadded=xp), x, dy,
-                      *((xp,) if xp is not None else ()))
+            run_wgrad(weight, lambda: native.conv_wgrad(x, dy, gw, kernel, stride, pad, dil, prepadded=xp, groups=groups),
+                      x, dy, *((xp,) if xp is not None else ()))
         # LAST: a ready bucket may launch its allreduce+update kernel on the side stream now; everything
         # this layer still needed from the weight arenas (gamma, wb) has been enqueued before the event
         for p in (gamma, beta, weight):
             if p.requires_grad:
                 notify_ready(p)
-        return (dx, dres) + (None,) * 12
+        return (dx, dres) + (None,) * 13
 
 
 def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad=0, dil=1, eps=1e-5, momentum=0.1,
-                relu=True, residual=None, training=True):
-    """z = act(BN(conv(x, weight)) [+ residual])  — the unit every ResNet/Inception layer is made of."""
+                relu=True, residual=None, training=True, groups=1):
+    """z = act(BN(conv(x, weight)) [+ residual])  — the unit every ResNet/Inception layer is made of.  ``groups`` > 1:
+    grouped convolution (``weight`` is [Cout, Cin/groups, R, S]); shapes outside ``native.supports_grouped`` take the
+    composite path."""
     if use_native(x) and native.supports_conv(x.shape[1], weight.shape[0]) \
+            and (groups == 1 or native.supports_grouped(x.shape[1], weight.shape[0], groups)) \
             and native.bn_supported(weight.shape[0]) and _krsc(weight):
         return _ConvBnAct.apply(x, residual, weight, gamma, beta, running_mean, running_var, stride, pad, dil, eps,
-                                momentum, relu, training)
-    xi = x[:, : weight.shape[1]] if x.shape[1] != weight.shape[1] else x     # NHWC4 stem input on the composite path
+                                momentum, relu, training, groups)
+    xi = x[:, : weight.shape[1]] if (x.shape[1] != weight.shape[1] and groups == 1) else x   # NHWC4 stem input
     y = F.conv2d(xi.to(weight.dtype) if not x.is_cuda else xi, weight.to(xi.dtype) if x.is_cuda else weight, None,
-                 stride, pad, dil)
+                 stride, pad, dil, groups)
     z = F.batch_norm(y.float(), running_mean, running_var, gamma, beta, training, momentum, eps).to(y.dtype)
     if residual is not None:
         z = z + residual
@@ -345,13 +360,14 @@ class _ConvBiasAct(torch.autograd.Function):
         return dx, None, None, None, None, None, None
 
 
-def conv_bias_act(x, weight, bias=None, stride=1, pad=0, dil=1, relu=True):
-    if use_native(x) and native.supports_conv(x.shape[1], weight.shape[0]) and _krsc(weight):
+def conv_bias_act(x, weight, bias=None, stride=1, pad=0, dil=1, relu=True, groups=1):
+    """Stand-alone conv (+ bias, + ReLU); grouped convolutions (no BN after them) run on the composite path."""
+    if use_native(x) and groups == 1 and native.supports_conv(x.shape[1], weight.shape[0]) and _krsc(weight):
         return _ConvBiasAct.apply(x, weight, bias, stride, pad, dil, relu)
-    xi = x[:, : weight.shape[1]] if x.shape[1] != weight.shape[1] else x
+    xi = x[:, : weight.shape[1]] if (x.shape[1] != weight.shape[1] and groups == 1) else x
     w = weight.to(xi.dtype) if x.is_cuda else weight
     b = bias.to(xi.dtype) if (bias is not None and x.is_cuda) else bias
-    y = F.conv2d(xi if x.is_cuda else xi.to(weight.dtype), w, b, stride, pad, dil)
+    y = F.conv2d(xi if x.is_cuda else xi.to(weight.dtype), w, b, stride, pad, dil, groups)
     return F.relu(y) if relu else y
 
 

@@ -53,14 +53,14 @@ VAR_PAIR = 1 << 8
 _TUNE = {"enabled": os.environ.get("DDL_CONV_AUTOTUNE", "1") == "1", "table": {}, "timings": {}}
 
 
-def conv_variants(n_total: int, m_rows: int, kb: int, b_mn_major: bool, fp8: bool = False):
+def conv_variants(n_total: int, m_rows: int, kb: int, b_mn_major: bool, fp8: bool = False, grouped: bool = False):
     """Variant words worth timing for an ``m_rows`` x ``n_total`` x ``kb*64`` problem (see launch_fwd_mode).  fp8
-    operands run on the one-tile kernel only."""
+    operands run on the one-tile kernel only; grouped tiles are 64 wide."""
     out = [VAR_ONE_TILE]
     if fp8 or m_rows < 128 * 132:     # less than one wave of 128-row tiles: the persistent kernels cannot pay
         return out
     out.append(VAR_PERSISTENT)
-    if not (b_mn_major and n_total % 128 != 0):       # MN-major weight tiles split into two 64-column boxes
+    if not (b_mn_major and (n_total % 128 != 0 or grouped)):   # MN-major weight tiles split into two 64-column boxes
         out.append(VAR_PERSISTENT | VAR_PAIR)
     return out
 
@@ -339,16 +339,64 @@ def supports_conv(cin: int, cout: int) -> bool:
     return cout % 8 == 0 and (cin % 8 == 0 or cin <= 4)
 
 
+def supports_grouped(cin: int, cout: int, groups: int) -> bool:
+    """Grouped convolutions the block-diagonal kernels handle: ``cin == cout``, a multiple of 64, split into groups whose
+    width divides 64 (a 64-channel tile then holds whole groups) and is a multiple of 4 (each 16-byte weight-gradient
+    vector lies in one group).  Other grouped shapes (depthwise among them) take the composite path."""
+    if groups <= 1:
+        return supports_conv(cin, cout)
+    if cin != cout or cin % groups != 0 or cin % 64 != 0:
+        return False
+    cg = cin // groups
+    return 64 % cg == 0 and cg % 4 == 0
+
+
+def expand_grouped_weight(w_bf16: torch.Tensor, taps: int, groups: int) -> torch.Tensor:
+    """Compact grouped weights ``[Cout, taps * cg]`` bf16 (KRSC of ``[Cout, cg, R, S]``) -> the block-diagonal operand
+    ``[Cout, taps * 64]`` of the grouped kernels: row ``co`` holds its ``cg`` input channels of each tap at columns
+    ``tap * 64 + (co % 64 - co % cg) + j``, zeros elsewhere.  Made once per step, in forward (so that a captured graph
+    re-derives it from the weights every replay), and kept for that step's data gradient."""
+    cout = w_bf16.shape[0]
+    cg = cout // groups
+    if w_bf16.dtype != torch.bfloat16 or w_bf16.numel() != cout * taps * cg or not w_bf16.is_contiguous():
+        raise ValueError("expand_grouped_weight: expected contiguous bf16 [Cout, taps * Cout / groups] weights")
+    out = torch.empty((cout, taps * 64), dtype=torch.bfloat16, device=w_bf16.device)
+    _C().expand_grouped_weight(w_bf16.data_ptr(), out.data_ptr(), cout, taps, cg, _stream())
+    return out
+
+
+def _check_grouped(cin: int, cout: int, groups: int, w_bf16: torch.Tensor, taps: int) -> None:
+    if not supports_grouped(cin, cout, groups):
+        raise ValueError(f"grouped conv {cin} -> {cout} in {groups} groups is not supported by the native kernels")
+    if tuple(w_bf16.shape) != (cout, taps * 64):
+        raise ValueError("grouped conv: pass the expanded weights of expand_grouped_weight ([Cout, R*S*64])")
+
+
+def _conv_grouped(mode: int, src: torch.Tensor, out: torch.Tensor, w_bf16: torch.Tensor, C: int, M: int, srcHW, dstHW,
+                  kernel, stride: int, ph: int, pw: int, dil: int, s_ptr: int = 0, ss_ptr: int = 0, batch: int = 0,
+                  tile=(0, 0, 0), zfill: int = 0, variant: int = 0) -> None:
+    """One launch of the block-diagonal grouped kernels (forward: tile / gather fwd; data gradient: tile / gather dgrad)
+    with one 64-channel k-block per tap."""
+    R, S = kernel
+    tma = mode in (_C().CONV_TILE_FWD, _C().CONV_TILE_DGRAD)
+    _C().conv_gemm(mode, 0 if tma else src.data_ptr(), out.data_ptr(), 0, 0, s_ptr, ss_ptr, M, R * S, C, srcHW[0],
+                   srcHW[1], C, dstHW[0], dstHW[1], R, S, stride, ph, dil, 1, 0, C, w_bf16.data_ptr(), C, R * S * 64, C,
+                   src.data_ptr() if tma else 0, C if tma else 0, batch, tile[0], tile[1], tile[2], zfill, _stream(), pw,
+                   64, variant=variant, grouped=1)
+
+
 # ------------------------------------------------------------------------------------------------
 # convolution forward / dgrad / wgrad
 # ------------------------------------------------------------------------------------------------
 def conv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, kernel: Tuple[int, int], stride: int, pad, dil: int = 1,
              stats: bool = False, bias: Optional[torch.Tensor] = None, relu: bool = False,
-             cout: Optional[int] = None, prepadded: Optional[torch.Tensor] = None):
+             cout: Optional[int] = None, prepadded: Optional[torch.Tensor] = None, groups: int = 1):
     """y = conv(x, w) [+ bias][ReLU]; optionally per-channel (sum, sumsq) of y for BatchNorm.
     ``prepadded``: result of :func:`stem_prepare` for this (x, geometry) — skips the internal padding copy.
 
     ``w_bf16``: [Cout, R*S*Cin] bf16 (or the packed stem matrix [Cout, KB*64]); ``pad``: int or (pad_h, pad_w).
+    ``groups`` > 1: a grouped convolution (:func:`supports_grouped`); ``w_bf16`` is then the expanded
+    [Cout, R*S*64] matrix of :func:`expand_grouped_weight`; no bias / ReLU.
     """
     C = _C()
     _check_act(x)
@@ -363,6 +411,21 @@ def conv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, kernel: Tuple[int, int], str
     y = empty_act(N, Cout, P, Q, x.device)
     st = zeros_f32((2, Cout), x.device) if stats else None
     s_ptr, ss_ptr = (st[0].data_ptr(), st[1].data_ptr()) if stats else (0, 0)
+    if groups > 1:
+        _check_grouped(Cin, Cout, groups, w_bf16, R * S)
+        if bias is not None or relu:
+            raise ValueError("conv_fwd: grouped convolutions take no bias / ReLU epilogue")
+        geo = dict(srcHW=(H, W), dstHW=(P, Q), kernel=kernel, stride=stride, ph=ph, pw=pw, dil=dil, s_ptr=s_ptr,
+                   ss_ptr=ss_ptr, batch=N)
+        if USE_TILE_TMA and (stride == 1 or (stride == 2 and R * S <= 16 and USE_TILE_S2)):
+            tile = tile_geometry(P, Q, N, 128)
+            _tuned(("fwd_g", N, H, W, Cin, Cout, R, S, stride, ph, pw, dil, stats, groups),
+                   conv_variants(Cout, M, R * S, False, grouped=True),
+                   lambda v: _conv_grouped(C.CONV_TILE_FWD, x, y, w_bf16, Cout, M, tile=tile, variant=v, **geo),
+                   (st,) if stats else ())
+        else:
+            _conv_grouped(C.CONV_FWD, x, y, w_bf16, Cout, M, **geo)
+        return (y, st) if stats else y
     n_total = _ceil_div(Cout, 64) * 64              # N tiles cover the padded width; stores / stats stop at Cout
     cch = _ceil_div(Cin, 64)
     wp, wr, wc = w_bf16.data_ptr(), w_bf16.shape[0], w_bf16.shape[1]
@@ -442,9 +505,9 @@ def conv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, kernel: Tuple[int, int], str
 
 def conv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, kernel: Tuple[int, int], stride: int, pad,
                dil: int = 1, add: Optional[torch.Tensor] = None, add_mask: Optional[torch.Tensor] = None,
-               bn_reduce: Optional[tuple] = None) -> torch.Tensor:
+               bn_reduce: Optional[tuple] = None, groups: int = 1) -> torch.Tensor:
     """dx = conv_transpose(dy, w) (+ add [gated by the bit mask ``add_mask``: uint8 [M, Cin/8]]).
-    ``w_bf16`` is the forward matrix [Cout, R*S*Cin].
+    ``w_bf16`` is the forward matrix [Cout, R*S*Cin] (``groups`` > 1: the expanded [Cout, R*S*64] matrix of the forward).
 
     ``bn_reduce = (y, gamma, beta, save, scratch[, zmask])``: dx is the output gradient of a BN+ReLU layer whose saved
     input is ``y``; the kernel's epilogue then also accumulates that BN's dbeta / dgamma sums into ``scratch`` (fp32
@@ -472,6 +535,28 @@ def conv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, kernel: Tuple[in
             zfill = 1
         elif R < 2 or S < 2 or not (covered_h and covered_w):
             dx.zero_()
+    if groups > 1:
+        # block-diagonal tiles: the N tile of input channels [n0, n0 + 64) reads dy channels [n0, n0 + 64) and the
+        # expanded weights MN-major; the shortcut add and the BN-backward reduction are not fused here
+        _check_grouped(Cin, Cout, groups, w_bf16, R * S)
+        if add is not None or add_mask is not None or bn_reduce is not None:
+            raise ValueError("conv_dgrad: grouped convolutions take no add / add_mask / bn_reduce")
+        geo = dict(srcHW=(P, Q), dstHW=(H, W), kernel=kernel, stride=stride, ph=ph, pw=pw, dil=dil, batch=N)
+        if stride == 1 and USE_TILE_TMA:
+            tile = tile_geometry(H, W, N, 128)
+            _tuned(("dgrad_g", N, H, W, Cin, Cout, R, S, 1, ph, pw, dil, groups),
+                   conv_variants(Cin, N * H * W, R * S, True, grouped=True),
+                   lambda v: _conv_grouped(C.CONV_TILE_DGRAD, dy, dx, w_bf16, Cin, N * H * W, tile=tile, variant=v,
+                                           **geo))
+        elif s2_tile:
+            tile = tile_geometry((H + 1) // 2, (W + 1) // 2, N, 128)
+            _tuned(("dgrad_s2_g", N, H, W, Cin, Cout, R, S, 2, ph, pw, dil, zfill, groups),
+                   conv_variants(Cin, N * ((H + 1) // 2) * ((W + 1) // 2), max(1, (R * S) // 4), True, grouped=True),
+                   lambda v: _conv_grouped(C.CONV_TILE_DGRAD, dy, dx, w_bf16, Cin, N * H * W, tile=tile, zfill=zfill,
+                                           variant=v, **geo))
+        else:
+            _conv_grouped(C.CONV_DGRAD, dy, dx, w_bf16, Cin, N * H * W, **geo)
+        return dx
     if add is not None:
         _check_act(add, "add")
     if add_mask is not None and (add is None or add_mask.dtype != torch.uint8 or add_mask.numel() != N * H * W * (Cin // 8)):
@@ -576,8 +661,9 @@ def _wgrad_splits(tiles: int, total_kb: int, device_index: int) -> int:
 
 
 def conv_wgrad(x: torch.Tensor, dy: torch.Tensor, grad_w: torch.Tensor, kernel: Tuple[int, int], stride: int,
-               pad, dil: int = 1, prepadded: Optional[torch.Tensor] = None) -> None:
-    """grad_w[Cout][R*S*Cin] (fp32, KRSC) += dy^T * im2col(x).  ``prepadded``: see :func:`stem_prepare`."""
+               pad, dil: int = 1, prepadded: Optional[torch.Tensor] = None, groups: int = 1) -> None:
+    """grad_w[Cout][R*S*Cin] (fp32, KRSC) += dy^T * im2col(x).  ``prepadded``: see :func:`stem_prepare`.
+    ``groups`` > 1: grad_w is the compact [Cout][R*S*Cin/groups] gradient of the grouped weight."""
     C = _C()
     _check_act(x)
     _check_act(dy, "dy")
@@ -589,6 +675,23 @@ def conv_wgrad(x: torch.Tensor, dy: torch.Tensor, grad_w: torch.Tensor, kernel: 
     dev = x.device.index or 0
     if grad_w.dtype != torch.float32:
         raise TypeError("grad_w must be fp32")
+    if groups > 1:
+        # tiles of 64 output channels x (tap, the same 64 input channels); the epilogue adds the in-group entries
+        if not supports_grouped(Cin, Cout, groups):
+            raise ValueError(f"grouped conv {Cin} -> {Cout} in {groups} groups is not supported by the native kernels")
+        cg = Cin // groups
+        if grad_w.numel() != Cout * R * S * cg:
+            raise ValueError("conv_wgrad: grad_w does not match the grouped weight [Cout, Cin/groups, R, S]")
+        ncols = R * S * 64
+        if USE_TILE_TMA and (stride == 1 or (stride == 2 and USE_TILE_S2)):
+            mode, (tw, th, tn) = C.CONV_TILE_FWD, tile_geometry(P, Q, N, 64)
+            total_kb = -(-Q // tw) * -(-P // th) * -(-N // tn)
+        else:
+            mode, (tw, th, tn), total_kb = C.CONV_FWD, (0, 0, 0), (M + 63) // 64
+        splits = _wgrad_splits(((ncols + 127) // 128) * (Cout // 64), total_kb, dev)
+        C.conv_wgrad(mode, x.data_ptr(), dy.data_ptr(), grad_w.data_ptr(), M, Cout, Cout, R * S * cg, ncols, H, W, Cin,
+                     P, Q, R, S, stride, ph, dil, 0, splits, N, tw, th, tn, _stream(), pw, 64, cg, group_width=cg)
+        return
     if Cin <= 4:
         SP, RPK, KB, RP = stem_geometry(R, S)
         ncols = KB * 64

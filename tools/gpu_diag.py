@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped","elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 
 
@@ -724,7 +724,8 @@ def _bn_twin(b):
 def _conv_twin(c):
     import torch
 
-    t = torch.nn.Conv2d(c.in_channels, c.out_channels, c.kernel_size, c.stride, c.padding, c.dilation, bias=False)
+    t = torch.nn.Conv2d(c.in_channels, c.out_channels, c.kernel_size, c.stride, c.padding, c.dilation, bias=False,
+                        groups=getattr(c, "groups", 1))
     with torch.no_grad():
         t.weight.copy_(c.weight)
     t.weight.requires_grad_(c.weight.requires_grad)
@@ -1339,6 +1340,206 @@ def g_avgdebug():
     print("ref", xr.grad[0, 0])
     print("got", got[0, 0].float())
     report("avgpool bwd tiny", got, xr.grad, 1e-2)
+
+
+# grouped 3x3 layers of ResNeXt-50 32x4d / 101 32x8d / 101 64x4d as (C, H=W, stride, group width), plus a whole-tile
+# group (cg = 64), an odd image with stride 2, and an M tail (N*P*Q not a multiple of 128)
+GROUPED_SHAPES = sorted({(128, 56, 1, 4), (256, 56, 2, 8), (256, 28, 1, 8), (512, 28, 2, 16), (512, 14, 1, 16),
+                         (1024, 14, 2, 32), (1024, 7, 1, 32),
+                         (256, 56, 1, 8), (512, 56, 2, 16), (512, 28, 1, 16), (1024, 28, 2, 32), (1024, 14, 1, 32),
+                         (2048, 14, 2, 64), (2048, 7, 1, 64),
+                         (256, 56, 1, 4), (512, 56, 2, 8), (512, 28, 1, 8), (1024, 28, 2, 16), (1024, 14, 1, 16),
+                         (2048, 14, 2, 32), (2048, 7, 1, 32),
+                         (128, 14, 1, 64), (256, 13, 2, 8), (192, 9, 1, 16)})
+
+
+def _grouped_layer(C, hw, stride, cg, n):
+    """fwd (+ BN statistics), dgrad and wgrad (accumulating onto a pre-filled slot, two passes) of one grouped 3x3 conv
+    against fp32 F.conv2d(groups=) on the same bf16-rounded operands, element-wise."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    g = C // cg
+    x = cl(bf(torch.randn(n, C, hw, hw, device="cuda")))
+    w = bf(torch.randn(C, cg, 3, 3, device="cuda") * (2.0 / (9 * cg)) ** 0.5).contiguous(memory_format=torch.channels_last)
+    wc = w.permute(0, 2, 3, 1).reshape(C, 9 * cg).contiguous()            # the compact [Cout][R*S*cg] operand
+    we = nv.expand_grouped_weight(wc, 9, g)
+    tag = f"C={C} {hw}x{hw} s{stride} cg={cg} N={n}"
+    y, st = nv.conv_fwd(x, we, (3, 3), stride, 1, stats=True, groups=g)
+    yr = F.conv2d(x.float(), w.float(), None, stride, 1, 1, g)
+    report_abs(f"grouped fwd  {tag}", y, yr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+    yb = y.float()
+    report_abs(f"grouped fwd sum   {tag}", st[0], yb.sum((0, 2, 3)), 2.0 ** -10, 0.0, arms=2.0 ** -10)
+    report_abs(f"grouped fwd sumsq {tag}", st[1], (yb * yb).sum((0, 2, 3)), 2.0 ** -10, 0.0, arms=2.0 ** -10)
+    dy = cl(bf(torch.randn(y.shape, device="cuda")))
+    dx = nv.conv_dgrad(dy, we, x.shape, (3, 3), stride, 1, groups=g)
+    dxr = torch.nn.grad.conv2d_input(x.shape, w.float(), dy.float(), stride, 1, 1, g)
+    report_abs(f"grouped dgrad {tag}", dx, dxr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+    dwr = torch.nn.grad.conv2d_weight(x.float(), w.shape, dy.float(), stride, 1, 1, g)
+    pre = torch.randn(w.shape, device="cuda").contiguous(memory_format=torch.channels_last)
+    gw = pre.clone()
+    nv.conv_wgrad(x, dy, gw, (3, 3), stride, 1, groups=g)
+    report_abs(f"grouped wgrad onto a filled slot {tag}", gw - pre, dwr, 2.0 ** -10, 0.0, arms=2.0 ** -10)
+    nv.conv_wgrad(x, dy, gw, (3, 3), stride, 1, groups=g)
+    report_abs(f"grouped wgrad two passes {tag}", gw - pre, 2 * dwr, 2.0 ** -10, 0.0, arms=2.0 ** -10)
+
+
+def _rx(inp, planes, stride=1, proj=False, groups=32, width=4):
+    import torch
+
+    from distributeddeeplearning_b200.models.layers import BatchNorm2d, Conv2d
+    from distributeddeeplearning_b200.models.resnet import Bottleneck
+
+    ds = torch.nn.Sequential(Conv2d(inp, planes * 4, 1, stride), BatchNorm2d(planes * 4)) if proj else None
+    return Bottleneck(inp, planes, stride, ds, groups, width)
+
+
+def _model_vs_torchvision(name, bs, hooks_on=None):
+    """zero_init_residual model vs torchvision fp32 with the same weights (and this repo's bf16 composite): logits cosine
+    and per-parameter gradient cosines, under g_model's bounds.  ``hooks_on``: module type whose forward outputs must
+    come from the native residual-block node."""
+    import torch
+    import torchvision
+
+    from distributeddeeplearning_b200 import models, ops
+
+    torch.manual_seed(0)
+    m = models.get_model(name, zero_init_residual=True).cuda().train()
+    tv = getattr(torchvision.models, name)().cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    paths = set()
+    hooks = [mod.register_forward_hook(lambda mod, i, o: paths.add(type(o.grad_fn).__name__))
+             for mod in m.modules() if hooks_on is not None and isinstance(mod, hooks_on)]
+    x = torch.randn(bs, 3, 224, 224, device="cuda").to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    out = m(x)
+    for h in hooks:
+        h.remove()
+    if hooks_on is not None:
+        RESULTS.append(paths == {"_ResidualBlockBackward"})
+        print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name}: every block on the native residual_block path {sorted(paths)}")
+    loss = ops.softmax_cross_entropy(out, y, 1000)
+    loss.backward()
+    ro = tv(x)
+    torch.nn.functional.cross_entropy(ro, y).backward()
+    os.environ["DDL_B200_IMPL"] = "torch"
+    co = m2(x)
+    ops.softmax_cross_entropy(co, y, 1000).backward()
+    os.environ["DDL_B200_IMPL"] = "native"
+    print(f"{name} logits cos vs fp32 {_cos(out, ro):.5f}   vs bf16-composite {_cos(out, co):.5f}")
+    RESULTS.append(_cos(out, ro) > 0.98)
+    gn, gc = dict(m.named_parameters()), dict(m2.named_parameters())
+    worst, lag = (1.0, ""), (0.0, "")
+    for k, p in tv.named_parameters():
+        if float(p.grad.norm()) == 0.0:
+            continue
+        c1, c2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if c1 < worst[0]:
+            worst = (c1, k)
+        if c2 - c1 > lag[0]:
+            lag = (c2 - c1, k)
+        if k in ("layer1.0.conv2.weight", "layer2.0.conv2.weight", "layer3.0.conv2.weight", "layer4.0.conv2.weight"):
+            print(f"   {k:32s} cos(native,fp32)={c1:.4f} cos(composite,fp32)={c2:.4f}")
+    ok = worst[0] > 0.80 and lag[0] < 0.08
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at {worst[1]}; "
+          f"largest deficit vs the bf16 composite = {lag[0]:.4f} at {lag[1]}", flush=True)
+    RESULTS.append(ok)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def g_grouped():
+    """Grouped convolutions (ResNeXt): the block-diagonal mode of the conv kernels per layer, in residual blocks against
+    the float64 twin of the `block` group, whole ResNeXt-50 / Wide ResNet-50 gradients against torchvision, CUDA-graph
+    replay of a training session, and fp8 mode keeping the grouped layers in bf16."""
+    import torch
+
+    from distributeddeeplearning_b200.models.resnet import Bottleneck
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.ops import native as nv
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    torch.manual_seed(0)
+    for C, hw, stride, cg in GROUPED_SHAPES:
+        _grouped_layer(C, hw, stride, cg, 3 if hw <= 14 else 2)
+    bad = []
+    for args in ((96, 96, 3), (128, 64, 32), (128, 128, 64), (128, 128, 128)):       # Cin != Cout, cg = 2, cg = 1
+        bad.append(nv.supports_grouped(*args))
+    RESULTS.append(not any(bad))
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] supports_grouped refuses unsupported grouped shapes {bad}", flush=True)
+
+    # residual blocks against the float64 twin (M = 98, 72, 162: none a multiple of 128)
+    _block_case("resnext bottleneck, identity (C = 128, cg = 4)", [_rx(256, 64)], (2, 256, 7, 7))
+    _block_case("resnext bottleneck, projection stride 2 on the grouped 3x3, 13x13 -> 7x7 (cg = 8)",
+                [_rx(256, 128, 2, True)], (2, 256, 13, 13))
+    _block_case("resnext chain of 3 (BN3 handoff)", [_rx(256, 64, 1, True), _rx(256, 64), _rx(256, 64)], (2, 256, 9, 9),
+                handoff=[True, True, False])
+    _block_case("resnext bottleneck, frozen grouped weight", [_rx(256, 64)], (2, 256, 9, 9),
+                frozen=("0.conv2.weight",))
+    _block_case("resnext bottleneck 64x4d width (C = 256, cg = 4), two passes", [_rx(256, 64, groups=64)],
+                (2, 256, 7, 7), passes=2)
+
+    # whole models
+    _model_vs_torchvision("resnext50_32x4d", 16, Bottleneck)
+    _model_vs_torchvision("wide_resnet50_2", 16, Bottleneck)
+
+    # training with the fused engine, eager then CUDA-graph replay: the replayed losses track the eager ones
+    dist.init()
+
+    def run(graph):
+        torch.manual_seed(0)
+        s = BenchmarkSession("resnext50_32x4d", 16, True, lr=0.01, momentum=0.9)
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out[-4:]
+
+    a, b = run(False), run(True)
+    ok = all(x == x for x in a + b) and all(abs(x - y) < 5e-2 * max(1.0, abs(x)) for x, y in zip(a, b))
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] resnext50_32x4d training: eager {[round(v, 4) for v in a]} "
+          f"graph replay {[round(v, 4) for v in b]}", flush=True)
+
+    # fp8 mode: the model runs, the 128-multiple dense layers take fp8, the grouped layers do not
+    fp8.reset()
+    fp8.enable(True)
+    calls = []
+    fwd, dgrad = nv.conv_fwd, nv.conv_dgrad
+
+    def spy(fn, kind):
+        def f(*a, **k):
+            before = fp8.launches()[kind]
+            r = fn(*a, **k)
+            if k.get("groups", 1) > 1:
+                calls.append(fp8.launches()[kind] - before)
+            return r
+        return f
+
+    nv.conv_fwd, nv.conv_dgrad = spy(fwd, "fwd"), spy(dgrad, "dgrad")
+    try:
+        torch.manual_seed(0)
+        s = BenchmarkSession("resnext50_32x4d", 16, True, lr=0.01, momentum=0.9)
+        losses = [float(s.step()) for _ in range(3)]
+        torch.cuda.synchronize()
+    finally:
+        nv.conv_fwd, nv.conv_dgrad = fwd, dgrad
+        fp8.enable(False)
+    n = fp8.launches()
+    ok = all(l == l for l in losses) and n["fwd"] > 0 and n["dgrad"] > 0 and len(calls) > 0 and not any(calls)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] resnext50_32x4d fp8: losses {[round(v, 3) for v in losses]}, fp8 launches {n}, "
+          f"grouped launches {len(calls)} of which fp8 {sum(calls)}", flush=True)
 
 
 def run_group(name):
