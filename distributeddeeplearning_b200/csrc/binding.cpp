@@ -372,6 +372,29 @@ PYBIND11_MODULE(_C, m) {
     check(ddl::launch_bn_pool_bwd(a, pool_args(N, H, W, C, Pq, Q, k, stride, pad), P<const __nv_bfloat16>(dy_pooled),
                                   P<const uint8_t>(argmax), sms, S(stream)), "bn_pool_bwd");
   });
+  // ------------------------------------------------------------------ depthwise 3x3 convolution
+  m.def("dwconv_fwd", [](ptr_t x, ptr_t w, ptr_t y, ptr_t sum, ptr_t sumsq, int N, int H, int W, int C, int Pq, int Q,
+                         int stride, int sms, ptr_t stream) {
+    ddl::DwConvArgs a{};
+    a.x = P<const __nv_bfloat16>(x); a.w = P<const __nv_bfloat16>(w); a.y = P<__nv_bfloat16>(y);
+    a.sum = P<float>(sum); a.sumsq = P<float>(sumsq);
+    a.N = N; a.H = H; a.W = W; a.C = C; a.P = Pq; a.Q = Q; a.stride = stride;
+    check(ddl::launch_dwconv_fwd(a, sms, S(stream)), "dwconv_fwd");
+  });
+  m.def("dwconv_dgrad", [](ptr_t dy, ptr_t w, ptr_t dx, int N, int H, int W, int C, int Pq, int Q, int stride, int sms,
+                           ptr_t stream) {
+    ddl::DwConvArgs a{};
+    a.dy = P<const __nv_bfloat16>(dy); a.w = P<const __nv_bfloat16>(w); a.y = P<__nv_bfloat16>(dx);
+    a.N = N; a.H = H; a.W = W; a.C = C; a.P = Pq; a.Q = Q; a.stride = stride;
+    check(ddl::launch_dwconv_dgrad(a, sms, S(stream)), "dwconv_dgrad");
+  });
+  m.def("dwconv_wgrad", [](ptr_t x, ptr_t dy, ptr_t gw, int N, int H, int W, int C, int Pq, int Q, int stride, int sms,
+                           ptr_t stream) {
+    ddl::DwConvArgs a{};
+    a.x = P<const __nv_bfloat16>(x); a.dy = P<const __nv_bfloat16>(dy); a.gw = P<float>(gw);
+    a.N = N; a.H = H; a.W = W; a.C = C; a.P = Pq; a.Q = Q; a.stride = stride;
+    check(ddl::launch_dwconv_wgrad(a, sms, S(stream)), "dwconv_wgrad");
+  });
   m.def("channel_stats", [](ptr_t x, ptr_t sum, ptr_t sumsq, int M, int C, int sms, ptr_t stream) {
     check(ddl::launch_channel_stats(P<const __nv_bfloat16>(x), P<float>(sum), P<float>(sumsq), M, C, sms, S(stream)),
           "channel_stats");

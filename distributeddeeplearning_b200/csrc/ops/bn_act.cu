@@ -9,6 +9,9 @@
 //             pass 2: dx = gamma*invstd * (dy - dbeta/M - xhat*dgamma/M),  dres = dy
 //   mask: none (no ReLU) | z > 0 (residual layers; z is read) | x*scale + shift > 0 (no residual: the
 //   mask is recomputed from x, so z is never read: 2 reads in pass 1, 2 reads + 1 write in pass 2)
+//   ReLU6 (relu == 2, MobileNetV2): z = min(max(v, 0), 6) and the gradient passes where 0 < v < 6 (PyTorch's hardtanh
+//   backward), v being z or the recomputed pre-activation.  Its own template instantiations, so that the ReLU
+//   kernels of the ResNet path keep their code and registers; not combined with the residual bit mask.
 //
 // Thread mapping: a thread owns 8 consecutive channels (one 16-byte vector) of a FIXED channel
 // group and walks rows with a grid stride, so per-channel constants live in registers.  The loops
@@ -23,7 +26,14 @@ namespace ddl {
 namespace {
 
 constexpr int kBnThreads = 256;
-enum { kMaskNone = 0, kMaskZ = 1, kMaskX = 2, kMaskBits = 3 };
+enum { kMaskNone = 0, kMaskZ = 1, kMaskX = 2, kMaskBits = 3, kMaskZ6 = 4, kMaskX6 = 5 };
+constexpr bool mask_from_z(int m) { return m == kMaskZ || m == kMaskZ6; }
+constexpr bool mask_from_x(int m) { return m == kMaskX || m == kMaskX6; }
+// whether the gradient passes the activation at pre-activation (or output) value v
+template <int MASK>
+DDL_DEVICE bool act_passes(float v) {
+  return (MASK == kMaskZ6 || MASK == kMaskX6) ? (v > 0.f && v < 6.f) : v > 0.f;
+}
 
 struct Vec8 {
   float v[8];
@@ -87,7 +97,7 @@ DDL_DEVICE void fp8_fold_amax(Fp8Slot* slot, float amax) {
   }
 }
 
-template <bool TRAIN, bool CHUNKED, bool FP8>
+template <bool TRAIN, bool CHUNKED, bool FP8, bool RELU6>
 __global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) {
   pdl_trigger();
   pdl_wait();      // nothing to prepare here: the gain is the launch latency and the block ramp-up
@@ -149,7 +159,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) 
         a.mask[off >> 3] = static_cast<uint8_t>(bits);
       }
 #pragma unroll
-      for (int i = 0; i < 8; ++i) z[i] = fmaxf(z[i], 0.f);
+      for (int i = 0; i < 8; ++i) z[i] = RELU6 ? fminf(fmaxf(z[i], 0.f), 6.f) : fmaxf(z[i], 0.f);
     }
     store8_bf16(a.z + off, z);
     if (FP8) {
@@ -200,7 +210,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
   float s1[8], s2[8], msc[8], msh[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) { s1[i] = 0.f; s2[i] = 0.f; msc[i] = 0.f; msh[i] = 0.f; }
-  if (MASK == kMaskX && live) {
+  if (mask_from_x(MASK) && live) {
     Vec8 mean = load8_f32(a.mean + c0), invstd = load8_f32(a.invstd + c0);
     Vec8 gam = load8_f32(a.gamma + c0), bet = load8_f32(a.beta + c0);
 #pragma unroll
@@ -210,17 +220,17 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
     float dz[8], x[8];
     unpack8(udz, dz);
     unpack8(ux, x);
-    if (MASK == kMaskZ) {
+    if (mask_from_z(MASK)) {
       float z[8];
       unpack8(uz, z);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) dz[i] = z[i] > 0.f ? dz[i] : 0.f;
+      for (int i = 0; i < 8; ++i) dz[i] = act_passes<MASK>(z[i]) ? dz[i] : 0.f;
     } else if (MASK == kMaskBits) {        // uz.x carries the 8 mask bits of this (row, channel group)
 #pragma unroll
       for (int i = 0; i < 8; ++i) dz[i] = ((uz.x >> i) & 1u) ? dz[i] : 0.f;
-    } else if (MASK == kMaskX) {
+    } else if (mask_from_x(MASK)) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) dz[i] = fmaf(x[i], msc[i], msh[i]) > 0.f ? dz[i] : 0.f;
+      for (int i = 0; i < 8; ++i) dz[i] = act_passes<MASK>(fmaf(x[i], msc[i], msh[i])) ? dz[i] : 0.f;
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -239,7 +249,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
     const uint4 d0 = ld_stream_u4(a.dz + off0), d1 = ld_stream_u4(a.dz + off1);
     const uint4 x0 = ld_stream_u4(a.x + off0), x1 = ld_stream_u4(a.x + off1);
     uint4 z0 = make_uint4(0, 0, 0, 0), z1 = z0;
-    if (MASK == kMaskZ) { z0 = ld_stream_u4(a.z + off0); z1 = ld_stream_u4(a.z + off1); }
+    if (mask_from_z(MASK)) { z0 = ld_stream_u4(a.z + off0); z1 = ld_stream_u4(a.z + off1); }
     if (MASK == kMaskBits) { z0.x = a.zmask[off0 >> 3]; z1.x = a.zmask[off1 >> 3]; }
     accumulate(d0, x0, z0);
     accumulate(d1, x1, z1);
@@ -249,7 +259,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
     const uint4 d0 = ld_stream_u4(a.dz + off0);
     const uint4 x0 = ld_stream_u4(a.x + off0);
     uint4 z0 = make_uint4(0, 0, 0, 0);
-    if (MASK == kMaskZ) z0 = ld_stream_u4(a.z + off0);
+    if (mask_from_z(MASK)) z0 = ld_stream_u4(a.z + off0);
     if (MASK == kMaskBits) z0.x = a.zmask[off0 >> 3];
     accumulate(d0, x0, z0);
   }
@@ -314,7 +324,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_apply_kernel(BnBwdAr
       cA[i] = -k1[i] * db.v[i] * inv_n - mean.v[i] * cB[i];
       msh[i] = 0.f;
     }
-    if (MASK == kMaskX) {
+    if (mask_from_x(MASK)) {
       Vec8 bet = load8_f32(a.beta + c0);
 #pragma unroll
       for (int i = 0; i < 8; ++i) msh[i] = bet.v[i] - mean.v[i] * k1[i];
@@ -325,18 +335,18 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_apply_kernel(BnBwdAr
     float dz[8], x[8];
     unpack8(ld_stream_u4(a.dz + off), dz);
     unpack8(ld_stream_u4(a.x + off), x);
-    if (MASK == kMaskZ) {
+    if (mask_from_z(MASK)) {
       float z[8];
       unpack8(ld_stream_u4(a.z + off), z);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) dz[i] = z[i] > 0.f ? dz[i] : 0.f;
+      for (int i = 0; i < 8; ++i) dz[i] = act_passes<MASK>(z[i]) ? dz[i] : 0.f;
     } else if (MASK == kMaskBits) {
       const uint32_t bits = a.zmask[off >> 3];
 #pragma unroll
       for (int i = 0; i < 8; ++i) dz[i] = ((bits >> i) & 1u) ? dz[i] : 0.f;
-    } else if (MASK == kMaskX) {
+    } else if (mask_from_x(MASK)) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) dz[i] = fmaf(x[i], k1[i], msh[i]) > 0.f ? dz[i] : 0.f;
+      for (int i = 0; i < 8; ++i) dz[i] = act_passes<MASK>(fmaf(x[i], k1[i], msh[i])) ? dz[i] : 0.f;
     }
     if (a.dres) store8_bf16(a.dres + off, dz);
 #pragma unroll
@@ -602,58 +612,73 @@ void set_bn_reverse(int on) { g_bn_reverse = on; }
 
 void pdl_early_bn(int trig) { cudaMemcpyToSymbol(c_pdl_trigger, &trig, sizeof(int)); }
 
+namespace {
+
+// ReLU6 layers get no fp8 twin (not instantiated: no MobileNetV2 convolution meets the fp8 shape rules)
+template <bool CHUNKED, bool RELU6>
+cudaError_t launch_bn_fwd_variant(const BnFwdArgs& a, bool train, bool f8, dim3 grid, cudaStream_t stream) {
+  if (f8) {
+    if constexpr (RELU6) return cudaErrorInvalidValue;
+    else return launch_pdl(bn_act_fwd_kernel<true, CHUNKED, true, false>, grid, dim3(kBnThreads), 0, stream, 1, a);
+  }
+  if (train) return launch_pdl(bn_act_fwd_kernel<true, CHUNKED, false, RELU6>, grid, dim3(kBnThreads), 0, stream, 1, a);
+  return launch_pdl(bn_act_fwd_kernel<false, CHUNKED, false, RELU6>, grid, dim3(kBnThreads), 0, stream, 1, a);
+}
+
+template <int MASK>
+cudaError_t launch_bn_bwd_mask(const BnBwdArgs& a, int sms, cudaStream_t stream, bool skip_reduce) {
+  const dim3 rgrid = bn_chunk_grid(a.M, a.C, sms);
+  if (!skip_reduce) {
+    const cudaError_t e = launch_pdl(bn_act_bwd_reduce_kernel<MASK>, rgrid, dim3(kBnThreads), 0, stream, 1, a);
+    if (e != cudaSuccess) return e;
+  }
+  const bool f8 = a.dxq != nullptr && a.dxq_slot != nullptr;
+  const bool flat = bn_flat_ok(a.C);
+  const dim3 grid = flat ? dim3(bn_grid(a.M, a.C, sms)) : rgrid;
+  if constexpr (MASK == kMaskZ6 || MASK == kMaskX6) {
+    if (f8) return cudaErrorInvalidValue;
+  } else if (f8) {
+    return flat ? launch_pdl(bn_act_bwd_apply_kernel<MASK, false, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                : launch_pdl(bn_act_bwd_apply_kernel<MASK, true, true>, grid, dim3(kBnThreads), 0, stream, 1, a);
+  }
+  return flat ? launch_pdl(bn_act_bwd_apply_kernel<MASK, false, false>, grid, dim3(kBnThreads), 0, stream, 1, a)
+              : launch_pdl(bn_act_bwd_apply_kernel<MASK, true, false>, grid, dim3(kBnThreads), 0, stream, 1, a);
+}
+
+}  // namespace
+
 cudaError_t launch_bn_act_fwd(const BnFwdArgs& a_in, bool train, int sms, cudaStream_t stream) {
   BnFwdArgs a = a_in;
   a.reverse = g_bn_reverse;
   if (a.C % 8 != 0 || a.C <= 0) return cudaErrorInvalidValue;
+  if (a.relu < 0 || a.relu > 2 || (a.relu == 2 && a.mask != nullptr)) return cudaErrorInvalidValue;   // no ReLU6 bit mask
   const bool f8 = a.zq != nullptr && a.zq_slot != nullptr && train;
-  cudaError_t e = cudaSuccess;
+  const bool r6 = a.relu == 2;
   if (bn_flat_ok(a.C)) {
-    const int grid = bn_grid(a.M, a.C, sms);
-    if (f8) e = launch_pdl(bn_act_fwd_kernel<true, false, true>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a);
-    else if (train) e = launch_pdl(bn_act_fwd_kernel<true, false, false>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a);
-    else e = launch_pdl(bn_act_fwd_kernel<false, false, false>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a);
-  } else {
-    const dim3 grid = bn_chunk_grid(a.M, a.C, sms);
-    if (f8) e = launch_pdl(bn_act_fwd_kernel<true, true, true>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a);
-    else if (train) e = launch_pdl(bn_act_fwd_kernel<true, true, false>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a);
-    else e = launch_pdl(bn_act_fwd_kernel<false, true, false>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a);
+    const dim3 grid(bn_grid(a.M, a.C, sms));
+    return r6 ? launch_bn_fwd_variant<false, true>(a, train, f8, grid, stream)
+              : launch_bn_fwd_variant<false, false>(a, train, f8, grid, stream);
   }
-  return e;
+  const dim3 grid = bn_chunk_grid(a.M, a.C, sms);
+  return r6 ? launch_bn_fwd_variant<true, true>(a, train, f8, grid, stream)
+            : launch_bn_fwd_variant<true, false>(a, train, f8, grid, stream);
 }
 
 cudaError_t launch_bn_act_bwd(const BnBwdArgs& a_in, int sms, cudaStream_t stream, bool skip_reduce) {
   BnBwdArgs a = a_in;
   a.reverse = g_bn_reverse;
   if (a.C % 8 != 0 || a.C <= 0) return cudaErrorInvalidValue;
-  const int mask = !a.relu ? kMaskNone : (a.mask_from_x ? kMaskX : (a.zmask ? kMaskBits : kMaskZ));
-  const dim3 rgrid = bn_chunk_grid(a.M, a.C, sms);
-  cudaError_t e = cudaSuccess;
-  if (!skip_reduce) switch (mask) {
-    case kMaskNone: e = launch_pdl(bn_act_bwd_reduce_kernel<kMaskNone>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); break;
-    case kMaskZ: e = launch_pdl(bn_act_bwd_reduce_kernel<kMaskZ>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); break;
-    case kMaskBits: e = launch_pdl(bn_act_bwd_reduce_kernel<kMaskBits>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); break;
-    default: e = launch_pdl(bn_act_bwd_reduce_kernel<kMaskX>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); break;
+  if (a.relu < 0 || a.relu > 2 || (a.relu == 2 && a.zmask != nullptr)) return cudaErrorInvalidValue;   // no ReLU6 bit mask
+  switch (!a.relu ? kMaskNone
+                  : a.relu == 2 ? (a.mask_from_x ? kMaskX6 : kMaskZ6)
+                                : (a.mask_from_x ? kMaskX : (a.zmask ? kMaskBits : kMaskZ))) {
+    case kMaskNone: return launch_bn_bwd_mask<kMaskNone>(a, sms, stream, skip_reduce);
+    case kMaskZ: return launch_bn_bwd_mask<kMaskZ>(a, sms, stream, skip_reduce);
+    case kMaskBits: return launch_bn_bwd_mask<kMaskBits>(a, sms, stream, skip_reduce);
+    case kMaskX: return launch_bn_bwd_mask<kMaskX>(a, sms, stream, skip_reduce);
+    case kMaskZ6: return launch_bn_bwd_mask<kMaskZ6>(a, sms, stream, skip_reduce);
+    default: return launch_bn_bwd_mask<kMaskX6>(a, sms, stream, skip_reduce);
   }
-  if (e != cudaSuccess) return e;
-  const bool f8 = a.dxq != nullptr && a.dxq_slot != nullptr;
-  if (bn_flat_ok(a.C)) {
-    const int grid = bn_grid(a.M, a.C, sms);
-    switch (mask) {
-      case kMaskNone: if (f8) e = launch_pdl(bn_act_bwd_apply_kernel<kMaskNone, false, true>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a); else e = launch_pdl(bn_act_bwd_apply_kernel<kMaskNone, false, false>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a); break;
-      case kMaskZ: if (f8) e = launch_pdl(bn_act_bwd_apply_kernel<kMaskZ, false, true>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a); else e = launch_pdl(bn_act_bwd_apply_kernel<kMaskZ, false, false>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a); break;
-      case kMaskBits: if (f8) e = launch_pdl(bn_act_bwd_apply_kernel<kMaskBits, false, true>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a); else e = launch_pdl(bn_act_bwd_apply_kernel<kMaskBits, false, false>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a); break;
-      default: if (f8) e = launch_pdl(bn_act_bwd_apply_kernel<kMaskX, false, true>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a); else e = launch_pdl(bn_act_bwd_apply_kernel<kMaskX, false, false>, dim3(grid), dim3(kBnThreads), 0, stream, 1, a); break;
-    }
-  } else {
-    switch (mask) {
-      case kMaskNone: if (f8) e = launch_pdl(bn_act_bwd_apply_kernel<kMaskNone, true, true>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); else e = launch_pdl(bn_act_bwd_apply_kernel<kMaskNone, true, false>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); break;
-      case kMaskZ: if (f8) e = launch_pdl(bn_act_bwd_apply_kernel<kMaskZ, true, true>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); else e = launch_pdl(bn_act_bwd_apply_kernel<kMaskZ, true, false>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); break;
-      case kMaskBits: if (f8) e = launch_pdl(bn_act_bwd_apply_kernel<kMaskBits, true, true>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); else e = launch_pdl(bn_act_bwd_apply_kernel<kMaskBits, true, false>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); break;
-      default: if (f8) e = launch_pdl(bn_act_bwd_apply_kernel<kMaskX, true, true>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); else e = launch_pdl(bn_act_bwd_apply_kernel<kMaskX, true, false>, dim3(rgrid), dim3(kBnThreads), 0, stream, 1, a); break;
-    }
-  }
-  return e;
 }
 
 

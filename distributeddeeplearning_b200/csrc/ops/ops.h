@@ -66,6 +66,23 @@ cudaError_t launch_bn_act_bwd(const BnBwdArgs& a, int sms, cudaStream_t stream, 
 cudaError_t launch_channel_stats(const __nv_bfloat16* x, float* sum, float* sumsq, int M, int C, int sms,
                                  cudaStream_t stream);
 
+// ---- depthwise 3x3 convolution (depthwise.cu) -------------------------------------------------------
+// groups == Cin == Cout = C (C % 8 == 0), 3x3, stride 1 or 2, padding 1; x [N][H][W][C], y / dy [N][P][Q][C] bf16
+struct DwConvArgs {
+  const __nv_bfloat16* x;         // forward / wgrad input
+  const __nv_bfloat16* dy;        // dgrad / wgrad output gradient
+  const __nv_bfloat16* w;         // [C][3][3] bf16
+  __nv_bfloat16* y;               // forward: y;  dgrad: dx [N][H][W][C]
+  float* sum;                     // forward, optional: per-channel sum / sum of squares of the bf16 y (+=, zeroed
+  float* sumsq;                   //   by the caller)
+  float* gw;                      // wgrad: fp32 [C][3][3] gradient, accumulated (+=)
+  int N, H, W, C, P, Q, stride;
+  int lg_gpc;                     // set by the launcher: log2 of the 8-channel groups per block
+};
+cudaError_t launch_dwconv_fwd(const DwConvArgs& a, int sms, cudaStream_t stream);
+cudaError_t launch_dwconv_dgrad(const DwConvArgs& a, int sms, cudaStream_t stream);
+cudaError_t launch_dwconv_wgrad(const DwConvArgs& a, int sms, cudaStream_t stream);
+
 // ---- pooling -------------------------------------------------------------------------------------
 struct PoolArgs {
   int N, H, W, C, P, Q, k, stride, pad;

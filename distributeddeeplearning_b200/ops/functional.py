@@ -165,7 +165,7 @@ class _ConvBnAct(torch.autograd.Function):
         y, stats = native.conv_fwd(x, wb, (R, S), stride, pad, dil, stats=train, cout=weight.shape[0], prepadded=xp,
                                    groups=groups) \
             if train else (native.conv_fwd(x, wb, (R, S), stride, pad, dil, cout=weight.shape[0], groups=groups), None)
-        use_bits = train and relu and residual is not None
+        use_bits = train and relu and relu != 2 and residual is not None
         if use_bits:      # residual layer: 1-bit ReLU mask for backward instead of re-reading z
             z, save, zmask = native.bn_act_fwd(y, stats, gamma, beta, running_mean, running_var, eps, momentum, relu,
                                                residual, train, want_mask=True)
@@ -215,22 +215,69 @@ class _ConvBnAct(torch.autograd.Function):
 
 
 def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad=0, dil=1, eps=1e-5, momentum=0.1,
-                relu=True, residual=None, training=True, groups=1):
+                relu=True, residual=None, training=True, groups=1, relu6=False):
     """z = act(BN(conv(x, weight)) [+ residual])  — the unit every ResNet/Inception layer is made of.  ``groups`` > 1:
-    grouped convolution (``weight`` is [Cout, Cin/groups, R, S]); shapes outside ``native.supports_grouped`` take the
-    composite path."""
+    grouped convolution (``weight`` is [Cout, Cin/groups, R, S]); depthwise shapes that ``native.supports_depthwise``
+    accepts run on the depthwise kernels, other shapes outside ``native.supports_grouped`` take the composite path.
+    ``relu6``: the activation is ReLU6 (clamp to [0, 6]) instead of ``relu``."""
+    act = 2 if relu6 else relu
+    if use_native(x) and groups > 1 and x.shape[1] == weight.shape[0] and weight.shape[1] == 1 \
+            and native.supports_depthwise(weight.shape[0], tuple(weight.shape[2:]), stride, pad, dil, groups) \
+            and _krsc(weight):
+        return _DwConvBnAct.apply(x, residual, weight, gamma, beta, running_mean, running_var, stride, eps, momentum,
+                                  act, training)
     if use_native(x) and native.supports_conv(x.shape[1], weight.shape[0]) \
             and (groups == 1 or native.supports_grouped(x.shape[1], weight.shape[0], groups)) \
             and native.bn_supported(weight.shape[0]) and _krsc(weight):
         return _ConvBnAct.apply(x, residual, weight, gamma, beta, running_mean, running_var, stride, pad, dil, eps,
-                                momentum, relu, training, groups)
+                                momentum, act, training, groups)
     xi = x[:, : weight.shape[1]] if (x.shape[1] != weight.shape[1] and groups == 1) else x   # NHWC4 stem input
     y = F.conv2d(xi.to(weight.dtype) if not x.is_cuda else xi, weight.to(xi.dtype) if x.is_cuda else weight, None,
                  stride, pad, dil, groups)
     z = F.batch_norm(y.float(), running_mean, running_var, gamma, beta, training, momentum, eps).to(y.dtype)
     if residual is not None:
         z = z + residual
+    if relu6:
+        return F.relu6(z)
     return F.relu(z) if relu else z
+
+
+# ------------------------------------------------------------------------------------------------
+# depthwise 3x3 conv + BN(train/eval) + ReLU / ReLU6 (+ residual)  (MobileNetV2)
+# ------------------------------------------------------------------------------------------------
+class _DwConvBnAct(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, residual, weight, gamma, beta, running_mean, running_var, stride, eps, momentum, relu, train):
+        wb = weight_bf16(weight, groups=weight.shape[0])          # [C, 9]
+        y, stats = native.dwconv_fwd(x, wb, stride, stats=True) if train else (native.dwconv_fwd(x, wb, stride), None)
+        z, save = native.bn_act_fwd(y, stats, gamma, beta, running_mean, running_var, eps, momentum, relu, residual,
+                                    train)
+        ctx.cfg = (stride, relu, residual is not None)
+        ctx.params = (weight, gamma, beta)
+        if train:
+            ctx.wb = wb       # view of the bf16 weight arena: see _ConvBnAct
+            ctx.save_for_backward(x, y, z, save)
+        return z
+
+    @staticmethod
+    def backward(ctx, dz):
+        stride, relu, has_res = ctx.cfg
+        weight, gamma, beta = ctx.params
+        x, y, z, save = ctx.saved_tensors
+        if not dz.is_contiguous(memory_format=CL):
+            dz = dz.contiguous(memory_format=CL)
+        gg = grad_buffer(gamma) if gamma.requires_grad else None
+        bg = grad_buffer(beta) if beta.requires_grad else None
+        dy, dres, _ = native.bn_act_bwd(dz, z, y, save, gamma, relu, has_res and ctx.needs_input_grad[1], gg, bg,
+                                        beta=beta, had_residual=has_res)
+        dx = native.dwconv_dgrad(dy, ctx.wb, x.shape, stride) if ctx.needs_input_grad[0] else None
+        if weight.requires_grad:
+            gw = grad_buffer(weight)
+            run_wgrad(weight, lambda: native.dwconv_wgrad(x, dy, gw, stride), x, dy)
+        for p in (gamma, beta, weight):       # LAST, as in _ConvBnAct
+            if p.requires_grad:
+                notify_ready(p)
+        return (dx, dres) + (None,) * 10
 
 
 # ------------------------------------------------------------------------------------------------
@@ -316,12 +363,15 @@ class _BnAct(torch.autograd.Function):
         return (dx if ctx.needs_input_grad[0] else None,) + (None,) * 8
 
 
-def batch_norm_act(x, gamma, beta, running_mean, running_var, eps=1e-5, momentum=0.1, relu=True, training=True):
-    """z = act(BN(x)) with the batch statistics reduced by the native channel_stats kernel."""
+def batch_norm_act(x, gamma, beta, running_mean, running_var, eps=1e-5, momentum=0.1, relu=True, training=True,
+                   relu6=False):
+    """z = act(BN(x)) with the batch statistics reduced by the native channel_stats kernel (``relu6``: ReLU6)."""
     if use_native(x) and x.dim() == 4 and x.dtype == torch.bfloat16 and native.bn_supported(x.shape[1]) \
             and (training or not torch.is_grad_enabled()):
-        return _BnAct.apply(x, gamma, beta, running_mean, running_var, eps, momentum, relu, training)
+        return _BnAct.apply(x, gamma, beta, running_mean, running_var, eps, momentum, 2 if relu6 else relu, training)
     z = F.batch_norm(x.float(), running_mean, running_var, gamma, beta, training, momentum, eps).to(x.dtype)
+    if relu6:
+        return F.relu6(z)
     return F.relu(z) if relu else z
 
 

@@ -351,6 +351,76 @@ def supports_grouped(cin: int, cout: int, groups: int) -> bool:
     return 64 % cg == 0 and cg % 4 == 0
 
 
+def supports_depthwise(c: int, kernel, stride: int, pad, dil: int, groups: int) -> bool:
+    """Depthwise convolutions the stencil kernels of csrc/ops/depthwise.cu handle: ``groups == Cin == Cout = c`` with
+    ``c % 8 == 0``, a 3x3 kernel, stride 1 or 2, padding 1 and dilation 1 (MobileNetV2's depthwise layers)."""
+    k = (kernel, kernel) if isinstance(kernel, int) else tuple(kernel)
+    return (groups == c and c > 0 and c % 8 == 0 and k == (3, 3) and stride in (1, 2) and _pad2(pad) == (1, 1)
+            and dil == 1)
+
+
+def _check_dw(c: int, w_bf16: torch.Tensor, stride: int) -> None:
+    if not supports_depthwise(c, (3, 3), stride, 1, 1, c):
+        raise ValueError(f"depthwise conv with {c} channels, stride {stride} is not supported by the native kernels")
+    if w_bf16.dtype != torch.bfloat16 or w_bf16.numel() != c * 9 or not w_bf16.is_contiguous() \
+            or w_bf16.device.type != "cuda":
+        raise ValueError("depthwise conv: expected contiguous CUDA bf16 weights [C, 9] (KRSC of [C, 1, 3, 3])")
+
+
+def _check_aligned(t: torch.Tensor, name: str) -> None:
+    if t.data_ptr() % 16 != 0:
+        raise ValueError(f"{name}: the depthwise kernels need 16-byte aligned activations")
+
+
+def dwconv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, stride: int, stats: bool = False):
+    """Depthwise 3x3 convolution, padding 1: y[n, c] = conv(x[n, c], w[c]).  ``w_bf16``: [C, 9] bf16.  With ``stats``
+    also the per-channel (sum, sumsq) of the bf16 y as fp32 [2, C] (same contract as ``conv_fwd(stats=True)``)."""
+    _check_act(x)
+    N, Ch, H, W = x.shape
+    _check_dw(Ch, w_bf16, stride)
+    _check_aligned(x, "x")
+    P, Q = conv_out_hw(H, W, (3, 3), stride, 1)
+    y = empty_act(N, Ch, P, Q, x.device)
+    st = zeros_f32((2, Ch), x.device) if stats else None
+    _C().dwconv_fwd(x.data_ptr(), w_bf16.data_ptr(), y.data_ptr(), st[0].data_ptr() if stats else 0,
+                    st[1].data_ptr() if stats else 0, N, H, W, Ch, P, Q, stride, sm_count(x.device.index or 0), _stream())
+    return (y, st) if stats else y
+
+
+def dwconv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, stride: int) -> torch.Tensor:
+    """dx = conv_transpose(dy, w) of :func:`dwconv_fwd` (every element written once)."""
+    _check_act(dy, "dy")
+    N, Ch, H, W = x_shape
+    _check_dw(Ch, w_bf16, stride)
+    _check_aligned(dy, "dy")
+    P, Q = conv_out_hw(H, W, (3, 3), stride, 1)
+    if tuple(dy.shape) != (N, Ch, P, Q):
+        raise ValueError(f"dwconv_dgrad: dy has shape {tuple(dy.shape)}, expected {(N, Ch, P, Q)}")
+    dx = empty_act(N, Ch, H, W, dy.device)
+    _C().dwconv_dgrad(dy.data_ptr(), w_bf16.data_ptr(), dx.data_ptr(), N, H, W, Ch, P, Q, stride,
+                      sm_count(dy.device.index or 0), _stream())
+    return dx
+
+
+def dwconv_wgrad(x: torch.Tensor, dy: torch.Tensor, grad_w: torch.Tensor, stride: int) -> None:
+    """grad_w[C][3][3] (fp32, KRSC of [C, 1, 3, 3]) += the weight gradient of :func:`dwconv_fwd`."""
+    _check_act(x)
+    _check_act(dy, "dy")
+    N, Ch, H, W = x.shape
+    if not supports_depthwise(Ch, (3, 3), stride, 1, 1, Ch):
+        raise ValueError(f"depthwise conv with {Ch} channels, stride {stride} is not supported by the native kernels")
+    _check_aligned(x, "x")
+    _check_aligned(dy, "dy")
+    P, Q = conv_out_hw(H, W, (3, 3), stride, 1)
+    if tuple(dy.shape) != (N, Ch, P, Q):
+        raise ValueError(f"dwconv_wgrad: dy has shape {tuple(dy.shape)}, expected {(N, Ch, P, Q)}")
+    if grad_w.dtype != torch.float32 or grad_w.numel() != Ch * 9 or not grad_w.is_contiguous(memory_format=CL) \
+            or not grad_w.is_cuda:
+        raise ValueError("dwconv_wgrad: grad_w must be a CUDA fp32 [C, 1, 3, 3] (KRSC) tensor")
+    _C().dwconv_wgrad(x.data_ptr(), dy.data_ptr(), grad_w.data_ptr(), N, H, W, Ch, P, Q, stride,
+                      sm_count(x.device.index or 0), _stream())
+
+
 def expand_grouped_weight(w_bf16: torch.Tensor, taps: int, groups: int) -> torch.Tensor:
     """Compact grouped weights ``[Cout, taps * cg]`` bf16 (KRSC of ``[Cout, cg, R, S]``) -> the block-diagonal operand
     ``[Cout, taps * 64]`` of the grouped kernels: row ``co`` holds its ``cg`` input channels of each tap at columns
@@ -790,9 +860,12 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
                eps: float, momentum: float, relu: bool, residual: Optional[torch.Tensor], train: bool,
                want_mask: bool = False):
     """z = act(BN(y) [+ residual]).  Returns (z, save) — with ``want_mask`` (train + ReLU) (z, save, mask): one bit per
-    element telling whether z > 0, which lets the backward of residual layers skip reading z (16x less mask traffic)."""
+    element telling whether z > 0, which lets the backward of residual layers skip reading z (16x less mask traffic).
+    ``relu``: False / True, or 2 for ReLU6 (clamp to [0, 6]; not with ``want_mask``)."""
     C = _C()
     _check_act(y, "y")
+    if int(relu) == 2 and want_mask:
+        raise ValueError("bn_act_fwd: ReLU6 has no bit-mask variant")
     N, Ch, H, W = y.shape
     M = N * H * W
     z = torch.empty_like(y)
@@ -808,7 +881,7 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
         zq = slot = None
         key = ("act", gamma.data_ptr(), N, H, W)
         # emit the e4m3 twin only when an fp8 convolution consumed this layer's output in an earlier step
-        twin = _fp8.enabled() and Ch % 128 == 0 and M >= 2048 and _fp8.note_producer(z, key)
+        twin = _fp8.enabled() and int(relu) != 2 and Ch % 128 == 0 and M >= 2048 and _fp8.note_producer(z, key)
         if twin:
             idx, fused = _fp8.producer_slot(key, y.device, z)
             if fused:       # the e4m3 twin rides in this kernel's pass (+1 B/element) instead of a 3 B/element pass
@@ -851,11 +924,14 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
         raise ValueError("pre_reduced sums are only defined for BN+ReLU layers (mask from y or from the bit mask)")
     if relu and not mask_from_x and zmask is None and z is None:
         raise ValueError("bn_act_bwd: need z or zmask for the ReLU mask of a residual layer")
+    if int(relu) == 2 and not mask_from_x and zmask is not None:
+        raise ValueError("bn_act_bwd: ReLU6 has no bit-mask variant (pass z)")
     from . import fp8 as _fp8
 
     dyq = slot = None
     key = ("grad", gamma.data_ptr(), N, H, W)
-    twin = _fp8.enabled() and Ch % 128 == 0 and M >= 2048 and _fp8.note_producer(dy, key)   # an fp8 dgrad consumed it before
+    twin = _fp8.enabled() and int(relu) != 2 and Ch % 128 == 0 and M >= 2048 and \
+        _fp8.note_producer(dy, key)                               # an fp8 dgrad consumed it before
     if twin:
         idx, fused = _fp8.producer_slot(key, y.device, dy, e5m2=True)
         if fused:

@@ -1,0 +1,104 @@
+#!/usr/bin/env python
+"""Per-layer timing of MobileNetV2's depthwise 3x3 convolutions: native stencil kernels (forward with BN statistics,
+data gradient, weight gradient) against cuDNN's bf16 channels_last F.conv2d(groups=C) and aten.convolution_backward.
+CUDA events, L2 flushed before every run, median of --iters runs.
+
+A depthwise 3x3 is bound by HBM bandwidth, so each row also gives the achieved bandwidth from the bytes the pass must
+move (forward: read x, write y; data gradient: read dy, write dx; weight gradient: read x and dy) and its fraction of
+the H100 SXM data sheet's 3.35 TB/s.  The card's name, power limit and maximum SM clock are printed with the table.
+
+    python tools/depthwise_bench.py [--batch 256] [--iters 20]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+# (C, H=W of the input, stride, layers of MobileNetV2 with this shape)
+SHAPES = [(32, 112, 1, 1), (96, 112, 2, 1), (144, 56, 1, 1), (144, 56, 2, 1), (192, 28, 1, 2), (192, 28, 2, 1),
+          (384, 14, 1, 4), (576, 14, 1, 2), (576, 14, 2, 1), (960, 7, 1, 3)]
+HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
+
+
+def timed(fn, iters, flush):
+    import torch
+
+    fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(iters):
+        flush.zero_()                         # evict the operands from L2 (50 MB on H100; 256 MB buffer)
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        b.synchronize()
+        ts.append(a.elapsed_time(b) * 1e3)
+    ts.sort()
+    return ts[len(ts) // 2]
+
+
+def card():
+    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "nvidia-smi unavailable"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--iters", type=int, default=20)
+    a = ap.parse_args()
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    if not torch.cuda.is_available():
+        raise SystemExit("depthwise_bench.py needs a GPU")
+    torch.backends.cudnn.benchmark = True
+    dev = torch.device("cuda")
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    info = card()
+    print(f"# {info} (name, power.limit, clocks.max.sm); batch {a.batch}, median of {a.iters} (us); GB/s from the "
+          f"bytes each pass must move; % of {HBM_BYTES_PER_S / 1e12:.2f} TB/s (bandwidth-bound)")
+    print(f"{'C':>4} {'HW':>3} {'s':>1} {'n':>1} | {'fwd':>7} {'cudnn':>7} {'GB/s':>5} {'%':>3} | {'dgrad':>7} {'cudnn':>7} "
+          f"{'GB/s':>5} {'%':>3} | {'wgrad':>7} {'cudnn':>7} {'GB/s':>5} {'%':>3}")
+    rows = []
+    for C, hw, s, n in SHAPES:
+        x = torch.randn(a.batch, C, hw, hw, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+        w = (torch.randn(C, 1, 3, 3, device=dev) * 0.3).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+        wb = w.reshape(C, 9).contiguous()
+        y = nv.dwconv_fwd(x, wb, s)
+        dy = torch.randn_like(y)
+        gw = torch.zeros(C, 1, 3, 3, device=dev).contiguous(memory_format=torch.channels_last)
+        bx, by = x.numel() * 2, y.numel() * 2
+        r = {"C": C, "HW": hw, "stride": s, "layers": n, "bytes_fwd": bx + by, "bytes_dgrad": by + bx,
+             "bytes_wgrad": bx + by}
+        r["fwd"] = timed(lambda: nv.dwconv_fwd(x, wb, s, stats=True), a.iters, flush)
+        r["fwd_cudnn"] = timed(lambda: F.conv2d(x, w, None, s, 1, 1, C), a.iters, flush)
+        r["dgrad"] = timed(lambda: nv.dwconv_dgrad(dy, wb, x.shape, s), a.iters, flush)
+        r["dgrad_cudnn"] = timed(lambda: torch.ops.aten.convolution_backward(
+            dy, x, w, None, [s, s], [1, 1], [1, 1], False, [0, 0], C, [True, False, False]), a.iters, flush)
+        r["wgrad"] = timed(lambda: nv.dwconv_wgrad(x, dy, gw, s), a.iters, flush)
+        r["wgrad_cudnn"] = timed(lambda: torch.ops.aten.convolution_backward(
+            dy, x, w, None, [s, s], [1, 1], [1, 1], False, [0, 0], C, [False, True, False]), a.iters, flush)
+        cells = []
+        for k in ("fwd", "dgrad", "wgrad"):
+            gbs = r[f"bytes_{k}"] / (r[k] * 1e-6) / 1e9
+            r[f"{k}_GBps"] = gbs
+            r[f"{k}_frac_peak"] = gbs * 1e9 / HBM_BYTES_PER_S
+            cells.append(f"{r[k]:7.1f} {r[k + '_cudnn']:7.1f} {gbs:5.0f} {100 * r[k + '_frac_peak']:3.0f}")
+        rows.append(r)
+        print(f"{C:4d} {hw:3d} {s:1d} {n:1d} | " + " | ".join(cells), flush=True)
+    tot = {k: sum(r[k] * r["layers"] for r in rows)
+           for k in ("fwd", "fwd_cudnn", "dgrad", "dgrad_cudnn", "wgrad", "wgrad_cudnn")}
+    print("all 17 layers (us): " + "  ".join(f"{k}={v:.0f}" for k, v in tot.items()))
+    print("JSON " + json.dumps({"device": info, "batch": a.batch, "rows": rows, "totals_us": tot}))
+
+
+if __name__ == "__main__":
+    sys.exit(main())
