@@ -373,27 +373,48 @@ PYBIND11_MODULE(_C, m) {
                                   P<const uint8_t>(argmax), sms, S(stream)), "bn_pool_bwd");
   });
   // ------------------------------------------------------------------ depthwise 3x3 convolution
+  // k: the kernel size, 3 (padding 1, depthwise.cu) or 5 (padding 2, depthwise5.cu)
   m.def("dwconv_fwd", [](ptr_t x, ptr_t w, ptr_t y, ptr_t sum, ptr_t sumsq, int N, int H, int W, int C, int Pq, int Q,
-                         int stride, int sms, ptr_t stream) {
+                         int stride, int sms, ptr_t stream, int k) {
     ddl::DwConvArgs a{};
     a.x = P<const __nv_bfloat16>(x); a.w = P<const __nv_bfloat16>(w); a.y = P<__nv_bfloat16>(y);
     a.sum = P<float>(sum); a.sumsq = P<float>(sumsq);
     a.N = N; a.H = H; a.W = W; a.C = C; a.P = Pq; a.Q = Q; a.stride = stride;
-    check(ddl::launch_dwconv_fwd(a, sms, S(stream)), "dwconv_fwd");
-  });
+    check(k == 3 ? ddl::launch_dwconv_fwd(a, sms, S(stream))
+                 : k == 5 ? ddl::launch_dwconv5_fwd(a, sms, S(stream)) : cudaErrorInvalidValue, "dwconv_fwd");
+  }, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("sum"), py::arg("sumsq"), py::arg("N"), py::arg("H"), py::arg("W"),
+     py::arg("C"), py::arg("P"), py::arg("Q"), py::arg("stride"), py::arg("sms"), py::arg("stream"), py::arg("k") = 3);
   m.def("dwconv_dgrad", [](ptr_t dy, ptr_t w, ptr_t dx, int N, int H, int W, int C, int Pq, int Q, int stride, int sms,
-                           ptr_t stream) {
+                           ptr_t stream, int k) {
     ddl::DwConvArgs a{};
     a.dy = P<const __nv_bfloat16>(dy); a.w = P<const __nv_bfloat16>(w); a.y = P<__nv_bfloat16>(dx);
     a.N = N; a.H = H; a.W = W; a.C = C; a.P = Pq; a.Q = Q; a.stride = stride;
-    check(ddl::launch_dwconv_dgrad(a, sms, S(stream)), "dwconv_dgrad");
-  });
+    check(k == 3 ? ddl::launch_dwconv_dgrad(a, sms, S(stream))
+                 : k == 5 ? ddl::launch_dwconv5_dgrad(a, sms, S(stream)) : cudaErrorInvalidValue, "dwconv_dgrad");
+  }, py::arg("dy"), py::arg("w"), py::arg("dx"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("C"), py::arg("P"),
+     py::arg("Q"), py::arg("stride"), py::arg("sms"), py::arg("stream"), py::arg("k") = 3);
   m.def("dwconv_wgrad", [](ptr_t x, ptr_t dy, ptr_t gw, int N, int H, int W, int C, int Pq, int Q, int stride, int sms,
-                           ptr_t stream) {
+                           ptr_t stream, int k) {
     ddl::DwConvArgs a{};
     a.x = P<const __nv_bfloat16>(x); a.dy = P<const __nv_bfloat16>(dy); a.gw = P<float>(gw);
     a.N = N; a.H = H; a.W = W; a.C = C; a.P = Pq; a.Q = Q; a.stride = stride;
-    check(ddl::launch_dwconv_wgrad(a, sms, S(stream)), "dwconv_wgrad");
+    check(k == 3 ? ddl::launch_dwconv_wgrad(a, sms, S(stream))
+                 : k == 5 ? ddl::launch_dwconv5_wgrad(a, sms, S(stream)) : cudaErrorInvalidValue, "dwconv_wgrad");
+  }, py::arg("x"), py::arg("dy"), py::arg("gw"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("C"), py::arg("P"),
+     py::arg("Q"), py::arg("stride"), py::arg("sms"), py::arg("stream"), py::arg("k") = 3);
+  // ------------------------------------------------------------------ squeeze-excitation
+  m.def("se_scale", [](ptr_t x, ptr_t s, int lds, ptr_t y, int N, int HW, int C, int sms, ptr_t stream) {
+    check(ddl::launch_se_scale(P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(s), lds, P<__nv_bfloat16>(y), N, HW, C,
+                               sms, S(stream)), "se_scale");
+  });
+  m.def("se_reduce", [](ptr_t dy, ptr_t x, ptr_t s, int lds, ptr_t ds, int ldd, int N, int HW, int C, ptr_t stream) {
+    check(ddl::launch_se_reduce(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(s), lds,
+                                P<__nv_bfloat16>(ds), ldd, N, HW, C, S(stream)), "se_reduce");
+  });
+  m.def("se_apply", [](ptr_t dy, ptr_t s, int lds, ptr_t dpooled, ptr_t dx, int N, int HW, int C, int sms,
+                       ptr_t stream) {
+    check(ddl::launch_se_apply(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(s), lds, P<const __nv_bfloat16>(dpooled),
+                               P<__nv_bfloat16>(dx), N, HW, C, sms, S(stream)), "se_apply");
   });
   m.def("channel_stats", [](ptr_t x, ptr_t sum, ptr_t sumsq, int M, int C, int sms, ptr_t stream) {
     check(ddl::launch_channel_stats(P<const __nv_bfloat16>(x), P<float>(sum), P<float>(sumsq), M, C, sms, S(stream)),
@@ -521,6 +542,13 @@ PYBIND11_MODULE(_C, m) {
     }
     a.whole = P<__nv_bfloat16>(whole); a.M = M;
     check(ddl::launch_concat_channels(a, scatter, S(stream)), "concat_channels");
+  });
+  m.def("hardswish_fwd", [](ptr_t x, ptr_t y, int64_t n, ptr_t stream) {
+    check(ddl::launch_hardswish_fwd(P<const __nv_bfloat16>(x), P<__nv_bfloat16>(y), n, S(stream)), "hardswish_fwd");
+  });
+  m.def("hardswish_bwd", [](ptr_t dy, ptr_t x, ptr_t dx, int64_t n, ptr_t stream) {
+    check(ddl::launch_hardswish_bwd(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(x), P<__nv_bfloat16>(dx), n,
+                                    S(stream)), "hardswish_bwd");
   });
   m.def("add_bf16", [](ptr_t a, ptr_t b, ptr_t y, int64_t n, ptr_t stream) {
     check(ddl::launch_add_bf16(P<const __nv_bfloat16>(a), P<const __nv_bfloat16>(b), P<__nv_bfloat16>(y), n,

@@ -12,6 +12,9 @@
 //   ReLU6 (relu == 2, MobileNetV2): z = min(max(v, 0), 6) and the gradient passes where 0 < v < 6 (PyTorch's hardtanh
 //   backward), v being z or the recomputed pre-activation.  Its own template instantiations, so that the ReLU
 //   kernels of the ResNet path keep their code and registers; not combined with the residual bit mask.
+//   Hardswish (relu == 3, MobileNetV3): z = v * clamp(v + 3, 0, 6) / 6; the gradient is dz * (0 for v <= -3,
+//   v / 3 + 1/2 for -3 < v < 3, 1 for v >= 3), v recomputed from x (mask-from-x mode only).  Its own forward kernel
+//   (bn_hswish_fwd_kernel, sharing the body) and backward mask value; no residual, bit mask or fp8 twin.
 //
 // Thread mapping: a thread owns 8 consecutive channels (one 16-byte vector) of a FIXED channel
 // group and walks rows with a grid stride, so per-channel constants live in registers.  The loops
@@ -26,14 +29,23 @@ namespace ddl {
 namespace {
 
 constexpr int kBnThreads = 256;
-enum { kMaskNone = 0, kMaskZ = 1, kMaskX = 2, kMaskBits = 3, kMaskZ6 = 4, kMaskX6 = 5 };
+enum { kMaskNone = 0, kMaskZ = 1, kMaskX = 2, kMaskBits = 3, kMaskZ6 = 4, kMaskX6 = 5, kMaskXH = 6 };
 constexpr bool mask_from_z(int m) { return m == kMaskZ || m == kMaskZ6; }
-constexpr bool mask_from_x(int m) { return m == kMaskX || m == kMaskX6; }
+constexpr bool mask_from_x(int m) { return m == kMaskX || m == kMaskX6 || m == kMaskXH; }
 // whether the gradient passes the activation at pre-activation (or output) value v
 template <int MASK>
 DDL_DEVICE bool act_passes(float v) {
   return (MASK == kMaskZ6 || MASK == kMaskX6) ? (v > 0.f && v < 6.f) : v > 0.f;
 }
+// the gradient dz of the activation's output as a gradient of its input, at pre-activation value v
+template <int MASK>
+DDL_DEVICE float act_bwd(float v, float dz) {
+  if (MASK == kMaskXH) return v <= -3.f ? 0.f : (v >= 3.f ? dz : dz * fmaf(v, 1.f / 3.f, 0.5f));
+  return act_passes<MASK>(v) ? dz : 0.f;
+}
+// forward activations of bn_act_fwd_body
+enum { kActRelu = 0, kActRelu6 = 1, kActHswish = 2 };
+DDL_DEVICE float hardswish(float v) { return v * fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f); }
 
 struct Vec8 {
   float v[8];
@@ -97,8 +109,9 @@ DDL_DEVICE void fp8_fold_amax(Fp8Slot* slot, float amax) {
   }
 }
 
-template <bool TRAIN, bool CHUNKED, bool FP8, bool RELU6>
-__global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) {
+// ACT: kActRelu (ReLU when a.relu, else none), kActRelu6 (when a.relu) or kActHswish (always)
+template <bool TRAIN, bool CHUNKED, bool FP8, int ACT>
+DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
   pdl_trigger();
   pdl_wait();      // nothing to prepare here: the gain is the launch latency and the block ramp-up
   int c0, row0, row_stride;
@@ -151,7 +164,10 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) 
 #pragma unroll
       for (int i = 0; i < 8; ++i) z[i] = fmaf(x[i], scale[i], shift[i]);
     }
-    if (a.relu) {
+    if (ACT == kActHswish) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) z[i] = hardswish(z[i]);
+    } else if (a.relu) {
       if (a.mask) {
         uint32_t bits = 0;
 #pragma unroll
@@ -159,7 +175,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) 
         a.mask[off >> 3] = static_cast<uint8_t>(bits);
       }
 #pragma unroll
-      for (int i = 0; i < 8; ++i) z[i] = RELU6 ? fminf(fmaxf(z[i], 0.f), 6.f) : fmaxf(z[i], 0.f);
+      for (int i = 0; i < 8; ++i) z[i] = ACT == kActRelu6 ? fminf(fmaxf(z[i], 0.f), 6.f) : fmaxf(z[i], 0.f);
     }
     store8_bf16(a.z + off, z);
     if (FP8) {
@@ -191,6 +207,16 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) 
     finish(x0, r0, off0);
   }
   if (FP8) fp8_fold_amax<!CHUNKED>(a.zq_slot, amax);
+}
+
+template <bool TRAIN, bool CHUNKED, bool FP8, bool RELU6>
+__global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) {
+  bn_act_fwd_body<TRAIN, CHUNKED, FP8, RELU6 ? kActRelu6 : kActRelu>(a);
+}
+
+template <bool TRAIN, bool CHUNKED>
+__global__ void __launch_bounds__(kBnThreads, 4) bn_hswish_fwd_kernel(BnFwdArgs a) {
+  bn_act_fwd_body<TRAIN, CHUNKED, false, kActHswish>(a);
 }
 
 // ---- backward pass 1: per-channel reductions ----------------------------------------------------
@@ -230,7 +256,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
       for (int i = 0; i < 8; ++i) dz[i] = ((uz.x >> i) & 1u) ? dz[i] : 0.f;
     } else if (mask_from_x(MASK)) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) dz[i] = act_passes<MASK>(fmaf(x[i], msc[i], msh[i])) ? dz[i] : 0.f;
+      for (int i = 0; i < 8; ++i) dz[i] = act_bwd<MASK>(fmaf(x[i], msc[i], msh[i]), dz[i]);
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -243,7 +269,14 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
   const int last = a.M - 1;
   auto phys = [&](int rr) { return a.reverse ? last - rr : rr; };      // see BnBwdArgs::reverse
   int r = live ? blockIdx.x * 32 + rl : a.M;
-  for (; r + rstep < a.M; r += 2 * rstep) {
+  if constexpr (MASK == kMaskXH) {
+    // one row per iteration: the hardswish gradient keeps more values live than a mask, and two rows would spill
+    for (; r < a.M; r += rstep) {
+      const size_t off0 = static_cast<size_t>(phys(r)) * a.C + c0;
+      accumulate(ld_stream_u4(a.dz + off0), ld_stream_u4(a.x + off0), make_uint4(0, 0, 0, 0));
+    }
+  }
+  for (; MASK != kMaskXH && r + rstep < a.M; r += 2 * rstep) {
     const size_t off0 = static_cast<size_t>(phys(r)) * a.C + c0;
     const size_t off1 = static_cast<size_t>(phys(r + rstep)) * a.C + c0;
     const uint4 d0 = ld_stream_u4(a.dz + off0), d1 = ld_stream_u4(a.dz + off1);
@@ -346,7 +379,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_apply_kernel(BnBwdAr
       for (int i = 0; i < 8; ++i) dz[i] = ((bits >> i) & 1u) ? dz[i] : 0.f;
     } else if (mask_from_x(MASK)) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) dz[i] = act_passes<MASK>(fmaf(x[i], k1[i], msh[i])) ? dz[i] : 0.f;
+      for (int i = 0; i < 8; ++i) dz[i] = act_bwd<MASK>(fmaf(x[i], k1[i], msh[i]), dz[i]);
     }
     if (a.dres) store8_bf16(a.dres + off, dz);
 #pragma unroll
@@ -635,7 +668,7 @@ cudaError_t launch_bn_bwd_mask(const BnBwdArgs& a, int sms, cudaStream_t stream,
   const bool f8 = a.dxq != nullptr && a.dxq_slot != nullptr;
   const bool flat = bn_flat_ok(a.C);
   const dim3 grid = flat ? dim3(bn_grid(a.M, a.C, sms)) : rgrid;
-  if constexpr (MASK == kMaskZ6 || MASK == kMaskX6) {
+  if constexpr (MASK == kMaskZ6 || MASK == kMaskX6 || MASK == kMaskXH) {
     if (f8) return cudaErrorInvalidValue;
   } else if (f8) {
     return flat ? launch_pdl(bn_act_bwd_apply_kernel<MASK, false, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
@@ -651,6 +684,17 @@ cudaError_t launch_bn_act_fwd(const BnFwdArgs& a_in, bool train, int sms, cudaSt
   BnFwdArgs a = a_in;
   a.reverse = g_bn_reverse;
   if (a.C % 8 != 0 || a.C <= 0) return cudaErrorInvalidValue;
+  if (a.relu == 3) {           // hardswish: no residual, bit mask or fp8 twin
+    if (a.residual != nullptr || a.mask != nullptr || (a.zq != nullptr && a.zq_slot != nullptr)) return cudaErrorInvalidValue;
+    if (bn_flat_ok(a.C)) {
+      const dim3 grid(bn_grid(a.M, a.C, sms));
+      return train ? launch_pdl(bn_hswish_fwd_kernel<true, false>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                   : launch_pdl(bn_hswish_fwd_kernel<false, false>, grid, dim3(kBnThreads), 0, stream, 1, a);
+    }
+    const dim3 grid = bn_chunk_grid(a.M, a.C, sms);
+    return train ? launch_pdl(bn_hswish_fwd_kernel<true, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                 : launch_pdl(bn_hswish_fwd_kernel<false, true>, grid, dim3(kBnThreads), 0, stream, 1, a);
+  }
   if (a.relu < 0 || a.relu > 2 || (a.relu == 2 && a.mask != nullptr)) return cudaErrorInvalidValue;   // no ReLU6 bit mask
   const bool f8 = a.zq != nullptr && a.zq_slot != nullptr && train;
   const bool r6 = a.relu == 2;
@@ -668,6 +712,10 @@ cudaError_t launch_bn_act_bwd(const BnBwdArgs& a_in, int sms, cudaStream_t strea
   BnBwdArgs a = a_in;
   a.reverse = g_bn_reverse;
   if (a.C % 8 != 0 || a.C <= 0) return cudaErrorInvalidValue;
+  if (a.relu == 3) {           // hardswish: pre-activation recomputed from x only, no residual gradient
+    if (!a.mask_from_x || a.zmask != nullptr || a.dres != nullptr) return cudaErrorInvalidValue;
+    return launch_bn_bwd_mask<kMaskXH>(a, sms, stream, skip_reduce);
+  }
   if (a.relu < 0 || a.relu > 2 || (a.relu == 2 && a.zmask != nullptr)) return cudaErrorInvalidValue;   // no ReLU6 bit mask
   switch (!a.relu ? kMaskNone
                   : a.relu == 2 ? (a.mask_from_x ? kMaskX6 : kMaskZ6)

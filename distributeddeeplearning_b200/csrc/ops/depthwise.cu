@@ -5,12 +5,10 @@
 // A depthwise 3x3 is 9 multiply-adds per output element: a stencil bound by HBM bandwidth, not a GEMM (the block-
 // diagonal mode of the conv kernels would do 64x the useful MMA work at one channel per group).
 //
-// Thread mapping (all three kernels): a thread owns 8 consecutive channels (one 16-byte vector) of a fixed channel slab
-// and walks output (dgrad: input) pixels with a grid stride, so its 72 filter taps stay in registers.  A block of 256
-// threads covers `gpc` channel groups x 256/gpc pixel lanes, gpc being the largest power of two <= 8 that divides C/8:
-// every thread is live for any C % 8 == 0 (MobileNetV2 has C = 96, 144, 960), and a pixel's slab is gpc*16 contiguous
-// bytes.  blockIdx.y picks the slab.  The 3x3 windows of the neighbouring pixels of a warp overlap and the rows above
-// and below were read moments earlier, so the taps are plain L1-cached 16-byte loads: HBM sees each input about once.
+// Thread mapping (all three kernels; depthwise.cuh): a thread owns 8 consecutive channels of a fixed channel slab and
+// walks output (dgrad: input) pixels with a grid stride, so its 72 filter taps stay in registers.  The 3x3 windows of
+// the neighbouring pixels of a warp overlap and the rows above and below were read moments earlier, so the taps are
+// plain L1-cached 16-byte loads: HBM sees each input about once.
 //
 //   forward   y[n,p,q,c]  = sum_{r,s} x[n, p*st-1+r, q*st-1+s, c] * w[c][r][s]
 //   dgrad     dx[n,h,w,c] = sum of dy[n,p,q,c] * w[c][r][s] over the taps with h = p*st-1+r, w = q*st-1+s (gather:
@@ -19,33 +17,13 @@
 #include "../common.cuh"
 #include "ops.h"
 #include "../launch.h"
+#include "depthwise.cuh"
 
 namespace ddl {
 
 namespace {
 
-constexpr int kDwThreads = 256;
-constexpr int kDwWarps = kDwThreads / 32;
-
-DDL_DEVICE void dw_unpack8(const uint4& u, float (&v)[8]) {
-  float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y; v[4] = c.x; v[5] = c.y; v[6] = d.x; v[7] = d.y;
-}
-DDL_DEVICE void dw_load8(const __nv_bfloat16* p, float (&v)[8]) {
-  dw_unpack8(__ldg(reinterpret_cast<const uint4*>(p)), v);
-}
-
-// this thread's channel slab and pixel lane
-struct DwMap {
-  int c0, lane, lanes;
-};
-DDL_DEVICE DwMap dw_map(int lg) {
-  DwMap m;
-  m.c0 = (static_cast<int>(blockIdx.y) << (lg + 3)) + ((threadIdx.x & ((1 << lg) - 1)) << 3);
-  m.lane = blockIdx.x * (kDwThreads >> lg) + (threadIdx.x >> lg);
-  m.lanes = gridDim.x * (kDwThreads >> lg);
-  return m;
-}
+using namespace dw;
 
 // the 9 taps of channels [c0, c0 + 8) of the bf16 [C][9] weights (72 contiguous elements) as wt[tap][channel]
 DDL_DEVICE void dw_load_weights(const __nv_bfloat16* w, int c0, float (&wt)[9][8]) {
@@ -53,31 +31,6 @@ DDL_DEVICE void dw_load_weights(const __nv_bfloat16* w, int c0, float (&wt)[9][8
   for (int i = 0; i < 8; ++i) {
 #pragma unroll
     for (int t = 0; t < 9; ++t) wt[t][i] = __bfloat162float(w[(c0 + i) * 9 + t]);
-  }
-}
-
-// Sum v[K] over the pixel lanes of the block that share this thread's channel group (v[k] belongs to channel k % 8),
-// then hand each of the block's gpc*K totals to `emit(channel, k / 8, total)` on one thread: the caller's one atomic per
-// channel and statistic (or tap) per block.  Lanes of a warp with the same channel group differ in lane bits >= lg.
-template <int K, typename Emit>
-DDL_DEVICE void dw_block_reduce(float (&v)[K], int lg, float* red /* [kDwWarps][8][K] */, Emit emit) {
-  for (int off = 1 << lg; off < 32; off <<= 1) {
-#pragma unroll
-    for (int k = 0; k < K; ++k) v[k] += __shfl_xor_sync(0xffffffffu, v[k], off);
-  }
-  const int warp = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l < (1 << lg)) {
-#pragma unroll
-    for (int k = 0; k < K; ++k) red[(warp * 8 + l) * K + k] = v[k];
-  }
-  __syncthreads();
-  const int slab0 = static_cast<int>(blockIdx.y) << (lg + 3);
-  for (int e = threadIdx.x; e < (K << lg); e += kDwThreads) {
-    const int g = e / K, k = e - g * K;
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < kDwWarps; ++w) t += red[(w * 8 + g) * K + k];
-    emit(slab0 + g * 8 + (k & 7), k >> 3, t);
   }
 }
 
@@ -215,26 +168,6 @@ __global__ void __launch_bounds__(kDwThreads, 2) dwconv_wgrad_kernel(DwConvArgs 
   }
   __shared__ float red[kDwWarps * 8 * 72];
   dw_block_reduce<72>(acc, a.lg_gpc, red, [&](int c, int tap, float v) { atomicAdd(a.gw + c * 9 + tap, v); });
-}
-
-// largest power of two <= 8 dividing C/8, as its log2
-inline int dw_lg_gpc(int C) {
-  const int groups = C / 8;
-  int lg = 0;
-  while (lg < 3 && groups % (2 << lg) == 0) ++lg;
-  return lg;
-}
-
-// (pixel blocks, channel slabs): at least 4 pixels per thread (amortises the weight loads), at most
-// `blocks_per_sm` * SMs blocks in all
-inline dim3 dw_grid(int pixels, int C, int lg, int sms, int blocks_per_sm) {
-  const int slabs = (C / 8) >> lg;
-  const int lanes = kDwThreads >> lg;
-  long long gx = (static_cast<long long>(pixels) + 4LL * lanes - 1) / (4LL * lanes);
-  const long long cap = (static_cast<long long>(sms) * blocks_per_sm + slabs - 1) / slabs;
-  if (gx > cap) gx = cap;
-  if (gx < 1) gx = 1;
-  return dim3(static_cast<unsigned>(gx), static_cast<unsigned>(slabs));
 }
 
 bool dw_args_ok(const DwConvArgs& a) {

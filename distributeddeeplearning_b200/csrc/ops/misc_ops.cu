@@ -638,6 +638,34 @@ __global__ void __launch_bounds__(256) add_bf16_kernel(const __nv_bfloat16* __re
   }
 }
 
+// hardswish on a [B][F] activation (MobileNetV3's classifier): y = x * clamp(x + 3, 0, 6) / 6, and its backward from the
+// saved pre-activation x: dx = dy * (0 for x <= -3, x / 3 + 1/2 for -3 < x < 3, 1 for x >= 3)
+__global__ void __launch_bounds__(256) hardswish_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* y,
+                                                            int64_t n8) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    float v[8];
+    unpack8(reinterpret_cast<const uint4*>(x)[i], v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = v[k] * fminf(fmaxf(v[k] + 3.f, 0.f), 6.f) * (1.f / 6.f);
+    reinterpret_cast<uint4*>(y)[i] = pack8(v);
+  }
+}
+
+__global__ void __launch_bounds__(256) hardswish_bwd_kernel(const __nv_bfloat16* __restrict__ dy,
+                                                            const __nv_bfloat16* __restrict__ x, __nv_bfloat16* dx,
+                                                            int64_t n8) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    float d[8], v[8];
+    unpack8(reinterpret_cast<const uint4*>(dy)[i], d);
+    unpack8(reinterpret_cast<const uint4*>(x)[i], v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) d[k] = v[k] <= -3.f ? 0.f : (v[k] >= 3.f ? d[k] : d[k] * fmaf(v[k], 1.f / 3.f, 0.5f));
+    reinterpret_cast<uint4*>(dx)[i] = pack8(d);
+  }
+}
+
 inline int grid_for(int64_t work, int per_block = 256, int cap = 132 * 16) {     // 16 blocks per SM of an H100 SXM
   int64_t b = (work + per_block - 1) / per_block;
   if (b > cap) b = cap;
@@ -807,6 +835,17 @@ cudaError_t launch_dropout(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, 
                            uint64_t offset, const int64_t* step, cudaStream_t stream) {
   if (n % 8 != 0) return cudaErrorInvalidValue;
   dropout_kernel<<<grid_for(n / 8), 256, 0, stream>>>(x, y, n / 8, p, seed, offset, step);
+  return cudaGetLastError();
+}
+cudaError_t launch_hardswish_fwd(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, cudaStream_t stream) {
+  if (n % 8 != 0) return cudaErrorInvalidValue;
+  hardswish_fwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>(x, y, n / 8);
+  return cudaGetLastError();
+}
+cudaError_t launch_hardswish_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* x, __nv_bfloat16* dx, int64_t n,
+                                 cudaStream_t stream) {
+  if (n % 8 != 0) return cudaErrorInvalidValue;
+  hardswish_bwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>(dy, x, dx, n / 8);
   return cudaGetLastError();
 }
 cudaError_t launch_pad_nhwc4(const __nv_bfloat16* in, __nv_bfloat16* out, int N, int H, int W, int Hp, int Wp, int pt,

@@ -66,22 +66,26 @@ cudaError_t launch_bn_act_bwd(const BnBwdArgs& a, int sms, cudaStream_t stream, 
 cudaError_t launch_channel_stats(const __nv_bfloat16* x, float* sum, float* sumsq, int M, int C, int sms,
                                  cudaStream_t stream);
 
-// ---- depthwise 3x3 convolution (depthwise.cu) -------------------------------------------------------
-// groups == Cin == Cout = C (C % 8 == 0), 3x3, stride 1 or 2, padding 1; x [N][H][W][C], y / dy [N][P][Q][C] bf16
+// ---- depthwise convolution (depthwise.cu: 3x3, depthwise5.cu: 5x5) ----------------------------------------
+// groups == Cin == Cout = C (C % 8 == 0), k x k with k = 3 (padding 1) or 5 (padding 2), stride 1 or 2;
+// x [N][H][W][C], y / dy [N][P][Q][C] bf16
 struct DwConvArgs {
   const __nv_bfloat16* x;         // forward / wgrad input
   const __nv_bfloat16* dy;        // dgrad / wgrad output gradient
-  const __nv_bfloat16* w;         // [C][3][3] bf16
+  const __nv_bfloat16* w;         // [C][k][k] bf16
   __nv_bfloat16* y;               // forward: y;  dgrad: dx [N][H][W][C]
   float* sum;                     // forward, optional: per-channel sum / sum of squares of the bf16 y (+=, zeroed
   float* sumsq;                   //   by the caller)
-  float* gw;                      // wgrad: fp32 [C][3][3] gradient, accumulated (+=)
+  float* gw;                      // wgrad: fp32 [C][k][k] gradient, accumulated (+=)
   int N, H, W, C, P, Q, stride;
   int lg_gpc;                     // set by the launcher: log2 of the 8-channel groups per block
 };
 cudaError_t launch_dwconv_fwd(const DwConvArgs& a, int sms, cudaStream_t stream);
 cudaError_t launch_dwconv_dgrad(const DwConvArgs& a, int sms, cudaStream_t stream);
 cudaError_t launch_dwconv_wgrad(const DwConvArgs& a, int sms, cudaStream_t stream);
+cudaError_t launch_dwconv5_fwd(const DwConvArgs& a, int sms, cudaStream_t stream);
+cudaError_t launch_dwconv5_dgrad(const DwConvArgs& a, int sms, cudaStream_t stream);
+cudaError_t launch_dwconv5_wgrad(const DwConvArgs& a, int sms, cudaStream_t stream);
 
 // ---- pooling -------------------------------------------------------------------------------------
 struct PoolArgs {
@@ -148,6 +152,21 @@ cudaError_t launch_bias_relu_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* z
                                  int M, int C, int c_valid, int relu, int sms, cudaStream_t stream);
 cudaError_t launch_dropout(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, float p, uint64_t seed,
                            uint64_t offset, const int64_t* step, cudaStream_t stream);
+// hardswish on n bf16 elements (n % 8 == 0) and its backward from the saved pre-activation x
+cudaError_t launch_hardswish_fwd(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, cudaStream_t stream);
+cudaError_t launch_hardswish_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* x, __nv_bfloat16* dx, int64_t n,
+                                 cudaStream_t stream);
+// ---- squeeze-excitation (squeeze_excite.cu) -------------------------------------------------------------------
+// x / y / dy / dx [N][HW][C] bf16 (C % 8 == 0); s = fc2 output [N][lds] bf16 (pre-hardsigmoid, lds % 8 == 0)
+// y = x * hsig(s)
+cudaError_t launch_se_scale(const __nv_bfloat16* x, const __nv_bfloat16* s, int lds, __nv_bfloat16* y, int N, int HW,
+                            int C, int sms, cudaStream_t stream);
+// ds [N][ldd] = hsig'(s) * sum_hw(dy * x), columns [C, ldd) zero (ldd <= C rounded up to 64); deterministic
+cudaError_t launch_se_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* x, const __nv_bfloat16* s, int lds,
+                             __nv_bfloat16* ds, int ldd, int N, int HW, int C, cudaStream_t stream);
+// dx = dy * hsig(s) + dpooled / HW  (dpooled [N][C])
+cudaError_t launch_se_apply(const __nv_bfloat16* dy, const __nv_bfloat16* s, int lds, const __nv_bfloat16* dpooled,
+                            __nv_bfloat16* dx, int N, int HW, int C, int sms, cudaStream_t stream);
 // y = a + b (bf16)
 // NHWC4 image [N][H][W] (8-byte pixels) -> zero-bordered, G-row-interleaved [N][Hp][Wp][G][4] with the source at
 // (pt, pl): position (h, w) holds the pixels of rows h .. h+G-1.  Operand layout of the TMA-fed stem convolution

@@ -5,7 +5,7 @@ Parity: the reference resolves ``--model`` with ``getattr(torchvision.models, na
 (``imagenet_pytorch_horovod.py:383``).  North-star zoo: ResNet-50/101/152, VGG-16, Inception-v3,
 AlexNet (SURVEY.md 2.7); ResNet-18/34, the other VGG depths, DenseNet and SqueezeNet (the rest of torchvision
 0.2.1's families) are here too, and the later ResNet family members of torchvision (ResNeXt-50 32x4d, ResNeXt-101
-32x8d / 64x4d, Wide ResNet-50-2 / 101-2) and MobileNetV2.
+32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2 and MobileNetV3-Large / -Small.
 """
 from __future__ import annotations
 
@@ -13,6 +13,7 @@ from .alexnet import AlexNet, alexnet  # noqa: F401
 from .densenet import DenseNet, densenet121, densenet161, densenet169, densenet201  # noqa: F401
 from .inception import Inception3, inception_v3  # noqa: F401
 from .mobilenet import MobileNetV2, mobilenet_v2  # noqa: F401
+from .mobilenetv3 import MobileNetV3, mobilenet_v3_large, mobilenet_v3_small  # noqa: F401
 from .resnet import (ResNet, resnet18, resnet34, resnet50, resnet101, resnet152, resnext50_32x4d,  # noqa: F401
                      resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2)
 from .squeezenet import SqueezeNet, squeezenet1_0, squeezenet1_1  # noqa: F401
@@ -20,7 +21,8 @@ from .vgg import VGG, vgg11, vgg11_bn, vgg13, vgg13_bn, vgg16, vgg16_bn, vgg19, 
 
 _REGISTRY = {
     f.__name__: f
-    for f in (alexnet, densenet121, densenet161, densenet169, densenet201, squeezenet1_0, squeezenet1_1, inception_v3, mobilenet_v2, resnet18, resnet34, resnet50, resnet101, resnet152,
+    for f in (alexnet, densenet121, densenet161, densenet169, densenet201, squeezenet1_0, squeezenet1_1, inception_v3, mobilenet_v2,
+              mobilenet_v3_large, mobilenet_v3_small, resnet18, resnet34, resnet50, resnet101, resnet152,
               resnext50_32x4d, resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2, vgg11, vgg11_bn, vgg13,
               vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn)
 }

@@ -75,13 +75,15 @@ class BatchNorm2d(nn.Module):
         return f"{self.num_features}, eps={self.eps}, momentum={self.momentum}"
 
 
-def conv_bn(x, conv: Conv2d, bn: BatchNorm2d, relu=True, residual=None, relu6=False):
-    """act(BN(conv(x)) [+ residual]) through the fused op (``relu6``: the activation is ReLU6)."""
+def conv_bn(x, conv: Conv2d, bn: BatchNorm2d, relu=True, residual=None, relu6=False, hardswish=False):
+    """act(BN(conv(x)) [+ residual]) through the fused op (``relu6``: the activation is ReLU6; ``hardswish``: it is
+    hardswish)."""
     return ops.conv_bn_act(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.stride,
                            conv.padding,
                            conv.dilation, bn.eps, bn.momentum, relu, residual, bn.training,
                            **({"groups": conv.groups} if conv.groups != 1 else {}),
-                           **({"relu6": True} if relu6 else {}))
+                           **({"relu6": True} if relu6 else {}),
+                           **({"hardswish": True} if hardswish else {}))
 
 
 def conv_bn_pool(x, conv: Conv2d, bn: BatchNorm2d, kernel=3, stride=2, padding=1):

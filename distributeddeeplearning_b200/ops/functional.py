@@ -215,14 +215,17 @@ class _ConvBnAct(torch.autograd.Function):
 
 
 def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad=0, dil=1, eps=1e-5, momentum=0.1,
-                relu=True, residual=None, training=True, groups=1, relu6=False):
+                relu=True, residual=None, training=True, groups=1, relu6=False, hardswish=False):
     """z = act(BN(conv(x, weight)) [+ residual])  — the unit every ResNet/Inception layer is made of.  ``groups`` > 1:
-    grouped convolution (``weight`` is [Cout, Cin/groups, R, S]); depthwise shapes that ``native.supports_depthwise``
-    accepts run on the depthwise kernels, other shapes outside ``native.supports_grouped`` take the composite path.
-    ``relu6``: the activation is ReLU6 (clamp to [0, 6]) instead of ``relu``."""
-    act = 2 if relu6 else relu
+    grouped convolution (``weight`` is [Cout, Cin/groups, R, S]); depthwise shapes that ``native.supports_depthwise`` (3x3)
+    or ``native.supports_depthwise5`` (5x5) accept run on the depthwise kernels, other shapes outside ``native.supports_grouped`` take the composite path.
+    ``relu6``: the activation is ReLU6 (clamp to [0, 6]) instead of ``relu``; ``hardswish``: it is hardswish
+    (v * clamp(v + 3, 0, 6) / 6), which takes no ``residual``."""
+    if hardswish and (relu6 or residual is not None):
+        raise ValueError("conv_bn_act: hardswish is neither combined with relu6 nor with a residual")
+    act = 3 if hardswish else (2 if relu6 else relu)
     if use_native(x) and groups > 1 and x.shape[1] == weight.shape[0] and weight.shape[1] == 1 \
-            and native.supports_depthwise(weight.shape[0], tuple(weight.shape[2:]), stride, pad, dil, groups) \
+            and native.depthwise_native(weight.shape[0], tuple(weight.shape[2:]), stride, pad, dil, groups) \
             and _krsc(weight):
         return _DwConvBnAct.apply(x, residual, weight, gamma, beta, running_mean, running_var, stride, eps, momentum,
                                   act, training)
@@ -237,22 +240,26 @@ def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad
     z = F.batch_norm(y.float(), running_mean, running_var, gamma, beta, training, momentum, eps).to(y.dtype)
     if residual is not None:
         z = z + residual
+    if hardswish:
+        return F.hardswish(z)
     if relu6:
         return F.relu6(z)
     return F.relu(z) if relu else z
 
 
 # ------------------------------------------------------------------------------------------------
-# depthwise 3x3 conv + BN(train/eval) + ReLU / ReLU6 (+ residual)  (MobileNetV2)
+# depthwise 3x3 / 5x5 conv + BN(train/eval) + ReLU / ReLU6 / hardswish (+ residual)  (MobileNetV2 / V3)
 # ------------------------------------------------------------------------------------------------
 class _DwConvBnAct(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, weight, gamma, beta, running_mean, running_var, stride, eps, momentum, relu, train):
-        wb = weight_bf16(weight, groups=weight.shape[0])          # [C, 9]
-        y, stats = native.dwconv_fwd(x, wb, stride, stats=True) if train else (native.dwconv_fwd(x, wb, stride), None)
+        k = weight.shape[2]
+        wb = weight_bf16(weight, groups=weight.shape[0])          # [C, k*k]
+        y, stats = native.dwconv_fwd(x, wb, stride, stats=True, k=k) if train else \
+            (native.dwconv_fwd(x, wb, stride, k=k), None)
         z, save = native.bn_act_fwd(y, stats, gamma, beta, running_mean, running_var, eps, momentum, relu, residual,
                                     train)
-        ctx.cfg = (stride, relu, residual is not None)
+        ctx.cfg = (stride, relu, residual is not None, k)
         ctx.params = (weight, gamma, beta)
         if train:
             ctx.wb = wb       # view of the bf16 weight arena: see _ConvBnAct
@@ -261,7 +268,7 @@ class _DwConvBnAct(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dz):
-        stride, relu, has_res = ctx.cfg
+        stride, relu, has_res, k = ctx.cfg
         weight, gamma, beta = ctx.params
         x, y, z, save = ctx.saved_tensors
         if not dz.is_contiguous(memory_format=CL):
@@ -270,10 +277,10 @@ class _DwConvBnAct(torch.autograd.Function):
         bg = grad_buffer(beta) if beta.requires_grad else None
         dy, dres, _ = native.bn_act_bwd(dz, z, y, save, gamma, relu, has_res and ctx.needs_input_grad[1], gg, bg,
                                         beta=beta, had_residual=has_res)
-        dx = native.dwconv_dgrad(dy, ctx.wb, x.shape, stride) if ctx.needs_input_grad[0] else None
+        dx = native.dwconv_dgrad(dy, ctx.wb, x.shape, stride, k=k) if ctx.needs_input_grad[0] else None
         if weight.requires_grad:
             gw = grad_buffer(weight)
-            run_wgrad(weight, lambda: native.dwconv_wgrad(x, dy, gw, stride), x, dy)
+            run_wgrad(weight, lambda: native.dwconv_wgrad(x, dy, gw, stride, k=k), x, dy)
         for p in (gamma, beta, weight):       # LAST, as in _ConvBnAct
             if p.requires_grad:
                 notify_ready(p)
@@ -463,6 +470,100 @@ def linear(x, weight, bias=None, relu=False):
     y = F.linear(x if not x.is_cuda else x, weight.to(x.dtype) if x.is_cuda else weight,
                  (bias.to(x.dtype) if x.is_cuda else bias) if bias is not None else None)
     return F.relu(y) if relu else y
+
+
+# ------------------------------------------------------------------------------------------------
+# hardswish on [B, F] (MobileNetV3's classifier)
+# ------------------------------------------------------------------------------------------------
+class _Hardswish(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        ctx.save_for_backward(x)
+        return native.hardswish_fwd(x)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        return native.hardswish_bwd(dy.contiguous(), x)
+
+
+def hardswish(x):
+    """x * clamp(x + 3, 0, 6) / 6; the native backward recomputes the gradient from the saved input."""
+    if use_native(x) and x.dtype == torch.bfloat16 and x.is_contiguous() and x.numel() % 8 == 0:
+        return _Hardswish.apply(x)
+    return F.hardswish(x)
+
+
+# ------------------------------------------------------------------------------------------------
+# squeeze-excitation: x * hardsigmoid(fc2(relu(fc1(mean_hw(x)))))  (MobileNetV3)
+# ------------------------------------------------------------------------------------------------
+class _SqueezeExcite(torch.autograd.Function):
+    """One autograd node with a hand-scheduled backward: the gradient of x from the scale path and from the pooling
+    path are formed by one kernel (se_apply), not summed by autograd, and the gate gradient is one deterministic
+    reduction (se_reduce) written straight into the fc2 GEMM's operand layout."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, train):
+        w1b, w2b = weight_bf16(w1), weight_bf16(w2)               # [C', C], [C, C'] (the 1x1 conv weights flattened)
+        cs = w1.shape[0]
+        pooled = native.global_avgpool_fwd(x)                     # [N, C]
+        h = native.linear_fwd(pooled, w1b, b1, relu=True)         # [N, C' rounded up to 64], pad columns 0
+        hc = h[:, :cs].contiguous()                               # fc2 takes exactly C' inputs
+        s = native.linear_fwd(hc, w2b, b2)                        # [N, C rounded up to 64]: the gate logits
+        y = native.se_scale(x, s)
+        ctx.params = (w1, b1, w2, b2)
+        if train:
+            ctx.wb = (w1b, w2b)       # views of the bf16 weight arena: see _ConvBnAct
+            ctx.save_for_backward(x, pooled, h, hc, s)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        w1, b1, w2, b2 = ctx.params
+        x, pooled, h, hc, s = ctx.saved_tensors
+        w1b, w2b = ctx.wb
+        if not dy.is_contiguous(memory_format=CL):
+            dy = dy.contiguous(memory_format=CL)
+        cs, c = w1.shape[0], w1.shape[1]
+        ds = native.se_reduce(dy, x, s)                           # [N, C rounded up to 64], pad columns 0
+        db2 = grad_buffer(b2) if b2.requires_grad else None
+        if db2 is not None:
+            native.bias_relu_bwd(ds, ds, db2, False, c_valid=c)
+        dh = native.linear_dgrad(ds, w2b)                         # [N, C']
+        if w2.requires_grad:
+            native.linear_wgrad(hc, ds, grad_buffer(w2))
+        # fc1's output gradient as its GEMM operand: C' rounded up to 64 columns, the pad zero (h is 0 there, so the
+        # ReLU mask clears it too)
+        dhp = torch.zeros((dh.shape[0], h.shape[1]), dtype=dh.dtype, device=dh.device)
+        dhp[:, :cs] = dh
+        dhp = native.bias_relu_bwd(dhp, h, grad_buffer(b1) if b1.requires_grad else None, True, c_valid=cs)
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dpooled = native.linear_dgrad(dhp, w1b)               # [N, C]
+            dx = native.se_apply(dy, s, dpooled)
+        if w1.requires_grad:
+            native.linear_wgrad(pooled, dhp, grad_buffer(w1))
+        for p in (b2, w2, b1, w1):                                # LAST, as in _ConvBnAct
+            if p.requires_grad:
+                notify_ready(p)
+        return dx, None, None, None, None, None
+
+
+def squeeze_excite(x, w1, b1, w2, b2):
+    """x * hardsigmoid(fc2(relu(fc1(mean_hw(x))))) with fc1 / fc2 the 1x1 convolutions ``w1`` [C', C, 1, 1] + ``b1``
+    and ``w2`` [C, C', 1, 1] + ``b2`` (torchvision's ``SqueezeExcitation`` with a hardsigmoid scale).  Native on
+    NHWC bf16 activations with C and C' multiples of 8; the composite is the CPU path."""
+    cs, c = w1.shape[0], w1.shape[1]
+    if use_native(x) and x.dim() == 4 and x.dtype == torch.bfloat16 and x.is_contiguous(memory_format=CL) \
+            and c % 8 == 0 and cs % 8 == 0 and x.shape[1] == c:
+        train = torch.is_grad_enabled() and any(t.requires_grad for t in (x, w1, b1, w2, b2))
+        return _SqueezeExcite.apply(x, w1, b1, w2, b2, train)
+    dt = x.dtype if x.is_cuda else w1.dtype
+    xi = x.to(dt)
+    sc = xi.float().mean((2, 3), keepdim=True).to(dt) if x.is_cuda else xi.mean((2, 3), keepdim=True)
+    sc = F.relu(F.conv2d(sc, w1.to(dt), b1.to(dt)))
+    sc = F.hardsigmoid(F.conv2d(sc, w2.to(dt), b2.to(dt)))
+    return xi * sc
 
 
 # ------------------------------------------------------------------------------------------------

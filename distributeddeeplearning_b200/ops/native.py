@@ -351,20 +351,38 @@ def supports_grouped(cin: int, cout: int, groups: int) -> bool:
     return 64 % cg == 0 and cg % 4 == 0
 
 
-def supports_depthwise(c: int, kernel, stride: int, pad, dil: int, groups: int) -> bool:
-    """Depthwise convolutions the stencil kernels of csrc/ops/depthwise.cu handle: ``groups == Cin == Cout = c`` with
-    ``c % 8 == 0``, a 3x3 kernel, stride 1 or 2, padding 1 and dilation 1 (MobileNetV2's depthwise layers)."""
+def _depthwise_ok(k_want: int, c: int, kernel, stride: int, pad, dil: int, groups: int) -> bool:
     k = (kernel, kernel) if isinstance(kernel, int) else tuple(kernel)
-    return (groups == c and c > 0 and c % 8 == 0 and k == (3, 3) and stride in (1, 2) and _pad2(pad) == (1, 1)
-            and dil == 1)
+    return (groups == c and c > 0 and c % 8 == 0 and k == (k_want, k_want) and stride in (1, 2)
+            and _pad2(pad) == (k_want // 2, k_want // 2) and dil == 1)
 
 
-def _check_dw(c: int, w_bf16: torch.Tensor, stride: int) -> None:
-    if not supports_depthwise(c, (3, 3), stride, 1, 1, c):
-        raise ValueError(f"depthwise conv with {c} channels, stride {stride} is not supported by the native kernels")
-    if w_bf16.dtype != torch.bfloat16 or w_bf16.numel() != c * 9 or not w_bf16.is_contiguous() \
+def supports_depthwise(c: int, kernel, stride: int, pad, dil: int, groups: int) -> bool:
+    """Depthwise convolutions the 3x3 stencil kernels of csrc/ops/depthwise.cu handle: ``groups == Cin == Cout = c``
+    with ``c % 8 == 0``, a 3x3 kernel, stride 1 or 2, padding 1 and dilation 1 (MobileNetV2's depthwise layers and
+    MobileNetV3's 3x3 ones).  The 5x5 kernels have their own predicate, :func:`supports_depthwise5`."""
+    return _depthwise_ok(3, c, kernel, stride, pad, dil, groups)
+
+
+def supports_depthwise5(c: int, kernel, stride: int, pad, dil: int, groups: int) -> bool:
+    """Depthwise convolutions the 5x5 stencil kernels of csrc/ops/depthwise5.cu handle: ``groups == Cin == Cout = c``
+    with ``c % 8 == 0``, a 5x5 kernel, stride 1 or 2, padding 2 and dilation 1 (MobileNetV3's 5x5 layers)."""
+    return _depthwise_ok(5, c, kernel, stride, pad, dil, groups)
+
+
+def depthwise_native(c: int, kernel, stride: int, pad, dil: int, groups: int) -> bool:
+    """Whether one of the native depthwise kernel families (3x3 or 5x5) takes this convolution."""
+    return supports_depthwise(c, kernel, stride, pad, dil, groups) or \
+        supports_depthwise5(c, kernel, stride, pad, dil, groups)
+
+
+def _check_dw(c: int, w_bf16: torch.Tensor, stride: int, k: int) -> None:
+    if not depthwise_native(c, (k, k), stride, k // 2, 1, c):
+        raise ValueError(f"depthwise {k}x{k} conv with {c} channels, stride {stride} is not supported by the native "
+                         "kernels")
+    if w_bf16.dtype != torch.bfloat16 or w_bf16.numel() != c * k * k or not w_bf16.is_contiguous() \
             or w_bf16.device.type != "cuda":
-        raise ValueError("depthwise conv: expected contiguous CUDA bf16 weights [C, 9] (KRSC of [C, 1, 3, 3])")
+        raise ValueError(f"depthwise conv: expected contiguous CUDA bf16 weights [C, {k * k}] (KRSC of [C, 1, {k}, {k}])")
 
 
 def _check_aligned(t: torch.Tensor, name: str) -> None:
@@ -372,53 +390,141 @@ def _check_aligned(t: torch.Tensor, name: str) -> None:
         raise ValueError(f"{name}: the depthwise kernels need 16-byte aligned activations")
 
 
-def dwconv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, stride: int, stats: bool = False):
-    """Depthwise 3x3 convolution, padding 1: y[n, c] = conv(x[n, c], w[c]).  ``w_bf16``: [C, 9] bf16.  With ``stats``
-    also the per-channel (sum, sumsq) of the bf16 y as fp32 [2, C] (same contract as ``conv_fwd(stats=True)``)."""
+def dwconv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, stride: int, stats: bool = False, k: int = 3):
+    """Depthwise k x k convolution (k = 3 with padding 1 or k = 5 with padding 2): y[n, c] = conv(x[n, c], w[c]).
+    ``w_bf16``: [C, k*k] bf16.  With ``stats`` also the per-channel (sum, sumsq) of the bf16 y as fp32 [2, C] (same
+    contract as ``conv_fwd(stats=True)``)."""
     _check_act(x)
     N, Ch, H, W = x.shape
-    _check_dw(Ch, w_bf16, stride)
+    _check_dw(Ch, w_bf16, stride, k)
     _check_aligned(x, "x")
-    P, Q = conv_out_hw(H, W, (3, 3), stride, 1)
+    P, Q = conv_out_hw(H, W, (k, k), stride, k // 2)
     y = empty_act(N, Ch, P, Q, x.device)
     st = zeros_f32((2, Ch), x.device) if stats else None
     _C().dwconv_fwd(x.data_ptr(), w_bf16.data_ptr(), y.data_ptr(), st[0].data_ptr() if stats else 0,
-                    st[1].data_ptr() if stats else 0, N, H, W, Ch, P, Q, stride, sm_count(x.device.index or 0), _stream())
+                    st[1].data_ptr() if stats else 0, N, H, W, Ch, P, Q, stride, sm_count(x.device.index or 0), _stream(),
+                    k)
     return (y, st) if stats else y
 
 
-def dwconv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, stride: int) -> torch.Tensor:
+def dwconv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, stride: int, k: int = 3) -> torch.Tensor:
     """dx = conv_transpose(dy, w) of :func:`dwconv_fwd` (every element written once)."""
     _check_act(dy, "dy")
     N, Ch, H, W = x_shape
-    _check_dw(Ch, w_bf16, stride)
+    _check_dw(Ch, w_bf16, stride, k)
     _check_aligned(dy, "dy")
-    P, Q = conv_out_hw(H, W, (3, 3), stride, 1)
+    P, Q = conv_out_hw(H, W, (k, k), stride, k // 2)
     if tuple(dy.shape) != (N, Ch, P, Q):
         raise ValueError(f"dwconv_dgrad: dy has shape {tuple(dy.shape)}, expected {(N, Ch, P, Q)}")
     dx = empty_act(N, Ch, H, W, dy.device)
     _C().dwconv_dgrad(dy.data_ptr(), w_bf16.data_ptr(), dx.data_ptr(), N, H, W, Ch, P, Q, stride,
-                      sm_count(dy.device.index or 0), _stream())
+                      sm_count(dy.device.index or 0), _stream(), k)
     return dx
 
 
-def dwconv_wgrad(x: torch.Tensor, dy: torch.Tensor, grad_w: torch.Tensor, stride: int) -> None:
-    """grad_w[C][3][3] (fp32, KRSC of [C, 1, 3, 3]) += the weight gradient of :func:`dwconv_fwd`."""
+def dwconv_wgrad(x: torch.Tensor, dy: torch.Tensor, grad_w: torch.Tensor, stride: int, k: int = 3) -> None:
+    """grad_w[C][k][k] (fp32, KRSC of [C, 1, k, k]) += the weight gradient of :func:`dwconv_fwd`."""
     _check_act(x)
     _check_act(dy, "dy")
     N, Ch, H, W = x.shape
-    if not supports_depthwise(Ch, (3, 3), stride, 1, 1, Ch):
-        raise ValueError(f"depthwise conv with {Ch} channels, stride {stride} is not supported by the native kernels")
+    if not depthwise_native(Ch, (k, k), stride, k // 2, 1, Ch):
+        raise ValueError(f"depthwise {k}x{k} conv with {Ch} channels, stride {stride} is not supported by the native "
+                         "kernels")
     _check_aligned(x, "x")
     _check_aligned(dy, "dy")
-    P, Q = conv_out_hw(H, W, (3, 3), stride, 1)
+    P, Q = conv_out_hw(H, W, (k, k), stride, k // 2)
     if tuple(dy.shape) != (N, Ch, P, Q):
         raise ValueError(f"dwconv_wgrad: dy has shape {tuple(dy.shape)}, expected {(N, Ch, P, Q)}")
-    if grad_w.dtype != torch.float32 or grad_w.numel() != Ch * 9 or not grad_w.is_contiguous(memory_format=CL) \
+    if grad_w.dtype != torch.float32 or grad_w.numel() != Ch * k * k or not grad_w.is_contiguous(memory_format=CL) \
             or not grad_w.is_cuda:
-        raise ValueError("dwconv_wgrad: grad_w must be a CUDA fp32 [C, 1, 3, 3] (KRSC) tensor")
+        raise ValueError(f"dwconv_wgrad: grad_w must be a CUDA fp32 [C, 1, {k}, {k}] (KRSC) tensor")
     _C().dwconv_wgrad(x.data_ptr(), dy.data_ptr(), grad_w.data_ptr(), N, H, W, Ch, P, Q, stride,
-                      sm_count(x.device.index or 0), _stream())
+                      sm_count(x.device.index or 0), _stream(), k)
+
+
+# ------------------------------------------------------------------------------------------------
+# squeeze-excitation (csrc/ops/squeeze_excite.cu) and hardswish on [B, F]
+# ------------------------------------------------------------------------------------------------
+def _check_gate(s: torch.Tensor, n: int, c: int) -> None:
+    """``s``: the fc2 output [N, >= C] bf16 (row stride a multiple of 8, unit column stride)."""
+    if s.dtype != torch.bfloat16 or not s.is_cuda or s.dim() != 2 or s.shape[0] != n or s.shape[1] < c \
+            or s.stride(1) != 1 or s.stride(0) % 8 != 0 or s.stride(0) < c:
+        raise ValueError(f"squeeze-excite: expected the CUDA bf16 gate logits [N={n}, >= {c}] with a row stride that is a "
+                         "multiple of 8")
+    _check_aligned(s, "s")
+
+
+def _check_se_act(x: torch.Tensor, name: str) -> None:
+    _check_act(x, name)
+    if x.dim() != 4 or x.shape[1] % 8 != 0:
+        raise ValueError(f"{name}: squeeze-excite needs a 4-D activation with a multiple of 8 channels")
+    _check_aligned(x, name)
+
+
+def se_scale(x: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """y = x * hardsigmoid(s[n, c]) for an NHWC activation x [N, C, H, W] and the gate logits s [N, >= C]."""
+    _check_se_act(x, "x")
+    N, Ch, H, W = x.shape
+    _check_gate(s, N, Ch)
+    y = torch.empty_like(x)
+    _C().se_scale(x.data_ptr(), s.data_ptr(), s.stride(0), y.data_ptr(), N, H * W, Ch, sm_count(x.device.index or 0),
+                  _stream())
+    return y
+
+
+def se_reduce(dy: torch.Tensor, x: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """ds [N, C rounded up to 64] bf16 = hardsigmoid'(s) * sum_hw(dy * x), pad columns zero: the gradient of the gate
+    logits of :func:`se_scale`, laid out as the fc2 GEMM operand.  Deterministic (no atomics)."""
+    _check_se_act(dy, "dy")
+    _check_se_act(x, "x")
+    N, Ch, H, W = x.shape
+    if tuple(dy.shape) != tuple(x.shape):
+        raise ValueError("se_reduce: dy and x differ in shape")
+    _check_gate(s, N, Ch)
+    ldd = _ceil_div(Ch, 64) * 64
+    ds = torch.empty((N, ldd), dtype=torch.bfloat16, device=x.device)
+    _C().se_reduce(dy.data_ptr(), x.data_ptr(), s.data_ptr(), s.stride(0), ds.data_ptr(), ldd, N, H * W, Ch, _stream())
+    return ds
+
+
+def se_apply(dy: torch.Tensor, s: torch.Tensor, dpooled: torch.Tensor) -> torch.Tensor:
+    """dx = dy * hardsigmoid(s[n, c]) + dpooled[n, c] / (H*W): the input gradient of squeeze-excitation from both of its
+    paths (the scale and the pooling) in one pass."""
+    _check_se_act(dy, "dy")
+    N, Ch, H, W = dy.shape
+    _check_gate(s, N, Ch)
+    if dpooled.dtype != torch.bfloat16 or tuple(dpooled.shape) != (N, Ch) or not dpooled.is_contiguous():
+        raise ValueError(f"se_apply: expected a contiguous bf16 dpooled [{N}, {Ch}]")
+    _check_aligned(dpooled, "dpooled")
+    dx = torch.empty_like(dy)
+    _C().se_apply(dy.data_ptr(), s.data_ptr(), s.stride(0), dpooled.data_ptr(), dx.data_ptr(), N, H * W, Ch,
+                  sm_count(dy.device.index or 0), _stream())
+    return dx
+
+
+def _check_flat(t: torch.Tensor, name: str) -> None:
+    if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous() or t.numel() % 8 != 0:
+        raise ValueError(f"{name}: expected a contiguous CUDA bf16 tensor with a multiple of 8 elements")
+    _check_aligned(t, name)
+
+
+def hardswish_fwd(x: torch.Tensor) -> torch.Tensor:
+    """y = x * clamp(x + 3, 0, 6) / 6 elementwise (MobileNetV3's classifier activation)."""
+    _check_flat(x, "x")
+    y = torch.empty_like(x)
+    _C().hardswish_fwd(x.data_ptr(), y.data_ptr(), x.numel(), _stream())
+    return y
+
+
+def hardswish_bwd(dy: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+    """dx = dy * hardswish'(x), x being the saved pre-activation."""
+    _check_flat(dy, "dy")
+    _check_flat(x, "x")
+    if dy.shape != x.shape:
+        raise ValueError("hardswish_bwd: dy and x differ in shape")
+    dx = torch.empty_like(dy)
+    _C().hardswish_bwd(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), x.numel(), _stream())
+    return dx
 
 
 def expand_grouped_weight(w_bf16: torch.Tensor, taps: int, groups: int) -> torch.Tensor:
@@ -825,13 +931,15 @@ def linear_fwd(x: torch.Tensor, w_bf16: torch.Tensor, bias: Optional[torch.Tenso
 
 
 def linear_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor) -> torch.Tensor:
-    """dy [B, Npad] bf16, w [Nout, K] -> dx [B, K]."""
+    """dy [B, Npad] bf16, w [Nout, K] -> dx [B, K].  K need not be a multiple of 64 (a squeeze-excitation fc2 has
+    C/4 inputs): the N tiles cover K rounded up to 64 and the stores stop at K, as in ``conv_dgrad``."""
     C = _C()
     B, Npad = dy.shape
     Nout, K = w_bf16.shape
     dx = torch.empty((B, K), dtype=torch.bfloat16, device=dy.device)
     C.conv_gemm(C.CONV_GEMM_DGRAD, 0, dx.data_ptr(), 0, 0, 0, 0, B, Npad // 64, K, 1, 1, Npad, 1, 1, 1, 1, 1, 0,
-                1, Npad // 64, 0, K, w_bf16.data_ptr(), Nout, K, K, dy.data_ptr(), Npad, B, 0, 0, 0, 0, _stream())
+                1, Npad // 64, 0, K, w_bf16.data_ptr(), Nout, K, _ceil_div(K, 64) * 64, dy.data_ptr(), Npad, B, 0, 0, 0, 0,
+                _stream())
     return dx
 
 
@@ -861,11 +969,14 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
                want_mask: bool = False):
     """z = act(BN(y) [+ residual]).  Returns (z, save) — with ``want_mask`` (train + ReLU) (z, save, mask): one bit per
     element telling whether z > 0, which lets the backward of residual layers skip reading z (16x less mask traffic).
-    ``relu``: False / True, or 2 for ReLU6 (clamp to [0, 6]; not with ``want_mask``)."""
+    ``relu``: False / True, 2 for ReLU6 (clamp to [0, 6]; not with ``want_mask``) or 3 for hardswish
+    (x * clamp(x + 3, 0, 6) / 6; not with ``want_mask`` or ``residual``)."""
     C = _C()
     _check_act(y, "y")
     if int(relu) == 2 and want_mask:
         raise ValueError("bn_act_fwd: ReLU6 has no bit-mask variant")
+    if int(relu) == 3 and (want_mask or residual is not None):
+        raise ValueError("bn_act_fwd: hardswish takes no residual and has no bit-mask variant")
     N, Ch, H, W = y.shape
     M = N * H * W
     z = torch.empty_like(y)
@@ -881,7 +992,8 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
         zq = slot = None
         key = ("act", gamma.data_ptr(), N, H, W)
         # emit the e4m3 twin only when an fp8 convolution consumed this layer's output in an earlier step
-        twin = _fp8.enabled() and int(relu) != 2 and Ch % 128 == 0 and M >= 2048 and _fp8.note_producer(z, key)
+        twin = _fp8.enabled() and int(relu) not in (2, 3) and Ch % 128 == 0 and M >= 2048 and \
+            _fp8.note_producer(z, key)
         if twin:
             idx, fused = _fp8.producer_slot(key, y.device, z)
             if fused:       # the e4m3 twin rides in this kernel's pass (+1 B/element) instead of a 3 B/element pass
@@ -926,11 +1038,13 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
         raise ValueError("bn_act_bwd: need z or zmask for the ReLU mask of a residual layer")
     if int(relu) == 2 and not mask_from_x and zmask is not None:
         raise ValueError("bn_act_bwd: ReLU6 has no bit-mask variant (pass z)")
+    if int(relu) == 3 and (not mask_from_x or want_dres):
+        raise ValueError("bn_act_bwd: hardswish recomputes its input from y (pass beta, had_residual=False)")
     from . import fp8 as _fp8
 
     dyq = slot = None
     key = ("grad", gamma.data_ptr(), N, H, W)
-    twin = _fp8.enabled() and int(relu) != 2 and Ch % 128 == 0 and M >= 2048 and \
+    twin = _fp8.enabled() and int(relu) not in (2, 3) and Ch % 128 == 0 and M >= 2048 and \
         _fp8.note_producer(dy, key)                               # an fp8 dgrad consumed it before
     if twin:
         idx, fused = _fp8.producer_slot(key, y.device, dy, e5m2=True)

@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 
 
@@ -1552,37 +1552,38 @@ DW_CASES = sorted({(32, 112, 112, 1, 2), (96, 112, 112, 2, 2), (144, 56, 56, 1, 
                    (96, 7, 7, 1, 1), (96, 8, 8, 2, 1)})
 
 
-def _dw_layer(C, H, W, stride, n):
-    """fwd (+ BN statistics), dgrad and wgrad (accumulating onto a pre-filled slot, two passes) of one depthwise 3x3
-    conv against fp32 F.conv2d(groups=C) on the same bf16 operands, element-wise."""
+def _dw_layer(C, H, W, stride, n, k=3):
+    """fwd (+ BN statistics), dgrad and wgrad (accumulating onto a pre-filled slot, two passes) of one depthwise k x k
+    conv (padding k // 2) against fp32 F.conv2d(groups=C) on the same bf16 operands, element-wise."""
     import torch
     import torch.nn.functional as F
 
     from distributeddeeplearning_b200.ops import native as nv
 
+    pad = k // 2
     x = cl(bf(torch.randn(n, C, H, W, device="cuda")))
-    w = bf(torch.randn(C, 1, 3, 3, device="cuda") * (2.0 / 9) ** 0.5).contiguous(memory_format=torch.channels_last)
-    wb = w.reshape(C, 9).contiguous()
-    tag = f"C={C} {H}x{W} s{stride} N={n}"
-    y, st = nv.dwconv_fwd(x, wb, stride, stats=True)
-    yr = F.conv2d(x.float(), w.float(), None, stride, 1, 1, C)
+    w = bf(torch.randn(C, 1, k, k, device="cuda") * (2.0 / (k * k)) ** 0.5).contiguous(memory_format=torch.channels_last)
+    wb = w.reshape(C, k * k).contiguous()
+    tag = f"C={C} {H}x{W} s{stride} N={n}" + (f" k={k}" if k != 3 else "")
+    y, st = nv.dwconv_fwd(x, wb, stride, stats=True, k=k)
+    yr = F.conv2d(x.float(), w.float(), None, stride, pad, 1, C)
     report_abs(f"dw fwd  {tag}", y, yr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
-    y2 = nv.dwconv_fwd(x, wb, stride)
+    y2 = nv.dwconv_fwd(x, wb, stride, k=k)
     RESULTS.append(torch.equal(y, y2))
     print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] dw fwd without statistics is the same y   {tag}", flush=True)
     yb = y.float()
     report_abs(f"dw fwd sum   {tag}", st[0], yb.sum((0, 2, 3)), 2.0 ** -10, 1e-4, arms=2.0 ** -10)
     report_abs(f"dw fwd sumsq {tag}", st[1], (yb * yb).sum((0, 2, 3)), 2.0 ** -10, 1e-4, arms=2.0 ** -10)
     dy = cl(bf(torch.randn(y.shape, device="cuda")))
-    dx = nv.dwconv_dgrad(dy, wb, x.shape, stride)
-    dxr = torch.nn.grad.conv2d_input(x.shape, w.float(), dy.float(), stride, 1, 1, C)
+    dx = nv.dwconv_dgrad(dy, wb, x.shape, stride, k=k)
+    dxr = torch.nn.grad.conv2d_input(x.shape, w.float(), dy.float(), stride, pad, 1, C)
     report_abs(f"dw dgrad {tag}", dx, dxr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
-    dwr = torch.nn.grad.conv2d_weight(x.float(), w.shape, dy.float(), stride, 1, 1, C)
+    dwr = torch.nn.grad.conv2d_weight(x.float(), w.shape, dy.float(), stride, pad, 1, C)
     pre = torch.randn(w.shape, device="cuda").contiguous(memory_format=torch.channels_last)
     gw = pre.clone()
-    nv.dwconv_wgrad(x, dy, gw, stride)
+    nv.dwconv_wgrad(x, dy, gw, stride, k=k)
     report_abs(f"dw wgrad onto a filled slot {tag}", gw - pre, dwr, 2.0 ** -10, 1e-4, arms=2.0 ** -10)
-    nv.dwconv_wgrad(x, dy, gw, stride)
+    nv.dwconv_wgrad(x, dy, gw, stride, k=k)
     report_abs(f"dw wgrad two passes {tag}", gw - pre, 2 * dwr, 2.0 ** -10, 1e-4, arms=2.0 ** -10)
 
 
@@ -1926,6 +1927,299 @@ def g_mobilenet():
     RESULTS.append(ok)
     print(f"[{'ok' if ok else 'FAIL'}] mobilenet_v2 fp8 session: losses {[round(v, 3) for v in losses]}, "
           f"fp8 launches {fp8.launches()}", flush=True)
+
+
+# depthwise 5x5 layers as (C, H, W, stride, batch): every 5x5 shape of MobileNetV3-Large and -Small (batch 3) plus C = 8
+# and 40 (one 8-channel group per block), odd / non-square images, 1x1 and 2x2 images, and batch 1
+DW5_CASES = sorted({(72, 56, 56, 2, 3), (120, 28, 28, 1, 3), (672, 14, 14, 2, 3), (960, 7, 7, 1, 3),
+                    (96, 28, 28, 2, 3), (240, 14, 14, 1, 3), (120, 14, 14, 1, 3), (144, 14, 14, 1, 3),
+                    (288, 14, 14, 2, 3), (576, 7, 7, 1, 3),
+                    (8, 9, 9, 1, 2), (8, 9, 9, 2, 2), (40, 15, 11, 2, 2), (40, 13, 17, 1, 2), (16, 1, 1, 1, 3),
+                    (16, 1, 1, 2, 3), (24, 2, 2, 1, 2), (24, 2, 2, 2, 2), (96, 7, 7, 1, 1), (96, 8, 8, 2, 1)})
+
+
+def _hswish_grad(v):
+    import torch
+
+    return torch.where(v <= -3, torch.zeros_like(v), torch.where(v >= 3, torch.ones_like(v), v / 3 + 0.5))
+
+
+def _hswish_bn(C):
+    """Hardswish in the fused BN kernels: train forward (z, running statistics), eval forward, and backward with the
+    pre-activation recomputed from y, on inputs straddling -3 and 3.  The reference gradient takes the hardswish
+    derivative at the kernel's own recomputed pre-activation (the derivative jumps at -3 and 3)."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    y = cl(bf(torch.randn(4, C, 9, 9, device="cuda") * 3))
+    g = torch.rand(C, device="cuda") * 2 + 0.5
+    b = torch.randn(C, device="cuda") * 2
+    rm, rv = torch.randn(C, device="cuda") * 0.1, torch.rand(C, device="cuda") + 0.5
+    rm2, rv2 = rm.clone(), rv.clone()
+    z, save = nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.01, 3, None, True)
+    v = F.batch_norm(y.float(), rm2, rv2, g, b, True, 0.01, 1e-3)
+    report_abs(f"hardswish bn fwd C={C}", z, F.hardswish(v), 2.0 ** -7, 2.0 ** -6)
+    frac = float(((v > 3).float().mean() * (v < -3).float().mean()) ** 0.5)
+    RESULTS.append(frac > 0.02)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] hardswish inputs straddle -3 and 3 (geometric mean fraction {frac:.3f})")
+    report_abs(f"hardswish bn running_mean C={C}", rm, rm2, 2.0 ** -8, 1e-5)
+    report_abs(f"hardswish bn running_var  C={C}", rv, rv2, 2.0 ** -8, 1e-5)
+    ze, _ = nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.01, 3, None, False)
+    report_abs(f"hardswish bn eval fwd C={C}", ze, F.hardswish(F.batch_norm(y.float(), rm, rv, g, b, False, 0.01, 1e-3)),
+               2.0 ** -7, 2.0 ** -6)
+    dz = cl(bf(torch.randn(y.shape, device="cuda")))
+    gg, bg = torch.zeros(C, device="cuda"), torch.zeros(C, device="cuda")
+    dy, _, _ = nv.bn_act_bwd(dz, None, y, save, g, 3, False, gg, bg, beta=b, had_residual=False)
+    vk = y.float() * (g * save[1]).view(1, -1, 1, 1) + (b - save[0] * g * save[1]).view(1, -1, 1, 1)
+    yr = y.float().requires_grad_(True)
+    gr, br = g.clone().requires_grad_(True), b.clone().requires_grad_(True)
+    vr = F.batch_norm(yr, None, None, gr, br, True, 0.01, 1e-3)
+    (vr * _hswish_grad(vk)).backward(dz.float())
+    report_abs(f"hardswish bn bwd dx C={C}", dy, yr.grad, 2.0 ** -6, 0.0, arms=2.0 ** -7)
+    report_abs(f"hardswish bn bwd dgamma C={C}", gg, gr.grad, 2.0 ** -8, 0.0, arms=2.0 ** -8)
+    report_abs(f"hardswish bn bwd dbeta C={C}", bg, br.grad, 2.0 ** -8, 0.0, arms=2.0 ** -8)
+    refused = []
+    for kw in ({"want_mask": True}, {"residual": y}):
+        try:
+            nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.01, 3, kw.get("residual"), True, kw.get("want_mask", False))
+            refused.append(False)
+        except ValueError:
+            refused.append(True)
+    RESULTS.append(all(refused))
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] bn_act_fwd refuses hardswish with the bit mask / a residual {refused}")
+
+
+def _se_shapes(name):
+    """(C, squeeze width, H=W) of every squeeze-excitation unit of a MobileNetV3 at 224x224."""
+    from distributeddeeplearning_b200 import models
+    from distributeddeeplearning_b200.models.mobilenetv3 import ConvBNAct, SqueezeExcitation
+
+    out, hw = [], 112
+    for blk in models.get_model(name).features[1:-1]:
+        for mod in blk.block:
+            if isinstance(mod, ConvBNAct) and mod[0].groups > 1:
+                hw = (hw - 1) // mod[0].stride + 1
+            elif isinstance(mod, SqueezeExcitation):
+                out.append((mod.fc1.in_channels, mod.fc1.out_channels, hw))
+    return out
+
+
+def _se_case(C, cs, hw, n):
+    """ops.squeeze_excite on the native node against a float64 reference on the same bf16 input and weights: output,
+    input gradient and the four parameter gradients.  The hardsigmoid derivative jumps at -3 and 3 and the ReLU's at 0,
+    and the native gate logits / fc1 outputs are bf16: the reference takes both derivatives' masks from the native
+    intermediates (recomputed with the same kernels), so a logit within rounding of a jump does not flip a whole
+    (sample, channel) of the parameter gradients."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import ops
+    from distributeddeeplearning_b200.ops import native as nv
+
+    x = cl(bf(torch.randn(n, C, hw, hw, device="cuda") * 2))
+    params = [bf(torch.randn(cs, C, 1, 1, device="cuda") * C ** -0.5).float(), torch.randn(cs, device="cuda") * 0.5,
+              bf(torch.randn(C, cs, 1, 1, device="cuda") * 2 * cs ** -0.5).float(), torch.randn(C, device="cuda")]
+    pn = [p.clone().requires_grad_(True) for p in params]
+    pr = [p.double().requires_grad_(True) for p in params]
+    xn, xr = x.clone().requires_grad_(True), x.double().requires_grad_(True)
+    y = ops.squeeze_excite(xn, *pn)
+    RESULTS.append(type(y.grad_fn).__name__ == "_SqueezeExciteBackward")
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] squeeze-excite on the native node: {type(y.grad_fn).__name__}")
+    with torch.no_grad():         # the native intermediates: fc1 output (after ReLU) and the gate logits
+        h = nv.linear_fwd(nv.global_avgpool_fwd(x), bf(params[0].view(cs, C)), params[1], relu=True)
+        sn = nv.linear_fwd(h[:, :cs].contiguous(), bf(params[2].view(C, cs)), params[3])
+        mh = (h[:, :cs] > 0).double()
+        ms = ((sn[:, :C] > -3) & (sn[:, :C] < 3)).double()
+    w1, b1, w2, b2 = pr
+    hr = F.linear(xr.mean((2, 3)), w1.view(cs, C), b1) * mh
+    sr = F.linear(hr, w2.view(C, cs), b2)
+    gate = ((sr + 3).clamp(0, 6) / 6).detach() + (sr - sr.detach()) * ms / 6
+    yr = xr * gate.view(n, C, 1, 1)
+    g = cl(bf(torch.randn(y.shape, device="cuda")))
+    y.backward(g)
+    yr.backward(g.double())
+    tag = f"C={C} C'={cs} {hw}x{hw} N={n}"
+    report_abs(f"se fwd {tag}", y, yr, 2.0 ** -6, 0.0, arms=2.0 ** -7)
+    report_abs(f"se dx {tag}", xn.grad, xr.grad, 2.0 ** -6, 0.0, arms=2.0 ** -6)
+    for nm, a, b in zip(("fc1.weight", "fc1.bias", "fc2.weight", "fc2.bias"), pn, pr):
+        report_abs(f"se d{nm} {tag}", a.grad, b.grad, 2.0 ** -5, 0.0, arms=2.0 ** -5)
+
+
+def _classifier_hardswish():
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import ops
+
+    x = bf(torch.linspace(-6, 6, 256 * 1280, device="cuda").view(256, 1280))
+    x = x[torch.randperm(256, device="cuda")].contiguous()
+    xn, xr = x.clone().requires_grad_(True), x.float().requires_grad_(True)
+    y = ops.hardswish(xn)
+    RESULTS.append(type(y.grad_fn).__name__ == "_HardswishBackward")
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] classifier hardswish on the native node: {type(y.grad_fn).__name__}")
+    g = bf(torch.randn(y.shape, device="cuda"))
+    y.backward(g)
+    report_abs("classifier hardswish fwd [256, 1280]", y, F.hardswish(xr), 2.0 ** -7, 1e-6)
+    report_abs("classifier hardswish bwd [256, 1280]", xn.grad, g.float() * _hswish_grad(xr.detach()), 2.0 ** -7, 1e-6)
+
+
+def _mobilenet_v3_vs_torchvision(name, bs):
+    """A MobileNetV3 against torchvision fp32 with the same weights (and this repo's bf16 composite), under g_mobilenet's
+    bounds: the last BN gamma of every residual block starts at zero in all three nets.  Forward hooks check that every
+    depthwise layer and every squeeze-excitation unit ran on its native node."""
+    import torch
+    import torchvision
+
+    from distributeddeeplearning_b200 import models, ops
+    from distributeddeeplearning_b200.models.mobilenetv3 import ConvBNAct, InvertedResidual, SqueezeExcitation
+
+    torch.manual_seed(0)
+    m = models.get_model(name).cuda().train()
+    with torch.no_grad():
+        for mod in m.modules():
+            if isinstance(mod, InvertedResidual) and mod.use_res_connect:
+                mod.block[-1][1].weight.zero_()
+    tv = getattr(torchvision.models, name)().cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    for net in (m, tv, m2):
+        net.classifier[2].p = 0.0          # dropout masks come from different generators
+    dw, se = [], []
+    hooks = [mod.register_forward_hook(lambda mod, i, o: dw.append(type(o.grad_fn).__name__))
+             for mod in m.modules() if isinstance(mod, ConvBNAct) and mod[0].groups > 1]
+    hooks += [mod.register_forward_hook(lambda mod, i, o: se.append(type(o.grad_fn).__name__))
+              for mod in m.modules() if isinstance(mod, SqueezeExcitation)]
+    x = torch.randn(bs, 3, 224, 224, device="cuda").to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    out = m(x)
+    for h in hooks:
+        h.remove()
+    n_dw, n_se = (15, 8) if name.endswith("large") else (11, 9)
+    RESULTS.append(len(dw) == n_dw and set(dw) == {"_DwConvBnActBackward"} and len(se) == n_se
+                   and set(se) == {"_SqueezeExciteBackward"})
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name}: {len(dw)} depthwise layers, nodes {sorted(set(dw))}; "
+          f"{len(se)} squeeze-excitation units, nodes {sorted(set(se))}")
+    ops.softmax_cross_entropy(out, y, 1000).backward()
+    ro = tv(x)
+    torch.nn.functional.cross_entropy(ro, y).backward()
+    os.environ["DDL_B200_IMPL"] = "torch"
+    co = m2(x)
+    ops.softmax_cross_entropy(co, y, 1000).backward()
+    os.environ["DDL_B200_IMPL"] = "native"
+    print(f"{name} logits cos vs fp32 {_cos(out, ro):.5f}   vs bf16-composite {_cos(out, co):.5f}")
+    RESULTS.append(_cos(out, ro) > 0.98)
+    gn, gc, tvp = dict(m.named_parameters()), dict(m2.named_parameters()), dict(tv.named_parameters())
+    # as in MobileNetV2: the projection-BN betas have an analytically zero gradient, and the gamma / beta gradients of
+    # the BNs whose output feeds a depthwise conv + BN are sums dominated by cancellation; both are printed, not judged
+    zero, cancel = set(), set()
+    for i, mod in enumerate(m.features):
+        if isinstance(mod, InvertedResidual):
+            zero.add(f"features.{i}.block.{len(mod.block) - 1}.1.bias")
+            if mod.block[0][0].groups == 1:
+                cancel |= {f"features.{i}.block.0.1.weight", f"features.{i}.block.0.1.bias"}
+    cancel |= {"features.0.1.weight", "features.0.1.bias"}
+    print(f"   projection-BN beta gradients (analytically zero), max |grad| native "
+          f"{max(float(gn[k].grad.abs().max()) for k in zero):.2e}, fp32 {max(float(tvp[k].grad.abs().max()) for k in zero):.2e}")
+    cc = sorted((_cos(gn[k].grad, tvp[k].grad), _cos(gc[k].grad, tvp[k].grad), k) for k in cancel)
+    print(f"   gamma / beta of BNs feeding a depthwise layer (not judged): lowest cos native {cc[0][0]:.3f} at {cc[0][2]}, "
+          f"composite {min(c[1] for c in cc):.3f}")
+    worst, worst_c, lag = (1.0, ""), 1.0, (0.0, "")
+    for k, p in tvp.items():
+        if float(p.grad.norm()) == 0.0 or k in zero or k in cancel:
+            continue
+        c1, c2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        worst_c = min(worst_c, c2)
+        if c1 < worst[0]:
+            worst = (c1, k)
+        if c2 - c1 > lag[0]:
+            lag = (c2 - c1, k)
+    ok = worst[0] > 0.60 and lag[0] < 0.08
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at {worst[1]} "
+          f"(bf16 composite {worst_c:.4f}); largest deficit vs the bf16 composite = {lag[0]:.4f} at {lag[1]}", flush=True)
+    RESULTS.append(ok)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        oe, re_ = m(x), tv(x)
+    ce = _cos(oe, re_)
+    RESULTS.append(ce > 0.98)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} eval-mode logits cos vs torchvision eval {ce:.5f}", flush=True)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def g_mobilenet_v3():
+    """MobileNetV3: 5x5 depthwise kernels per layer shape, hardswish in the fused BN kernels, squeeze-excitation at every
+    SE shape of both models, the classifier hardswish, and both models against torchvision, eager vs CUDA-graph training
+    and an fp8 session."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.ops import native as nv
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.manual_seed(0)
+    for C, H, W, s, n in DW5_CASES:
+        _dw_layer(C, H, W, s, n, k=5)
+    bad = [nv.supports_depthwise5(*a) for a in ((32, 5, 1, 1, 1, 32), (36, 5, 1, 2, 1, 36), (32, 5, 3, 2, 1, 32),
+                                                (32, 7, 1, 3, 1, 32), (64, 5, 1, 2, 1, 16), (32, 3, 1, 1, 1, 32))]
+    RESULTS.append(not any(bad))
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] supports_depthwise5 refuses unsupported shapes {bad}", flush=True)
+    for C in (64, 120):         # flat and 64-channel-chunk thread mappings of the BN kernels
+        _hswish_bn(C)
+    for name in ("mobilenet_v3_large", "mobilenet_v3_small"):
+        for C, cs, hw in sorted(set(_se_shapes(name))):
+            _se_case(C, cs, hw, 4)
+    _classifier_hardswish()
+    for name in ("mobilenet_v3_large", "mobilenet_v3_small"):
+        _mobilenet_v3_vs_torchvision(name, 16)
+    dist.init()
+
+    def run(name, graph):
+        torch.manual_seed(0)
+        s = BenchmarkSession(name, 16, True, lr=0.01, momentum=0.9)
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out[-4:]
+
+    for name in ("mobilenet_v3_large", "mobilenet_v3_small"):
+        a, b = run(name, False), run(name, True)
+        ok = all(x == x for x in a + b) and all(abs(x - y) < 5e-2 * max(1.0, abs(x)) for x, y in zip(a, b))
+        RESULTS.append(ok)
+        print(f"[{'ok' if ok else 'FAIL'}] {name} training: eager {[round(v, 4) for v in a]} "
+              f"graph replay {[round(v, 4) for v in b]}", flush=True)
+
+    for name in ("mobilenet_v3_large", "mobilenet_v3_small"):
+        fp8.reset()
+        fp8.enable(True)
+        try:
+            torch.manual_seed(0)
+            s = BenchmarkSession(name, 16, True, lr=0.01, momentum=0.9)
+            losses = [float(s.step()) for _ in range(4)]
+            torch.cuda.synchronize()
+            s.optimizer.check_errors()
+        finally:
+            fp8.enable(False)
+        n = fp8.launches()
+        # no MobileNetV3 convolution meets the fp8 shape rules (input channels a multiple of 128): every layer stays bf16
+        ok = all(l == l and abs(l) < 1e4 for l in losses) and n["fwd"] == 0 and n["dgrad"] == 0
+        RESULTS.append(ok)
+        print(f"[{'ok' if ok else 'FAIL'}] {name} fp8 session: losses {[round(v, 3) for v in losses]}, fp8 launches {n}",
+              flush=True)
+        del s
+        torch.cuda.empty_cache()
 
 
 def run_group(name):
