@@ -156,7 +156,8 @@ KERNEL_LAUNCHES = {
     "nhwc_u8_to_nhwc4": 1, "cast_f32_bf16": 1, "pack_stem_weight": 1, "unpack_stem_grad": 1, "bias_relu_bwd": 1,
     "dropout": 1, "add_bf16": 1, "fp8_quantize": 1, "fp8_quantize_mx": 1, "fp8_transpose_taps": 1, "fp8_amax": 1, "fp8_update_scales": 1, "pad_nhwc4": 1, "expand_grouped_weight": 1, "concat_channels": 1, "bn_relu_maxpool_fwd": 1, "bn_pool_bwd": 2,
     "dwconv_fwd": 1, "dwconv_dgrad": 1, "dwconv_wgrad": 1, "se_scale": 1, "se_reduce": 1, "se_apply": 1,
-    "hardswish_fwd": 1, "hardswish_bwd": 1,
+    "hardswish_fwd": 1, "hardswish_bwd": 1, "se_sig_scale": 1, "se_sig_reduce": 1, "se_sig_apply": 1, "pad_cols_bf16": 1,
+    "fold_cols_f32": 1, "silu_rows_fwd": 1, "silu_rows_bwd": 1, "stochastic_depth_keep": 1,
 }
 LAUNCH_COUNT = [0]          # kernels of THIS repo launched so far (bench.py reports the per-region delta)
 

@@ -317,9 +317,11 @@ PYBIND11_MODULE(_C, m) {
   // ------------------------------------------------------------------ BN / activation
   m.def("bn_act_fwd", [](ptr_t x, ptr_t residual, ptr_t z, ptr_t sum, ptr_t sumsq, ptr_t gamma, ptr_t beta,
                          ptr_t mean, ptr_t invstd, ptr_t rmean, ptr_t rvar, float eps, float momentum, int M, int C,
-                         int relu, bool train, int sms, ptr_t stream, ptr_t mask, ptr_t zq, ptr_t zq_slot) {
+                         int relu, bool train, int sms, ptr_t stream, ptr_t mask, ptr_t zq, ptr_t zq_slot,
+                         ptr_t sample_scale, int hw) {
     BnFwdArgs a{};
     a.mask = P<uint8_t>(mask);
+    a.sample_scale = P<const float>(sample_scale); a.hw = hw;
     a.zq = P<uint8_t>(zq); a.zq_slot = P<ddl::Fp8Slot>(zq_slot);
     a.x = P<const __nv_bfloat16>(x); a.residual = P<const __nv_bfloat16>(residual); a.z = P<__nv_bfloat16>(z);
     a.sum = P<const float>(sum); a.sumsq = P<const float>(sumsq); a.gamma = P<const float>(gamma);
@@ -330,13 +332,14 @@ PYBIND11_MODULE(_C, m) {
   }, py::arg("x"), py::arg("residual"), py::arg("z"), py::arg("sum"), py::arg("sumsq"), py::arg("gamma"), py::arg("beta"),
      py::arg("mean"), py::arg("invstd"), py::arg("rmean"), py::arg("rvar"), py::arg("eps"), py::arg("momentum"),
      py::arg("M"), py::arg("C"), py::arg("relu"), py::arg("train"), py::arg("sms"), py::arg("stream"), py::arg("mask") = 0,
-     py::arg("zq") = 0, py::arg("zq_slot") = 0);
+     py::arg("zq") = 0, py::arg("zq_slot") = 0, py::arg("sample_scale") = 0, py::arg("hw") = 0);
   m.def("bn_act_bwd", [](ptr_t dz, ptr_t z, ptr_t x, ptr_t dx, ptr_t dres, ptr_t mean, ptr_t invstd, ptr_t gamma,
                          ptr_t beta, ptr_t dgamma, ptr_t dbeta, ptr_t gamma_grad, ptr_t beta_grad, int M, int C,
                          int relu, int mask_from_x, int sms, ptr_t stream, ptr_t zmask, bool skip_reduce, ptr_t dxq,
-                         ptr_t dxq_slot) {
+                         ptr_t dxq_slot, ptr_t sample_scale, int hw) {
     BnBwdArgs a{};
     a.zmask = P<const uint8_t>(zmask);
+    a.sample_scale = P<const float>(sample_scale); a.hw = hw;
     a.dxq = P<uint8_t>(dxq); a.dxq_slot = P<ddl::Fp8Slot>(dxq_slot);
     a.dz = P<const __nv_bfloat16>(dz); a.z = P<const __nv_bfloat16>(z); a.x = P<const __nv_bfloat16>(x);
     a.dx = P<__nv_bfloat16>(dx); a.dres = P<__nv_bfloat16>(dres); a.mean = P<const float>(mean);
@@ -347,7 +350,8 @@ PYBIND11_MODULE(_C, m) {
   }, py::arg("dz"), py::arg("z"), py::arg("x"), py::arg("dx"), py::arg("dres"), py::arg("mean"), py::arg("invstd"),
      py::arg("gamma"), py::arg("beta"), py::arg("dgamma"), py::arg("dbeta"), py::arg("gamma_grad"), py::arg("beta_grad"),
      py::arg("M"), py::arg("C"), py::arg("relu"), py::arg("mask_from_x"), py::arg("sms"), py::arg("stream"),
-     py::arg("zmask") = 0, py::arg("skip_reduce") = false, py::arg("dxq") = 0, py::arg("dxq_slot") = 0);
+     py::arg("zmask") = 0, py::arg("skip_reduce") = false, py::arg("dxq") = 0, py::arg("dxq_slot") = 0,
+     py::arg("sample_scale") = 0, py::arg("hw") = 0);
   m.def("bn_relu_maxpool_fwd", [](ptr_t x, ptr_t pooled, ptr_t argmax, ptr_t sum, ptr_t sumsq, ptr_t gamma, ptr_t beta,
                                   ptr_t mean, ptr_t invstd, ptr_t rmean, ptr_t rvar, float eps, float momentum, int N, int H,
                                   int W, int C, int Pq, int Q, int k, int stride, int pad, int sms, ptr_t stream) {
@@ -415,6 +419,40 @@ PYBIND11_MODULE(_C, m) {
                        ptr_t stream) {
     check(ddl::launch_se_apply(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(s), lds, P<const __nv_bfloat16>(dpooled),
                                P<__nv_bfloat16>(dx), N, HW, C, sms, S(stream)), "se_apply");
+  });
+  // sigmoid gate (EfficientNet): same arguments as the hardsigmoid kernels above
+  m.def("se_sig_scale", [](ptr_t x, ptr_t s, int lds, ptr_t y, int N, int HW, int C, int sms, ptr_t stream) {
+    check(ddl::launch_se_sig_scale(P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(s), lds, P<__nv_bfloat16>(y), N, HW,
+                                   C, sms, S(stream)), "se_sig_scale");
+  });
+  m.def("se_sig_reduce", [](ptr_t dy, ptr_t x, ptr_t s, int lds, ptr_t ds, int ldd, int N, int HW, int C, ptr_t stream) {
+    check(ddl::launch_se_sig_reduce(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(s), lds,
+                                    P<__nv_bfloat16>(ds), ldd, N, HW, C, S(stream)), "se_sig_reduce");
+  });
+  m.def("se_sig_apply", [](ptr_t dy, ptr_t s, int lds, ptr_t dpooled, ptr_t dx, int N, int HW, int C, int sms,
+                           ptr_t stream) {
+    check(ddl::launch_se_sig_apply(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(s), lds,
+                                   P<const __nv_bfloat16>(dpooled), P<__nv_bfloat16>(dx), N, HW, C, sms, S(stream)),
+          "se_sig_apply");
+  });
+  m.def("pad_cols_bf16", [](ptr_t src, ptr_t dst, int rows, int k, int kp, ptr_t stream) {
+    check(ddl::launch_pad_cols_bf16(P<const __nv_bfloat16>(src), P<__nv_bfloat16>(dst), rows, k, kp, S(stream)),
+          "pad_cols_bf16");
+  });
+  m.def("fold_cols_f32", [](ptr_t src, ptr_t dst, int rows, int k, int kp, ptr_t stream) {
+    check(ddl::launch_fold_cols_f32(P<const float>(src), P<float>(dst), rows, k, kp, S(stream)), "fold_cols_f32");
+  });
+  m.def("silu_rows_fwd", [](ptr_t x, int ldx, ptr_t y, int ldy, int N, ptr_t stream) {
+    check(ddl::launch_silu_rows_fwd(P<const __nv_bfloat16>(x), ldx, P<__nv_bfloat16>(y), ldy, N, S(stream)),
+          "silu_rows_fwd");
+  });
+  m.def("silu_rows_bwd", [](ptr_t dy, int ldy, ptr_t x, int ldx, ptr_t dx, int c_valid, int N, ptr_t stream) {
+    check(ddl::launch_silu_rows_bwd(P<const __nv_bfloat16>(dy), ldy, P<const __nv_bfloat16>(x), ldx, P<__nv_bfloat16>(dx),
+                                    c_valid, N, S(stream)), "silu_rows_bwd");
+  });
+  m.def("stochastic_depth_keep", [](ptr_t keep, int n, float p, uint64_t seed, uint64_t offset, ptr_t stream, ptr_t step) {
+    check(ddl::launch_stochastic_depth_keep(P<float>(keep), n, p, seed, offset, P<const int64_t>(step), S(stream)),
+          "stochastic_depth_keep");
   });
   m.def("channel_stats", [](ptr_t x, ptr_t sum, ptr_t sumsq, int M, int C, int sms, ptr_t stream) {
     check(ddl::launch_channel_stats(P<const __nv_bfloat16>(x), P<float>(sum), P<float>(sumsq), M, C, sms, S(stream)),

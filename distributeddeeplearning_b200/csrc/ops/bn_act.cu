@@ -15,6 +15,11 @@
 //   Hardswish (relu == 3, MobileNetV3): z = v * clamp(v + 3, 0, 6) / 6; the gradient is dz * (0 for v <= -3,
 //   v / 3 + 1/2 for -3 < v < 3, 1 for v >= 3), v recomputed from x (mask-from-x mode only).  Its own forward kernel
 //   (bn_hswish_fwd_kernel, sharing the body) and backward mask value; no residual, bit mask or fp8 twin.
+//   SiLU (relu == 4, EfficientNet): z = v * sigmoid(v); the gradient is dz * s * (1 + v * (1 - s)) with s = sigmoid(v),
+//   v recomputed from x.  Own forward kernel (bn_silu_fwd_kernel) and mask value; the same refusals as hardswish.
+//   Stochastic depth (sample_scale, EfficientNet's residual blocks): z = BN(x) * keep[n] + residual with one scale per
+//   sample (row / hw), no activation.  The statistics cover every sample, dropped ones included; backward feeds
+//   dz * keep[n] to the BN and returns dres = dz.  Own forward kernel (bn_sd_fwd_kernel, train only) and mask value.
 //
 // Thread mapping: a thread owns 8 consecutive channels (one 16-byte vector) of a FIXED channel
 // group and walks rows with a grid stride, so per-channel constants live in registers.  The loops
@@ -29,9 +34,14 @@ namespace ddl {
 namespace {
 
 constexpr int kBnThreads = 256;
-enum { kMaskNone = 0, kMaskZ = 1, kMaskX = 2, kMaskBits = 3, kMaskZ6 = 4, kMaskX6 = 5, kMaskXH = 6 };
+enum { kMaskNone = 0, kMaskZ = 1, kMaskX = 2, kMaskBits = 3, kMaskZ6 = 4, kMaskX6 = 5, kMaskXH = 6, kMaskXS = 7,
+       kMaskSD = 8 };
 constexpr bool mask_from_z(int m) { return m == kMaskZ || m == kMaskZ6; }
-constexpr bool mask_from_x(int m) { return m == kMaskX || m == kMaskX6 || m == kMaskXH; }
+constexpr bool mask_from_x(int m) { return m == kMaskX || m == kMaskX6 || m == kMaskXH || m == kMaskXS; }
+// sigmoid on the MUFU exp and reciprocal (__fdividef, no IEEE division: with `1.f / (...)` the SiLU backward's chunked
+// apply pass spilled at 64 registers).  Relative accuracy holds in the negative tail, where sigmoid(v) is tiny; for
+// v < -87 the denominator overflows to inf and the result is 0.
+DDL_DEVICE float sigmoid(float v) { return __fdividef(1.f, 1.f + __expf(-v)); }
 // whether the gradient passes the activation at pre-activation (or output) value v
 template <int MASK>
 DDL_DEVICE bool act_passes(float v) {
@@ -41,10 +51,14 @@ DDL_DEVICE bool act_passes(float v) {
 template <int MASK>
 DDL_DEVICE float act_bwd(float v, float dz) {
   if (MASK == kMaskXH) return v <= -3.f ? 0.f : (v >= 3.f ? dz : dz * fmaf(v, 1.f / 3.f, 0.5f));
+  if (MASK == kMaskXS) {
+    const float sg = sigmoid(v);
+    return dz * sg * fmaf(v, 1.f - sg, 1.f);
+  }
   return act_passes<MASK>(v) ? dz : 0.f;
 }
 // forward activations of bn_act_fwd_body
-enum { kActRelu = 0, kActRelu6 = 1, kActHswish = 2 };
+enum { kActRelu = 0, kActRelu6 = 1, kActHswish = 2, kActSilu = 3, kActSD = 4 };
 DDL_DEVICE float hardswish(float v) { return v * fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f); }
 
 struct Vec8 {
@@ -109,7 +123,8 @@ DDL_DEVICE void fp8_fold_amax(Fp8Slot* slot, float amax) {
   }
 }
 
-// ACT: kActRelu (ReLU when a.relu, else none), kActRelu6 (when a.relu) or kActHswish (always)
+// ACT: kActRelu (ReLU when a.relu, else none), kActRelu6 (when a.relu), kActHswish / kActSilu (always) or kActSD (no
+// activation; the BN output scaled by the row's sample scale before the residual add)
 template <bool TRAIN, bool CHUNKED, bool FP8, int ACT>
 DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
   pdl_trigger();
@@ -155,7 +170,13 @@ DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
   auto finish = [&](const uint4& ux, const uint4& ur, size_t off) {
     float x[8], z[8];
     unpack8(ux, x);
-    if (a.residual) {
+    if (ACT == kActSD) {
+      float res[8];
+      unpack8(ur, res);
+      const float ks = a.sample_scale[off / (static_cast<size_t>(a.hw) * a.C)];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) z[i] = fmaf(fmaf(x[i], scale[i], shift[i]), ks, res[i]);
+    } else if (a.residual) {
       float res[8];
       unpack8(ur, res);
 #pragma unroll
@@ -167,7 +188,10 @@ DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
     if (ACT == kActHswish) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) z[i] = hardswish(z[i]);
-    } else if (a.relu) {
+    } else if (ACT == kActSilu) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) z[i] *= sigmoid(z[i]);
+    } else if (ACT != kActSD && a.relu) {
       if (a.mask) {
         uint32_t bits = 0;
 #pragma unroll
@@ -217,6 +241,17 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_fwd_kernel(BnFwdArgs a) 
 template <bool TRAIN, bool CHUNKED>
 __global__ void __launch_bounds__(kBnThreads, 4) bn_hswish_fwd_kernel(BnFwdArgs a) {
   bn_act_fwd_body<TRAIN, CHUNKED, false, kActHswish>(a);
+}
+
+template <bool TRAIN, bool CHUNKED>
+__global__ void __launch_bounds__(kBnThreads, 4) bn_silu_fwd_kernel(BnFwdArgs a) {
+  bn_act_fwd_body<TRAIN, CHUNKED, false, kActSilu>(a);
+}
+
+// stochastic depth is drawn in training only: eval takes the plain residual kernels
+template <bool CHUNKED>
+__global__ void __launch_bounds__(kBnThreads, 4) bn_sd_fwd_kernel(BnFwdArgs a) {
+  bn_act_fwd_body<true, CHUNKED, false, kActSD>(a);
 }
 
 // ---- backward pass 1: per-channel reductions ----------------------------------------------------
@@ -269,14 +304,29 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
   const int last = a.M - 1;
   auto phys = [&](int rr) { return a.reverse ? last - rr : rr; };      // see BnBwdArgs::reverse
   int r = live ? blockIdx.x * 32 + rl : a.M;
-  if constexpr (MASK == kMaskXH) {
-    // one row per iteration: the hardswish gradient keeps more values live than a mask, and two rows would spill
+  if constexpr (MASK == kMaskXH || MASK == kMaskXS) {
+    // one row per iteration: the hardswish / SiLU gradient keeps more values live than a mask, and two rows would spill
     for (; r < a.M; r += rstep) {
       const size_t off0 = static_cast<size_t>(phys(r)) * a.C + c0;
       accumulate(ld_stream_u4(a.dz + off0), ld_stream_u4(a.x + off0), make_uint4(0, 0, 0, 0));
     }
   }
-  for (; MASK != kMaskXH && r + rstep < a.M; r += 2 * rstep) {
+  if constexpr (MASK == kMaskSD) {        // the BN sees dz * keep[sample]
+    for (; r < a.M; r += rstep) {
+      const int pr = phys(r);
+      const size_t off0 = static_cast<size_t>(pr) * a.C + c0;
+      const float ks = a.sample_scale[pr / a.hw];
+      float dz[8], x[8];
+      unpack8(ld_stream_u4(a.dz + off0), dz);
+      unpack8(ld_stream_u4(a.x + off0), x);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        s1[i] = fmaf(dz[i], ks, s1[i]);
+        s2[i] = fmaf(dz[i] * ks, x[i], s2[i]);
+      }
+    }
+  }
+  for (; MASK != kMaskXH && MASK != kMaskXS && MASK != kMaskSD && r + rstep < a.M; r += 2 * rstep) {
     const size_t off0 = static_cast<size_t>(phys(r)) * a.C + c0;
     const size_t off1 = static_cast<size_t>(phys(r + rstep)) * a.C + c0;
     const uint4 d0 = ld_stream_u4(a.dz + off0), d1 = ld_stream_u4(a.dz + off1);
@@ -382,6 +432,11 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_apply_kernel(BnBwdAr
       for (int i = 0; i < 8; ++i) dz[i] = act_bwd<MASK>(fmaf(x[i], k1[i], msh[i]), dz[i]);
     }
     if (a.dres) store8_bf16(a.dres + off, dz);
+    if constexpr (MASK == kMaskSD) {
+      const float ks = a.sample_scale[r / a.hw];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) dz[i] *= ks;
+    }
 #pragma unroll
     for (int i = 0; i < 8; ++i) x[i] = fmaf(dz[i], k1[i], fmaf(x[i], cB[i], cA[i]));
     store8_bf16(a.dx + off, x);
@@ -668,7 +723,7 @@ cudaError_t launch_bn_bwd_mask(const BnBwdArgs& a, int sms, cudaStream_t stream,
   const bool f8 = a.dxq != nullptr && a.dxq_slot != nullptr;
   const bool flat = bn_flat_ok(a.C);
   const dim3 grid = flat ? dim3(bn_grid(a.M, a.C, sms)) : rgrid;
-  if constexpr (MASK == kMaskZ6 || MASK == kMaskX6 || MASK == kMaskXH) {
+  if constexpr (MASK == kMaskZ6 || MASK == kMaskX6 || MASK == kMaskXH || MASK == kMaskXS || MASK == kMaskSD) {
     if (f8) return cudaErrorInvalidValue;
   } else if (f8) {
     return flat ? launch_pdl(bn_act_bwd_apply_kernel<MASK, false, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
@@ -684,26 +739,37 @@ cudaError_t launch_bn_act_fwd(const BnFwdArgs& a_in, bool train, int sms, cudaSt
   BnFwdArgs a = a_in;
   a.reverse = g_bn_reverse;
   if (a.C % 8 != 0 || a.C <= 0) return cudaErrorInvalidValue;
-  if (a.relu == 3) {           // hardswish: no residual, bit mask or fp8 twin
+  const bool flat = bn_flat_ok(a.C);
+  const dim3 grid = flat ? dim3(bn_grid(a.M, a.C, sms)) : bn_chunk_grid(a.M, a.C, sms);
+  if (a.sample_scale != nullptr) {     // stochastic depth: train only, a residual, no activation, bit mask or fp8 twin
+    if (!train || a.relu != 0 || a.residual == nullptr || a.mask != nullptr || (a.zq != nullptr && a.zq_slot != nullptr) ||
+        a.hw <= 0 || a.M % a.hw != 0)
+      return cudaErrorInvalidValue;
+    return flat ? launch_pdl(bn_sd_fwd_kernel<false>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                : launch_pdl(bn_sd_fwd_kernel<true>, grid, dim3(kBnThreads), 0, stream, 1, a);
+  }
+  if (a.relu == 3 || a.relu == 4) {    // hardswish / SiLU: no residual, bit mask or fp8 twin
     if (a.residual != nullptr || a.mask != nullptr || (a.zq != nullptr && a.zq_slot != nullptr)) return cudaErrorInvalidValue;
-    if (bn_flat_ok(a.C)) {
-      const dim3 grid(bn_grid(a.M, a.C, sms));
+    if (a.relu == 4) {
+      if (flat)
+        return train ? launch_pdl(bn_silu_fwd_kernel<true, false>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                     : launch_pdl(bn_silu_fwd_kernel<false, false>, grid, dim3(kBnThreads), 0, stream, 1, a);
+      return train ? launch_pdl(bn_silu_fwd_kernel<true, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                   : launch_pdl(bn_silu_fwd_kernel<false, true>, grid, dim3(kBnThreads), 0, stream, 1, a);
+    }
+    if (flat)
       return train ? launch_pdl(bn_hswish_fwd_kernel<true, false>, grid, dim3(kBnThreads), 0, stream, 1, a)
                    : launch_pdl(bn_hswish_fwd_kernel<false, false>, grid, dim3(kBnThreads), 0, stream, 1, a);
-    }
-    const dim3 grid = bn_chunk_grid(a.M, a.C, sms);
     return train ? launch_pdl(bn_hswish_fwd_kernel<true, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
                  : launch_pdl(bn_hswish_fwd_kernel<false, true>, grid, dim3(kBnThreads), 0, stream, 1, a);
   }
   if (a.relu < 0 || a.relu > 2 || (a.relu == 2 && a.mask != nullptr)) return cudaErrorInvalidValue;   // no ReLU6 bit mask
   const bool f8 = a.zq != nullptr && a.zq_slot != nullptr && train;
   const bool r6 = a.relu == 2;
-  if (bn_flat_ok(a.C)) {
-    const dim3 grid(bn_grid(a.M, a.C, sms));
+  if (flat) {
     return r6 ? launch_bn_fwd_variant<false, true>(a, train, f8, grid, stream)
               : launch_bn_fwd_variant<false, false>(a, train, f8, grid, stream);
   }
-  const dim3 grid = bn_chunk_grid(a.M, a.C, sms);
   return r6 ? launch_bn_fwd_variant<true, true>(a, train, f8, grid, stream)
             : launch_bn_fwd_variant<true, false>(a, train, f8, grid, stream);
 }
@@ -712,9 +778,16 @@ cudaError_t launch_bn_act_bwd(const BnBwdArgs& a_in, int sms, cudaStream_t strea
   BnBwdArgs a = a_in;
   a.reverse = g_bn_reverse;
   if (a.C % 8 != 0 || a.C <= 0) return cudaErrorInvalidValue;
-  if (a.relu == 3) {           // hardswish: pre-activation recomputed from x only, no residual gradient
+  if (a.sample_scale != nullptr) {     // stochastic depth: no activation, no fp8 twin, sums not pre-reduced
+    if (a.relu != 0 || a.zmask != nullptr || skip_reduce || (a.dxq != nullptr && a.dxq_slot != nullptr) || a.hw <= 0 ||
+        a.M % a.hw != 0)
+      return cudaErrorInvalidValue;
+    return launch_bn_bwd_mask<kMaskSD>(a, sms, stream, false);
+  }
+  if (a.relu == 3 || a.relu == 4) {    // hardswish / SiLU: pre-activation recomputed from x only, no residual gradient
     if (!a.mask_from_x || a.zmask != nullptr || a.dres != nullptr) return cudaErrorInvalidValue;
-    return launch_bn_bwd_mask<kMaskXH>(a, sms, stream, skip_reduce);
+    return a.relu == 3 ? launch_bn_bwd_mask<kMaskXH>(a, sms, stream, skip_reduce)
+                       : launch_bn_bwd_mask<kMaskXS>(a, sms, stream, skip_reduce);
   }
   if (a.relu < 0 || a.relu > 2 || (a.relu == 2 && a.zmask != nullptr)) return cudaErrorInvalidValue;   // no ReLU6 bit mask
   switch (!a.relu ? kMaskNone

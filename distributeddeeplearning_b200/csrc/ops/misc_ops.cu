@@ -666,6 +666,61 @@ __global__ void __launch_bounds__(256) hardswish_bwd_kernel(const __nv_bfloat16*
   }
 }
 
+// SiLU on the rows of a small bf16 matrix (EfficientNet's squeeze-excitation fc1 output [N][ldx]): y = x * sigmoid(x) into
+// [N][ldy] (ldy <= ldx: the next GEMM's K), and its backward from the saved x into a zero-padded GEMM operand
+// [N][ldx]: dx = dy * s * (1 + x * (1 - s)) for columns < c_valid, 0 beyond.  One thread per 8-column vector.
+__global__ void __launch_bounds__(256) silu_rows_fwd_kernel(const __nv_bfloat16* __restrict__ x, int ldx,
+                                                            __nv_bfloat16* __restrict__ y, int ldy, int64_t total) {
+  const int g8 = ldy / 8;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t n = i / g8;
+    const int c = static_cast<int>(i % g8) * 8;
+    float v[8];
+    unpack8(*reinterpret_cast<const uint4*>(x + n * ldx + c), v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = v[k] / (1.f + __expf(-v[k]));
+    *reinterpret_cast<uint4*>(y + n * ldy + c) = pack8(v);
+  }
+}
+
+__global__ void __launch_bounds__(256) silu_rows_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int ldy,
+                                                            const __nv_bfloat16* __restrict__ x, int ldx,
+                                                            __nv_bfloat16* __restrict__ dx, int c_valid, int64_t total) {
+  const int g8 = ldx / 8;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t n = i / g8;
+    const int c = static_cast<int>(i % g8) * 8;
+    float d[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (c < c_valid) {
+      float v[8];
+      unpack8(*reinterpret_cast<const uint4*>(x + n * ldx + c), v);
+      unpack8(*reinterpret_cast<const uint4*>(dy + n * ldy + c), d);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float sg = 1.f / (1.f + __expf(-v[k]));
+        d[k] = c + k < c_valid ? d[k] * sg * fmaf(v[k], 1.f - sg, 1.f) : 0.f;
+      }
+    }
+    *reinterpret_cast<uint4*>(dx + n * ldx + c) = pack8(d);
+  }
+}
+
+// stochastic depth ("row" mode): one keep scale per sample, 0 or 1 / (1 - p), from the dropout Philox stream (same key
+// and device step counter as dropout_kernel, its own counter word) so that CUDA-graph replays draw fresh vectors
+__global__ void __launch_bounds__(256) stochastic_depth_keep_kernel(float* __restrict__ keep, int n, float p,
+                                                                    uint64_t seed, uint64_t offset,
+                                                                    const int64_t* __restrict__ step) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint64_t sd = seed + (step ? static_cast<uint64_t>(*step) * 0x9E3779B97F4A7C15ull : 0ull);
+  const uint2 key = make_uint2(static_cast<uint32_t>(sd), static_cast<uint32_t>(sd >> 32));
+  const uint64_t ctr = offset + static_cast<uint64_t>(i);
+  const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(ctr), static_cast<uint32_t>(ctr >> 32), 0x5344u, 0), key);
+  keep[i] = u32_to_unit(r.x) > p ? 1.f / (1.f - p) : 0.f;
+}
+
 inline int grid_for(int64_t work, int per_block = 256, int cap = 132 * 16) {     // 16 blocks per SM of an H100 SXM
   int64_t b = (work + per_block - 1) / per_block;
   if (b > cap) b = cap;
@@ -846,6 +901,25 @@ cudaError_t launch_hardswish_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* x
                                  cudaStream_t stream) {
   if (n % 8 != 0) return cudaErrorInvalidValue;
   hardswish_bwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>(dy, x, dx, n / 8);
+  return cudaGetLastError();
+}
+cudaError_t launch_silu_rows_fwd(const __nv_bfloat16* x, int ldx, __nv_bfloat16* y, int ldy, int N, cudaStream_t stream) {
+  if (N <= 0 || ldy <= 0 || ldy % 8 != 0 || ldx % 8 != 0 || ldy > ldx) return cudaErrorInvalidValue;
+  const int64_t total = static_cast<int64_t>(N) * (ldy / 8);
+  silu_rows_fwd_kernel<<<grid_for(total), 256, 0, stream>>>(x, ldx, y, ldy, total);
+  return cudaGetLastError();
+}
+cudaError_t launch_silu_rows_bwd(const __nv_bfloat16* dy, int ldy, const __nv_bfloat16* x, int ldx, __nv_bfloat16* dx,
+                                 int c_valid, int N, cudaStream_t stream) {
+  if (N <= 0 || ldy % 8 != 0 || ldx % 8 != 0 || c_valid <= 0 || c_valid > ldy || ldy > ldx) return cudaErrorInvalidValue;
+  const int64_t total = static_cast<int64_t>(N) * (ldx / 8);
+  silu_rows_bwd_kernel<<<grid_for(total), 256, 0, stream>>>(dy, ldy, x, ldx, dx, c_valid, total);
+  return cudaGetLastError();
+}
+cudaError_t launch_stochastic_depth_keep(float* keep, int n, float p, uint64_t seed, uint64_t offset, const int64_t* step,
+                                         cudaStream_t stream) {
+  if (n <= 0 || !(p > 0.f && p < 1.f)) return cudaErrorInvalidValue;
+  stochastic_depth_keep_kernel<<<(n + 255) / 256, 256, 0, stream>>>(keep, n, p, seed, offset, step);
   return cudaGetLastError();
 }
 cudaError_t launch_pad_nhwc4(const __nv_bfloat16* in, __nv_bfloat16* out, int N, int H, int W, int Hp, int Wp, int pt,

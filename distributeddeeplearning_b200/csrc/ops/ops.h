@@ -33,6 +33,8 @@ struct BnFwdArgs {
   Fp8Slot* zq_slot;               //   z * slot->scale, amax(|z|) folded into the slot (ops/fp8.py: no separate quantise pass)
   int reverse;                    // walk the rows from the END: the producing conv wrote x front to back, so the tail of a
                                   //   tensor larger than L2 is what is still cached (set by the launcher: set_bn_reverse)
+  const float* sample_scale;      // optional [M / hw] per-sample scale of the BN output before the residual add
+  int hw;                         //   (stochastic depth: z = BN(x) * sample_scale[row / hw] + residual; no activation)
 };
 
 struct BnBwdArgs {
@@ -56,6 +58,8 @@ struct BnBwdArgs {
   Fp8Slot* dxq_slot;
   int reverse;                    // the REDUCE pass walks the rows from the end (dz was just written front to back; the apply
                                   //   pass then walks forward and finds the rows the reduce pass read last)
+  const float* sample_scale;      // optional, as in BnFwdArgs: BN sees dz * sample_scale[row / hw], dres = dz
+  int hw;
 };
 
 cudaError_t launch_bn_act_fwd(const BnFwdArgs& a, bool train, int sms, cudaStream_t stream);
@@ -167,6 +171,26 @@ cudaError_t launch_se_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* x, co
 // dx = dy * hsig(s) + dpooled / HW  (dpooled [N][C])
 cudaError_t launch_se_apply(const __nv_bfloat16* dy, const __nv_bfloat16* s, int lds, const __nv_bfloat16* dpooled,
                             __nv_bfloat16* dx, int N, int HW, int C, int sms, cudaStream_t stream);
+// ---- squeeze-excitation with a sigmoid gate (squeeze_excite_sigmoid.cu; EfficientNet) -------------------------------
+// same operands as above; gate sigmoid(s), reduce ds = g (1 - g) * sum_hw(dy * x)
+cudaError_t launch_se_sig_scale(const __nv_bfloat16* x, const __nv_bfloat16* s, int lds, __nv_bfloat16* y, int N, int HW,
+                                int C, int sms, cudaStream_t stream);
+cudaError_t launch_se_sig_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* x, const __nv_bfloat16* s, int lds,
+                                 __nv_bfloat16* ds, int ldd, int N, int HW, int C, cudaStream_t stream);
+cudaError_t launch_se_sig_apply(const __nv_bfloat16* dy, const __nv_bfloat16* s, int lds, const __nv_bfloat16* dpooled,
+                                __nv_bfloat16* dx, int N, int HW, int C, int sms, cudaStream_t stream);
+// bf16 [rows][k] -> [rows][kp] with zero columns [k, kp) (the squeeze dimension of fc2's weight padded to 8)
+cudaError_t launch_pad_cols_bf16(const __nv_bfloat16* src, __nv_bfloat16* dst, int rows, int k, int kp, cudaStream_t stream);
+// fp32 dst [rows][k] += src [rows][kp] columns [0, k)  (fc2's weight gradient folded into its compact slot)
+cudaError_t launch_fold_cols_f32(const float* src, float* dst, int rows, int k, int kp, cudaStream_t stream);
+// SiLU on the rows of a bf16 matrix: y [N][ldy] = silu(x [N][ldx]) for columns [0, ldy) (ldy <= ldx, both % 8 == 0), and
+// its backward dx [N][ldx] = dy [N][ldy] * silu'(x) for columns < c_valid, zero elsewhere (a GEMM operand with zero pad)
+cudaError_t launch_silu_rows_fwd(const __nv_bfloat16* x, int ldx, __nv_bfloat16* y, int ldy, int N, cudaStream_t stream);
+cudaError_t launch_silu_rows_bwd(const __nv_bfloat16* dy, int ldy, const __nv_bfloat16* x, int ldx, __nv_bfloat16* dx,
+                                 int c_valid, int N, cudaStream_t stream);
+// stochastic depth: keep[i] = (uniform(seed, step, offset + i) > p) / (1 - p) for i < n, from the dropout Philox stream
+cudaError_t launch_stochastic_depth_keep(float* keep, int n, float p, uint64_t seed, uint64_t offset, const int64_t* step,
+                                         cudaStream_t stream);
 // y = a + b (bf16)
 // NHWC4 image [N][H][W] (8-byte pixels) -> zero-bordered, G-row-interleaved [N][Hp][Wp][G][4] with the source at
 // (pt, pl): position (h, w) holds the pixels of rows h .. h+G-1.  Operand layout of the TMA-fed stem convolution

@@ -5,12 +5,15 @@ Parity: the reference resolves ``--model`` with ``getattr(torchvision.models, na
 (``imagenet_pytorch_horovod.py:383``).  North-star zoo: ResNet-50/101/152, VGG-16, Inception-v3,
 AlexNet (SURVEY.md 2.7); ResNet-18/34, the other VGG depths, DenseNet and SqueezeNet (the rest of torchvision
 0.2.1's families) are here too, and the later ResNet family members of torchvision (ResNeXt-50 32x4d, ResNeXt-101
-32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2 and MobileNetV3-Large / -Small.
+32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2, MobileNetV3-Large / -Small and EfficientNet-B0 to -B7.
 """
 from __future__ import annotations
 
 from .alexnet import AlexNet, alexnet  # noqa: F401
 from .densenet import DenseNet, densenet121, densenet161, densenet169, densenet201  # noqa: F401
+from .efficientnet import (INPUT_SIZE as _EFFICIENTNET_INPUT_SIZE, EfficientNet, efficientnet_b0,  # noqa: F401
+                           efficientnet_b1, efficientnet_b2, efficientnet_b3, efficientnet_b4, efficientnet_b5,
+                           efficientnet_b6, efficientnet_b7)
 from .inception import Inception3, inception_v3  # noqa: F401
 from .mobilenet import MobileNetV2, mobilenet_v2  # noqa: F401
 from .mobilenetv3 import MobileNetV3, mobilenet_v3_large, mobilenet_v3_small  # noqa: F401
@@ -21,7 +24,9 @@ from .vgg import VGG, vgg11, vgg11_bn, vgg13, vgg13_bn, vgg16, vgg16_bn, vgg19, 
 
 _REGISTRY = {
     f.__name__: f
-    for f in (alexnet, densenet121, densenet161, densenet169, densenet201, squeezenet1_0, squeezenet1_1, inception_v3, mobilenet_v2,
+    for f in (alexnet, densenet121, densenet161, densenet169, densenet201, efficientnet_b0, efficientnet_b1,
+              efficientnet_b2, efficientnet_b3, efficientnet_b4, efficientnet_b5, efficientnet_b6, efficientnet_b7,
+              squeezenet1_0, squeezenet1_1, inception_v3, mobilenet_v2,
               mobilenet_v3_large, mobilenet_v3_small, resnet18, resnet34, resnet50, resnet101, resnet152,
               resnext50_32x4d, resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2, vgg11, vgg11_bn, vgg13,
               vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn)
@@ -43,7 +48,10 @@ def get_model(name: str, **kw):
 
 
 def input_size(model_or_name) -> int:
-    """Spatial input size (299 for Inception-v3 — the reference hard-codes 224 and breaks, SURVEY.md Q2)."""
+    """Spatial input size (299 for Inception-v3 — the reference hard-codes 224 and breaks, SURVEY.md Q2; torchvision's
+    crop size for EfficientNet-B0 to -B7, 224 to 600)."""
     if isinstance(model_or_name, str):
+        if model_or_name in _EFFICIENTNET_INPUT_SIZE:
+            return _EFFICIENTNET_INPUT_SIZE[model_or_name]
         return 299 if model_or_name.startswith("inception") else 224
     return int(getattr(model_or_name, "input_size", 224))

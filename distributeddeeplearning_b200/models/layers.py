@@ -75,15 +75,19 @@ class BatchNorm2d(nn.Module):
         return f"{self.num_features}, eps={self.eps}, momentum={self.momentum}"
 
 
-def conv_bn(x, conv: Conv2d, bn: BatchNorm2d, relu=True, residual=None, relu6=False, hardswish=False):
+def conv_bn(x, conv: Conv2d, bn: BatchNorm2d, relu=True, residual=None, relu6=False, hardswish=False, silu=False,
+            sample_scale=None):
     """act(BN(conv(x)) [+ residual]) through the fused op (``relu6``: the activation is ReLU6; ``hardswish``: it is
-    hardswish)."""
+    hardswish; ``silu``: it is SiLU).  ``sample_scale``: per-sample scales of stochastic depth applied to the BN output
+    before the residual add (no activation)."""
     return ops.conv_bn_act(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.stride,
                            conv.padding,
                            conv.dilation, bn.eps, bn.momentum, relu, residual, bn.training,
                            **({"groups": conv.groups} if conv.groups != 1 else {}),
                            **({"relu6": True} if relu6 else {}),
-                           **({"hardswish": True} if hardswish else {}))
+                           **({"hardswish": True} if hardswish else {}),
+                           **({"silu": True} if silu else {}),
+                           **({"sample_scale": sample_scale} if sample_scale is not None else {}))
 
 
 def conv_bn_pool(x, conv: Conv2d, bn: BatchNorm2d, kernel=3, stride=2, padding=1):

@@ -110,7 +110,8 @@ def is_stem_weight(p: torch.Tensor, groups: Optional[int] = None) -> bool:
     return p.dim() == 4 and p.shape[1] <= 4 and g == 1
 
 
-def weight_bf16(p: torch.Tensor, kernel: Optional[Tuple[int, int]] = None, groups: Optional[int] = None) -> torch.Tensor:
+def weight_bf16(p: torch.Tensor, kernel: Optional[Tuple[int, int]] = None, groups: Optional[int] = None,
+                stem: Optional[bool] = None) -> torch.Tensor:
     """bf16 GEMM operand of a parameter.
 
     With a fused engine attached the copy is a view into the bf16 weight arena that the
@@ -118,8 +119,10 @@ def weight_bf16(p: torch.Tensor, kernel: Optional[Tuple[int, int]] = None, group
     demand and cached against the parameter's version counter.  Stem weights (Cin <= 4) are
     re-packed to the padded [Cout, KB*64] matrix.  Grouped weights come as the compact
     [Cout, R*S*Cin/groups] matrix (``native.expand_grouped_weight`` derives the kernels' operand from it).
+    ``stem=False``: a weight with <= 4 input channels that is not an image convolution (a squeeze-excitation fc2 with a
+    squeeze width of 4) keeps the plain [Cout, Cin*R*S] layout.
     """
-    stem = is_stem_weight(p, groups)
+    stem = is_stem_weight(p, groups) if stem is None else stem
     view = getattr(p, "_ddl_bf16", None)
     if view is not None and not stem:
         return view
@@ -155,7 +158,7 @@ def _krsc(p: torch.Tensor) -> bool:
 class _ConvBnAct(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, weight, gamma, beta, running_mean, running_var, stride, pad, dil, eps, momentum,
-                relu, train, groups):
+                relu, train, groups, sample_scale=None):
         R, S = weight.shape[2], weight.shape[3]
         wb = weight_bf16(weight, groups=groups)
         if groups > 1:      # this step's block-diagonal operand, shared by the forward and the data gradient
@@ -171,9 +174,10 @@ class _ConvBnAct(torch.autograd.Function):
                                                residual, train, want_mask=True)
         else:
             z, save = native.bn_act_fwd(y, stats, gamma, beta, running_mean, running_var, eps, momentum, relu, residual,
-                                        train)
+                                        train, sample_scale=sample_scale)
             zmask = None
         ctx.cfg = (stride, pad, dil, relu, residual is not None, (R, S), groups)
+        ctx.sample_scale = sample_scale
         ctx.params = (weight, gamma, beta)
         if train:
             # wb is a view of the engine's bf16 weight arena: kept as a plain attribute (no autograd
@@ -197,7 +201,7 @@ class _ConvBnAct(torch.autograd.Function):
         bg = grad_buffer(beta) if beta.requires_grad else None
         dy, dres, _ = native.bn_act_bwd(dz, None if zmask is not None else z, y, save, gamma, relu,
                                         has_res and ctx.needs_input_grad[1], gg, bg, beta=beta, had_residual=has_res,
-                                        zmask=zmask)
+                                        zmask=zmask, sample_scale=ctx.sample_scale)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = native.conv_dgrad(dy, wb, x.shape, kernel, stride, pad, dil, groups=groups)
@@ -211,19 +215,34 @@ class _ConvBnAct(torch.autograd.Function):
         for p in (gamma, beta, weight):
             if p.requires_grad:
                 notify_ready(p)
-        return (dx, dres) + (None,) * 13
+        return (dx, dres) + (None,) * 14
 
 
 def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad=0, dil=1, eps=1e-5, momentum=0.1,
-                relu=True, residual=None, training=True, groups=1, relu6=False, hardswish=False):
+                relu=True, residual=None, training=True, groups=1, relu6=False, hardswish=False, silu=False,
+                sample_scale=None):
     """z = act(BN(conv(x, weight)) [+ residual])  — the unit every ResNet/Inception layer is made of.  ``groups`` > 1:
     grouped convolution (``weight`` is [Cout, Cin/groups, R, S]); depthwise shapes that ``native.supports_depthwise`` (3x3)
     or ``native.supports_depthwise5`` (5x5) accept run on the depthwise kernels, other shapes outside ``native.supports_grouped`` take the composite path.
     ``relu6``: the activation is ReLU6 (clamp to [0, 6]) instead of ``relu``; ``hardswish``: it is hardswish
-    (v * clamp(v + 3, 0, 6) / 6), which takes no ``residual``."""
+    (v * clamp(v + 3, 0, 6) / 6), which takes no ``residual``; ``silu``: it is SiLU (v * sigmoid(v)), which takes no
+    ``residual`` either.  ``sample_scale``: fp32 [N] per-sample scales of stochastic depth (``stochastic_depth_keep``):
+    z = BN(conv(x)) * sample_scale[n] + residual, with a ``residual``, no activation and in training; the batch
+    statistics cover every sample, dropped ones included."""
     if hardswish and (relu6 or residual is not None):
         raise ValueError("conv_bn_act: hardswish is neither combined with relu6 nor with a residual")
-    act = 3 if hardswish else (2 if relu6 else relu)
+    if silu and (relu6 or hardswish or residual is not None):
+        raise ValueError("conv_bn_act: SiLU is neither combined with relu6 / hardswish nor with a residual")
+    if sample_scale is not None and (residual is None or relu or relu6 or hardswish or silu or not training):
+        raise ValueError("conv_bn_act: sample_scale needs a residual, no activation and training")
+    act = 4 if silu else (3 if hardswish else (2 if relu6 else relu))
+    if use_native(x) and sample_scale is not None:
+        if not (native.supports_conv(x.shape[1], weight.shape[0]) and groups == 1 and native.bn_supported(weight.shape[0])
+                and _krsc(weight)):
+            raise ValueError("conv_bn_act: stochastic depth is fused for dense convolutions with a multiple of 8 "
+                             "output channels only")
+        return _ConvBnAct.apply(x, residual, weight, gamma, beta, running_mean, running_var, stride, pad, dil, eps,
+                                momentum, act, training, groups, sample_scale)
     if use_native(x) and groups > 1 and x.shape[1] == weight.shape[0] and weight.shape[1] == 1 \
             and native.depthwise_native(weight.shape[0], tuple(weight.shape[2:]), stride, pad, dil, groups) \
             and _krsc(weight):
@@ -238,8 +257,12 @@ def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad
     y = F.conv2d(xi.to(weight.dtype) if not x.is_cuda else xi, weight.to(xi.dtype) if x.is_cuda else weight, None,
                  stride, pad, dil, groups)
     z = F.batch_norm(y.float(), running_mean, running_var, gamma, beta, training, momentum, eps).to(y.dtype)
+    if sample_scale is not None:
+        z = z * sample_scale.to(z.dtype).view(-1, 1, 1, 1)
     if residual is not None:
         z = z + residual
+    if silu:
+        return F.silu(z)
     if hardswish:
         return F.hardswish(z)
     if relu6:
@@ -549,20 +572,92 @@ class _SqueezeExcite(torch.autograd.Function):
         return dx, None, None, None, None, None
 
 
-def squeeze_excite(x, w1, b1, w2, b2):
-    """x * hardsigmoid(fc2(relu(fc1(mean_hw(x))))) with fc1 / fc2 the 1x1 convolutions ``w1`` [C', C, 1, 1] + ``b1``
-    and ``w2`` [C, C', 1, 1] + ``b2`` (torchvision's ``SqueezeExcitation`` with a hardsigmoid scale).  Native on
-    NHWC bf16 activations with C and C' multiples of 8; the composite is the CPU path."""
+class _SqueezeExciteSiLU(torch.autograd.Function):
+    """x * sigmoid(fc2(silu(fc1(mean_hw(x))))) (EfficientNet) as one node, with _SqueezeExcite's backward schedule.  Any
+    squeeze width C': fc2's K = C' is padded with zero columns to C'8 = C' rounded up to 8 (a 16-byte GEMM operand row),
+    through a padded bf16 copy of its weight made in forward (so a captured graph rebuilds it from the weight arena every
+    replay) and a padded fp32 weight-gradient scratch folded into the compact slot."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, train):
+        cs, c = w1.shape[0], w1.shape[1]
+        cs8 = _ceil8(cs)
+        w1b, w2b = weight_bf16(w1), weight_bf16(w2, stem=False)   # [C', C], [C, C']
+        w2p = w2b if cs8 == cs else native.pad_cols_bf16(w2b, cs8)                    # [C, C'8]
+        pooled = native.global_avgpool_fwd(x)                     # [N, C]
+        h = native.linear_fwd(pooled, w1b, b1)                    # [N, C' rounded up to 64]: fc1 logits, pad columns 0
+        a = native.silu_rows_fwd(h, cs8)                          # [N, C'8]: fc2's input, pad columns silu(0) = 0
+        s = native.linear_fwd(a, w2p, b2)                         # [N, C rounded up to 64]: the gate logits
+        y = native.se_scale(x, s, gate="sigmoid")
+        ctx.params = (w1, b1, w2, b2)
+        if train:
+            ctx.wb = (w1b, w2p)       # views of the bf16 weight arena / this step's padded copy: see _ConvBnAct
+            ctx.save_for_backward(x, pooled, h, a, s)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        w1, b1, w2, b2 = ctx.params
+        x, pooled, h, a, s = ctx.saved_tensors
+        w1b, w2p = ctx.wb
+        if not dy.is_contiguous(memory_format=CL):
+            dy = dy.contiguous(memory_format=CL)
+        cs, c = w1.shape[0], w1.shape[1]
+        cs8 = a.shape[1]
+        ds = native.se_reduce(dy, x, s, gate="sigmoid")           # [N, C rounded up to 64], pad columns 0
+        if b2.requires_grad:
+            native.bias_relu_bwd(ds, ds, grad_buffer(b2), False, c_valid=c)
+        da = native.linear_dgrad(ds, w2p)                         # [N, C'8]
+        if w2.requires_grad:
+            if cs8 == cs:
+                native.linear_wgrad(a, ds, grad_buffer(w2))
+            else:
+                gw = native.zeros_f32((c, cs8), ds.device)
+                native.linear_wgrad(a, ds, gw)
+                native.fold_cols_f32(gw, grad_buffer(w2))
+        dh = native.silu_rows_bwd(da, h, cs)                      # [N, C' rounded up to 64]: fc1's GEMM operand, pad 0
+        if b1.requires_grad:
+            native.bias_relu_bwd(dh, dh, grad_buffer(b1), False, c_valid=cs)
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dpooled = native.linear_dgrad(dh, w1b)                # [N, C]
+            dx = native.se_apply(dy, s, dpooled, gate="sigmoid")
+        if w1.requires_grad:
+            native.linear_wgrad(pooled, dh, grad_buffer(w1))
+        for p in (b2, w2, b1, w1):                                # LAST, as in _ConvBnAct
+            if p.requires_grad:
+                notify_ready(p)
+        return dx, None, None, None, None, None
+
+
+def _ceil8(n: int) -> int:
+    return (n + 7) // 8 * 8
+
+
+def squeeze_excite(x, w1, b1, w2, b2, gate="hardsigmoid", act="relu"):
+    """x * gate(fc2(act(fc1(mean_hw(x))))) with fc1 / fc2 the 1x1 convolutions ``w1`` [C', C, 1, 1] + ``b1``
+    and ``w2`` [C, C', 1, 1] + ``b2`` (torchvision's ``SqueezeExcitation``).  ``gate="hardsigmoid", act="relu"``
+    (MobileNetV3): native on NHWC bf16 activations with C and C' multiples of 8.  ``gate="sigmoid", act="silu"``
+    (EfficientNet): native with C a multiple of 8 and any C'.  The composite is the CPU path."""
+    if (gate, act) not in (("hardsigmoid", "relu"), ("sigmoid", "silu")):
+        raise ValueError(f"squeeze_excite: (gate, act) must be ('hardsigmoid', 'relu') or ('sigmoid', 'silu'), "
+                         f"got {(gate, act)}")
     cs, c = w1.shape[0], w1.shape[1]
-    if use_native(x) and x.dim() == 4 and x.dtype == torch.bfloat16 and x.is_contiguous(memory_format=CL) \
-            and c % 8 == 0 and cs % 8 == 0 and x.shape[1] == c:
+    native_act = use_native(x) and x.dim() == 4 and x.dtype == torch.bfloat16 and x.is_contiguous(memory_format=CL) \
+        and c % 8 == 0 and x.shape[1] == c
+    if native_act and gate == "sigmoid":
+        train = torch.is_grad_enabled() and any(t.requires_grad for t in (x, w1, b1, w2, b2))
+        return _SqueezeExciteSiLU.apply(x, w1, b1, w2, b2, train)
+    if native_act and cs % 8 == 0:
         train = torch.is_grad_enabled() and any(t.requires_grad for t in (x, w1, b1, w2, b2))
         return _SqueezeExcite.apply(x, w1, b1, w2, b2, train)
     dt = x.dtype if x.is_cuda else w1.dtype
     xi = x.to(dt)
     sc = xi.float().mean((2, 3), keepdim=True).to(dt) if x.is_cuda else xi.mean((2, 3), keepdim=True)
-    sc = F.relu(F.conv2d(sc, w1.to(dt), b1.to(dt)))
-    sc = F.hardsigmoid(F.conv2d(sc, w2.to(dt), b2.to(dt)))
+    sc = F.conv2d(sc, w1.to(dt), b1.to(dt))
+    sc = F.silu(sc) if act == "silu" else F.relu(sc)
+    sc = F.conv2d(sc, w2.to(dt), b2.to(dt))
+    sc = torch.sigmoid(sc) if gate == "sigmoid" else F.hardsigmoid(sc)
     return xi * sc
 
 
@@ -701,6 +796,22 @@ class _Dropout(torch.autograd.Function):
         p, seed, off, cl, step = ctx.cfg
         dy = dy.contiguous(memory_format=CL) if cl else dy.contiguous()
         return native.dropout(dy, p, seed, off, step), None
+
+
+def stochastic_depth_keep(n: int, p: float, device) -> torch.Tensor:
+    """fp32 [n] per-sample scales of stochastic depth ("row" mode): 0 with probability p, else 1 / (1 - p).  On CUDA
+    they are drawn on the device from the dropout Philox stream (seed, offset and the device step counter), so a step
+    replayed from a CUDA graph draws a fresh vector; the data-parallel rank is mixed into the key, so that the ranks
+    drop independent samples of the global batch.  On CPU from torch's generator (the composite path)."""
+    device = torch.device(device)
+    if device.type != "cuda":
+        return torch.empty(n).bernoulli_(1.0 - p).div_(1.0 - p)
+    from ..parallel import dist
+
+    seed, off = _DROPOUT_STATE["seed"], _DROPOUT_STATE["offset"]
+    _DROPOUT_STATE["offset"] = off + n
+    seed = (seed + dist.rank() * 0xD1B54A32D192ED03) & 0xFFFFFFFFFFFFFFFF
+    return native.stochastic_depth_keep(n, p, seed, off, _dropout_step(device), device)
 
 
 def dropout(x, p=0.5, training=True):

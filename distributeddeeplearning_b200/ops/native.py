@@ -461,20 +461,32 @@ def _check_se_act(x: torch.Tensor, name: str) -> None:
     _check_aligned(x, name)
 
 
-def se_scale(x: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
-    """y = x * hardsigmoid(s[n, c]) for an NHWC activation x [N, C, H, W] and the gate logits s [N, >= C]."""
+_SE_GATES = ("hardsigmoid", "sigmoid")
+
+
+def _se_kernel(name: str, gate: str):
+    """The hardsigmoid kernels (squeeze_excite.cu) or the sigmoid ones (squeeze_excite_sigmoid.cu)."""
+    if gate not in _SE_GATES:
+        raise ValueError(f"squeeze-excite: gate must be one of {_SE_GATES}, got {gate!r}")
+    return getattr(_C(), name if gate == "hardsigmoid" else name.replace("se_", "se_sig_"))
+
+
+def se_scale(x: torch.Tensor, s: torch.Tensor, gate: str = "hardsigmoid") -> torch.Tensor:
+    """y = x * gate(s[n, c]) for an NHWC activation x [N, C, H, W] and the gate logits s [N, >= C]; ``gate`` is
+    "hardsigmoid" (MobileNetV3) or "sigmoid" (EfficientNet)."""
     _check_se_act(x, "x")
     N, Ch, H, W = x.shape
     _check_gate(s, N, Ch)
     y = torch.empty_like(x)
-    _C().se_scale(x.data_ptr(), s.data_ptr(), s.stride(0), y.data_ptr(), N, H * W, Ch, sm_count(x.device.index or 0),
+    _se_kernel("se_scale", gate)(x.data_ptr(), s.data_ptr(), s.stride(0), y.data_ptr(), N, H * W, Ch, sm_count(x.device.index or 0),
                   _stream())
     return y
 
 
-def se_reduce(dy: torch.Tensor, x: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
-    """ds [N, C rounded up to 64] bf16 = hardsigmoid'(s) * sum_hw(dy * x), pad columns zero: the gradient of the gate
-    logits of :func:`se_scale`, laid out as the fc2 GEMM operand.  Deterministic (no atomics)."""
+def se_reduce(dy: torch.Tensor, x: torch.Tensor, s: torch.Tensor, gate: str = "hardsigmoid") -> torch.Tensor:
+    """ds [N, C rounded up to 64] bf16 = gate'(s) * sum_hw(dy * x), pad columns zero: the gradient of the gate
+    logits of :func:`se_scale`, laid out as the fc2 GEMM operand.  Deterministic (no atomics).  The sigmoid's
+    derivative is g (1 - g), g = sigmoid(s) recomputed from the saved logits."""
     _check_se_act(dy, "dy")
     _check_se_act(x, "x")
     N, Ch, H, W = x.shape
@@ -483,12 +495,13 @@ def se_reduce(dy: torch.Tensor, x: torch.Tensor, s: torch.Tensor) -> torch.Tenso
     _check_gate(s, N, Ch)
     ldd = _ceil_div(Ch, 64) * 64
     ds = torch.empty((N, ldd), dtype=torch.bfloat16, device=x.device)
-    _C().se_reduce(dy.data_ptr(), x.data_ptr(), s.data_ptr(), s.stride(0), ds.data_ptr(), ldd, N, H * W, Ch, _stream())
+    _se_kernel("se_reduce", gate)(dy.data_ptr(), x.data_ptr(), s.data_ptr(), s.stride(0), ds.data_ptr(), ldd, N, H * W,
+                                   Ch, _stream())
     return ds
 
 
-def se_apply(dy: torch.Tensor, s: torch.Tensor, dpooled: torch.Tensor) -> torch.Tensor:
-    """dx = dy * hardsigmoid(s[n, c]) + dpooled[n, c] / (H*W): the input gradient of squeeze-excitation from both of its
+def se_apply(dy: torch.Tensor, s: torch.Tensor, dpooled: torch.Tensor, gate: str = "hardsigmoid") -> torch.Tensor:
+    """dx = dy * gate(s[n, c]) + dpooled[n, c] / (H*W): the input gradient of squeeze-excitation from both of its
     paths (the scale and the pooling) in one pass."""
     _check_se_act(dy, "dy")
     N, Ch, H, W = dy.shape
@@ -497,9 +510,61 @@ def se_apply(dy: torch.Tensor, s: torch.Tensor, dpooled: torch.Tensor) -> torch.
         raise ValueError(f"se_apply: expected a contiguous bf16 dpooled [{N}, {Ch}]")
     _check_aligned(dpooled, "dpooled")
     dx = torch.empty_like(dy)
-    _C().se_apply(dy.data_ptr(), s.data_ptr(), s.stride(0), dpooled.data_ptr(), dx.data_ptr(), N, H * W, Ch,
-                  sm_count(dy.device.index or 0), _stream())
+    _se_kernel("se_apply", gate)(dy.data_ptr(), s.data_ptr(), s.stride(0), dpooled.data_ptr(), dx.data_ptr(), N, H * W,
+                                  Ch, sm_count(dy.device.index or 0), _stream())
     return dx
+
+
+def pad_cols_bf16(w: torch.Tensor, kp: int) -> torch.Tensor:
+    """bf16 [rows, k] -> [rows, kp] with zero columns [k, kp): fc2's weight with its squeeze dimension padded to a
+    multiple of 8, so that its rows are 16-byte GEMM operand rows."""
+    if w.dtype != torch.bfloat16 or not w.is_cuda or w.dim() != 2 or not w.is_contiguous() or kp < w.shape[1]:
+        raise ValueError(f"pad_cols_bf16: expected a contiguous CUDA bf16 matrix with at most {kp} columns")
+    out = torch.empty((w.shape[0], kp), dtype=torch.bfloat16, device=w.device)
+    _C().pad_cols_bf16(w.data_ptr(), out.data_ptr(), w.shape[0], w.shape[1], kp, _stream())
+    return out
+
+
+def fold_cols_f32(src: torch.Tensor, dst: torch.Tensor) -> None:
+    """dst [rows, k] (fp32, any contiguous shape of rows * k elements) += src [rows, kp][:, :k]."""
+    rows, kp = src.shape
+    if src.dtype != torch.float32 or dst.dtype != torch.float32 or not src.is_contiguous() or not dst.is_contiguous() \
+            or dst.numel() % rows != 0 or dst.numel() // rows > kp:
+        raise ValueError("fold_cols_f32: expected contiguous fp32 src [rows, kp] and dst [rows, k <= kp]")
+    _C().fold_cols_f32(src.data_ptr(), dst.data_ptr(), rows, dst.numel() // rows, kp, _stream())
+
+
+def silu_rows_fwd(x: torch.Tensor, cols: int) -> torch.Tensor:
+    """y [N, cols] = silu(x[:, :cols]) for a bf16 matrix x [N, ld] (cols <= ld, both multiples of 8)."""
+    _check_act(x, "x")
+    if x.dim() != 2 or x.shape[1] % 8 != 0 or cols % 8 != 0 or not 0 < cols <= x.shape[1]:
+        raise ValueError("silu_rows_fwd: expected a bf16 [N, ld] matrix and cols <= ld, both multiples of 8")
+    y = torch.empty((x.shape[0], cols), dtype=torch.bfloat16, device=x.device)
+    _C().silu_rows_fwd(x.data_ptr(), x.shape[1], y.data_ptr(), cols, x.shape[0], _stream())
+    return y
+
+
+def silu_rows_bwd(dy: torch.Tensor, x: torch.Tensor, c_valid: int) -> torch.Tensor:
+    """dx [N, ld] = dy * silu'(x) in columns < c_valid and 0 beyond, for the saved pre-activation x [N, ld] and
+    dy [N, <= ld]: the gradient of :func:`silu_rows_fwd` laid out as a zero-padded GEMM operand."""
+    _check_act(dy, "dy")
+    _check_act(x, "x")
+    if dy.dim() != 2 or x.dim() != 2 or dy.shape[0] != x.shape[0] or dy.shape[1] % 8 != 0 or x.shape[1] % 8 != 0 \
+            or dy.shape[1] > x.shape[1] or not 0 < c_valid <= dy.shape[1]:
+        raise ValueError("silu_rows_bwd: expected bf16 dy [N, k] and x [N, ld >= k] (multiples of 8), 0 < c_valid <= k")
+    dx = torch.empty_like(x)
+    _C().silu_rows_bwd(dy.data_ptr(), dy.shape[1], x.data_ptr(), x.shape[1], dx.data_ptr(), c_valid, x.shape[0], _stream())
+    return dx
+
+
+def stochastic_depth_keep(n: int, p: float, seed: int, offset: int, step: Optional[torch.Tensor], device) -> torch.Tensor:
+    """fp32 [n] per-sample scales, 0 or 1 / (1 - p), drawn on the device from the dropout Philox stream (``step``: the
+    device step counter mixed into the key, see :func:`dropout`)."""
+    if not 0.0 < p < 1.0 or n <= 0:
+        raise ValueError(f"stochastic_depth_keep: need n > 0 and 0 < p < 1, got n={n}, p={p}")
+    keep = torch.empty(n, dtype=torch.float32, device=device)
+    _C().stochastic_depth_keep(keep.data_ptr(), n, p, seed, offset, _stream(), _ptr(step))
+    return keep
 
 
 def _check_flat(t: torch.Tensor, name: str) -> None:
@@ -966,13 +1031,18 @@ def bn_supported(c: int) -> bool:
 
 def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, running_mean, running_var,
                eps: float, momentum: float, relu: bool, residual: Optional[torch.Tensor], train: bool,
-               want_mask: bool = False):
+               want_mask: bool = False, sample_scale: Optional[torch.Tensor] = None):
     """z = act(BN(y) [+ residual]).  Returns (z, save) — with ``want_mask`` (train + ReLU) (z, save, mask): one bit per
     element telling whether z > 0, which lets the backward of residual layers skip reading z (16x less mask traffic).
     ``relu``: False / True, 2 for ReLU6 (clamp to [0, 6]; not with ``want_mask``) or 3 for hardswish
-    (x * clamp(x + 3, 0, 6) / 6; not with ``want_mask`` or ``residual``)."""
+    (x * clamp(x + 3, 0, 6) / 6; not with ``want_mask`` or ``residual``), 4 for SiLU (x * sigmoid(x); the same
+    refusals).  ``sample_scale``: fp32 [N] (stochastic depth, train only): z = BN(y) * sample_scale[n] + residual, with
+    no activation."""
     C = _C()
     _check_act(y, "y")
+    if int(relu) == 4 and (want_mask or residual is not None):
+        raise ValueError("bn_act_fwd: SiLU takes no residual and has no bit-mask variant")
+    _check_sample_scale(sample_scale, y, relu, residual, train)
     if int(relu) == 2 and want_mask:
         raise ValueError("bn_act_fwd: ReLU6 has no bit-mask variant")
     if int(relu) == 3 and (want_mask or residual is not None):
@@ -992,8 +1062,8 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
         zq = slot = None
         key = ("act", gamma.data_ptr(), N, H, W)
         # emit the e4m3 twin only when an fp8 convolution consumed this layer's output in an earlier step
-        twin = _fp8.enabled() and int(relu) not in (2, 3) and Ch % 128 == 0 and M >= 2048 and \
-            _fp8.note_producer(z, key)
+        twin = _fp8.enabled() and int(relu) not in (2, 3, 4) and sample_scale is None and Ch % 128 == 0 and M >= 2048 \
+            and _fp8.note_producer(z, key)
         if twin:
             idx, fused = _fp8.producer_slot(key, y.device, z)
             if fused:       # the e4m3 twin rides in this kernel's pass (+1 B/element) instead of a 3 B/element pass
@@ -1001,7 +1071,7 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
         C.bn_act_fwd(y.data_ptr(), _ptr(residual), z.data_ptr(), stats[0].data_ptr(), stats[1].data_ptr(),
                      gamma.data_ptr(), beta.data_ptr(), save[0].data_ptr(), save[1].data_ptr(), _ptr(running_mean),
                      _ptr(running_var), eps, momentum, M, Ch, int(relu), True, sm_count(y.device.index or 0), _stream(),
-                     _ptr(mask), _ptr(zq), slot or 0)
+                     _ptr(mask), _ptr(zq), slot or 0, _ptr(sample_scale), H * W)
         if twin:
             if zq is not None:
                 _fp8.attach_twin(z, zq, idx)
@@ -1014,18 +1084,33 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
     return (z, None, None) if want_mask else (z, None)
 
 
+def _check_sample_scale(sample_scale, y, relu, residual, train) -> None:
+    if sample_scale is None:
+        return
+    if int(relu) != 0 or residual is None or not train:
+        raise ValueError("bn: a per-sample scale (stochastic depth) needs training, a residual and no activation")
+    if sample_scale.dtype != torch.float32 or not sample_scale.is_cuda or sample_scale.dim() != 1 \
+            or sample_scale.shape[0] != y.shape[0] or not sample_scale.is_contiguous():
+        raise ValueError(f"bn: sample_scale must be a contiguous CUDA fp32 [{y.shape[0]}] tensor")
+
+
 def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, save: torch.Tensor, gamma: torch.Tensor,
                relu: bool, want_dres: bool, gamma_grad: Optional[torch.Tensor], beta_grad: Optional[torch.Tensor],
                beta: Optional[torch.Tensor] = None, had_residual: bool = True, zmask: Optional[torch.Tensor] = None,
-               pre_reduced: Optional[torch.Tensor] = None):
+               pre_reduced: Optional[torch.Tensor] = None, sample_scale: Optional[torch.Tensor] = None):
     """Returns (dy, dres|None, scratch); accumulates into gamma_grad / beta_grad (fp32) when given.
     ``pre_reduced``: fp32 [2, C] holding (dbeta, dgamma) already (``conv_dgrad(..., bn_reduce=...)``): only the
     elementwise pass runs.
 
     ReLU mask source: recomputed from y when the layer had no residual (``beta`` given), else the bit mask written by
-    the forward (``zmask``), else the saved output ``z``."""
+    the forward (``zmask``), else the saved output ``z``.  ``sample_scale``: the forward's per-sample scale (stochastic
+    depth): the BN sees dz * sample_scale[n] while dres = dz."""
     C = _C()
     _check_act(dz, "dz")
+    if sample_scale is not None:
+        _check_sample_scale(sample_scale, y, relu, True, True)
+        if pre_reduced is not None or zmask is not None:
+            raise ValueError("bn_act_bwd: a per-sample scale takes neither pre-reduced sums nor a bit mask")
     N, Ch, H, W = y.shape
     M = N * H * W
     dy = torch.empty_like(y)
@@ -1038,14 +1123,14 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
         raise ValueError("bn_act_bwd: need z or zmask for the ReLU mask of a residual layer")
     if int(relu) == 2 and not mask_from_x and zmask is not None:
         raise ValueError("bn_act_bwd: ReLU6 has no bit-mask variant (pass z)")
-    if int(relu) == 3 and (not mask_from_x or want_dres):
-        raise ValueError("bn_act_bwd: hardswish recomputes its input from y (pass beta, had_residual=False)")
+    if int(relu) in (3, 4) and (not mask_from_x or want_dres):
+        raise ValueError("bn_act_bwd: hardswish / SiLU recompute their input from y (pass beta, had_residual=False)")
     from . import fp8 as _fp8
 
     dyq = slot = None
     key = ("grad", gamma.data_ptr(), N, H, W)
-    twin = _fp8.enabled() and int(relu) not in (2, 3) and Ch % 128 == 0 and M >= 2048 and \
-        _fp8.note_producer(dy, key)                               # an fp8 dgrad consumed it before
+    twin = _fp8.enabled() and int(relu) not in (2, 3, 4) and sample_scale is None and Ch % 128 == 0 and M >= 2048 \
+        and _fp8.note_producer(dy, key)                           # an fp8 dgrad consumed it before
     if twin:
         idx, fused = _fp8.producer_slot(key, y.device, dy, e5m2=True)
         if fused:
@@ -1054,7 +1139,7 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
                  save[1].data_ptr(), gamma.data_ptr(), _ptr(beta), scratch[0].data_ptr(), scratch[1].data_ptr(),
                  _ptr(gamma_grad), _ptr(beta_grad), M, Ch, int(relu), int(mask_from_x), sm_count(y.device.index or 0),
                  _stream(), _ptr(zmask) if (relu and not mask_from_x) else 0, pre_reduced is not None, _ptr(dyq),
-                 slot or 0)
+                 slot or 0, _ptr(sample_scale), H * W)
     if twin:
         if dyq is not None:
             _fp8.attach_twin(dy, dyq, idx)

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Per-layer timing of the depthwise convolutions of MobileNetV2 (3x3) or MobileNetV3-Large / -Small (3x3 and 5x5):
+"""Per-layer timing of the depthwise convolutions of MobileNetV2 (3x3), MobileNetV3-Large / -Small or EfficientNet-B0
+(3x3 and 5x5):
 native stencil kernels (forward with BN statistics, data gradient, weight gradient) against cuDNN's bf16 channels_last
 F.conv2d(groups=C) and aten.convolution_backward.  CUDA events, L2 flushed before every run, median of --iters runs.
 
@@ -7,7 +8,8 @@ A depthwise convolution is bound by HBM bandwidth, so each row also gives the ac
 move (forward: read x, write y; data gradient: read dy, write dx; weight gradient: read x and dy) and its fraction of
 the H100 SXM data sheet's 3.35 TB/s.  The card's name, power limit and maximum SM clock are printed with the table.
 
-    python tools/depthwise_bench.py [--model mobilenet_v2|mobilenet_v3_large|mobilenet_v3_small] [--batch 256]
+    python tools/depthwise_bench.py [--model mobilenet_v2|mobilenet_v3_large|mobilenet_v3_small|efficientnet_b0]
+                                    [--batch 256]
                                     [--iters 20]
 """
 import argparse
@@ -29,6 +31,9 @@ SHAPES_V3 = {
     "mobilenet_v3_small": [(16, 112, 3, 2, 1), (72, 56, 3, 2, 1), (88, 28, 3, 1, 1), (96, 28, 5, 2, 1),
                            (240, 14, 5, 1, 2), (120, 14, 5, 1, 1), (144, 14, 5, 1, 1), (288, 14, 5, 2, 1),
                            (576, 7, 5, 1, 2)],
+    "efficientnet_b0": [(32, 112, 3, 1, 1), (96, 112, 3, 2, 1), (144, 56, 3, 1, 1), (144, 56, 5, 2, 1),
+                        (240, 28, 5, 1, 1), (240, 28, 3, 2, 1), (480, 14, 3, 1, 2), (480, 14, 5, 1, 1),
+                        (672, 14, 5, 1, 2), (672, 14, 5, 2, 1), (1152, 7, 5, 1, 3), (1152, 7, 3, 1, 1)],
 }
 HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
 
