@@ -158,6 +158,8 @@ KERNEL_LAUNCHES = {
     "dwconv_fwd": 1, "dwconv_dgrad": 1, "dwconv_wgrad": 1, "se_scale": 1, "se_reduce": 1, "se_apply": 1,
     "hardswish_fwd": 1, "hardswish_bwd": 1, "se_sig_scale": 1, "se_sig_reduce": 1, "se_sig_apply": 1, "pad_cols_bf16": 1,
     "fold_cols_f32": 1, "silu_rows_fwd": 1, "silu_rows_bwd": 1, "stochastic_depth_keep": 1,
+    "dwconv7_fwd": 1, "dwconv7_dgrad": 1, "dwconv7_wgrad": 1, "layer_norm_fwd": 1, "layer_norm_bwd": 1, "gelu_fwd": 1,
+    "gelu_bwd": 1, "layer_scale_fwd": 1, "layer_scale_bwd": 1,
 }
 LAUNCH_COUNT = [0]          # kernels of THIS repo launched so far (bench.py reports the per-region delta)
 

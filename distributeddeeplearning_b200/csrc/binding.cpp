@@ -406,6 +406,62 @@ PYBIND11_MODULE(_C, m) {
                  : k == 5 ? ddl::launch_dwconv5_wgrad(a, sms, S(stream)) : cudaErrorInvalidValue, "dwconv_wgrad");
   }, py::arg("x"), py::arg("dy"), py::arg("gw"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("C"), py::arg("P"),
      py::arg("Q"), py::arg("stride"), py::arg("sms"), py::arg("stream"), py::arg("k") = 3);
+  // ------------------------------------------------------------------ depthwise 7x7 with a bias (ConvNeXt)
+  // l1: the L1 mapping instead of the halo tile (tools/depthwise_bench.py compares the two)
+  m.def("dwconv7_fwd", [](ptr_t x, ptr_t w, ptr_t bias, ptr_t y, int N, int H, int W, int C, int sms, ptr_t stream,
+                          int l1) {
+    ddl::Dw7Args a{};
+    a.x = P<const __nv_bfloat16>(x); a.w = P<const __nv_bfloat16>(w); a.bias = P<const float>(bias);
+    a.y = P<__nv_bfloat16>(y); a.N = N; a.H = H; a.W = W; a.C = C;
+    check(ddl::launch_dwconv7_fwd(a, sms, l1 != 0, S(stream)), "dwconv7_fwd");
+  }, py::arg("x"), py::arg("w"), py::arg("bias"), py::arg("y"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("C"),
+     py::arg("sms"), py::arg("stream"), py::arg("l1") = 0);
+  m.def("dwconv7_dgrad", [](ptr_t dy, ptr_t w, ptr_t add, ptr_t dx, int N, int H, int W, int C, int sms, ptr_t stream,
+                            int l1) {
+    ddl::Dw7Args a{};
+    a.dy = P<const __nv_bfloat16>(dy); a.w = P<const __nv_bfloat16>(w); a.add = P<const __nv_bfloat16>(add);
+    a.y = P<__nv_bfloat16>(dx); a.N = N; a.H = H; a.W = W; a.C = C;
+    check(ddl::launch_dwconv7_dgrad(a, sms, l1 != 0, S(stream)), "dwconv7_dgrad");
+  }, py::arg("dy"), py::arg("w"), py::arg("add"), py::arg("dx"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("C"),
+     py::arg("sms"), py::arg("stream"), py::arg("l1") = 0);
+  m.def("dwconv7_wgrad", [](ptr_t x, ptr_t dy, ptr_t gw, ptr_t gb, int N, int H, int W, int C, int sms, ptr_t stream) {
+    ddl::Dw7Args a{};
+    a.x = P<const __nv_bfloat16>(x); a.dy = P<const __nv_bfloat16>(dy); a.gw = P<float>(gw); a.gb = P<float>(gb);
+    a.N = N; a.H = H; a.W = W; a.C = C;
+    check(ddl::launch_dwconv7_wgrad(a, sms, S(stream)), "dwconv7_wgrad");
+  });
+  // ------------------------------------------------------------------ ConvNeXt row kernels (LayerNorm, GELU, layer scale)
+  m.def("layer_norm_fwd", [](ptr_t x, ptr_t gamma, ptr_t beta, ptr_t y, ptr_t mean, ptr_t rstd, int M, int C, float eps,
+                             int sms, ptr_t stream) {
+    check(ddl::launch_layer_norm_fwd(P<const __nv_bfloat16>(x), P<const float>(gamma), P<const float>(beta),
+                                     P<__nv_bfloat16>(y), P<float>(mean), P<float>(rstd), M, C, eps, sms, S(stream)),
+          "layer_norm_fwd");
+  });
+  m.def("layer_norm_bwd", [](ptr_t dy, ptr_t x, ptr_t mean, ptr_t rstd, ptr_t gamma, ptr_t dx, ptr_t dgamma, ptr_t dbeta,
+                             int M, int C, int sms, ptr_t stream) {
+    check(ddl::launch_layer_norm_bwd(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(x), P<const float>(mean),
+                                     P<const float>(rstd), P<const float>(gamma), P<__nv_bfloat16>(dx), P<float>(dgamma),
+                                     P<float>(dbeta), M, C, sms, S(stream)), "layer_norm_bwd");
+  });
+  m.def("gelu_fwd", [](ptr_t h, ptr_t g, int64_t n, int sms, ptr_t stream) {
+    check(ddl::launch_gelu_fwd(P<const __nv_bfloat16>(h), P<__nv_bfloat16>(g), n, sms, S(stream)), "gelu_fwd");
+  });
+  m.def("gelu_bwd", [](ptr_t dg, ptr_t h, ptr_t dh, ptr_t dbias, int M, int C, int sms, ptr_t stream) {
+    check(ddl::launch_gelu_bwd(P<const __nv_bfloat16>(dg), P<const __nv_bfloat16>(h), P<__nv_bfloat16>(dh), P<float>(dbias),
+                               M, C, sms, S(stream)), "gelu_bwd");
+  });
+  m.def("layer_scale_fwd", [](ptr_t y, ptr_t ls, ptr_t keep, ptr_t x, ptr_t z, int M, int C, int hw, int sms,
+                              ptr_t stream) {
+    check(ddl::launch_layer_scale_fwd(P<const __nv_bfloat16>(y), P<const float>(ls), P<const float>(keep),
+                                      P<const __nv_bfloat16>(x), P<__nv_bfloat16>(z), M, C, hw, sms, S(stream)),
+          "layer_scale_fwd");
+  });
+  m.def("layer_scale_bwd", [](ptr_t dz, ptr_t y, ptr_t ls, ptr_t keep, ptr_t dy, ptr_t dls, ptr_t dbias, int M, int C,
+                              int hw, int sms, ptr_t stream) {
+    check(ddl::launch_layer_scale_bwd(P<const __nv_bfloat16>(dz), P<const __nv_bfloat16>(y), P<const float>(ls),
+                                      P<const float>(keep), P<__nv_bfloat16>(dy), P<float>(dls), P<float>(dbias), M, C, hw,
+                                      sms, S(stream)), "layer_scale_bwd");
+  });
   // ------------------------------------------------------------------ squeeze-excitation
   m.def("se_scale", [](ptr_t x, ptr_t s, int lds, ptr_t y, int N, int HW, int C, int sms, ptr_t stream) {
     check(ddl::launch_se_scale(P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(s), lds, P<__nv_bfloat16>(y), N, HW, C,

@@ -90,6 +90,49 @@ cudaError_t launch_dwconv_wgrad(const DwConvArgs& a, int sms, cudaStream_t strea
 cudaError_t launch_dwconv5_fwd(const DwConvArgs& a, int sms, cudaStream_t stream);
 cudaError_t launch_dwconv5_dgrad(const DwConvArgs& a, int sms, cudaStream_t stream);
 cudaError_t launch_dwconv5_wgrad(const DwConvArgs& a, int sms, cudaStream_t stream);
+// ---- depthwise 7x7 with a bias (depthwise7.cu; ConvNeXt): stride 1, padding 3, x / y / dy / dx [N][H][W][C] bf16 ----
+struct Dw7Args {
+  const __nv_bfloat16* x;         // forward / wgrad input
+  const __nv_bfloat16* dy;        // dgrad / wgrad output gradient
+  const __nv_bfloat16* w;         // [C][7][7] bf16
+  const float* bias;              // forward: fp32 [C]
+  const __nv_bfloat16* add;       // dgrad, optional: added to dx in its store (the block's residual gradient)
+  __nv_bfloat16* y;               // forward: y;  dgrad: dx
+  float* gw;                      // wgrad: fp32 [C][7][7] gradient, accumulated (+=)
+  float* gb;                      // wgrad, optional: fp32 [C] bias gradient, accumulated (+=)
+  int N, H, W, C;
+  int lg_gpc;                     // set by the launcher: log2 of the 8-channel groups per block
+};
+// l1: the L1 mapping of the 5x5 kernels instead of the shared-memory halo tile (for timing the two against each other)
+cudaError_t launch_dwconv7_fwd(const Dw7Args& a, int sms, bool l1, cudaStream_t stream);
+cudaError_t launch_dwconv7_dgrad(const Dw7Args& a, int sms, bool l1, cudaStream_t stream);
+cudaError_t launch_dwconv7_wgrad(const Dw7Args& a, int sms, cudaStream_t stream);
+
+// ---- ConvNeXt row kernels (convnext.cu) ------------------------------------------------------------------------------
+// LayerNorm over the C channels of each row of a bf16 [M][C] matrix (an NHWC activation or [N][C]), C % 8 == 0 and
+// C / 8 = T * V with T a power of two <= 32 threads per row and V <= 6 vectors per thread.
+// forward: y = (x - mean) * rstd * gamma + beta, saving fp32 mean / rstd [M]
+cudaError_t launch_layer_norm_fwd(const __nv_bfloat16* x, const float* gamma, const float* beta, __nv_bfloat16* y,
+                                  float* mean, float* rstd, int M, int C, float eps, int sms, cudaStream_t stream);
+// backward: dx = rstd * (g dy - mean_c(g dy) - xhat * mean_c(g dy xhat)), g = gamma; dgamma += sum_m dy xhat,
+// dbeta += sum_m dy (each optional)
+cudaError_t launch_layer_norm_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* x, const float* mean, const float* rstd,
+                                  const float* gamma, __nv_bfloat16* dx, float* dgamma, float* dbeta, int M, int C, int sms,
+                                  cudaStream_t stream);
+// exact GELU on n bf16 elements (n % 8 == 0): g = h * Phi(h)
+cudaError_t launch_gelu_fwd(const __nv_bfloat16* h, __nv_bfloat16* g, int64_t n, int sms, cudaStream_t stream);
+// dh = dg * (Phi(h) + h * phi(h)) on [M][C]; dbias[c] += sum_m dh (optional): fc1's bias gradient, summed over the
+// stored bf16 dh (as bias_relu_bwd sums its bf16 dy)
+cudaError_t launch_gelu_bwd(const __nv_bfloat16* dg, const __nv_bfloat16* h, __nv_bfloat16* dh, float* dbias, int M, int C,
+                            int sms, cudaStream_t stream);
+// layer scale + stochastic depth + residual on [M][C] (M = N * hw): z = ls[c] * y * keep[m / hw] + x (keep optional)
+cudaError_t launch_layer_scale_fwd(const __nv_bfloat16* y, const float* ls, const float* keep, const __nv_bfloat16* x,
+                                   __nv_bfloat16* z, int M, int C, int hw, int sms, cudaStream_t stream);
+// dy = dz * ls[c] * keep[m / hw];  dls[c] += sum_m dz * keep * y;  dbias[c] += sum_m dy over the stored bf16 dy
+// (dls / dbias optional)
+cudaError_t launch_layer_scale_bwd(const __nv_bfloat16* dz, const __nv_bfloat16* y, const float* ls, const float* keep,
+                                   __nv_bfloat16* dy, float* dls, float* dbias, int M, int C, int hw, int sms,
+                                   cudaStream_t stream);
 
 // ---- pooling -------------------------------------------------------------------------------------
 struct PoolArgs {

@@ -5,11 +5,13 @@ Parity: the reference resolves ``--model`` with ``getattr(torchvision.models, na
 (``imagenet_pytorch_horovod.py:383``).  North-star zoo: ResNet-50/101/152, VGG-16, Inception-v3,
 AlexNet (SURVEY.md 2.7); ResNet-18/34, the other VGG depths, DenseNet and SqueezeNet (the rest of torchvision
 0.2.1's families) are here too, and the later ResNet family members of torchvision (ResNeXt-50 32x4d, ResNeXt-101
-32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2, MobileNetV3-Large / -Small and EfficientNet-B0 to -B7.
+32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2, MobileNetV3-Large / -Small, EfficientNet-B0 to -B7 and
+ConvNeXt-Tiny / -Small / -Base / -Large.
 """
 from __future__ import annotations
 
 from .alexnet import AlexNet, alexnet  # noqa: F401
+from .convnext import ConvNeXt, convnext_base, convnext_large, convnext_small, convnext_tiny  # noqa: F401
 from .densenet import DenseNet, densenet121, densenet161, densenet169, densenet201  # noqa: F401
 from .efficientnet import (INPUT_SIZE as _EFFICIENTNET_INPUT_SIZE, EfficientNet, efficientnet_b0,  # noqa: F401
                            efficientnet_b1, efficientnet_b2, efficientnet_b3, efficientnet_b4, efficientnet_b5,
@@ -24,8 +26,9 @@ from .vgg import VGG, vgg11, vgg11_bn, vgg13, vgg13_bn, vgg16, vgg16_bn, vgg19, 
 
 _REGISTRY = {
     f.__name__: f
-    for f in (alexnet, densenet121, densenet161, densenet169, densenet201, efficientnet_b0, efficientnet_b1,
-              efficientnet_b2, efficientnet_b3, efficientnet_b4, efficientnet_b5, efficientnet_b6, efficientnet_b7,
+    for f in (alexnet, convnext_tiny, convnext_small, convnext_base, convnext_large, densenet121, densenet161,
+              densenet169, densenet201, efficientnet_b0, efficientnet_b1, efficientnet_b2, efficientnet_b3,
+              efficientnet_b4, efficientnet_b5, efficientnet_b6, efficientnet_b7,
               squeezenet1_0, squeezenet1_1, inception_v3, mobilenet_v2,
               mobilenet_v3_large, mobilenet_v3_small, resnet18, resnet34, resnet50, resnet101, resnet152,
               resnext50_32x4d, resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2, vgg11, vgg11_bn, vgg13,

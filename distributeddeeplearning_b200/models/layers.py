@@ -75,6 +75,23 @@ class BatchNorm2d(nn.Module):
         return f"{self.num_features}, eps={self.eps}, momentum={self.momentum}"
 
 
+class LayerNorm(nn.Module):
+    """Affine parameters holder of a LayerNorm over channels (same state_dict as nn.LayerNorm(C)); ``forward``
+    normalises the channels of an NHWC activation [N, C, H, W] or of a matrix [N, C]."""
+
+    def __init__(self, num_features, eps=1e-5):
+        super().__init__()
+        self.normalized_shape, self.eps = (num_features,), eps
+        self.weight = nn.Parameter(torch.ones(num_features))
+        self.bias = nn.Parameter(torch.zeros(num_features))
+
+    def forward(self, x):
+        return ops.layer_norm_channels(x, self.weight, self.bias, self.eps)
+
+    def extra_repr(self):
+        return f"{self.normalized_shape}, eps={self.eps}"
+
+
 def conv_bn(x, conv: Conv2d, bn: BatchNorm2d, relu=True, residual=None, relu6=False, hardswish=False, silu=False,
             sample_scale=None):
     """act(BN(conv(x)) [+ residual]) through the fused op (``relu6``: the activation is ReLU6; ``hardswish``: it is

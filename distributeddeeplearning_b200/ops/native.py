@@ -376,6 +376,13 @@ def depthwise_native(c: int, kernel, stride: int, pad, dil: int, groups: int) ->
         supports_depthwise5(c, kernel, stride, pad, dil, groups)
 
 
+def supports_depthwise7(c: int, kernel, stride: int, pad, dil: int, groups: int) -> bool:
+    """Depthwise convolutions the 7x7 kernels of csrc/ops/depthwise7.cu handle: ``groups == Cin == Cout = c`` with
+    ``c % 8 == 0``, a 7x7 kernel, stride 1, padding 3 and dilation 1 (ConvNeXt's depthwise layers, which carry a bias).
+    They are separate from :func:`depthwise_native`, which decides what ``conv_bn_act`` sends to its depthwise node."""
+    return _depthwise_ok(7, c, kernel, stride, pad, dil, groups) and stride == 1
+
+
 def _check_dw(c: int, w_bf16: torch.Tensor, stride: int, k: int) -> None:
     if not depthwise_native(c, (k, k), stride, k // 2, 1, c):
         raise ValueError(f"depthwise {k}x{k} conv with {c} channels, stride {stride} is not supported by the native "
@@ -440,6 +447,197 @@ def dwconv_wgrad(x: torch.Tensor, dy: torch.Tensor, grad_w: torch.Tensor, stride
         raise ValueError(f"dwconv_wgrad: grad_w must be a CUDA fp32 [C, 1, {k}, {k}] (KRSC) tensor")
     _C().dwconv_wgrad(x.data_ptr(), dy.data_ptr(), grad_w.data_ptr(), N, H, W, Ch, P, Q, stride,
                       sm_count(x.device.index or 0), _stream(), k)
+
+
+# ------------------------------------------------------------------------------------------------
+# depthwise 7x7 with a bias (csrc/ops/depthwise7.cu) and the ConvNeXt row kernels (csrc/ops/convnext.cu)
+# ------------------------------------------------------------------------------------------------
+def _check_dw7(x: torch.Tensor, name: str, w_bf16: Optional[torch.Tensor] = None) -> None:
+    _check_act(x, name)
+    if x.dim() != 4 or not supports_depthwise7(x.shape[1], (7, 7), 1, 3, 1, x.shape[1]):
+        raise ValueError(f"{name}: the depthwise 7x7 kernels need a 4-D activation with a multiple of 8 channels")
+    _check_aligned(x, name)
+    if w_bf16 is not None and (w_bf16.dtype != torch.bfloat16 or w_bf16.numel() != x.shape[1] * 49
+                               or not w_bf16.is_contiguous() or not w_bf16.is_cuda):
+        raise ValueError("depthwise 7x7: expected contiguous CUDA bf16 weights [C, 49] (KRSC of [C, 1, 7, 7])")
+
+
+def _check_f32_vec(t: Optional[torch.Tensor], n: int, name: str) -> None:
+    if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.numel() != n or not t.is_contiguous()):
+        raise ValueError(f"{name}: expected a contiguous CUDA fp32 tensor of {n} elements")
+
+
+def dwconv7_fwd(x: torch.Tensor, w_bf16: torch.Tensor, bias: torch.Tensor, l1: bool = False) -> torch.Tensor:
+    """y = depthwise 7x7 conv (stride 1, padding 3) of x with the bf16 weights [C, 49], plus the fp32 bias [C].
+    ``l1``: run the L1 mapping of the 5x5 kernels instead of the shared-memory halo tile (tools/depthwise_bench.py times
+    the two against each other; the model path uses the halo tile)."""
+    _check_dw7(x, "x", w_bf16)
+    N, Ch, H, W = x.shape
+    _check_f32_vec(bias, Ch, "bias")
+    y = torch.empty_like(x)
+    _C().dwconv7_fwd(x.data_ptr(), w_bf16.data_ptr(), bias.data_ptr(), y.data_ptr(), N, H, W, Ch,
+                     sm_count(x.device.index or 0), _stream(), int(l1))
+    return y
+
+
+def dwconv7_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, add: Optional[torch.Tensor] = None,
+                  l1: bool = False) -> torch.Tensor:
+    """dx = conv_transpose(dy, w) of :func:`dwconv7_fwd` (+ ``add``, a same-shape tensor added in the store); ``l1`` as
+    in :func:`dwconv7_fwd`."""
+    _check_dw7(dy, "dy", w_bf16)
+    if add is not None:
+        _check_act(add, "add")
+        _check_aligned(add, "add")
+        if add.shape != dy.shape:
+            raise ValueError("dwconv7_dgrad: add must have the shape of dy")
+    N, Ch, H, W = dy.shape
+    dx = torch.empty_like(dy)
+    _C().dwconv7_dgrad(dy.data_ptr(), w_bf16.data_ptr(), _ptr(add), dx.data_ptr(), N, H, W, Ch,
+                       sm_count(dy.device.index or 0), _stream(), int(l1))
+    return dx
+
+
+def dwconv7_wgrad(x: torch.Tensor, dy: torch.Tensor, grad_w: torch.Tensor, grad_b: Optional[torch.Tensor]) -> None:
+    """grad_w [C, 1, 7, 7] (fp32 KRSC) += the weight gradient of :func:`dwconv7_fwd`; grad_b [C] += sum of dy."""
+    _check_dw7(x, "x")
+    _check_dw7(dy, "dy")
+    if dy.shape != x.shape:
+        raise ValueError("dwconv7_wgrad: dy must have the shape of x")
+    N, Ch, H, W = x.shape
+    if grad_w.dtype != torch.float32 or grad_w.numel() != Ch * 49 or not grad_w.is_contiguous(memory_format=CL) \
+            or not grad_w.is_cuda:
+        raise ValueError("dwconv7_wgrad: grad_w must be a CUDA fp32 [C, 1, 7, 7] (KRSC) tensor")
+    _check_f32_vec(grad_b, Ch, "grad_b")
+    _C().dwconv7_wgrad(x.data_ptr(), dy.data_ptr(), grad_w.data_ptr(), _ptr(grad_b), N, H, W, Ch,
+                       sm_count(x.device.index or 0), _stream())
+
+
+def supports_layer_norm(c: int) -> bool:
+    """Channel counts the LayerNorm kernels take: C % 8 == 0 with C / 8 = T * V, T the largest power of two <= 32
+    dividing C / 8 and V <= 6 (every ConvNeXt width, 96 to 1536)."""
+    if c <= 0 or c % 8 != 0:
+        return False
+    v = c // 8
+    t = 1
+    while t < 32 and v % (2 * t) == 0:
+        t *= 2
+    return v // t <= 6
+
+
+def _rows(x: torch.Tensor) -> Tuple[int, int]:
+    """(rows, channels) of an NHWC activation [N, C, H, W] or a matrix [N, C]."""
+    if x.dim() == 4:
+        return x.shape[0] * x.shape[2] * x.shape[3], x.shape[1]
+    if x.dim() == 2:
+        return x.shape[0], x.shape[1]
+    raise ValueError("expected an NHWC activation [N, C, H, W] or a matrix [N, C]")
+
+
+def layer_norm_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float):
+    """LayerNorm over the channels of every row: returns (y bf16 like x, mean fp32 [rows], rstd fp32 [rows])."""
+    _check_act(x)
+    _check_aligned(x, "x")
+    M, Ch = _rows(x)
+    if not supports_layer_norm(Ch):
+        raise ValueError(f"layer_norm: {Ch} channels are not supported by the native kernels")
+    _check_f32_vec(gamma, Ch, "gamma")
+    _check_f32_vec(beta, Ch, "beta")
+    y = torch.empty_like(x)
+    mean = torch.empty(M, dtype=torch.float32, device=x.device)
+    rstd = torch.empty(M, dtype=torch.float32, device=x.device)
+    _C().layer_norm_fwd(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
+                        M, Ch, float(eps), sm_count(x.device.index or 0), _stream())
+    return y, mean, rstd
+
+
+def layer_norm_bwd(dy: torch.Tensor, x: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor, gamma: torch.Tensor,
+                   grad_gamma: Optional[torch.Tensor], grad_beta: Optional[torch.Tensor]) -> torch.Tensor:
+    """dx of :func:`layer_norm_fwd` from the saved x, mean and rstd; grad_gamma += sum dy * xhat, grad_beta += sum dy."""
+    _check_act(dy, "dy")
+    _check_act(x)
+    _check_aligned(dy, "dy")
+    if dy.shape != x.shape:
+        raise ValueError("layer_norm_bwd: dy must have the shape of x")
+    M, Ch = _rows(x)
+    for t, name in ((gamma, "gamma"), (grad_gamma, "grad_gamma"), (grad_beta, "grad_beta")):
+        _check_f32_vec(t, Ch, name)
+    dx = torch.empty_like(x)
+    _C().layer_norm_bwd(dy.data_ptr(), x.data_ptr(), mean.data_ptr(), rstd.data_ptr(), gamma.data_ptr(), dx.data_ptr(),
+                        _ptr(grad_gamma), _ptr(grad_beta), M, Ch, sm_count(x.device.index or 0), _stream())
+    return dx
+
+
+def gelu_fwd(h: torch.Tensor) -> torch.Tensor:
+    """g = h * Phi(h) (exact GELU) elementwise."""
+    _check_act(h, "h")           # dense NHWC or a contiguous matrix: elementwise over the memory
+    if h.numel() % 8 != 0:
+        raise ValueError("gelu_fwd: expected a multiple of 8 elements")
+    _check_aligned(h, "h")
+    g = torch.empty_like(h)
+    _C().gelu_fwd(h.data_ptr(), g.data_ptr(), h.numel(), sm_count(h.device.index or 0), _stream())
+    return g
+
+
+def gelu_bwd(dg: torch.Tensor, h: torch.Tensor, grad_bias: Optional[torch.Tensor]) -> torch.Tensor:
+    """dh = dg * (Phi(h) + h phi(h)) from the saved pre-activation h; grad_bias [C] += the column sums of dh."""
+    _check_act(dg, "dg")
+    _check_act(h, "h")
+    if dg.shape != h.shape:
+        raise ValueError("gelu_bwd: dg must have the shape of h")
+    M, Ch = _rows(h)
+    if Ch % 8 != 0 or Ch > 8192:
+        raise ValueError("gelu_bwd: the channel count must be a multiple of 8, at most 8192")
+    _check_aligned(dg, "dg")
+    _check_aligned(h, "h")
+    _check_f32_vec(grad_bias, Ch, "grad_bias")
+    dh = torch.empty_like(h)
+    _C().gelu_bwd(dg.data_ptr(), h.data_ptr(), dh.data_ptr(), _ptr(grad_bias), M, Ch, sm_count(h.device.index or 0),
+                  _stream())
+    return dh
+
+
+def _check_keep(keep: Optional[torch.Tensor], n: int) -> None:
+    if keep is not None and (keep.dtype != torch.float32 or not keep.is_cuda or keep.dim() != 1 or keep.shape[0] != n
+                             or not keep.is_contiguous()):
+        raise ValueError(f"layer scale: keep must be a contiguous CUDA fp32 [{n}] tensor")
+
+
+def layer_scale_fwd(y: torch.Tensor, ls: torch.Tensor, keep: Optional[torch.Tensor], x: torch.Tensor) -> torch.Tensor:
+    """z = ls[c] * y * keep[n] + x for NHWC activations y, x [N, C, H, W] (``keep``: stochastic depth, or None)."""
+    _check_act(y, "y")
+    _check_act(x)
+    if y.dim() != 4 or y.shape != x.shape or y.shape[1] % 8 != 0:
+        raise ValueError("layer_scale_fwd: y and x must be NHWC activations of one shape, C a multiple of 8")
+    _check_aligned(y, "y")
+    _check_aligned(x, "x")
+    N, Ch, H, W = y.shape
+    _check_f32_vec(ls, Ch, "ls")
+    _check_keep(keep, N)
+    z = torch.empty_like(x)
+    _C().layer_scale_fwd(y.data_ptr(), ls.data_ptr(), _ptr(keep), x.data_ptr(), z.data_ptr(), N * H * W, Ch, H * W,
+                         sm_count(y.device.index or 0), _stream())
+    return z
+
+
+def layer_scale_bwd(dz: torch.Tensor, y: torch.Tensor, ls: torch.Tensor, keep: Optional[torch.Tensor],
+                    grad_ls: Optional[torch.Tensor], grad_bias: Optional[torch.Tensor]) -> torch.Tensor:
+    """dy = dz * ls[c] * keep[n]; grad_ls += sum dz * keep * y; grad_bias (fc2's) += sum dy."""
+    _check_act(dz, "dz")
+    _check_act(y, "y")
+    if dz.shape != y.shape or y.dim() != 4:
+        raise ValueError("layer_scale_bwd: dz must have the shape of y")
+    _check_aligned(dz, "dz")
+    _check_aligned(y, "y")
+    N, Ch, H, W = y.shape
+    if Ch % 8 != 0 or Ch > 4096:
+        raise ValueError("layer_scale_bwd: the channel count must be a multiple of 8, at most 4096")
+    for t, name in ((ls, "ls"), (grad_ls, "grad_ls"), (grad_bias, "grad_bias")):
+        _check_f32_vec(t, Ch, name)
+    _check_keep(keep, N)
+    dy = torch.empty_like(y)
+    _C().layer_scale_bwd(dz.data_ptr(), y.data_ptr(), ls.data_ptr(), _ptr(keep), dy.data_ptr(), _ptr(grad_ls),
+                         _ptr(grad_bias), N * H * W, Ch, H * W, sm_count(y.device.index or 0), _stream())
+    return dy
 
 
 # ------------------------------------------------------------------------------------------------

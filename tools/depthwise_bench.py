@@ -1,14 +1,18 @@
 #!/usr/bin/env python
 """Per-layer timing of the depthwise convolutions of MobileNetV2 (3x3), MobileNetV3-Large / -Small or EfficientNet-B0
-(3x3 and 5x5):
+(3x3 and 5x5), or ConvNeXt-Tiny (7x7 with a bias):
 native stencil kernels (forward with BN statistics, data gradient, weight gradient) against cuDNN's bf16 channels_last
 F.conv2d(groups=C) and aten.convolution_backward.  CUDA events, L2 flushed before every run, median of --iters runs.
+For 7x7 the forward adds the bias (cuDNN's too), the weight gradient also reduces the bias gradient, and the forward and
+data gradient are timed twice: with the shared-memory halo tile the model uses, and with the L1 mapping of the 5x5
+kernels (columns fwd-L1, dgrad-L1), the comparison that decides which of the two the model keeps.
 
 A depthwise convolution is bound by HBM bandwidth, so each row also gives the achieved bandwidth from the bytes the pass must
 move (forward: read x, write y; data gradient: read dy, write dx; weight gradient: read x and dy) and its fraction of
 the H100 SXM data sheet's 3.35 TB/s.  The card's name, power limit and maximum SM clock are printed with the table.
 
-    python tools/depthwise_bench.py [--model mobilenet_v2|mobilenet_v3_large|mobilenet_v3_small|efficientnet_b0]
+    python tools/depthwise_bench.py [--model mobilenet_v2|mobilenet_v3_large|mobilenet_v3_small|efficientnet_b0|
+                                             convnext_tiny]
                                     [--batch 256]
                                     [--iters 20]
 """
@@ -34,6 +38,7 @@ SHAPES_V3 = {
     "efficientnet_b0": [(32, 112, 3, 1, 1), (96, 112, 3, 2, 1), (144, 56, 3, 1, 1), (144, 56, 5, 2, 1),
                         (240, 28, 5, 1, 1), (240, 28, 3, 2, 1), (480, 14, 3, 1, 2), (480, 14, 5, 1, 1),
                         (672, 14, 5, 1, 2), (672, 14, 5, 2, 1), (1152, 7, 5, 1, 3), (1152, 7, 3, 1, 1)],
+    "convnext_tiny": [(96, 56, 7, 1, 3), (192, 28, 7, 1, 3), (384, 14, 7, 1, 9), (768, 7, 7, 1, 3)],
 }
 HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
 
@@ -86,25 +91,36 @@ def main():
     if v3:
         print(f"# {a.model}")
     print(f"{'C':>4} {'HW':>3} " + (f"{'k':>1} " if v3 else "") + f"{'s':>1} {'n':>1} | {'fwd':>7} {'cudnn':>7} {'GB/s':>5} {'%':>3} | {'dgrad':>7} {'cudnn':>7} "
-          f"{'GB/s':>5} {'%':>3} | {'wgrad':>7} {'cudnn':>7} {'GB/s':>5} {'%':>3}")
+          f"{'GB/s':>5} {'%':>3} | {'wgrad':>7} {'cudnn':>7} {'GB/s':>5} {'%':>3}"
+          + (f" | {'fwd-L1':>7} {'dgrad-L1':>8}" if a.model == "convnext_tiny" else ""))
     rows = []
     for C, hw, k, s, n in shapes:
         p = k // 2
         x = torch.randn(a.batch, C, hw, hw, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
         w = (torch.randn(C, 1, k, k, device=dev) * 0.3).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
         wb = w.reshape(C, k * k).contiguous()
-        y = nv.dwconv_fwd(x, wb, s, k=k)
+        b = torch.randn(C, device=dev)
+        y = nv.dwconv7_fwd(x, wb, b) if k == 7 else nv.dwconv_fwd(x, wb, s, k=k)
         dy = torch.randn_like(y)
         gw = torch.zeros(C, 1, k, k, device=dev).contiguous(memory_format=torch.channels_last)
+        gb = torch.zeros(C, device=dev)
         bx, by = x.numel() * 2, y.numel() * 2
         r = {"C": C, "HW": hw, **({"k": k} if v3 else {}), "stride": s, "layers": n, "bytes_fwd": bx + by,
              "bytes_dgrad": by + bx, "bytes_wgrad": bx + by}
-        r["fwd"] = timed(lambda: nv.dwconv_fwd(x, wb, s, stats=True, k=k), a.iters, flush)
-        r["fwd_cudnn"] = timed(lambda: F.conv2d(x, w, None, s, p, 1, C), a.iters, flush)
-        r["dgrad"] = timed(lambda: nv.dwconv_dgrad(dy, wb, x.shape, s, k=k), a.iters, flush)
+        if k == 7:
+            r["fwd"] = timed(lambda: nv.dwconv7_fwd(x, wb, b), a.iters, flush)
+            r["fwd_L1"] = timed(lambda: nv.dwconv7_fwd(x, wb, b, l1=True), a.iters, flush)
+            r["fwd_cudnn"] = timed(lambda: F.conv2d(x, w, b.to(torch.bfloat16), s, p, 1, C), a.iters, flush)
+            r["dgrad"] = timed(lambda: nv.dwconv7_dgrad(dy, wb), a.iters, flush)
+            r["dgrad_L1"] = timed(lambda: nv.dwconv7_dgrad(dy, wb, l1=True), a.iters, flush)
+            r["wgrad"] = timed(lambda: nv.dwconv7_wgrad(x, dy, gw, gb), a.iters, flush)
+        else:
+            r["fwd"] = timed(lambda: nv.dwconv_fwd(x, wb, s, stats=True, k=k), a.iters, flush)
+            r["fwd_cudnn"] = timed(lambda: F.conv2d(x, w, None, s, p, 1, C), a.iters, flush)
+            r["dgrad"] = timed(lambda: nv.dwconv_dgrad(dy, wb, x.shape, s, k=k), a.iters, flush)
+            r["wgrad"] = timed(lambda: nv.dwconv_wgrad(x, dy, gw, s, k=k), a.iters, flush)
         r["dgrad_cudnn"] = timed(lambda: torch.ops.aten.convolution_backward(
             dy, x, w, None, [s, s], [p, p], [1, 1], False, [0, 0], C, [True, False, False]), a.iters, flush)
-        r["wgrad"] = timed(lambda: nv.dwconv_wgrad(x, dy, gw, s, k=k), a.iters, flush)
         r["wgrad_cudnn"] = timed(lambda: torch.ops.aten.convolution_backward(
             dy, x, w, None, [s, s], [p, p], [1, 1], False, [0, 0], C, [False, True, False]), a.iters, flush)
         cells = []
@@ -113,10 +129,13 @@ def main():
             r[f"{ph}_GBps"] = gbs
             r[f"{ph}_frac_peak"] = gbs * 1e9 / HBM_BYTES_PER_S
             cells.append(f"{r[ph]:7.1f} {r[ph + '_cudnn']:7.1f} {gbs:5.0f} {100 * r[ph + '_frac_peak']:3.0f}")
+        if k == 7:
+            cells.append(f"{r['fwd_L1']:7.1f} {r['dgrad_L1']:8.1f}")
         rows.append(r)
         print(f"{C:4d} {hw:3d} " + (f"{k:1d} " if v3 else "") + f"{s:1d} {n:1d} | " + " | ".join(cells), flush=True)
     tot = {k: sum(r[k] * r["layers"] for r in rows)
-           for k in ("fwd", "fwd_cudnn", "dgrad", "dgrad_cudnn", "wgrad", "wgrad_cudnn")}
+           for k in ("fwd", "fwd_cudnn", "dgrad", "dgrad_cudnn", "wgrad", "wgrad_cudnn", "fwd_L1", "dgrad_L1")
+           if k in rows[0]}
     print(f"all {sum(r['layers'] for r in rows)} layers (us): " + "  ".join(f"{k}={v:.0f}" for k, v in tot.items()))
     print("JSON " + json.dumps({"device": info, "batch": a.batch, **({"model": a.model} if v3 else {}), "rows": rows,
                                 "totals_us": tot}))

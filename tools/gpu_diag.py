@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 
 
@@ -2583,6 +2583,321 @@ def g_efficientnet():
     ok = all(l == l and abs(l) < 1e4 for l in losses)
     RESULTS.append(ok)
     print(f"[{'ok' if ok else 'FAIL'}] efficientnet_b0 fp8 session: losses {[round(v, 3) for v in losses]}, "
+          f"fp8 launches {fp8.launches()}", flush=True)
+    del s
+    torch.cuda.empty_cache()
+
+
+# depthwise 7x7 layers as (C, H, W, batch): the stage shapes of ConvNeXt-T/S (96..768), -B (128..1024) and -L
+# (192..1536), plus C = 8 / 40 / 48 (one / one / two 8-channel groups per block), batch 1, 1x1 and odd-sized images
+DW7_CASES = [(96, 56, 56, 2), (192, 28, 28, 2), (384, 14, 14, 2), (768, 7, 7, 2), (128, 56, 56, 2), (256, 28, 28, 2),
+             (512, 14, 14, 2), (1024, 7, 7, 2), (192, 56, 56, 1), (384, 28, 28, 2), (768, 14, 14, 2), (1536, 7, 7, 2),
+             (8, 9, 9, 1), (40, 15, 15, 2), (48, 9, 13, 1), (16, 1, 1, 3), (24, 2, 3, 1), (96, 17, 5, 1)]
+
+
+def _dw7_layer(C, H, W, n):
+    """dwconv7 fwd (+bias), dgrad with and without the addend, wgrad + bias gradient (onto pre-filled slots, two
+    passes) against fp32 F.conv2d(groups=C) on the same bf16 operands, element-wise."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    x = cl(bf(torch.randn(n, C, H, W, device="cuda")))
+    w = bf(torch.randn(C, 1, 7, 7, device="cuda") * (2.0 / 49) ** 0.5).contiguous(memory_format=torch.channels_last)
+    b = torch.randn(C, device="cuda")
+    wb = w.reshape(C, 49).contiguous()
+    tag = f"C={C} {H}x{W} N={n}"
+    y = nv.dwconv7_fwd(x, wb, b)
+    yr = F.conv2d(x.float(), w.float(), b, 1, 3, 1, C)
+    report_abs(f"dw7 fwd  {tag}", y, yr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+    report_abs(f"dw7 fwd, L1 mapping {tag}", nv.dwconv7_fwd(x, wb, b, l1=True), yr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+    dy = cl(bf(torch.randn(y.shape, device="cuda")))
+    dxr = torch.nn.grad.conv2d_input(x.shape, w.float(), dy.float(), 1, 3, 1, C)
+    report_abs(f"dw7 dgrad {tag}", nv.dwconv7_dgrad(dy, wb), dxr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+    add = cl(bf(torch.randn(x.shape, device="cuda")))
+    report_abs(f"dw7 dgrad + addend {tag}", nv.dwconv7_dgrad(dy, wb, add=add), dxr + add.float(), 2.0 ** -7, 0.0,
+               arms=2.0 ** -8)
+    report_abs(f"dw7 dgrad + addend, L1 mapping {tag}", nv.dwconv7_dgrad(dy, wb, add=add, l1=True), dxr + add.float(),
+               2.0 ** -7, 0.0, arms=2.0 ** -8)
+    dwr = torch.nn.grad.conv2d_weight(x.float(), w.shape, dy.float(), 1, 3, 1, C)
+    dbr = dy.float().sum((0, 2, 3))
+    pre = torch.randn(w.shape, device="cuda").contiguous(memory_format=torch.channels_last)
+    preb = torch.randn(C, device="cuda")
+    gw, gb = pre.clone(), preb.clone()
+    nv.dwconv7_wgrad(x, dy, gw, gb)
+    report_abs(f"dw7 wgrad onto a filled slot {tag}", gw - pre, dwr, 2.0 ** -10, 1e-4, arms=2.0 ** -10)
+    report_abs(f"dw7 bias grad onto a filled slot {tag}", gb - preb, dbr, 2.0 ** -10, 1e-4, arms=2.0 ** -10)
+    nv.dwconv7_wgrad(x, dy, gw, gb)
+    report_abs(f"dw7 wgrad two passes {tag}", gw - pre, 2 * dwr, 2.0 ** -10, 1e-4, arms=2.0 ** -10)
+    report_abs(f"dw7 bias grad two passes {tag}", gb - preb, 2 * dbr, 2.0 ** -10, 1e-4, arms=2.0 ** -10)
+
+
+def _layer_norm_case(C, rows, offset, four_d):
+    """LayerNorm fwd (y, mean, rstd) and bwd (dx, dgamma, dbeta onto filled slots) against fp32 torch; ``offset``: the
+    rows' mean in units of their standard deviation."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    if four_d:
+        x = cl(bf(torch.randn(2, C, rows // 2, 1, device="cuda") + offset))
+        xr = x.float().permute(0, 2, 3, 1).reshape(-1, C)
+    else:
+        x = bf(torch.randn(rows, C, device="cuda") + offset)
+        xr = x.float()
+    g, b = torch.rand(C, device="cuda") + 0.5, torch.randn(C, device="cuda")
+    tag = f"C={C} rows={rows} mean={offset:g}sd {'NHWC' if four_d else '[N, C]'}"
+    y, mean, rstd = nv.layer_norm_fwd(x, g, b, 1e-6)
+    yr = F.layer_norm(xr, (C,), g, b, 1e-6)
+    yv = y.float().permute(0, 2, 3, 1).reshape(-1, C) if four_d else y.float()
+    report_abs(f"LN fwd {tag}", yv, yr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+    var = xr.double().var(1, unbiased=False)
+    report_abs(f"LN mean {tag}", mean, xr.double().mean(1), 2.0 ** -20, 1e-6)
+    report_abs(f"LN rstd {tag}", rstd, (var + 1e-6).rsqrt(), 2.0 ** -14, 0.0)
+    dy = torch.randn_like(x.float()).to(torch.bfloat16)
+    dy = cl(dy) if four_d else dy
+    dyr = dy.float().permute(0, 2, 3, 1).reshape(-1, C) if four_d else dy.float()
+    xq, gq, bq = xr.clone().requires_grad_(True), g.clone().requires_grad_(True), b.clone().requires_grad_(True)
+    F.layer_norm(xq, (C,), gq, bq, 1e-6).backward(dyr)
+    pg, pb = torch.randn(C, device="cuda"), torch.randn(C, device="cuda")
+    gg, gbb = pg.clone(), pb.clone()
+    dx = nv.layer_norm_bwd(dy, x, mean, rstd, g, gg, gbb)
+    dxv = dx.float().permute(0, 2, 3, 1).reshape(-1, C) if four_d else dx.float()
+    report_abs(f"LN dx {tag}", dxv, xq.grad, 2.0 ** -6, 0.0, arms=2.0 ** -7)
+    report_abs(f"LN dgamma {tag}", gg - pg, gq.grad, 2.0 ** -8, 1e-4, arms=2.0 ** -9)
+    report_abs(f"LN dbeta {tag}", gbb - pb, bq.grad, 2.0 ** -8, 1e-4, arms=2.0 ** -9)
+
+
+def _gelu_and_layer_scale():
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    for C in (384, 1536, 8):
+        h = cl(bf(torch.linspace(-12, 12, 4 * C * 9 * 7, device="cuda")[torch.randperm(4 * C * 63, device="cuda")]
+                  .view(4, 9, 7, C).permute(0, 3, 1, 2)))        # tails included: gelu(-12) ~ 0, gelu(12) = 12
+        report_abs(f"GELU fwd C={C} h in [-12, 12]", nv.gelu_fwd(h), F.gelu(h.float()), 2.0 ** -7, 1e-6)
+        dg = cl(bf(torch.randn(h.shape, device="cuda")))
+        hq = h.float().requires_grad_(True)
+        F.gelu(hq).backward(dg.float())
+        pre = torch.randn(C, device="cuda")
+        db = pre.clone()
+        dh = nv.gelu_bwd(dg, h, db)
+        report_abs(f"GELU bwd C={C}", dh, hq.grad, 2.0 ** -7, 1e-6)
+        report_abs(f"GELU bwd bias grad (sum of the stored bf16 dh) C={C}", db - pre, dh.float().sum((0, 2, 3)), 2.0 ** -10, 1e-4,
+                   arms=2.0 ** -10)
+    for C, hw in ((96, 56), (768, 7), (40, 5)):
+        for with_keep in (False, True):
+            N = 8
+            y = cl(bf(torch.randn(N, C, hw, hw, device="cuda")))
+            x = cl(bf(torch.randn(N, C, hw, hw, device="cuda")))
+            ls = torch.rand(C, device="cuda") + 0.25
+            keep = torch.tensor([0.0, 2.0] * (N // 2), device="cuda") if with_keep else None
+            k = keep.view(-1, 1, 1, 1) if with_keep else 1.0
+            tag = f"C={C} {hw}x{hw} {'with' if with_keep else 'without'} stochastic depth"
+            z = nv.layer_scale_fwd(y, ls, keep, x)
+            report_abs(f"layer scale fwd {tag}", z, ls.view(-1, 1, 1) * y.float() * k + x.float(), 2.0 ** -7, 0.0,
+                       arms=2.0 ** -9)
+            dz = cl(bf(torch.randn(y.shape, device="cuda")))
+            pl, pb = torch.randn(C, device="cuda"), torch.randn(C, device="cuda")
+            gl, gbias = pl.clone(), pb.clone()
+            dy = nv.layer_scale_bwd(dz, y, ls, keep, gl, gbias)
+            dyr = dz.float() * ls.view(-1, 1, 1) * k
+            report_abs(f"layer scale dy {tag}", dy, dyr, 2.0 ** -7, 0.0)
+            report_abs(f"layer scale dls {tag}", gl - pl, (dz.float() * k * y.float()).sum((0, 2, 3)), 2.0 ** -10,
+                       1e-4, arms=2.0 ** -10)
+            report_abs(f"layer scale fc2 bias grad {tag}", gbias - pb, dy.float().sum((0, 2, 3)), 2.0 ** -10, 1e-4,
+                       arms=2.0 ** -10)
+
+
+def _strided_bias_conv(cin, cout, hw, k, n):
+    """ConvNeXt's stem (4x4 / 4 on the NHWC4 image) and downsample (2x2 / 2) convs with bias through conv_bias_act:
+    forward, data and weight gradients and the bias gradient against fp32 torch."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import ops
+    from distributeddeeplearning_b200.models.layers import prepare_input
+
+    img = cin == 3
+    xf = torch.randn(n, cin, hw, hw, device="cuda")
+    x = prepare_input(xf) if img else cl(bf(xf))
+    xs = x.clone().requires_grad_(not img)
+    w = (torch.randn(cout, cin, k, k, device="cuda") * 0.1).contiguous(memory_format=torch.channels_last)
+    wn, bn_ = w.clone().requires_grad_(True), torch.randn(cout, device="cuda").requires_grad_(True)
+    y = ops.conv_bias_act(xs, wn, bn_, k, 0, 1, False)
+    xr = (x[:, :3].float() if img else x.float()).requires_grad_(not img)
+    wr, br = bf(w).float().requires_grad_(True), bn_.detach().clone().requires_grad_(True)
+    yr = F.conv2d(xr, wr, br, k)
+    tag = f"{k}x{k}/{k} {cin}->{cout} {hw}x{hw} N={n}"
+    RESULTS.append(type(y.grad_fn).__name__ == "_ConvBiasActBackward")
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {tag} runs on the native conv node ({type(y.grad_fn).__name__})")
+    report_abs(f"conv+bias fwd {tag}", y, yr, 2.0 ** -7, 1e-3, arms=2.0 ** -8)
+    dy = cl(bf(torch.randn(y.shape, device="cuda")))
+    y.backward(dy)
+    yr.backward(dy.float())
+    if not img:
+        report_abs(f"conv+bias dgrad {tag}", xs.grad, xr.grad, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+    report_abs(f"conv+bias wgrad {tag}", wn.grad, wr.grad, 2.0 ** -8, 1e-4, arms=2.0 ** -9)
+    report_abs(f"conv+bias bias grad {tag}", bn_.grad, br.grad, 2.0 ** -8, 1e-4, arms=2.0 ** -9)
+
+
+def _convnext_vs_torchvision(name, bs):
+    """A ConvNeXt against torchvision fp32 with the same weights (non-trivial layer scales) and stochastic-depth vectors,
+    and this repo's bf16 composite; forward hooks check that every block ran on the native node."""
+    import torch
+    import torchvision
+    from torchvision.ops import StochasticDepth
+
+    from distributeddeeplearning_b200 import models, ops
+    from distributeddeeplearning_b200.models.convnext import CNBlock
+
+    torch.manual_seed(0)
+    m = models.get_model(name).cuda().train()
+    with torch.no_grad():
+        for k, p in m.named_parameters():
+            if k.endswith("layer_scale"):
+                p.copy_(torch.rand_like(p) * 0.5 + 0.25)
+    tv = getattr(torchvision.models, name)().cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    keeps, replay = [], []
+    draw = ops.stochastic_depth_keep
+
+    def record(n, p, device):
+        keeps.append(draw(n, p, device))
+        return keeps[-1]
+
+    orig_sd = StochasticDepth.forward
+    StochasticDepth.forward = lambda self, x: x if self.p == 0.0 else x * replay.pop(0).view(-1, 1, 1, 1).to(x.dtype)
+    nodes = []
+    hooks = [mod.register_forward_hook(lambda mod, i, o: nodes.append(type(o.grad_fn).__name__))
+             for mod in m.modules() if isinstance(mod, CNBlock)]
+    x = torch.randn(bs, 3, 224, 224, device="cuda").to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    try:
+        ops.stochastic_depth_keep = record
+        out = m(x)
+        for h in hooks:
+            h.remove()
+        ops.softmax_cross_entropy(out, y, 1000).backward()
+        replay[:] = list(keeps)
+        ro = tv(x)
+        torch.nn.functional.cross_entropy(ro, y).backward()
+        replay[:] = list(keeps)
+        ops.stochastic_depth_keep = lambda n, p, device: replay.pop(0)
+        os.environ["DDL_B200_IMPL"] = "torch"
+        co = m2(x)
+        ops.softmax_cross_entropy(co, y, 1000).backward()
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+        ops.stochastic_depth_keep = draw
+        StochasticDepth.forward = orig_sd
+    n_blocks = sum(1 for mod in m.modules() if isinstance(mod, CNBlock))
+    ok = len(nodes) == n_blocks and set(nodes) == {"_ConvNeXtBlockBackward"}
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: {len(nodes)} of {n_blocks} blocks ran on {sorted(set(nodes))}; "
+          f"{len(keeps)} stochastic-depth draws, {sum(int((k == 0).sum()) for k in keeps)} dropped samples", flush=True)
+    c1, c2 = _cos(out, ro), _cos(out, co)
+    RESULTS.append(c1 > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} logits cos vs fp32 {c1:.5f}   vs bf16-composite {c2:.5f}")
+    gn, gc, tvp = dict(m.named_parameters()), dict(m2.named_parameters()), dict(tv.named_parameters())
+    worst, lag = (1.0, "", 1.0), (-1.0, "")
+    for k, p in tvp.items():
+        if float(p.grad.norm()) == 0.0:
+            continue
+        a1, a2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if a1 < worst[0]:
+            worst = (a1, k, a2)
+        if a2 - a1 > lag[0]:
+            lag = (a2 - a1, k)
+    ok = lag[0] <= 0.01 and worst[0] > 0.6
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at {worst[1]} "
+          f"(bf16 composite {worst[2]:.4f}); largest deficit vs the bf16 composite = {lag[0]:.4f} at {lag[1]}", flush=True)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        oe, re_ = m(x), tv(x)
+    ce = _cos(oe, re_)
+    RESULTS.append(ce > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} eval-mode logits cos vs torchvision eval {ce:.5f}", flush=True)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def g_convnext():
+    """ConvNeXt: the depthwise 7x7 kernels at every ConvNeXt-T/S/B/L shape plus edge cases, LayerNorm over channels at
+    every width (and rows whose mean is 100x their spread), GELU, layer scale with and without stochastic depth, the
+    stem / downsample convs with bias, convnext_tiny against torchvision, eager vs CUDA-graph training and fp8."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.manual_seed(0)
+    for case in DW7_CASES:
+        _dw7_layer(*case)
+    for C in (96, 128, 192, 256, 384, 512, 768, 1024, 1536, 8, 40):
+        _layer_norm_case(C, 1000, 0.0, True)
+        _layer_norm_case(C, 37, 100.0, False)
+    _layer_norm_case(96, 20000, 100.0, True)
+    _gelu_and_layer_scale()
+    for args in ((3, 96, 224, 4, 2), (3, 128, 64, 4, 1), (96, 192, 56, 2, 2), (384, 768, 14, 2, 4), (768, 1536, 14, 2, 2)):
+        _strided_bias_conv(*args)
+    _convnext_vs_torchvision("convnext_tiny", 16)
+    dist.init()
+
+    def run(graph, random_drops):
+        torch.manual_seed(0)
+        s = BenchmarkSession("convnext_tiny", 16, True, lr=0.01, momentum=0.9)
+        if not random_drops:        # the eager and the replayed step draw their vectors from different counters
+            for mod in s.model.modules():
+                if hasattr(mod, "sd_prob"):
+                    mod.sd_prob = 0.0
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out[-4:]
+
+    a, b = run(False, False), run(True, False)
+    rel = max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(a, b))
+    ok = all(x == x for x in a + b) and rel < 5e-2
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] convnext_tiny training without random drops: eager {[round(v, 4) for v in a]} "
+          f"graph replay {[round(v, 4) for v in b]} (largest relative difference {rel:.2e})", flush=True)
+    c = run(True, True)
+    ok = all(x == x and abs(x) < 1e4 for x in c)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] convnext_tiny graph-replayed training with stochastic depth: "
+          f"{[round(v, 4) for v in c]}", flush=True)
+    fp8.reset()
+    fp8.enable(True)
+    try:
+        torch.manual_seed(0)
+        s = BenchmarkSession("convnext_tiny", 16, True, lr=0.01, momentum=0.9)
+        losses = [float(s.step()) for _ in range(4)]
+        torch.cuda.synchronize()
+        s.optimizer.check_errors()
+    finally:
+        fp8.enable(False)
+    # the pointwise convs that meet fp8's multiple-of-128 rule (fc2 of stages 2-4, fc1 of stage 4) must take it
+    n8 = fp8.launches()
+    ok = all(l == l and abs(l) < 1e4 for l in losses) and n8.get("fwd", 0) > 0 and n8.get("dgrad", 0) > 0
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] convnext_tiny fp8 session: losses {[round(v, 3) for v in losses]}, "
           f"fp8 launches {fp8.launches()}", flush=True)
     del s
     torch.cuda.empty_cache()
