@@ -15,8 +15,9 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
+WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
 
 def report(name, got, ref, tol=2e-2, atol=None):
@@ -57,12 +58,15 @@ def _bound_ratio(got, ref, rtol, atol, arms):
     return int((err > bound).sum().item()), float((err / bound).max().item()), bool(torch.isfinite(got).all().item())
 
 
-def report_abs(name, got, ref, rtol, atol, arms=0.0, also=None):
+def report_abs(name, got, ref, rtol, atol, arms=0.0, also=None, kind=None):
     """allclose-style check: |got - ref| <= atol + arms * rms(ref) + rtol * |ref| ELEMENT-WISE (small-magnitude errors
     are not hidden behind max|ref| the way `report` normalises).  ``also = (got2, ref2)``: a second implementation of
-    the same tensor (not checked) whose worst ratio to the same bound is printed alongside.  Returns the worst ratio."""
+    the same tensor (not checked) whose worst ratio to the same bound is printed alongside.  ``kind``: the tensor kind
+    under which the worst ratio is kept in WORST.  Returns the worst ratio."""
     bad, worst, finite = _bound_ratio(got, ref, rtol, atol, arms)
     ok = bad == 0 and finite
+    if kind is not None:
+        WORST[kind] = max(WORST.get(kind, 0.0), worst)
     desc = f"atol {atol:g} + " if atol else ""
     desc += f"{arms:g}*rms(ref) + " if arms else ""
     other = ""
@@ -337,6 +341,11 @@ def g_gemm():
         report(f"  stats sumsq M{M} K{K} N{N}", st[1], (yb * yb).sum((0, 2, 3)), 2e-3)
 
 
+# image stems (R = S, stride, pad, H = W, Cout) of g_conv_fwd / g_conv_wgrad
+STEM_CASES = [(7, 2, 3, 32, 64), (11, 4, 2, 63, 64), (3, 1, 1, 16, 64), (3, 2, 0, 35, 64), (7, 2, 0, 41, 64),
+              (7, 2, 3, 224, 64), (3, 2, 0, 299, 32), (7, 2, 0, 224, 96), (7, 2, 3, 224, 96)]
+
+
 def g_conv_fwd():
     import torch
 
@@ -359,17 +368,18 @@ def g_conv_fwd():
     b = torch.randn(128, device=dev)
     y = nv.conv_fwd(x, _w_bf16(w), (3, 3), 1, 1, bias=b, relu=True)
     report("conv_fwd bias+relu", y, torch.relu(_conv_ref(x, w, 1, 1) + b.view(1, -1, 1, 1)), 2e-2)
-    # stems: ResNet 7x7/2, AlexNet 11x11/4, VGG 3x3/1
+    # stems: ResNet 7x7/2, AlexNet 11x11/4, VGG 3x3/1, and the stems with Cout != 64: Inception-v3 (3x3/2/p0 -> 32),
+    # SqueezeNet 1.0 (7x7/2/p0 -> 96) and DenseNet-161 (7x7/2/p3 -> 96)
     for tma in (True, False):       # TMA-fed (row-interleaved padded image) and cp.async gather stems
         nv.USE_STEM_TMA = tma
-        for (k, s, p, hw) in [(7, 2, 3, 32), (11, 4, 2, 63), (3, 1, 1, 16), (3, 2, 0, 35), (7, 2, 0, 41), (7, 2, 3, 224)]:
+        for (k, s, p, hw, co) in STEM_CASES:
             img = torch.randn(2, 3, hw, hw, device=dev)
             x4 = nv.nchw_to_nhwc4(img)
-            w = torch.randn(64, 3, k, k, device=dev) * 0.1
+            w = torch.randn(co, 3, k, k, device=dev) * 0.1
             wp = nv.pack_stem_weight(cl(w), k, k)
-            y, st = nv.conv_fwd(x4, wp, (k, k), s, p, stats=True, cout=64)
+            y, st = nv.conv_fwd(x4, wp, (k, k), s, p, stats=True, cout=co)
             ref = _conv_ref(bf(img), bf(w), s, p)
-            report(f"stem conv {'tma' if tma else 'gather'} k{k}s{s}p{p} {hw}x{hw}", y, ref, 2e-2)
+            report(f"stem conv {'tma' if tma else 'gather'} k{k}s{s}p{p} {hw}x{hw} ->{co}", y, ref, 2e-2)
     nv.USE_STEM_TMA = True
 
 
@@ -546,16 +556,16 @@ def g_conv_wgrad():
         report(f"conv_wgrad n{n} c{ci} {h}x{w_} ->{co} k{k}s{s}p{p}", gw, w.grad, 2e-2)
     for tma in (True, False):
         nv.USE_STEM_TMA = tma
-        for (k, s, p, hw) in [(7, 2, 3, 32), (11, 4, 2, 63), (3, 1, 1, 16), (3, 2, 0, 35), (7, 2, 0, 41), (7, 2, 3, 224)]:
+        for (k, s, p, hw, co) in STEM_CASES:
             img = torch.randn(2, 3, hw, hw, device=dev)
             x4 = nv.nchw_to_nhwc4(img)
-            w = torch.randn(64, 3, k, k, device=dev).requires_grad_(True)
+            w = torch.randn(co, 3, k, k, device=dev).requires_grad_(True)
             yr = _conv_ref(bf(img), w, s, p)
             dy = cl(bf(torch.randn_like(yr)))
             yr.backward(dy.float())
-            gw = cl(torch.zeros(64, 3, k, k, device=dev))
+            gw = cl(torch.zeros(co, 3, k, k, device=dev))
             nv.conv_wgrad(x4, dy, gw, (k, k), s, p)
-            report(f"stem wgrad {'tma' if tma else 'gather'} k{k}s{s}p{p}", gw, w.grad, 2e-2)
+            report(f"stem wgrad {'tma' if tma else 'gather'} k{k}s{s}p{p} {hw}x{hw} ->{co}", gw, w.grad, 2e-2)
     nv.USE_STEM_TMA = True
 
 
@@ -1353,37 +1363,48 @@ GROUPED_SHAPES = sorted({(128, 56, 1, 4), (256, 56, 2, 8), (256, 28, 1, 8), (512
                          (128, 14, 1, 64), (256, 13, 2, 8), (192, 9, 1, 16)})
 
 
-def _grouped_layer(C, hw, stride, cg, n):
-    """fwd (+ BN statistics), dgrad and wgrad (accumulating onto a pre-filled slot, two passes) of one grouped 3x3 conv
-    against fp32 F.conv2d(groups=) on the same bf16-rounded operands, element-wise."""
+def _conv_layer(cin, cout, kernel, stride, pad, h, w_, n, groups=1):
+    """fwd (+ BN statistics), dgrad and wgrad (accumulating onto a pre-filled slot, two passes) of one convolution
+    (dense, or grouped through the block-diagonal operand) against float64 F.conv2d on the same bf16-rounded operands,
+    element-wise.  ``pad`` is (pad_h, pad_w)."""
     import torch
     import torch.nn.functional as F
 
     from distributeddeeplearning_b200.ops import native as nv
 
-    g = C // cg
-    x = cl(bf(torch.randn(n, C, hw, hw, device="cuda")))
-    w = bf(torch.randn(C, cg, 3, 3, device="cuda") * (2.0 / (9 * cg)) ** 0.5).contiguous(memory_format=torch.channels_last)
-    wc = w.permute(0, 2, 3, 1).reshape(C, 9 * cg).contiguous()            # the compact [Cout][R*S*cg] operand
-    we = nv.expand_grouped_weight(wc, 9, g)
-    tag = f"C={C} {hw}x{hw} s{stride} cg={cg} N={n}"
-    y, st = nv.conv_fwd(x, we, (3, 3), stride, 1, stats=True, groups=g)
-    yr = F.conv2d(x.float(), w.float(), None, stride, 1, 1, g)
-    report_abs(f"grouped fwd  {tag}", y, yr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
-    yb = y.float()
-    report_abs(f"grouped fwd sum   {tag}", st[0], yb.sum((0, 2, 3)), 2.0 ** -10, 0.0, arms=2.0 ** -10)
-    report_abs(f"grouped fwd sumsq {tag}", st[1], (yb * yb).sum((0, 2, 3)), 2.0 ** -10, 0.0, arms=2.0 ** -10)
+    R, S = kernel
+    cg = cin // groups
+    x = cl(bf(torch.randn(n, cin, h, w_, device="cuda")))
+    w = bf(torch.randn(cout, cg, R, S, device="cuda") * (2.0 / (R * S * cg)) ** 0.5).contiguous(
+        memory_format=torch.channels_last)
+    wk = w.permute(0, 2, 3, 1).reshape(cout, R * S * cg).contiguous()     # the [Cout][R*S*Cin/groups] operand
+    if groups > 1:
+        wk = nv.expand_grouped_weight(wk, R * S, groups)
+        label, tag = "grouped", f"C={cin} {h}x{w_} s{stride} cg={cg} N={n}"
+    else:
+        label, tag = "conv", f"{cin}->{cout} {R}x{S} s{stride} p{pad[0]},{pad[1]} {h}x{w_} N={n}"
+    xd, wd = x.double(), w.double()
+    y, st = nv.conv_fwd(x, wk, kernel, stride, pad, stats=True, groups=groups)
+    yr = F.conv2d(xd, wd, None, stride, pad, 1, groups)
+    report_abs(f"{label} fwd  {tag}", y, yr, 2.0 ** -7, 0.0, arms=2.0 ** -8, kind=f"{label} fwd")
+    yb = y.double()
+    report_abs(f"{label} fwd sum   {tag}", st[0], yb.sum((0, 2, 3)), 2.0 ** -10, 0.0, arms=2.0 ** -10,
+               kind=f"{label} BN statistics")
+    report_abs(f"{label} fwd sumsq {tag}", st[1], (yb * yb).sum((0, 2, 3)), 2.0 ** -10, 0.0, arms=2.0 ** -10,
+               kind=f"{label} BN statistics")
     dy = cl(bf(torch.randn(y.shape, device="cuda")))
-    dx = nv.conv_dgrad(dy, we, x.shape, (3, 3), stride, 1, groups=g)
-    dxr = torch.nn.grad.conv2d_input(x.shape, w.float(), dy.float(), stride, 1, 1, g)
-    report_abs(f"grouped dgrad {tag}", dx, dxr, 2.0 ** -7, 0.0, arms=2.0 ** -8)
-    dwr = torch.nn.grad.conv2d_weight(x.float(), w.shape, dy.float(), stride, 1, 1, g)
+    dx = nv.conv_dgrad(dy, wk, x.shape, kernel, stride, pad, groups=groups)
+    dxr = torch.nn.grad.conv2d_input(x.shape, wd, dy.double(), stride, pad, 1, groups)
+    report_abs(f"{label} dgrad {tag}", dx, dxr, 2.0 ** -7, 0.0, arms=2.0 ** -8, kind=f"{label} dgrad")
+    dwr = torch.nn.grad.conv2d_weight(xd, w.shape, dy.double(), stride, pad, 1, groups)
     pre = torch.randn(w.shape, device="cuda").contiguous(memory_format=torch.channels_last)
     gw = pre.clone()
-    nv.conv_wgrad(x, dy, gw, (3, 3), stride, 1, groups=g)
-    report_abs(f"grouped wgrad onto a filled slot {tag}", gw - pre, dwr, 2.0 ** -10, 0.0, arms=2.0 ** -10)
-    nv.conv_wgrad(x, dy, gw, (3, 3), stride, 1, groups=g)
-    report_abs(f"grouped wgrad two passes {tag}", gw - pre, 2 * dwr, 2.0 ** -10, 0.0, arms=2.0 ** -10)
+    nv.conv_wgrad(x, dy, gw, kernel, stride, pad, groups=groups)
+    report_abs(f"{label} wgrad onto a filled slot {tag}", gw - pre, dwr, 2.0 ** -10, 0.0, arms=2.0 ** -10,
+               kind=f"{label} wgrad")
+    nv.conv_wgrad(x, dy, gw, kernel, stride, pad, groups=groups)
+    report_abs(f"{label} wgrad two passes {tag}", gw - pre, 2 * dwr, 2.0 ** -10, 0.0, arms=2.0 ** -10,
+               kind=f"{label} wgrad")
 
 
 def _rx(inp, planes, stride=1, proj=False, groups=32, width=4):
@@ -1466,7 +1487,7 @@ def g_grouped():
 
     torch.manual_seed(0)
     for C, hw, stride, cg in GROUPED_SHAPES:
-        _grouped_layer(C, hw, stride, cg, 3 if hw <= 14 else 2)
+        _conv_layer(C, C, (3, 3), stride, (1, 1), hw, hw, 3 if hw <= 14 else 2, groups=C // cg)
     bad = []
     for args in ((96, 96, 3), (128, 64, 32), (128, 128, 64), (128, 128, 128)):       # Cin != Cout, cg = 2, cg = 1
         bad.append(nv.supports_grouped(*args))
@@ -2713,36 +2734,46 @@ def _gelu_and_layer_scale():
                        arms=2.0 ** -10)
 
 
-def _strided_bias_conv(cin, cout, hw, k, n):
-    """ConvNeXt's stem (4x4 / 4 on the NHWC4 image) and downsample (2x2 / 2) convs with bias through conv_bias_act:
-    forward, data and weight gradients and the bias gradient against fp32 torch."""
+def _bias_conv(cin, cout, hw, k, n, stride=None, pad=0, relu=False):
+    """A conv with bias (and ReLU) through conv_bias_act: ConvNeXt's stem (4x4 / 4 on the NHWC4 image) and downsample
+    (2x2 / 2) convs, every conv of SqueezeNet.  Forward, data and weight gradients and the bias gradient (after
+    bias_relu_bwd's ReLU mask) against float64 torch on the same bf16 operands.  ``stride`` defaults to ``k``.  Where
+    the float64 pre-activation lies within 2^-8 * rms of zero (far beyond the fp32 accumulation error) the ReLU mask takes
+    the side of the tested output."""
     import torch
     import torch.nn.functional as F
 
     from distributeddeeplearning_b200 import ops
     from distributeddeeplearning_b200.models.layers import prepare_input
 
+    stride = k if stride is None else stride
     img = cin == 3
     xf = torch.randn(n, cin, hw, hw, device="cuda")
-    x = prepare_input(xf) if img else cl(bf(xf))
+    x = prepare_input(xf) if img else cl(bf(xf.relu() if relu else xf))      # a ReLU net's convs see post-ReLU inputs
     xs = x.clone().requires_grad_(not img)
     w = (torch.randn(cout, cin, k, k, device="cuda") * 0.1).contiguous(memory_format=torch.channels_last)
     wn, bn_ = w.clone().requires_grad_(True), torch.randn(cout, device="cuda").requires_grad_(True)
-    y = ops.conv_bias_act(xs, wn, bn_, k, 0, 1, False)
-    xr = (x[:, :3].float() if img else x.float()).requires_grad_(not img)
-    wr, br = bf(w).float().requires_grad_(True), bn_.detach().clone().requires_grad_(True)
-    yr = F.conv2d(xr, wr, br, k)
-    tag = f"{k}x{k}/{k} {cin}->{cout} {hw}x{hw} N={n}"
+    y = ops.conv_bias_act(xs, wn, bn_, stride, pad, 1, relu)
+    xr = (x[:, :3].double() if img else x.double()).requires_grad_(not img)
+    wr, br = bf(w).double().requires_grad_(True), bn_.detach().double().requires_grad_(True)
+    vr = F.conv2d(xr, wr, br, stride, pad)
+    yr = vr
+    if relu:
+        tie = vr.abs() <= 2.0 ** -8 * vr.detach().pow(2).mean().sqrt()
+        yr = vr * torch.where(tie, y.double() > 0, vr > 0)
+    tag = f"{k}x{k}/{stride} p{pad} {cin}->{cout} {hw}x{hw} N={n}"
+    what = "conv+bias+relu" if relu else "conv+bias"
     RESULTS.append(type(y.grad_fn).__name__ == "_ConvBiasActBackward")
     print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {tag} runs on the native conv node ({type(y.grad_fn).__name__})")
-    report_abs(f"conv+bias fwd {tag}", y, yr, 2.0 ** -7, 1e-3, arms=2.0 ** -8)
+    report_abs(f"{what} fwd {tag}", y, vr.clamp(min=0) if relu else vr, 2.0 ** -7, 1e-3, arms=2.0 ** -8,
+               kind=f"{what} fwd")
     dy = cl(bf(torch.randn(y.shape, device="cuda")))
     y.backward(dy)
-    yr.backward(dy.float())
+    yr.backward(dy.double())
     if not img:
-        report_abs(f"conv+bias dgrad {tag}", xs.grad, xr.grad, 2.0 ** -7, 0.0, arms=2.0 ** -8)
-    report_abs(f"conv+bias wgrad {tag}", wn.grad, wr.grad, 2.0 ** -8, 1e-4, arms=2.0 ** -9)
-    report_abs(f"conv+bias bias grad {tag}", bn_.grad, br.grad, 2.0 ** -8, 1e-4, arms=2.0 ** -9)
+        report_abs(f"{what} dgrad {tag}", xs.grad, xr.grad, 2.0 ** -7, 0.0, arms=2.0 ** -8, kind=f"{what} dgrad")
+    report_abs(f"{what} wgrad {tag}", wn.grad, wr.grad, 2.0 ** -8, 1e-4, arms=2.0 ** -9, kind=f"{what} wgrad")
+    report_abs(f"{what} bias grad {tag}", bn_.grad, br.grad, 2.0 ** -8, 1e-4, arms=2.0 ** -9, kind=f"{what} bias grad")
 
 
 def _convnext_vs_torchvision(name, bs):
@@ -2850,7 +2881,7 @@ def g_convnext():
     _layer_norm_case(96, 20000, 100.0, True)
     _gelu_and_layer_scale()
     for args in ((3, 96, 224, 4, 2), (3, 128, 64, 4, 1), (96, 192, 56, 2, 2), (384, 768, 14, 2, 4), (768, 1536, 14, 2, 2)):
-        _strided_bias_conv(*args)
+        _bias_conv(*args)
     _convnext_vs_torchvision("convnext_tiny", 16)
     dist.init()
 
@@ -2901,6 +2932,477 @@ def g_convnext():
           f"fp8 launches {fp8.launches()}", flush=True)
     del s
     torch.cuda.empty_cache()
+
+
+# ------------------------------------------------------------------------------------------------
+# classic zoo: Inception-v3, DenseNet, SqueezeNet
+# ------------------------------------------------------------------------------------------------
+# Budgets of the `classic` group's stand-alone kernels as (rtol, atol, arms) of report_abs, by tensor kind.  Each
+# reference is float64 on the same bf16 operands.
+# - pool out / pool grad: the kernels sum at most 25 window terms (<= ceil(k/s)^2 = 4 for a max-pool gradient) in fp32
+#   and round once to bf16.  Half a bf16 ulp is at most 2^-8 of the value; 2^-14 * rms covers the fp32 sum where its
+#   terms cancel.  A wrong divisor or a gradient routed to another window tap is an error of order |ref|.
+# - global pool out: the same rounding after an fp32 sum over up to 169 pixels: 2^-12 * rms.
+# - bn out / running stats / dx / dgamma / dbeta: the budgets of the other fused-BN checks (_relu6_bn, _silu_bn).
+CLASSIC_BUDGET = {"pool out": (2.0 ** -8, 0.0, 2.0 ** -14), "pool grad": (2.0 ** -8, 0.0, 2.0 ** -14),
+                  "global pool out": (2.0 ** -8, 0.0, 2.0 ** -12), "global pool grad": (2.0 ** -8, 0.0, 2.0 ** -14),
+                  "bn out": (2.0 ** -7, 2.0 ** -6, 0.0), "bn running_mean": (2.0 ** -8, 1e-5, 0.0),
+                  "bn running_var": (2.0 ** -8, 1e-5, 0.0), "bn dx": (2.0 ** -6, 0.0, 2.0 ** -7),
+                  "bn dgamma": (2.0 ** -8, 0.0, 2.0 ** -8), "bn dbeta": (2.0 ** -8, 0.0, 2.0 ** -8)}
+# Whole models against torchvision fp32: the running statistics after one training step differ by the bf16 rounding
+# of every activation upstream of each BN, which grows with depth.  Element-wise bounds with about 2x margin over the
+# worst ratio the repo's bf16 composite (same rounding points, stock cuDNN kernels) reaches on DenseNet-121; a BN where
+# the composite itself gets past half of the bound (Inception-v3's aux head normalises 8 values per channel) must stay
+# within 2x of the composite's ratio instead.  Both ratios are printed.
+CLASSIC_RUNNING_BUDGET = {"running_mean": (2.0 ** -4, 0.0, 2.0 ** -4), "running_var": (2.0 ** -5, 0.0, 2.0 ** -5)}
+CLASSIC_RESOLVED = 0.9      # cosine with fp32 above which the bf16 composite resolves a gradient
+# autograd nodes of the torch composites: none of them may appear in a native model's graph
+FALLBACK_NODES = ("CatBackward0", "MaxPool2DWithIndicesBackward0", "AvgPool2DBackward0", "NativeBatchNormBackward0",
+                  "CudnnBatchNormBackward0", "ConvolutionBackward0", "ReluBackward0", "MeanBackward1")
+
+
+def _classic(kind, name, got, ref):
+    rtol, atol, arms = CLASSIC_BUDGET[kind]
+    return report_abs(name, got, ref, rtol, atol, arms, kind=kind)
+
+
+def _exact(name, ok):
+    RESULTS.append(bool(ok))
+    print(f"[{'ok' if ok else 'FAIL'}] {name}", flush=True)
+
+
+def _uncovered(size, k, s, p, out):
+    """Input rows (or columns) of a pooling axis that no window covers."""
+    cov = [False] * size
+    for o in range(out):
+        for i in range(max(o * s - p, 0), min(o * s - p + k, size)):
+            cov[i] = True
+    return [i for i in range(size) if not cov[i]]
+
+
+def _check_uncovered(name, dx, k, s, p):
+    from distributeddeeplearning_b200.ops import native as nv
+
+    H, W = dx.shape[2], dx.shape[3]
+    rows = _uncovered(H, k, s, p, nv._pool_out(H, k, s, p, False))
+    cols = _uncovered(W, k, s, p, nv._pool_out(W, k, s, p, False))
+    if rows or cols:
+        zero = all(float(dx[:, :, r].abs().max()) == 0 for r in rows) and \
+            all(float(dx[:, :, :, c].abs().max()) == 0 for c in cols)
+        _exact(f"{name}: rows {rows} / columns {cols} no window covers get exactly zero gradient", zero)
+
+
+def _concat_case(chans, n, h, w):
+    """concat_channels (gather) and split_channels (scatter) against torch.cat / slicing, bit for bit."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    parts = [cl(bf(torch.randn(n, c, h, w, device="cuda"))) for c in chans]
+    out = nv.concat_channels(parts)
+    fwd = out.is_contiguous(memory_format=torch.channels_last) and torch.equal(out, torch.cat(parts, 1))
+    dy = cl(bf(torch.randn(out.shape, device="cuda")))
+    back, o = nv.split_channels(dy, chans), 0
+    bwd = True
+    for c, b in zip(chans, back):
+        bwd = bwd and torch.equal(b, dy[:, o:o + c])
+        o += c
+    _exact(f"concat {'+'.join(map(str, chans))} N={n} {h}x{w}: gather {'==' if fwd else '!='} torch.cat, "
+           f"scatter {'==' if bwd else '!='} slices", fwd and bwd)
+
+
+def _concat_dispatch(chans, node):
+    """ops.concat_channels: the native node for <= 8 parts of multiples of 8 channels, torch.cat otherwise; either way
+    the values and the part gradients are exact."""
+    import torch
+
+    from distributeddeeplearning_b200 import ops
+
+    parts = [cl(bf(torch.randn(2, c, 5, 7, device="cuda"))).requires_grad_(True) for c in chans]
+    out = ops.concat_channels(parts)
+    got = type(out.grad_fn).__name__
+    dy = cl(bf(torch.randn(out.shape, device="cuda")))
+    out.backward(dy)
+    ok = got == node and torch.equal(out, torch.cat([p.detach() for p in parts], 1))
+    o = 0
+    for c, p in zip(chans, parts):
+        ok = ok and torch.equal(p.grad, dy[:, o:o + c])
+        o += c
+    _exact(f"ops.concat_channels of {len(chans)} parts {chans[:3]}...: {got} (want {node}), values and gradients exact", ok)
+
+
+def _pool_input(kind, shape):
+    import torch
+
+    x = torch.randn(shape, device="cuda")
+    if kind == "post-relu":           # (N(0,1) - 1)^+: 84 % exact zeros, a fifth of 3x3 windows all zero
+        x = (x - 1.0).relu()
+    elif kind == "coarse":            # 7 levels: most windows hold their maximum more than once
+        x = (x * 1.5).round().clamp(-3, 3) * 0.5
+    return cl(bf(x))
+
+
+def _maxpool_case(C, H, k, s, p, ceil, n, kind):
+    """maxpool_fwd bit for bit, maxpool_bwd element-wise against torch's float64 CPU max-pool and its backward on the
+    same bf16 values; both take the first maximum of a window in row-major order."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    x = _pool_input(kind, (n, C, H, H))
+    y, arg = nv.maxpool_fwd(x, k, s, p, ceil)
+    xr = x.cpu().double().contiguous().requires_grad_(True)
+    yr = F.max_pool2d(xr, k, s, p, ceil_mode=ceil)
+    tag = f"maxpool {k}/{s}/{p}{' ceil' if ceil else ''} C={C} {H}->{y.shape[2]} N={n} {kind}"
+    _exact(f"{tag} fwd bit-exact", y.shape == yr.shape and torch.equal(y.cpu().double(), yr.detach()))
+    dy = cl(bf(torch.randn(y.shape, device="cuda")))
+    yr.backward(dy.cpu().double().contiguous())
+    dx = nv.maxpool_bwd(dy, arg, x.shape, k, s, p)
+    _classic("pool grad", f"{tag} bwd", dx.cpu(), xr.grad)
+    if not ceil:
+        _check_uncovered(tag, dx, k, s, p)
+
+
+def _avgpool_case(C, H, k, s, p, cip, n):
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    x = cl(bf(torch.randn(n, C, H, H, device="cuda")))
+    y = nv.avgpool_fwd(x, k, s, p, cip)
+    xr = x.cpu().double().contiguous().requires_grad_(True)
+    yr = F.avg_pool2d(xr, k, s, p, count_include_pad=cip)
+    tag = f"avgpool {k}/{s}/{p} count_include_pad={cip} C={C} {H}->{y.shape[2]} N={n}"
+    _classic("pool out", f"{tag} fwd", y.cpu(), yr.detach())
+    dy = cl(bf(torch.randn(y.shape, device="cuda")))
+    yr.backward(dy.cpu().double().contiguous())
+    dx = nv.avgpool_bwd(dy, x.shape, k, s, p, cip)
+    _classic("pool grad", f"{tag} bwd", dx.cpu(), xr.grad)
+    _check_uncovered(tag, dx, k, s, p)
+
+
+def _global_pool_case(C, hw, n):
+    import torch
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    x = cl(bf(torch.randn(n, C, hw, hw, device="cuda")))
+    tag = f"global avgpool C={C} HW={hw * hw} N={n}"
+    _classic("global pool out", f"{tag} fwd", nv.global_avgpool_fwd(x), x.double().mean((2, 3)))
+    dy = bf(torch.randn(n, C, device="cuda"))
+    _classic("global pool grad", f"{tag} bwd", nv.global_avgpool_bwd(dy, x.shape),
+             (dy.double() / (hw * hw))[:, :, None, None].expand(n, C, hw, hw))
+
+
+def _bn_relu_case(C, c_relu, hw, n):
+    """ops.batch_norm_act in training (channel_stats -> bn_act_fwd / bn_act_bwd) on a DenseNet-like input: c_relu
+    post-ReLU channels followed by raw-conv-like channels of assorted scales and offsets.  z, dx, dgamma, dbeta and the
+    running statistics against float64 F.batch_norm; where the float64 BN output lies within 2^-7 of zero (inside the
+    forward budget) the ReLU mask takes the side of the tested output."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import ops
+
+    dev = "cuda"
+    xf = torch.randn(n, C, hw, hw, device=dev)
+    raw = xf[:, c_relu:] * (torch.rand(C - c_relu, device=dev) * 1.5 + 0.5).view(1, -1, 1, 1) + \
+        (torch.randn(C - c_relu, device=dev) * 0.5).view(1, -1, 1, 1)
+    x = cl(bf(torch.cat([xf[:, :c_relu].relu(), raw], 1))).requires_grad_(True)
+    g = (torch.rand(C, device=dev) + 0.5).requires_grad_(True)
+    b = (torch.randn(C, device=dev) * 0.3).requires_grad_(True)
+    rm, rv = torch.randn(C, device=dev) * 0.1, torch.rand(C, device=dev) + 0.5
+    rmd, rvd = rm.double(), rv.double()
+    z = ops.batch_norm_act(x, g, b, rm, rv, 1e-5, 0.1, True, True)
+    tag = f"C={C} {hw}x{hw} N={n}"
+    if type(z.grad_fn).__name__ != "_BnActBackward":
+        _exact(f"bn+relu {tag} runs on the native node ({type(z.grad_fn).__name__})", False)
+    xd = x.detach().double().requires_grad_(True)
+    gd, bd = g.detach().double().requires_grad_(True), b.detach().double().requires_grad_(True)
+    v = F.batch_norm(xd, rmd, rvd, gd, bd, True, 0.1, 1e-5)
+    _classic("bn out", f"bn+relu fwd {tag}", z, v.detach().clamp(min=0))
+    _classic("bn running_mean", f"bn+relu running_mean {tag}", rm, rmd)
+    _classic("bn running_var", f"bn+relu running_var {tag}", rv, rvd)
+    dz = cl(bf(torch.randn(z.shape, device=dev)))
+    z.backward(dz)
+    mask = torch.where(v.detach().abs() <= 2.0 ** -7, z.detach().double() > 0, v.detach() > 0)
+    (v * mask).backward(dz.double())
+    _classic("bn dx", f"bn+relu dx {tag}", x.grad, xd.grad)
+    _classic("bn dgamma", f"bn+relu dgamma {tag}", g.grad, gd.grad)
+    _classic("bn dbeta", f"bn+relu dbeta {tag}", b.grad, bd.grad)
+
+
+def _densenet_layout(name):
+    """DenseNet at 224: [(C, growth, H=W)] of every dense layer's input, [(C, H=W)] of the transition norms and norm5,
+    and the stem width."""
+    from distributeddeeplearning_b200 import models
+
+    f = models.get_model(name).features
+    layers, norms, hw = [], [], 56
+    for cname, mod in f.named_children():
+        if cname.startswith("denseblock"):
+            layers += [(lay.norm1.num_features, lay.conv2.out_channels, hw) for lay in mod.children()]
+        elif cname.startswith("transition"):
+            norms.append((mod.norm.num_features, hw))
+            hw //= 2
+    norms.append((f.norm5.num_features, hw))
+    return layers, norms, f.conv0.out_channels
+
+
+def _conv_geometries(name, size, unit):
+    """Every distinct (Cin, Cout, (R, S), stride, (ph, pw), H, W) of the convolutions of a zoo model at input ``size``,
+    from forward hooks on the modules of type ``unit`` during a CPU forward of batch 2 in training."""
+    import torch
+
+    from distributeddeeplearning_b200 import models
+
+    m = models.get_model(name).train()
+    seen = set()
+
+    def hook(mod, inp, out):
+        c = getattr(mod, "conv", mod)
+        pad = c.padding if isinstance(c.padding, tuple) else (c.padding, c.padding)
+        seen.add((c.in_channels, c.out_channels, tuple(c.kernel_size), c.stride, tuple(pad), inp[0].shape[2],
+                  inp[0].shape[3]))
+
+    hooks = [mod.register_forward_hook(hook) for mod in m.modules() if isinstance(mod, unit)]
+    with torch.no_grad():
+        m(torch.randn(2, 3, size, size))
+    for h in hooks:
+        h.remove()
+    return sorted(seen)
+
+
+def _graph_nodes(*roots):
+    """Counter of the autograd node types reachable from ``roots``."""
+    import collections
+
+    counts, seen = collections.Counter(), set()
+    stack = [r.grad_fn for r in roots if r.grad_fn is not None]
+    while stack:
+        fn = stack.pop()
+        if fn in seen:
+            continue
+        seen.add(fn)
+        counts[type(fn).__name__] += 1
+        stack += [nxt for nxt, _ in fn.next_functions if nxt is not None]
+    return counts
+
+
+def _classic_vs_torchvision(name, bs):
+    """A model (dropout 0) against torchvision fp32 with the same weights and this repo's bf16 composite, under
+    g_model's bounds, plus every BN's running statistics element-wise, the eval-mode logits and an autograd graph free
+    of torch-composite nodes.  Inception-v3's loss is main + 0.4 * aux, and both logits are checked."""
+    import torch
+    import torch.nn.functional as F
+    import torchvision
+
+    from distributeddeeplearning_b200 import models, ops
+    from distributeddeeplearning_b200.models.layers import BatchNorm2d
+
+    torch.manual_seed(0)
+    kw = {"dropout": 0.0} if name.startswith(("inception", "squeezenet")) else {}
+    m = models.get_model(name, **kw).cuda().train()
+    tv = getattr(torchvision.models, name)(**kw, **({"init_weights": False} if name.startswith("inception") else {}))
+    tv = tv.cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name, **kw).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    size = m.input_size
+    # images of different contrast: on i.i.d. noise images of one scale the deep features of a randomly initialised net
+    # are nearly the same for every sample, and a BN over few values (Inception's aux head: 1x1 maps) would normalise
+    # differences hundreds of times smaller than their mean, where one bf16 rounding is no longer small
+    contrast = torch.linspace(0.25, 2.0, bs, device="cuda").view(-1, 1, 1, 1)
+    x = (torch.randn(bs, 3, size, size, device="cuda") * contrast).to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+
+    def heads(out):        # the native classifier may return padded logits
+        return [o[:, :1000] for o in out] if isinstance(out, tuple) else [out[:, :1000]]
+
+    def loss_of(outs, xent):
+        return sum(w * xent(o) for w, o in zip((1.0, 0.4), outs))
+
+    out = heads(m(x))
+    loss = loss_of(out, lambda o: ops.softmax_cross_entropy(o, y, 1000))
+    nodes = _graph_nodes(loss)
+    loss.backward()
+    ro = heads(tv(x))
+    loss_of(ro, lambda o: F.cross_entropy(o, y)).backward()
+    os.environ["DDL_B200_IMPL"] = "torch"
+    try:
+        co = heads(m2(x))
+        loss_of(co, lambda o: ops.softmax_cross_entropy(o, y, 1000)).backward()
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+    fallback = {k: nodes[k] for k in FALLBACK_NODES if nodes[k]}
+    native = {k: v for k, v in sorted(nodes.items()) if k.startswith("_")}
+    _exact(f"{name}: no torch-composite node in the training graph {fallback}; native nodes {native}", not fallback)
+    # Logits: cosine with fp32 above 0.98, or at most 0.01 below the bf16 composite's (Inception-v3's aux head, behind a
+    # BN over 8 values per channel, reaches about 0.98 in bf16 on either implementation).  A gradient the bf16 composite
+    # itself does not resolve (cosine with fp32 below CLASSIC_RESOLVED: the BN parameters of a stem, whose gradients
+    # cancel down to rounding) is noise for any bf16 implementation: the bounds apply to the others, and the unresolved
+    # ones are counted and printed
+    for head, a, r, c in zip(("logits", "aux logits"), out, ro, co):
+        c1, c2 = _cos(a, r), _cos(c, r)
+        _exact(f"{name} {head} cos vs fp32 {c1:.5f} (bf16 composite {c2:.5f})   vs bf16-composite {_cos(a, c):.5f}",
+               c1 > 0.98 or c1 > c2 - 0.01)
+    gn, gc = dict(m.named_parameters()), dict(m2.named_parameters())
+    worst, lag, noise = (1.0, "", 1.0), (0.0, ""), []
+    for k, p in tv.named_parameters():
+        if float(p.grad.norm()) == 0.0:
+            continue
+        c1, c2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if c2 < CLASSIC_RESOLVED:
+            noise.append(f"{k} {c1:.2f}/{c2:.2f}")
+            continue
+        if c1 < worst[0]:
+            worst = (c1, k, c2)
+        if c2 - c1 > lag[0]:
+            lag = (c2 - c1, k)
+    _exact(f"{name}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at {worst[1]} (bf16 composite "
+           f"{worst[2]:.4f}); largest deficit vs the bf16 composite = {lag[0]:.4f} at {lag[1]}; "
+           f"{len(noise)} gradients the composite does not resolve (native/composite cosine): {noise}",
+           worst[0] > 0.80 and lag[0] < 0.08)
+    tvb, cb = dict(tv.named_buffers()), dict(m2.named_buffers())
+    bns = [k for k, mod in m.named_modules() if isinstance(mod, BatchNorm2d)]
+    for stat, (rtol, atol, arms) in CLASSIC_RUNNING_BUDGET.items() if bns else ():
+        worst_n, worst_c, where, bad, finite = 0.0, 0.0, "", 0, True
+        for k in bns:
+            got = getattr(m.get_submodule(k), stat)
+            nb, r, fin = _bound_ratio(got, tvb[f"{k}.{stat}"], rtol, atol, arms)
+            rc = _bound_ratio(cb[f"{k}.{stat}"], tvb[f"{k}.{stat}"], rtol, atol, arms)[1]
+            if nb and r <= 2 * rc:       # where the composite is half-way to the budget, within 2x of the composite
+                nb = 0
+            bad, finite, worst_c = bad + nb, finite and fin, max(worst_c, rc)
+            if r > worst_n:
+                worst_n, where = r, k
+        WORST[f"model {stat}"] = max(WORST.get(f"model {stat}", 0.0), worst_n)
+        _exact(f"{name} {stat} of {len(bns)} BNs vs fp32: violations={bad} worst={worst_n:.3f}x at {where} "
+               f"(bf16 composite {worst_c:.3f}x) of ({arms:g}*rms(ref) + rtol {rtol:g}*|ref|)", bad == 0 and finite)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        oe, re_ = m(x), tv(x)
+    ce = _cos(oe[:, :1000], re_)
+    _exact(f"{name} eval-mode logits cos vs torchvision eval {ce:.5f}", ce > 0.98)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def _graph_replay(name, bs):
+    """Training with the fused engine, eager then CUDA-graph replay: the capture succeeds and the replayed losses track
+    the eager ones.  Dropout is off: the eager and the replayed step draw their masks from different counters.  A second
+    eager run measures how far two eager runs drift apart: Inception-v3's randomly initialised loss on noise images
+    depends on the order of the kernels' fp32 atomics (two eager runs differ by ~1 % at the first step and ~10 % after
+    five), so the replay is held to 5 % or twice that drift, whichever is larger."""
+    import torch
+
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    captured = []
+
+    def run(graph):
+        torch.manual_seed(0)
+        s = BenchmarkSession(name, bs, True, lr=0.01)
+        if hasattr(s.model, "p"):
+            s.model.p = 0.0
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            captured.append(s.enable_graph(warmup=1))
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out[-4:]
+
+    def drift(u, v):
+        return max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(u, v))
+
+    a, a2, b = run(False), run(False), run(True)
+    rel, noise = drift(a, b), drift(a, a2)
+    _exact(f"{name} training: captured={captured[0]} eager {[round(v, 4) for v in a]} graph replay "
+           f"{[round(v, 4) for v in b]} (largest relative difference {rel:.2e}; between two eager runs {noise:.2e})",
+           captured[0] and all(x == x for x in a + b) and rel < max(5e-2, 2 * noise))
+
+
+def g_classic():
+    """Inception-v3, DenseNet and SqueezeNet: the channel concat, max / average / global pooling, stand-alone BN+ReLU
+    and conv+bias+ReLU kernels at every shape these models use (plus edge cases) against float64, every Inception-v3
+    convolution per layer, the three families against torchvision with a native-only autograd graph, and CUDA-graph
+    replay of Inception-v3 and DenseNet-121 training."""
+    import torch
+
+    from distributeddeeplearning_b200.models.inception import BasicConv2d
+    from distributeddeeplearning_b200.models.layers import Conv2d
+    from distributeddeeplearning_b200.parallel import dist
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.manual_seed(0)
+    dn = {name: _densenet_layout(name) for name in ("densenet121", "densenet161")}
+
+    # ---- channel concat: Inception-v3, DenseNet-121 / -161 (C + growth at every layer), SqueezeNet, edges
+    for chans, hw in [((64, 64, 96, 32), 35), ((64, 64, 96, 64), 35), ((384, 96, 288), 17), ((192,) * 4, 17),
+                      ((320, 192, 768), 8), ((384, 384), 8), ((320, 768, 768, 192), 8)]:
+        _concat_case(chans, 2, hw, hw)
+    for layers, _, _ in dn.values():
+        for c, growth, hw in layers:
+            _concat_case((c, growth), 2, hw, hw)
+    for c, hw in [(64, 55), (64, 54), (128, 54), (128, 27), (192, 27), (256, 27), (192, 13), (256, 13)]:
+        _concat_case((c, c), 2, hw, hw)
+    for chans, n, h, w in [((8,) * 8, 2, 5, 3), ((8, 8), 1, 1, 1), ((8,) * 8, 1, 1, 1),
+                           ((8, 16, 24, 64, 8, 120, 40, 8), 3, 7, 11), ((24, 40), 1, 13, 17)]:
+        _concat_case(chans, n, h, w)
+    _concat_dispatch((8,) * 8, "_ConcatBackward")
+    _concat_dispatch((8,) * 9, "CatBackward0")
+    _concat_dispatch((16, 12, 8), "CatBackward0")
+
+    # ---- max pool: SqueezeNet's ceil-mode pools, Inception's pad-0 pools, DenseNet's 3/2/1 stem pool (k3s2 kernels),
+    # and floor-mode edges with an input row / column no window covers
+    for C, H, k, s, p, ceil in [(96, 109, 3, 2, 0, True), (64, 111, 3, 2, 0, True), (128, 55, 3, 2, 0, True),
+                                (256, 54, 3, 2, 0, True), (256, 27, 3, 2, 0, True), (512, 27, 3, 2, 0, True),
+                                (64, 147, 3, 2, 0, False), (192, 71, 3, 2, 0, False), (288, 35, 3, 2, 0, False),
+                                (768, 17, 3, 2, 0, False), (64, 112, 3, 2, 1, False), (96, 112, 3, 2, 1, False),
+                                (64, 16, 3, 2, 0, False), (64, 15, 2, 2, 0, False)]:
+        for kind in ("post-relu", "coarse"):
+            _maxpool_case(C, H, k, s, p, ceil, 2, kind)
+
+    # ---- average pool: Inception 3/1/1 and the aux head's 5/3/0, DenseNet-121 / -161 transitions, odd sizes
+    cases = [(192, 35, 3, 1, 1), (256, 35, 3, 1, 1), (288, 35, 3, 1, 1), (768, 17, 3, 1, 1), (1280, 8, 3, 1, 1),
+             (2048, 8, 3, 1, 1), (768, 17, 5, 3, 0), (64, 15, 2, 2, 0), (64, 7, 2, 2, 0)]
+    cases += [(c // 2, hw, 2, 2, 0) for _, norms, _ in dn.values() for c, hw in norms[:-1]]
+    for C, H, k, s, p in cases:
+        for cip in (True, False):
+            _avgpool_case(C, H, k, s, p, cip, 2)
+    for C, hw in [(2048, 8), (2208, 7), (1000, 13), (512, 1)]:
+        _global_pool_case(C, hw, 4)
+
+    # ---- stand-alone BN + ReLU at every norm1 / transition / norm5 width of DenseNet-121 and -161
+    for layers, norms, c0 in dn.values():
+        for c, hw in [(c, hw) for c, _, hw in layers] + norms:
+            _bn_relu_case(c, c0, hw, {56: 2, 28: 3}.get(hw, 4))
+
+    # ---- conv + bias + ReLU at every SqueezeNet 1.0 / 1.1 geometry (the stems on the NHWC4 image)
+    for name in ("squeezenet1_0", "squeezenet1_1"):
+        for cin, cout, (k, _), s, (p, _), h, _ in _conv_geometries(name, 224, Conv2d):
+            _bias_conv(cin, cout, h, k, 2, stride=s, pad=p, relu=True)
+
+    # ---- every Inception-v3 convolution (the stem is a case of g_conv_fwd / g_conv_wgrad)
+    for cin, cout, kernel, s, pad, h, w in _conv_geometries("inception_v3", 299, BasicConv2d):
+        if cin > 4:
+            _conv_layer(cin, cout, kernel, s, pad, h, w, 2)
+
+    # ---- whole models
+    for name, bs in [("inception_v3", 8), ("densenet121", 16), ("squeezenet1_0", 16), ("squeezenet1_1", 16)]:
+        _classic_vs_torchvision(name, bs)
+    dist.init()
+    _graph_replay("inception_v3", 8)
+    _graph_replay("densenet121", 16)
+    for kind, r in sorted(WORST.items()):
+        print(f"worst ratio to budget: {kind:24s} {r:.3f}x", flush=True)
 
 
 def run_group(name):
