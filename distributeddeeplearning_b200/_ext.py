@@ -160,6 +160,8 @@ KERNEL_LAUNCHES = {
     "fold_cols_f32": 1, "silu_rows_fwd": 1, "silu_rows_bwd": 1, "stochastic_depth_keep": 1,
     "dwconv7_fwd": 1, "dwconv7_dgrad": 1, "dwconv7_wgrad": 1, "layer_norm_fwd": 1, "layer_norm_bwd": 1, "gelu_fwd": 1,
     "gelu_bwd": 1, "layer_scale_fwd": 1, "layer_scale_bwd": 1,
+    "attention_fwd": 1, "attention_bwd": 2, "add_layer_norm_fwd": 1, "layer_norm_bwd_add": 1, "patchify": 1,
+    "tokens_fwd": 1, "tokens_bwd": 2,
 }
 LAUNCH_COUNT = [0]          # kernels of THIS repo launched so far (bench.py reports the per-region delta)
 

@@ -462,6 +462,43 @@ PYBIND11_MODULE(_C, m) {
                                       P<const float>(keep), P<__nv_bfloat16>(dy), P<float>(dls), P<float>(dbias), M, C, hw,
                                       sms, S(stream)), "layer_scale_bwd");
   });
+  // ------------------------------------------------------------------ ViT: attention and row kernels
+  m.def("attention_fwd", [](ptr_t qkv, ptr_t o, ptr_t lse, int N, int L, int H, int C, ptr_t stream) {
+    check(ddl::launch_attention_fwd(P<const __nv_bfloat16>(qkv), P<__nv_bfloat16>(o), P<float>(lse), N, L, H, C,
+                                    S(stream)), "attention_fwd");
+  });
+  m.def("attention_bwd", [](ptr_t qkv, ptr_t o, ptr_t dout, ptr_t lse, ptr_t delta, ptr_t dqkv, int N, int L, int H,
+                            int C, ptr_t stream) {
+    check(ddl::launch_attention_bwd(P<const __nv_bfloat16>(qkv), P<const __nv_bfloat16>(o), P<const __nv_bfloat16>(dout),
+                                    P<const float>(lse), P<float>(delta), P<__nv_bfloat16>(dqkv), N, L, H, C, S(stream)),
+          "attention_bwd");
+  });
+  m.def("add_layer_norm_fwd", [](ptr_t x, ptr_t add, ptr_t gamma, ptr_t beta, ptr_t x1, ptr_t y, ptr_t mean, ptr_t rstd,
+                                 int M, int C, float eps, int sms, ptr_t stream) {
+    check(ddl::launch_add_layer_norm_fwd(P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(add), P<const float>(gamma),
+                                         P<const float>(beta), P<__nv_bfloat16>(x1), P<__nv_bfloat16>(y), P<float>(mean),
+                                         P<float>(rstd), M, C, eps, sms, S(stream)), "add_layer_norm_fwd");
+  });
+  m.def("layer_norm_bwd_add", [](ptr_t dy, ptr_t x, ptr_t mean, ptr_t rstd, ptr_t gamma, ptr_t dres, ptr_t dx,
+                                 ptr_t dgamma, ptr_t dbeta, int M, int C, int sms, ptr_t stream) {
+    check(ddl::launch_layer_norm_bwd_add(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(x), P<const float>(mean),
+                                         P<const float>(rstd), P<const float>(gamma), P<const __nv_bfloat16>(dres),
+                                         P<__nv_bfloat16>(dx), P<float>(dgamma), P<float>(dbeta), M, C, sms, S(stream)),
+          "layer_norm_bwd_add");
+  });
+  m.def("patchify", [](ptr_t img, ptr_t out, int N, int H, int W, int P_, int sms, ptr_t stream) {
+    check(ddl::launch_patchify(P<const __nv_bfloat16>(img), P<__nv_bfloat16>(out), N, H, W, P_, sms, S(stream)),
+          "patchify");
+  });
+  m.def("tokens_fwd", [](ptr_t patch, ptr_t cls, ptr_t pos, ptr_t tok, int N, int L, int C, int sms, ptr_t stream) {
+    check(ddl::launch_tokens_fwd(P<const __nv_bfloat16>(patch), P<const float>(cls), P<const float>(pos),
+                                 P<__nv_bfloat16>(tok), N, L, C, sms, S(stream)), "tokens_fwd");
+  });
+  m.def("tokens_bwd", [](ptr_t dtok, ptr_t dpatch, ptr_t colsum, ptr_t dpos, ptr_t dcls, ptr_t dbias, int N, int L, int C,
+                         ptr_t stream) {
+    check(ddl::launch_tokens_bwd(P<const __nv_bfloat16>(dtok), P<__nv_bfloat16>(dpatch), P<float>(colsum), P<float>(dpos),
+                                 P<float>(dcls), P<float>(dbias), N, L, C, S(stream)), "tokens_bwd");
+  });
   // ------------------------------------------------------------------ squeeze-excitation
   m.def("se_scale", [](ptr_t x, ptr_t s, int lds, ptr_t y, int N, int HW, int C, int sms, ptr_t stream) {
     check(ddl::launch_se_scale(P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(s), lds, P<__nv_bfloat16>(y), N, HW, C,

@@ -134,6 +134,37 @@ cudaError_t launch_layer_scale_bwd(const __nv_bfloat16* dz, const __nv_bfloat16*
                                    __nv_bfloat16* dy, float* dls, float* dbias, int M, int C, int hw, int sms,
                                    cudaStream_t stream);
 
+// ---- multi-head self-attention, head dim 64 (attention.cu; ViT) -------------------------------------------------------
+// qkv [N*L][3C] bf16 (head h: Q, K, V at columns 64h, C + 64h, 2C + 64h), C = 64 H.  forward: o [N*L][C] =
+// softmax(Q K^T / 8) V per (image, head), lse [N][H][L] fp32 natural-log log-sum-exp of the scaled scores.
+cudaError_t launch_attention_fwd(const __nv_bfloat16* qkv, __nv_bfloat16* o, float* lse, int N, int L, int H, int C,
+                                 cudaStream_t stream);
+// backward (two kernels): dqkv [N*L][3C] in qkv's layout from dout [N*L][C] and the saved qkv, o, lse; delta [N][H][L]
+// fp32 receives D = rowsum(dout o o)
+cudaError_t launch_attention_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, const __nv_bfloat16* dout,
+                                 const float* lse, float* delta, __nv_bfloat16* dqkv, int N, int L, int H, int C,
+                                 cudaStream_t stream);
+
+// ---- ViT row kernels (vit.cu) ------------------------------------------------------------------------------------------
+// x1 = x + add, y = LayerNorm(x1) on [M][C] rows (the LayerNorm mapping of convnext.cu), saving fp32 mean / rstd [M]
+cudaError_t launch_add_layer_norm_fwd(const __nv_bfloat16* x, const __nv_bfloat16* add, const float* gamma,
+                                      const float* beta, __nv_bfloat16* x1, __nv_bfloat16* y, float* mean, float* rstd,
+                                      int M, int C, float eps, int sms, cudaStream_t stream);
+// dx = LayerNorm_bwd(dy) + dres; dgamma / dbeta as launch_layer_norm_bwd (optional)
+cudaError_t launch_layer_norm_bwd_add(const __nv_bfloat16* dy, const __nv_bfloat16* x, const float* mean,
+                                      const float* rstd, const float* gamma, const __nv_bfloat16* dres, __nv_bfloat16* dx,
+                                      float* dgamma, float* dbeta, int M, int C, int sms, cudaStream_t stream);
+// NHWC4 image [N][H][W][4] -> patch rows [N * (H/P) * (W/P)][P*P*3] in (r, s, c) order
+cudaError_t launch_patchify(const __nv_bfloat16* img, __nv_bfloat16* out, int N, int H, int W, int P, int sms,
+                            cudaStream_t stream);
+// tok [N*L][C] = (cls | patch [N*(L-1)][C]) + pos [L][C]  (cls, pos fp32)
+cudaError_t launch_tokens_fwd(const __nv_bfloat16* patch, const float* cls, const float* pos, __nv_bfloat16* tok, int N,
+                              int L, int C, int sms, cudaStream_t stream);
+// dpatch = rows 1.. of every image of dtok (optional); colsum [L][C] fp32 scratch; dpos[l] += sum_n dtok[n, l],
+// dcls += sum_n dtok[n, 0], dbias += sum_{n, l >= 1} dtok[n, l] (each optional), in a fixed order (two kernels)
+cudaError_t launch_tokens_bwd(const __nv_bfloat16* dtok, __nv_bfloat16* dpatch, float* colsum, float* dpos, float* dcls,
+                              float* dbias, int N, int L, int C, cudaStream_t stream);
+
 // ---- pooling -------------------------------------------------------------------------------------
 struct PoolArgs {
   int N, H, W, C, P, Q, k, stride, pad;

@@ -5,8 +5,8 @@ Parity: the reference resolves ``--model`` with ``getattr(torchvision.models, na
 (``imagenet_pytorch_horovod.py:383``).  North-star zoo: ResNet-50/101/152, VGG-16, Inception-v3,
 AlexNet (SURVEY.md 2.7); ResNet-18/34, the other VGG depths, DenseNet and SqueezeNet (the rest of torchvision
 0.2.1's families) are here too, and the later ResNet family members of torchvision (ResNeXt-50 32x4d, ResNeXt-101
-32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2, MobileNetV3-Large / -Small, EfficientNet-B0 to -B7 and
-ConvNeXt-Tiny / -Small / -Base / -Large.
+32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2, MobileNetV3-Large / -Small, EfficientNet-B0 to -B7,
+ConvNeXt-Tiny / -Small / -Base / -Large and the Vision Transformers ViT-B/16, -B/32, -L/16 and -L/32.
 """
 from __future__ import annotations
 
@@ -23,6 +23,7 @@ from .resnet import (ResNet, resnet18, resnet34, resnet50, resnet101, resnet152,
                      resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2)
 from .squeezenet import SqueezeNet, squeezenet1_0, squeezenet1_1  # noqa: F401
 from .vgg import VGG, vgg11, vgg11_bn, vgg13, vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn  # noqa: F401
+from .vit import VisionTransformer, vit_b_16, vit_b_32, vit_l_16, vit_l_32  # noqa: F401
 
 _REGISTRY = {
     f.__name__: f
@@ -32,7 +33,7 @@ _REGISTRY = {
               squeezenet1_0, squeezenet1_1, inception_v3, mobilenet_v2,
               mobilenet_v3_large, mobilenet_v3_small, resnet18, resnet34, resnet50, resnet101, resnet152,
               resnext50_32x4d, resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2, vgg11, vgg11_bn, vgg13,
-              vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn)
+              vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn, vit_b_16, vit_b_32, vit_l_16, vit_l_32)
 }
 
 
@@ -52,7 +53,7 @@ def get_model(name: str, **kw):
 
 def input_size(model_or_name) -> int:
     """Spatial input size (299 for Inception-v3 — the reference hard-codes 224 and breaks, SURVEY.md Q2; torchvision's
-    crop size for EfficientNet-B0 to -B7, 224 to 600)."""
+    crop size for EfficientNet-B0 to -B7, 224 to 600; a Vision Transformer's ``image_size``)."""
     if isinstance(model_or_name, str):
         if model_or_name in _EFFICIENTNET_INPUT_SIZE:
             return _EFFICIENTNET_INPUT_SIZE[model_or_name]

@@ -20,3 +20,4 @@ from .functional import (  # noqa: F401
     topk_correct,
     use_native,
 )
+from .vit import self_attention, vit_embed, vit_encoder_block  # noqa: F401

@@ -641,6 +641,142 @@ def layer_scale_bwd(dz: torch.Tensor, y: torch.Tensor, ls: torch.Tensor, keep: O
 
 
 # ------------------------------------------------------------------------------------------------
+# ViT: multi-head self-attention (csrc/ops/attention.cu) and the token-row kernels (csrc/ops/vit.cu)
+# ------------------------------------------------------------------------------------------------
+def supports_attention(L: int, heads: int, head_dim: int) -> bool:
+    """Shapes the attention kernels take: head dim 64 and C = 64 * heads (any L >= 1)."""
+    return head_dim == 64 and 0 < heads <= 65535 and L >= 1
+
+
+def _check_rows(t: torch.Tensor, rows: int, cols: int, name: str) -> None:
+    if t.dtype != torch.bfloat16 or not t.is_cuda or t.dim() != 2 or tuple(t.shape) != (rows, cols) \
+            or not t.is_contiguous():
+        raise ValueError(f"{name}: expected a contiguous CUDA bf16 [{rows}, {cols}] matrix, got {t.dtype} "
+                         f"{tuple(t.shape)} on {t.device}")
+    _check_aligned(t, name)
+
+
+def _attn_dims(qkv: torch.Tensor, num_heads: int, L: int) -> Tuple[int, int]:
+    if qkv.dim() != 2 or qkv.shape[1] % 3 != 0 or L <= 0 or qkv.shape[0] % L != 0:
+        raise ValueError("attention: qkv must be [N*L, 3C]")
+    C = qkv.shape[1] // 3
+    if C % num_heads != 0 or not supports_attention(L, num_heads, C // num_heads):
+        raise ValueError(f"attention: head dim {C // max(num_heads, 1)} is not supported by the native kernels (64 only)")
+    return qkv.shape[0] // L, C
+
+
+def attention_fwd(qkv: torch.Tensor, num_heads: int, L: int):
+    """O [N*L, C] = softmax(Q K^T / sqrt(64)) V per (image, head) from the packed in-projection output qkv [N*L, 3C];
+    returns (O, lse fp32 [N, H, L])."""
+    N, C = _attn_dims(qkv, num_heads, L)
+    _check_rows(qkv, N * L, 3 * C, "qkv")
+    o = torch.empty((N * L, C), dtype=torch.bfloat16, device=qkv.device)
+    lse = torch.empty((N, num_heads, L), dtype=torch.float32, device=qkv.device)
+    _C().attention_fwd(qkv.data_ptr(), o.data_ptr(), lse.data_ptr(), N, L, num_heads, C, _stream())
+    return o, lse
+
+
+def attention_bwd(dout: torch.Tensor, qkv: torch.Tensor, o: torch.Tensor, lse: torch.Tensor, num_heads: int,
+                  L: int) -> torch.Tensor:
+    """dqkv [N*L, 3C] (qkv's layout) of :func:`attention_fwd` from dO and the saved qkv, O and lse."""
+    N, C = _attn_dims(qkv, num_heads, L)
+    _check_rows(qkv, N * L, 3 * C, "qkv")
+    _check_rows(o, N * L, C, "o")
+    _check_rows(dout, N * L, C, "dout")
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (N, num_heads, L) or not lse.is_contiguous():
+        raise ValueError("attention_bwd: lse must be the contiguous fp32 [N, H, L] of the forward")
+    dqkv = torch.empty_like(qkv)
+    delta = torch.empty((N, num_heads, L), dtype=torch.float32, device=qkv.device)
+    _C().attention_bwd(qkv.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(), delta.data_ptr(),
+                       dqkv.data_ptr(), N, L, num_heads, C, _stream())
+    return dqkv
+
+
+def add_layer_norm_fwd(x: torch.Tensor, a: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float):
+    """x1 = x + a and t = LayerNorm(x1) over the rows of [M, C] matrices: returns (x1, t, mean fp32 [M], rstd fp32 [M])."""
+    M, Ch = _rows(x)
+    _check_rows(x, M, Ch, "x")
+    _check_rows(a, M, Ch, "a")
+    if x.dim() != 2 or not supports_layer_norm(Ch):
+        raise ValueError(f"add_layer_norm: {Ch} channels are not supported by the native kernels")
+    _check_f32_vec(gamma, Ch, "gamma")
+    _check_f32_vec(beta, Ch, "beta")
+    x1, t = torch.empty_like(x), torch.empty_like(x)
+    mean = torch.empty(M, dtype=torch.float32, device=x.device)
+    rstd = torch.empty(M, dtype=torch.float32, device=x.device)
+    _C().add_layer_norm_fwd(x.data_ptr(), a.data_ptr(), gamma.data_ptr(), beta.data_ptr(), x1.data_ptr(), t.data_ptr(),
+                            mean.data_ptr(), rstd.data_ptr(), M, Ch, float(eps), sm_count(x.device.index or 0), _stream())
+    return x1, t, mean, rstd
+
+
+def layer_norm_bwd_add(dy: torch.Tensor, x: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor, gamma: torch.Tensor,
+                       dres: torch.Tensor, grad_gamma: Optional[torch.Tensor],
+                       grad_beta: Optional[torch.Tensor]) -> torch.Tensor:
+    """dx = :func:`layer_norm_bwd` (dy) + dres over [M, C] rows, with the same grad_gamma / grad_beta sums."""
+    M, Ch = _rows(x)
+    for t, name in ((dy, "dy"), (x, "x"), (dres, "dres")):
+        _check_rows(t, M, Ch, name)
+    if not supports_layer_norm(Ch):
+        raise ValueError(f"layer_norm_bwd_add: {Ch} channels are not supported by the native kernels")
+    _check_f32_vec(mean, M, "mean")
+    _check_f32_vec(rstd, M, "rstd")
+    for t, name in ((gamma, "gamma"), (grad_gamma, "grad_gamma"), (grad_beta, "grad_beta")):
+        _check_f32_vec(t, Ch, name)
+    dx = torch.empty_like(x)
+    _C().layer_norm_bwd_add(dy.data_ptr(), x.data_ptr(), mean.data_ptr(), rstd.data_ptr(), gamma.data_ptr(),
+                            dres.data_ptr(), dx.data_ptr(), _ptr(grad_gamma), _ptr(grad_beta), M, Ch,
+                            sm_count(x.device.index or 0), _stream())
+    return dx
+
+
+def patchify(img: torch.Tensor, patch: int) -> torch.Tensor:
+    """NHWC4 image [N, 4, H, W] -> patch rows [N * (H/P) * (W/P), P*P*3] in (r, s, c) order: the GEMM operand of a
+    channels_last conv_proj weight [C, 3, P, P] taken as the [C, 3*P*P] matrix it is in memory."""
+    _check_act(img, "img")
+    N, c4, H, W = img.shape
+    if img.dim() != 4 or c4 != 4 or H % patch != 0 or W % patch != 0:
+        raise ValueError(f"patchify: expected an NHWC4 image whose sides are multiples of {patch}")
+    rows = N * (H // patch) * (W // patch)
+    out = torch.empty((rows, 3 * patch * patch), dtype=torch.bfloat16, device=img.device)
+    _C().patchify(img.data_ptr(), out.data_ptr(), N, H, W, patch, sm_count(img.device.index or 0), _stream())
+    return out
+
+
+def tokens_fwd(patch_rows: torch.Tensor, cls: torch.Tensor, pos: torch.Tensor, N: int) -> torch.Tensor:
+    """tokens [N*L, C]: row (n, 0) = cls + pos[0], row (n, 1+p) = patch_rows[n*(L-1) + p] + pos[1+p] (cls [C] and
+    pos [L, C] fp32)."""
+    C = cls.numel()
+    L = pos.numel() // max(C, 1)
+    if C % 8 != 0 or L < 2 or pos.numel() != L * C:
+        raise ValueError("tokens_fwd: pos must hold L >= 2 rows of C (a multiple of 8) columns")
+    _check_rows(patch_rows, N * (L - 1), C, "patch_rows")
+    _check_f32_vec(cls, C, "cls")
+    _check_f32_vec(pos, L * C, "pos")
+    tok = torch.empty((N * L, C), dtype=torch.bfloat16, device=patch_rows.device)
+    _C().tokens_fwd(patch_rows.data_ptr(), cls.data_ptr(), pos.data_ptr(), tok.data_ptr(), N, L, C,
+                    sm_count(tok.device.index or 0), _stream())
+    return tok
+
+
+def tokens_bwd(dtok: torch.Tensor, N: int, L: int, grad_pos: Optional[torch.Tensor], grad_cls: Optional[torch.Tensor],
+               grad_bias: Optional[torch.Tensor], want_dpatch: bool = True) -> Optional[torch.Tensor]:
+    """Backward of :func:`tokens_fwd`: returns dpatch [N*(L-1), C] (the patch rows of dtok, or None); grad_pos [L, C] +=
+    sum over images, grad_cls [C] += that of token 0, grad_bias [C] += sum over the patch tokens (each optional)."""
+    C = dtok.shape[1]
+    if L < 2 or C % 8 != 0:
+        raise ValueError("tokens_bwd: L >= 2 and C a multiple of 8")
+    _check_rows(dtok, N * L, C, "dtok")
+    _check_f32_vec(grad_pos, L * C, "grad_pos")
+    _check_f32_vec(grad_cls, C, "grad_cls")
+    _check_f32_vec(grad_bias, C, "grad_bias")
+    dpatch = torch.empty((N * (L - 1), C), dtype=torch.bfloat16, device=dtok.device) if want_dpatch else None
+    colsum = torch.empty((L, C), dtype=torch.float32, device=dtok.device)
+    _C().tokens_bwd(dtok.data_ptr(), _ptr(dpatch), colsum.data_ptr(), _ptr(grad_pos), _ptr(grad_cls), _ptr(grad_bias),
+                    N, L, C, _stream())
+    return dpatch
+
+
+# ------------------------------------------------------------------------------------------------
 # squeeze-excitation (csrc/ops/squeeze_excite.cu) and hardswish on [B, F]
 # ------------------------------------------------------------------------------------------------
 def _check_gate(s: torch.Tensor, n: int, c: int) -> None:

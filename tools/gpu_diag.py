@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -2932,6 +2932,263 @@ def g_convnext():
           f"fp8 launches {fp8.launches()}", flush=True)
     del s
     torch.cuda.empty_cache()
+
+
+# ------------------------------------------------------------------------------------------------
+# ViT: attention, add + LayerNorm, LayerNorm backward with an addend, patchify, token assembly, vit_b_16
+# ------------------------------------------------------------------------------------------------
+# Budgets as (rtol, atol, arms) of report_abs; every reference is float64 on the same bf16 operands.
+# - attn o: P is rounded to bf16 (relative 2^-9) before P V and O is rounded once (2^-9): 2^-7 of |ref| plus 2^-7 of
+#   rms(ref) for rows whose terms cancel.
+# - attn lse: fp32 scores of exact bf16 products, fp32 exp2 / log2: 1e-4 absolute.
+# - attn dq / dk / dv: dS = P (dP - D) cancels where dP is close to D, and P, dS are bf16 operands: 2^-6 of |ref| plus
+#   2^-5 of rms(ref).  Where the exact dQ / dK is 0 (L = 1: P = 1 and dP = D) the kernels' fp32 dP and D differ in
+#   their summation order, so dQ / dK also get 2^-8 of rms(dV) absolute.  A masking or indexing bug is an error of order
+#   rms(ref).
+# - ln out / ln dx: one bf16 rounding of an fp32 row computation: 2^-7 of |ref| plus 2^-8 of rms(ref);
+#   ln dgamma / dbeta: fp32 sums over the rows: 2^-8 of |ref| plus 2^-10 of rms(ref).
+# - token sums: fp32 sums of n bf16 terms (n = N for dpos / dcls, N (L - 1) for dbias): 1e-5 of |ref| plus
+#   2^-22 n rms(terms) absolute, the rounding of an n-term fp32 sum where the terms cancel.
+VIT_BUDGET = {"attn o": (2.0 ** -7, 0.0, 2.0 ** -7), "attn lse": (0.0, 1e-4, 0.0), "attn dq": (2.0 ** -6, 0.0, 2.0 ** -5),
+              "attn dk": (2.0 ** -6, 0.0, 2.0 ** -5), "attn dv": (2.0 ** -6, 0.0, 2.0 ** -5),
+              "ln out": (2.0 ** -7, 0.0, 2.0 ** -8), "ln dx": (2.0 ** -7, 0.0, 2.0 ** -8),
+              "ln dgamma": (2.0 ** -8, 0.0, 2.0 ** -10), "ln dbeta": (2.0 ** -8, 0.0, 2.0 ** -10),
+              "token sums": (1e-5, 1e-6, 0.0)}
+
+
+def _vit_check(name, kind, got, ref, atol=None):
+    rtol, atol0, arms = VIT_BUDGET[kind]
+    report_abs(f"{name} {kind}", got, ref, rtol, atol0 if atol is None else atol, arms, kind=kind)
+
+
+def _attn_case(N, L, H, special=None):
+    import torch
+
+    from distributeddeeplearning_b200.ops import native
+
+    C = 64 * H
+    qkv = torch.randn(N, L, 3 * C, device="cuda")
+    if special == "dominant":          # query 0 of every head aligned with key L // 2, scaled: one logit far above the rest
+        for h in range(H):
+            qkv[:, 0, 64 * h:64 * h + 64] = 4.0 * qkv[:, L // 2, C + 64 * h:C + 64 * h + 64]
+    elif special == "constant":        # every key of image 0 equal: a constant score row, O = mean of V
+        qkv[0, :, C:2 * C] = qkv[0, :1, C:2 * C]
+    qkv = qkv.to(torch.bfloat16)
+    dout = torch.randn(N * L, C, device="cuda").to(torch.bfloat16)
+    o, lse = native.attention_fwd(qkv.view(N * L, 3 * C), H, L)
+    dqkv = native.attention_bwd(dout, qkv.view(N * L, 3 * C), o, lse, H, L)
+    qd = qkv.double().requires_grad_(True)
+    q, k, v = (t.reshape(N, L, H, 64).transpose(1, 2) for t in qd.split(C, dim=2))
+    s = q @ k.transpose(-2, -1) / 8.0
+    ref = (torch.softmax(s, -1) @ v).transpose(1, 2).reshape(N * L, C)
+    ref.backward(dout.double())
+    tag = f"attention N={N} L={L} heads={H}" + (f" {special}" if special else "")
+    _vit_check(tag, "attn o", o, ref.detach())
+    _vit_check(tag, "attn lse", lse, torch.logsumexp(s.detach(), -1))
+    g = qd.grad.view(N * L, 3 * C)
+    floor = 2.0 ** -8 * float(g[:, 2 * C:].pow(2).mean().sqrt())
+    for i, kind in enumerate(("attn dq", "attn dk", "attn dv")):
+        _vit_check(tag, kind, dqkv[:, i * C:(i + 1) * C], g[:, i * C:(i + 1) * C], atol=floor if i < 2 else None)
+
+
+def _add_ln_case(M, C, offset):
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native
+
+    x = (torch.randn(M, C, device="cuda") + offset).to(torch.bfloat16)
+    a = torch.randn(M, C, device="cuda").to(torch.bfloat16)
+    gamma = torch.randn(C, device="cuda") * 0.5 + 1.0
+    beta = torch.randn(C, device="cuda") * 0.1
+    x1, t, mean, rstd = native.add_layer_norm_fwd(x, a, gamma, beta, 1e-6)
+    tag = f"add+LN M={M} C={C} offset={offset:g}"
+    ok = torch.equal(x1, (x.float() + a.float()).to(torch.bfloat16))
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {tag} x1 bit for bit", flush=True)
+    xd = x1.double().requires_grad_(True)
+    gd, bd = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
+    ref = F.layer_norm(xd, (C,), gd, bd, 1e-6)
+    _vit_check(tag, "ln out", t, ref.detach())
+    dt = torch.randn(M, C, device="cuda").to(torch.bfloat16)
+    dres = torch.randn(M, C, device="cuda").to(torch.bfloat16)
+    ref.backward(dt.double())
+    dg, db = torch.zeros(C, device="cuda"), torch.zeros(C, device="cuda")
+    dx = native.layer_norm_bwd_add(dt, x1, mean, rstd, gamma, dres, dg, db)
+    tag = f"LN bwd + addend M={M} C={C} offset={offset:g}"
+    _vit_check(tag, "ln dx", dx, xd.grad + dres.double())
+    _vit_check(tag, "ln dgamma", dg, gd.grad)
+    _vit_check(tag, "ln dbeta", db, bd.grad)
+
+
+def _embed_cases():
+    import torch
+
+    from distributeddeeplearning_b200.ops import native
+
+    for N, size, P in ((4, 224, 16), (4, 224, 32), (2, 384, 32)):
+        img = torch.randn(N, 4, size, size, device="cuda").to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+        rows = native.patchify(img, P)
+        g = size // P
+        ref = img.permute(0, 2, 3, 1)[..., :3].reshape(N, g, P, g, P, 3).permute(0, 1, 3, 2, 4, 5).reshape(-1, 3 * P * P)
+        ok = torch.equal(rows, ref)
+        RESULTS.append(ok)
+        print(f"[{'ok' if ok else 'FAIL'}] patchify N={N} {size}x{size} P={P} bit for bit", flush=True)
+    for N, L, C in ((32, 197, 768), (3, 50, 1024), (2, 577, 768)):
+        patch = torch.randn(N * (L - 1), C, device="cuda").to(torch.bfloat16)
+        cls, pos = torch.randn(C, device="cuda"), torch.randn(L, C, device="cuda")
+        tok = native.tokens_fwd(patch, cls, pos, N)
+        ref = (torch.cat([cls.expand(N, 1, C), patch.float().view(N, L - 1, C)], 1) + pos).to(torch.bfloat16)
+        ok = torch.equal(tok.view(N, L, C), ref)
+        RESULTS.append(ok)
+        print(f"[{'ok' if ok else 'FAIL'}] token assembly N={N} L={L} C={C} bit for bit", flush=True)
+        dtok = torch.randn(N * L, C, device="cuda").to(torch.bfloat16)
+        gpos, gcls, gb = torch.ones(L, C, device="cuda"), torch.ones(C, device="cuda"), torch.ones(C, device="cuda")
+        dpatch = native.tokens_bwd(dtok, N, L, gpos, gcls, gb)
+        d = dtok.view(N, L, C)
+        ok = torch.equal(dpatch.view(N, L - 1, C), d[:, 1:])
+        RESULTS.append(ok)
+        print(f"[{'ok' if ok else 'FAIL'}] token assembly backward N={N} L={L} C={C} dpatch bit for bit", flush=True)
+        s = d.double().sum(0)
+        tag = f"token assembly backward N={N} L={L} C={C}"
+        rms = float(d.double().pow(2).mean().sqrt())
+        _vit_check(tag + " dpos", "token sums", gpos, s + 1, atol=2.0 ** -22 * N * rms)
+        _vit_check(tag + " dcls", "token sums", gcls, s[0] + 1, atol=2.0 ** -22 * N * rms)
+        _vit_check(tag + " dbias", "token sums", gb, s[1:].sum(0) + 1, atol=2.0 ** -22 * N * (L - 1) * rms)
+
+
+def _vit_vs_torchvision(name, bs):
+    """A ViT against torchvision fp32 with the same weights (a random head: the zero head would zero every other
+    gradient) and this repo's bf16 composite; forward hooks check that every block ran on the native node."""
+    import torch
+    import torchvision
+
+    from distributeddeeplearning_b200 import models, ops
+    from distributeddeeplearning_b200.models.vit import EncoderBlock
+
+    torch.manual_seed(0)
+    m = models.get_model(name).cuda().train()
+    with torch.no_grad():
+        m.heads.head.weight.normal_(std=0.02)
+        m.class_token.normal_(std=0.02)
+    tv = getattr(torchvision.models, name)().cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    nodes = []
+    hooks = [mod.register_forward_hook(lambda mod, i, o: nodes.append(type(o.grad_fn).__name__))
+             for mod in m.modules() if isinstance(mod, EncoderBlock)]
+    x = torch.randn(bs, 3, 224, 224, device="cuda").to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    try:
+        out = m(x)
+        for h in hooks:
+            h.remove()
+        ops.softmax_cross_entropy(out, y, 1000).backward()
+        ro = tv(x)
+        torch.nn.functional.cross_entropy(ro, y).backward()
+        os.environ["DDL_B200_IMPL"] = "torch"
+        co = m2(x)
+        ops.softmax_cross_entropy(co, y, 1000).backward()
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+    n_blocks = len(m.encoder.layers)
+    ok = len(nodes) == n_blocks and set(nodes) == {"_EncoderBlockBackward"}
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: {len(nodes)} of {n_blocks} blocks ran on {sorted(set(nodes))}", flush=True)
+    c1, c2 = _cos(out, ro), _cos(co, ro)
+    RESULTS.append(c1 > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} logits cos vs fp32 {c1:.5f}   (bf16 composite {c2:.5f})")
+    gn, gc, tvp = dict(m.named_parameters()), dict(m2.named_parameters()), dict(tv.named_parameters())
+    worst, lag = (1.0, "", 1.0), (-1.0, "")
+    for k, p in tvp.items():
+        if float(p.grad.norm()) == 0.0:
+            continue
+        a1, a2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if a1 < worst[0]:
+            worst = (a1, k, a2)
+        if a2 - a1 > lag[0]:
+            lag = (a2 - a1, k)
+    ok = lag[0] <= 0.01 and worst[0] > 0.6
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at {worst[1]} "
+          f"(bf16 composite {worst[2]:.4f}); largest deficit vs the bf16 composite = {lag[0]:.4f} at {lag[1]}", flush=True)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        oe, re_ = m(x), tv(x)
+    ce = _cos(oe, re_)
+    RESULTS.append(ce > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} eval-mode logits cos vs torchvision eval {ce:.5f}", flush=True)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def g_vit():
+    """ViT: attention forward / backward at every zoo shape and edge cases (L = 1, 63, 64, 65, a dominant logit, a
+    constant score row), add + LayerNorm and LayerNorm backward with an addend, patchify and token assembly,
+    vit_b_16 against torchvision, eager vs CUDA-graph training and an fp8 session."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.manual_seed(0)
+    for N, L in ((8, 50), (4, 145), (4, 197), (2, 577)):
+        for H in (12, 16):
+            _attn_case(N, L, H)
+    for L in (1, 63, 64, 65):
+        _attn_case(3, L, 12)
+    _attn_case(2, 197, 12, "dominant")
+    _attn_case(2, 50, 16, "constant")
+    for C in (768, 1024):
+        _add_ln_case(4 * 197, C, 0.0)
+        _add_ln_case(37, C, 100.0)
+    _embed_cases()
+    _vit_vs_torchvision("vit_b_16", 16)
+    dist.init()
+
+    def run(graph):
+        torch.manual_seed(0)
+        s = BenchmarkSession("vit_b_16", 16, True, lr=0.01, momentum=0.9)
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out
+
+    a, b = run(False), run(True)
+    rel = max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(a[-4:], b[-4:]))
+    ok = all(x == x for x in a + b) and rel < 5e-2 and a[-1] < a[0]
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] vit_b_16 training: eager {[round(v, 4) for v in a]} graph replay "
+          f"{[round(v, 4) for v in b]} (largest relative difference of the last 4 {rel:.2e})", flush=True)
+    fp8.reset()
+    fp8.enable(True)
+    try:
+        torch.manual_seed(0)
+        s = BenchmarkSession("vit_b_16", 16, True, lr=0.01, momentum=0.9)
+        losses = [float(s.step()) for _ in range(4)]
+        torch.cuda.synchronize()
+        s.optimizer.check_errors()
+    finally:
+        fp8.enable(False)
+    n8 = fp8.launches()
+    ok = all(l == l and abs(l) < 1e4 for l in losses) and n8.get("fwd", 0) > 0
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] vit_b_16 fp8 session: losses {[round(v, 3) for v in losses]}, fp8 launches {n8}",
+          flush=True)
+    del s
+    torch.cuda.empty_cache()
+    for kind, r in sorted(WORST.items()):
+        print(f"worst ratio to budget: {kind:24s} {r:.3f}x", flush=True)
 
 
 # ------------------------------------------------------------------------------------------------
