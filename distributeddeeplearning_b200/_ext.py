@@ -162,6 +162,7 @@ KERNEL_LAUNCHES = {
     "gelu_bwd": 1, "layer_scale_fwd": 1, "layer_scale_bwd": 1,
     "attention_fwd": 1, "attention_bwd": 2, "add_layer_norm_fwd": 1, "layer_norm_bwd_add": 1, "patchify": 1,
     "tokens_fwd": 1, "tokens_bwd": 2,
+    "window_attention_fwd": 1, "window_attention_bwd": 3, "patch_merge_fwd": 1, "patch_merge_bwd": 2,
 }
 LAUNCH_COUNT = [0]          # kernels of THIS repo launched so far (bench.py reports the per-region delta)
 

@@ -499,6 +499,36 @@ PYBIND11_MODULE(_C, m) {
     check(ddl::launch_tokens_bwd(P<const __nv_bfloat16>(dtok), P<__nv_bfloat16>(dpatch), P<float>(colsum), P<float>(dpos),
                                  P<float>(dcls), P<float>(dbias), N, L, C, S(stream)), "tokens_bwd");
   });
+  // ------------------------------------------------------------------ Swin: window attention and patch merging
+  m.def("window_attention_fwd", [](ptr_t qkv, ptr_t table, ptr_t o, ptr_t lse, int N, int H, int W, int heads, int C,
+                                   int sy, int sx, ptr_t stream) {
+    check(ddl::launch_window_attention_fwd(P<const __nv_bfloat16>(qkv), P<const float>(table), P<__nv_bfloat16>(o),
+                                           P<float>(lse), N, H, W, heads, C, sy, sx, S(stream)), "window_attention_fwd");
+  });
+  m.def("window_attention_bwd", [](ptr_t qkv, ptr_t table, ptr_t o, ptr_t dout, ptr_t lse, ptr_t dqkv, ptr_t dtable,
+                                   ptr_t scratch, int N, int H, int W, int heads, int C, int sy, int sx, ptr_t stream) {
+    check(ddl::launch_window_attention_bwd(P<const __nv_bfloat16>(qkv), P<const float>(table),
+                                           P<const __nv_bfloat16>(o), P<const __nv_bfloat16>(dout), P<const float>(lse),
+                                           P<__nv_bfloat16>(dqkv), P<float>(dtable), P<float>(scratch), N, H, W, heads, C,
+                                           sy, sx, S(stream)), "window_attention_bwd");
+  });
+  m.def("window_attention_bwd_scratch_floats", [](int N, int H, int heads) {
+    return ddl::window_attention_bwd_scratch_floats(N, H, heads);
+  });
+  m.def("patch_merge_fwd", [](ptr_t x, ptr_t gamma, ptr_t beta, ptr_t y, ptr_t mean, ptr_t rstd, int N, int H, int W,
+                              int C, float eps, int sms, ptr_t stream) {
+    check(ddl::launch_patch_merge_fwd(P<const __nv_bfloat16>(x), P<const float>(gamma), P<const float>(beta),
+                                      P<__nv_bfloat16>(y), P<float>(mean), P<float>(rstd), N, H, W, C, eps, sms,
+                                      S(stream)), "patch_merge_fwd");
+  });
+  m.def("patch_merge_bwd", [](ptr_t dy, ptr_t x, ptr_t mean, ptr_t rstd, ptr_t gamma, ptr_t dx, ptr_t dgamma,
+                              ptr_t dbeta, ptr_t scratch, int N, int H, int W, int C, int sms, ptr_t stream) {
+    check(ddl::launch_patch_merge_bwd(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(x), P<const float>(mean),
+                                      P<const float>(rstd), P<const float>(gamma), P<__nv_bfloat16>(dx), P<float>(dgamma),
+                                      P<float>(dbeta), P<float>(scratch), N, H, W, C, sms, S(stream)),
+          "patch_merge_bwd");
+  });
+  m.def("patch_merge_bwd_blocks", [](int sms) { return ddl::patch_merge_bwd_blocks(sms); });
   // ------------------------------------------------------------------ squeeze-excitation
   m.def("se_scale", [](ptr_t x, ptr_t s, int lds, ptr_t y, int N, int HW, int C, int sms, ptr_t stream) {
     check(ddl::launch_se_scale(P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(s), lds, P<__nv_bfloat16>(y), N, HW, C,

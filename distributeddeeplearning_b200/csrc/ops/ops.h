@@ -165,6 +165,33 @@ cudaError_t launch_tokens_fwd(const __nv_bfloat16* patch, const float* cls, cons
 cudaError_t launch_tokens_bwd(const __nv_bfloat16* dtok, __nv_bfloat16* dpatch, float* colsum, float* dpos, float* dcls,
                               float* dbias, int N, int L, int C, cudaStream_t stream);
 
+// ---- Swin: shifted-window attention, window 7, head dim 32 (window_attention.cu) ---------------------------------------
+// qkv [N*H*W][3C] bf16 in image order (head h: Q, K, V at columns 32h, C + 32h, 2C + 32h), C = 32 heads, H and W
+// multiples of 7, shift (sy, sx) in [0, 7) (0 on a side of 7).  forward: o [N*H*W][C] and lse [N*H*W][heads] fp32 of the
+// windows of the map rolled by -shift, with the relative-position bias table [169][heads] fp32 and the shifted-window mask.
+cudaError_t launch_window_attention_fwd(const __nv_bfloat16* qkv, const float* table, __nv_bfloat16* o, float* lse,
+                                        int N, int H, int W, int heads, int C, int sy, int sx, cudaStream_t stream);
+// backward (three kernels, deterministic): dqkv [N*H*W][3C] in qkv's layout; dtable [169][heads] += the bias gradient
+// (optional); scratch holds window_attention_bwd_scratch_floats(N, H, heads) fp32
+cudaError_t launch_window_attention_bwd(const __nv_bfloat16* qkv, const float* table, const __nv_bfloat16* o,
+                                        const __nv_bfloat16* dout, const float* lse, __nv_bfloat16* dqkv, float* dtable,
+                                        float* scratch, int N, int H, int W, int heads, int C, int sy, int sx,
+                                        cudaStream_t stream);
+size_t window_attention_bwd_scratch_floats(int N, int H, int heads);
+
+// ---- Swin: patch merging (swin.cu) -------------------------------------------------------------------------------------
+// y [N * H/2 * W/2][4C] = LayerNorm over 4C of the 2x2 gather (x0, x1, x2, x3) of the NHWC x [N][H][W][C] (H, W even,
+// C % 8 == 0, C <= 512), saving fp32 mean / rstd [rows]
+cudaError_t launch_patch_merge_fwd(const __nv_bfloat16* x, const float* gamma, const float* beta, __nv_bfloat16* y,
+                                   float* mean, float* rstd, int N, int H, int W, int C, float eps, int sms,
+                                   cudaStream_t stream);
+// dx [N][H][W][C] of the forward from dy [rows][4C]; dgamma / dbeta [4C] += fixed-order sums (optional, two kernels);
+// scratch holds patch_merge_bwd_blocks(sms) * 8C fp32
+cudaError_t launch_patch_merge_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* x, const float* mean, const float* rstd,
+                                   const float* gamma, __nv_bfloat16* dx, float* dgamma, float* dbeta, float* scratch,
+                                   int N, int H, int W, int C, int sms, cudaStream_t stream);
+int patch_merge_bwd_blocks(int sms);
+
 // ---- pooling -------------------------------------------------------------------------------------
 struct PoolArgs {
   int N, H, W, C, P, Q, k, stride, pad;

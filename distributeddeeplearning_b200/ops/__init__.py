@@ -20,4 +20,5 @@ from .functional import (  # noqa: F401
     topk_correct,
     use_native,
 )
+from .swin import patch_merging, swin_block, window_attention  # noqa: F401
 from .vit import self_attention, vit_embed, vit_encoder_block  # noqa: F401

@@ -777,6 +777,116 @@ def tokens_bwd(dtok: torch.Tensor, N: int, L: int, grad_pos: Optional[torch.Tens
 
 
 # ------------------------------------------------------------------------------------------------
+# Swin: shifted-window attention (csrc/ops/window_attention.cu) and patch merging (csrc/ops/swin.cu)
+# ------------------------------------------------------------------------------------------------
+def supports_window_attention(H: int, W: int, window: int, heads: int, head_dim: int) -> bool:
+    """Shapes the window-attention kernels take: window 7, head dim 32, H and W multiples of 7 (no padding)."""
+    return (window == 7 and head_dim == 32 and 0 < heads <= 65535 and H > 0 and W > 0 and H % 7 == 0 and W % 7 == 0
+            and (H // 7) * (W // 7) <= 65535)
+
+
+def supports_patch_merge(H: int, W: int, C: int) -> bool:
+    """Maps the patch-merging kernels take: H and W even, C a multiple of 8 up to 512 (LayerNorm over 4C <= 2048)."""
+    return H > 0 and W > 0 and H % 2 == 0 and W % 2 == 0 and 8 <= C <= 512 and C % 8 == 0
+
+
+def window_shift(H: int, W: int, window: int, shift: int) -> Tuple[int, int]:
+    """torchvision's per-side shift: 0 on a side whose (padded) size is at most the window."""
+    ph, pw = -(-H // window) * window, -(-W // window) * window
+    return (0 if ph <= window else shift), (0 if pw <= window else shift)
+
+
+def _win_check(qkv: torch.Tensor, table: torch.Tensor, heads: int, N: int, H: int, W: int, shift: int):
+    C = qkv.shape[1] // 3 if qkv.dim() == 2 else 0
+    if C == 0 or C % heads != 0 or not supports_window_attention(H, W, 7, heads, C // heads):
+        raise ValueError(f"window_attention: H={H}, W={W}, {heads} heads of {C // max(heads, 1)} are not supported by the "
+                         "native kernels (window 7, head dim 32, H and W multiples of 7)")
+    if not 0 <= shift < 7:
+        raise ValueError("window_attention: shift must be in [0, 7)")
+    _check_rows(qkv, N * H * W, 3 * C, "qkv")
+    if table.dtype != torch.float32 or tuple(table.shape) != (169, heads) or not table.is_contiguous():
+        raise ValueError(f"window_attention: table must be the contiguous fp32 [169, {heads}] parameter")
+    return C
+
+
+def window_attention_fwd(qkv: torch.Tensor, table: torch.Tensor, heads: int, N: int, H: int, W: int, shift: int):
+    """Shifted-window attention (window 7, head dim 32) on the image-order qkv rows [N*H*W, 3C] with the relative-position
+    bias ``table`` [169, heads] fp32: returns (O [N*H*W, C] in image order, lse fp32 [N*H*W, heads])."""
+    C = _win_check(qkv, table, heads, N, H, W, shift)
+    sy, sx = window_shift(H, W, 7, shift)
+    o = torch.empty((N * H * W, C), dtype=torch.bfloat16, device=qkv.device)
+    lse = torch.empty((N * H * W, heads), dtype=torch.float32, device=qkv.device)
+    _C().window_attention_fwd(qkv.data_ptr(), table.data_ptr(), o.data_ptr(), lse.data_ptr(), N, H, W, heads, C, sy, sx,
+                              _stream())
+    return o, lse
+
+
+def window_attention_bwd(dout: torch.Tensor, qkv: torch.Tensor, table: torch.Tensor, o: torch.Tensor, lse: torch.Tensor,
+                         heads: int, N: int, H: int, W: int, shift: int,
+                         grad_table: Optional[torch.Tensor]) -> torch.Tensor:
+    """dqkv [N*H*W, 3C] (qkv's layout) of :func:`window_attention_fwd`; grad_table [169, heads] += the bias gradient
+    (optional).  Deterministic: no atomics."""
+    C = _win_check(qkv, table, heads, N, H, W, shift)
+    sy, sx = window_shift(H, W, 7, shift)
+    _check_rows(o, N * H * W, C, "o")
+    _check_rows(dout, N * H * W, C, "dout")
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (N * H * W, heads) or not lse.is_contiguous():
+        raise ValueError("window_attention_bwd: lse must be the contiguous fp32 [N*H*W, heads] of the forward")
+    if grad_table is not None and (grad_table.dtype != torch.float32 or tuple(grad_table.shape) != (169, heads)
+                                   or not grad_table.is_contiguous()):
+        raise ValueError("window_attention_bwd: grad_table must be a contiguous fp32 [169, heads] buffer")
+    dqkv = torch.empty_like(qkv)
+    scratch = torch.empty(_C().window_attention_bwd_scratch_floats(N, H, heads), dtype=torch.float32,
+                          device=qkv.device)
+    _C().window_attention_bwd(qkv.data_ptr(), table.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(),
+                              dqkv.data_ptr(), _ptr(grad_table), scratch.data_ptr(), N, H, W, heads, C, sy, sx,
+                              _stream())
+    return dqkv
+
+
+def _merge_check(x: torch.Tensor) -> Tuple[int, int, int, int]:
+    _check_act(x)
+    _check_aligned(x, "x")
+    N, C, H, W = x.shape
+    if not supports_patch_merge(H, W, C):
+        raise ValueError(f"patch_merge: an [N, {C}, {H}, {W}] map is not supported by the native kernels")
+    return N, C, H, W
+
+
+def patch_merge_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float):
+    """LayerNorm over 4C of the 2x2 gather (x[0::2, 0::2], x[1::2, 0::2], x[0::2, 1::2], x[1::2, 1::2]) of the NHWC
+    activation x [N, C, H, W]: returns (rows bf16 [N*H/2*W/2, 4C], mean fp32 [rows], rstd fp32 [rows])."""
+    N, C, H, W = _merge_check(x)
+    _check_f32_vec(gamma, 4 * C, "gamma")
+    _check_f32_vec(beta, 4 * C, "beta")
+    M = N * (H // 2) * (W // 2)
+    y = torch.empty((M, 4 * C), dtype=torch.bfloat16, device=x.device)
+    mean = torch.empty(M, dtype=torch.float32, device=x.device)
+    rstd = torch.empty(M, dtype=torch.float32, device=x.device)
+    _C().patch_merge_fwd(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
+                         N, H, W, C, float(eps), sm_count(x.device.index or 0), _stream())
+    return y, mean, rstd
+
+
+def patch_merge_bwd(dy: torch.Tensor, x: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor, gamma: torch.Tensor,
+                    grad_gamma: Optional[torch.Tensor], grad_beta: Optional[torch.Tensor]) -> torch.Tensor:
+    """dx (like x) of :func:`patch_merge_fwd` from dy [rows, 4C]; grad_gamma / grad_beta [4C] += fixed-order sums."""
+    N, C, H, W = _merge_check(x)
+    M = N * (H // 2) * (W // 2)
+    _check_rows(dy, M, 4 * C, "dy")
+    _check_f32_vec(mean, M, "mean")
+    _check_f32_vec(rstd, M, "rstd")
+    for t, name in ((gamma, "gamma"), (grad_gamma, "grad_gamma"), (grad_beta, "grad_beta")):
+        _check_f32_vec(t, 4 * C, name)
+    sms = sm_count(x.device.index or 0)
+    dx = torch.empty_like(x)
+    scratch = torch.empty(_C().patch_merge_bwd_blocks(sms) * 8 * C, dtype=torch.float32, device=x.device)
+    _C().patch_merge_bwd(dy.data_ptr(), x.data_ptr(), mean.data_ptr(), rstd.data_ptr(), gamma.data_ptr(), dx.data_ptr(),
+                         _ptr(grad_gamma), _ptr(grad_beta), scratch.data_ptr(), N, H, W, C, sms, _stream())
+    return dx
+
+
+# ------------------------------------------------------------------------------------------------
 # squeeze-excitation (csrc/ops/squeeze_excite.cu) and hardswish on [B, F]
 # ------------------------------------------------------------------------------------------------
 def _check_gate(s: torch.Tensor, n: int, c: int) -> None:

@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "swin", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -3184,6 +3184,274 @@ def g_vit():
     ok = all(l == l and abs(l) < 1e4 for l in losses) and n8.get("fwd", 0) > 0
     RESULTS.append(ok)
     print(f"[{'ok' if ok else 'FAIL'}] vit_b_16 fp8 session: losses {[round(v, 3) for v in losses]}, fp8 launches {n8}",
+          flush=True)
+    del s
+    torch.cuda.empty_cache()
+    for kind, r in sorted(WORST.items()):
+        print(f"worst ratio to budget: {kind:24s} {r:.3f}x", flush=True)
+
+
+# ------------------------------------------------------------------------------------------------
+# Swin Transformer: shifted-window attention, patch merging
+# ------------------------------------------------------------------------------------------------
+# Budgets of the `swin` group as (rtol, atol, arms) of report_abs.  The window-attention kernels are the ViT kernels'
+# arithmetic at head dim 32 (bf16 operands, fp32 accumulation, P and dS rounded to bf16 as A operands, D from the
+# stored bf16 O), so lse and dV take VIT_BUDGET's attention entries.  O, dQ and dK take twice its rms term: a window row
+# has at most 49 keys, and the -100 mask and the bias leave fewer effective keys per row than ViT's L >= 50, so the bf16
+# rounding of P and dS is a larger share of rms(ref); at VIT_BUDGET's rms term 1 to 2 elements in 10^6 went up to 1.04x.
+# - win dtable: fp32 sums of fp32 dS over every (image, window, pair) of one relative index; dS carries the error of
+#   dQ / dK before their bf16 rounding: 2^-6 of |ref| plus 2^-5 of rms(ref).
+# - merge out / dx / dgamma / dbeta: the LayerNorm budgets of VIT_BUDGET (one bf16 rounding of an fp32 row computation;
+#   fp32 sums over the rows).
+SWIN_BUDGET = {"win o": (2.0 ** -7, 0.0, 2.0 ** -6), "win lse": VIT_BUDGET["attn lse"], "win dq": (2.0 ** -6, 0.0, 2.0 ** -4),
+               "win dk": (2.0 ** -6, 0.0, 2.0 ** -4), "win dv": VIT_BUDGET["attn dv"],
+               "win dtable": (2.0 ** -6, 0.0, 2.0 ** -5),
+               "merge out": VIT_BUDGET["ln out"], "merge dx": VIT_BUDGET["ln dx"],
+               "merge dgamma": VIT_BUDGET["ln dgamma"], "merge dbeta": VIT_BUDGET["ln dbeta"]}
+
+
+def _swin_check(name, kind, got, ref, atol=None):
+    rtol, atol0, arms = SWIN_BUDGET[kind]
+    report_abs(f"{name} {kind}", got, ref, rtol, atol0 if atol is None else atol, arms, kind=kind)
+
+
+def _win_lse_ref(qkv, table, heads, N, H, W, shift):
+    """float64 log-sum-exp [N*H*W, heads] of torchvision's logits (scaled scores + bias + the -100 mask of its slices)."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import native
+    from distributeddeeplearning_b200.ops.swin import relative_position_index
+
+    C = qkv.shape[1] // 3
+    sy, sx = native.window_shift(H, W, 7, shift)
+    idx = torch.arange(N * H * W, device=qkv.device).view(N, H, W)
+    reg = torch.zeros(H, W, device=qkv.device)
+    if sy + sx > 0:
+        idx = torch.roll(idx, (-sy, -sx), (1, 2))
+        count = 0
+        for h in ((0, -7), (-7, -sy), (-sy, None)):
+            for w in ((0, -7), (-7, -sx), (-sx, None)):
+                reg[h[0]:h[1], w[0]:w[1]] = count
+                count += 1
+    nW = (H // 7) * (W // 7)
+    idx = idx.view(N, H // 7, 7, W // 7, 7).permute(0, 1, 3, 2, 4).reshape(N * nW, 49)
+    reg = reg.view(H // 7, 7, W // 7, 7).permute(0, 2, 1, 3).reshape(nW, 49)
+    mask = ((reg[:, None, :] - reg[:, :, None]) != 0).double() * -100.0
+    t = qkv.double()[idx].view(N * nW, 49, 3, heads, C // heads).permute(2, 0, 3, 1, 4)
+    s = (t[0] * (C // heads) ** -0.5) @ t[1].transpose(-2, -1)
+    s = s + table.double()[relative_position_index(7).to(qkv.device)].view(49, 49, heads).permute(2, 0, 1)
+    s = (s.view(N, nW, heads, 49, 49) + mask[None, :, None]).view(N * nW, heads, 49, 49)
+    lse = torch.empty(N * H * W, heads, dtype=torch.float64, device=qkv.device)
+    lse[idx.reshape(-1)] = torch.logsumexp(s, -1).permute(0, 2, 1).reshape(-1, heads)
+    return lse
+
+
+def _win_case(N, H, W, heads, shift, special=None, determinism=False):
+    import torch
+
+    from distributeddeeplearning_b200 import ops
+    from distributeddeeplearning_b200.ops import native
+
+    C = 32 * heads
+    qkv = torch.randn(N * H * W, 3 * C, device="cuda")
+    if special == "dominant":          # token 0 of every head aligned with the token 3 rows below, scaled
+        for h in range(heads):
+            qkv[0, 32 * h:32 * h + 32] = 4.0 * qkv[3 * W, C + 32 * h:C + 32 * h + 32]
+    elif special == "constant":        # every key of image 0 equal (and a zero table): constant score rows
+        qkv[:H * W, C:2 * C] = qkv[:1, C:2 * C]
+    qkv = qkv.to(torch.bfloat16)
+    table = torch.randn(169, heads, device="cuda") * (0.0 if special == "constant" else 0.5)
+    dout = torch.randn(N * H * W, C, device="cuda").to(torch.bfloat16)
+    o, lse = native.window_attention_fwd(qkv, table, heads, N, H, W, shift)
+    dt = torch.zeros(169, heads, device="cuda")
+    dqkv = native.window_attention_bwd(dout, qkv, table, o, lse, heads, N, H, W, shift, dt)
+    tag = f"window attention N={N} {H}x{W} heads={heads} shift={shift}" + (f" {special}" if special else "")
+    if determinism:
+        dt2 = torch.zeros(169, heads, device="cuda")
+        dqkv2 = native.window_attention_bwd(dout, qkv, table, o, lse, heads, N, H, W, shift, dt2)
+        ok = torch.equal(dqkv, dqkv2) and torch.equal(dt, dt2)
+        RESULTS.append(ok)
+        print(f"[{'ok' if ok else 'FAIL'}] {tag} dqkv and dtable bitwise equal across two backward calls", flush=True)
+    qd, td = qkv.double().requires_grad_(True), table.double().requires_grad_(True)
+    ref = ops.window_attention(qd, td, heads, H, W, 7, shift)        # the float64 composite: torchvision's maths
+    ref.backward(dout.double())
+    _swin_check(tag, "win o", o, ref.detach())
+    _swin_check(tag, "win lse", lse, _win_lse_ref(qkv, table, heads, N, H, W, shift))
+    g = qd.grad
+    floor = 2.0 ** -8 * float(g[:, 2 * C:].pow(2).mean().sqrt())
+    for i, kind in enumerate(("win dq", "win dk", "win dv")):
+        _swin_check(tag, kind, dqkv[:, i * C:(i + 1) * C], g[:, i * C:(i + 1) * C], atol=floor if i < 2 else None)
+    _swin_check(tag, "win dtable", dt, td.grad)
+
+
+def _merge_case(N, H, C, offset):
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native
+
+    x = (torch.randn(N, C, H, H, device="cuda") + offset).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    gamma = torch.randn(4 * C, device="cuda") * 0.5 + 1.0
+    beta = torch.randn(4 * C, device="cuda") * 0.1
+    y, mean, rstd = native.patch_merge_fwd(x, gamma, beta, 1e-5)
+    xd = x.double().requires_grad_(True)
+    gd, bd = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
+    t = xd.permute(0, 2, 3, 1)
+    t = torch.cat([t[:, 0::2, 0::2], t[:, 1::2, 0::2], t[:, 0::2, 1::2], t[:, 1::2, 1::2]], -1).reshape(-1, 4 * C)
+    ref = F.layer_norm(t, (4 * C,), gd, bd, 1e-5)
+    tag = f"patch merge + LN N={N} {H}x{H} 4C={4 * C} offset={offset:g}"
+    _swin_check(tag, "merge out", y, ref.detach())
+    dy = torch.randn_like(y)
+    ref.backward(dy.double())
+    dg, db = torch.ones(4 * C, device="cuda"), torch.ones(4 * C, device="cuda")
+    dx = native.patch_merge_bwd(dy, x, mean, rstd, gamma, dg, db)
+    _swin_check(tag, "merge dx", dx, xd.grad)
+    _swin_check(tag, "merge dgamma", dg, gd.grad + 1)
+    _swin_check(tag, "merge dbeta", db, bd.grad + 1)
+    dg2, db2 = torch.ones(4 * C, device="cuda"), torch.ones(4 * C, device="cuda")
+    dx2 = native.patch_merge_bwd(dy, x, mean, rstd, gamma, dg2, db2)
+    ok = torch.equal(dx, dx2) and torch.equal(dg, dg2) and torch.equal(db, db2)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {tag} backward bitwise equal across two calls", flush=True)
+
+
+def _swin_vs_torchvision(name, bs):
+    """A Swin against torchvision fp32 with the same weights (stochastic depth 0, so that both draw nothing) and this
+    repo's bf16 composite; forward hooks check that every block and patch merge ran on the native node."""
+    import torch
+    from torchvision.models.swin_transformer import SwinTransformer as TvSwin
+
+    from distributeddeeplearning_b200 import models, ops
+    from distributeddeeplearning_b200.models.swin import _VARIANTS, PatchMerging, SwinTransformerBlock
+
+    dim, depths, heads, _ = _VARIANTS[name]
+    torch.manual_seed(0)
+    m = models.get_model(name, stochastic_depth_prob=0.0).cuda().train()
+    tv = TvSwin([4, 4], dim, list(depths), list(heads), [7, 7], stochastic_depth_prob=0.0).cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name, stochastic_depth_prob=0.0).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    nodes = []
+    hooks = [mod.register_forward_hook(lambda mod, i, o: nodes.append(type(o.grad_fn).__name__))
+             for mod in m.modules() if isinstance(mod, (SwinTransformerBlock, PatchMerging))]
+    x = torch.randn(bs, 3, 224, 224, device="cuda").to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    try:
+        out = m(x)
+        for h in hooks:
+            h.remove()
+        ops.softmax_cross_entropy(out, y, 1000).backward()
+        ro = tv(x)
+        torch.nn.functional.cross_entropy(ro, y).backward()
+        os.environ["DDL_B200_IMPL"] = "torch"
+        co = m2(x)
+        ops.softmax_cross_entropy(co, y, 1000).backward()
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+    want = sum(depths) + len(depths) - 1
+    ok = len(nodes) == want and set(nodes) == {"_SwinBlockBackward", "_PatchMergingBackward"}
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: {len(nodes)} of {want} blocks / merges ran on {sorted(set(nodes))}",
+          flush=True)
+    c1, c2 = _cos(out, ro), _cos(co, ro)
+    RESULTS.append(c1 > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} logits cos vs fp32 {c1:.5f}   (bf16 composite {c2:.5f})")
+    gn, gc, tvp = dict(m.named_parameters()), dict(m2.named_parameters()), dict(tv.named_parameters())
+    worst, lag = (1.0, "", 1.0), (-1.0, "")
+    for k, p in tvp.items():
+        if float(p.grad.norm()) == 0.0:
+            continue
+        a1, a2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if a1 < worst[0]:
+            worst = (a1, k, a2)
+        if a2 - a1 > lag[0]:
+            lag = (a2 - a1, k)
+    ok = lag[0] <= 0.01 and worst[0] > 0.6
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at {worst[1]} "
+          f"(bf16 composite {worst[2]:.4f}); largest deficit vs the bf16 composite = {lag[0]:.4f} at {lag[1]}", flush=True)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        oe, re_ = m(x), tv(x)
+    ce = _cos(oe, re_)
+    RESULTS.append(ce > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} eval-mode logits cos vs torchvision eval {ce:.5f}", flush=True)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def g_swin():
+    """Swin: window attention forward / backward at every stage shape of swin_t and swin_b with shift 0 and 3 (stage 4's
+    shift forced to 0), a non-square map, a map shifted on one axis only, a dominant logit and constant score rows, and
+    bitwise-repeatable backward; patch merge + LayerNorm at all six widths; swin_t against torchvision, eager vs
+    CUDA-graph training and an fp8 session."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.manual_seed(0)
+    for heads0 in (3, 4):                       # swin_t / _s and swin_b
+        for stage, (N, H) in enumerate(((2, 56), (4, 28), (8, 14), (16, 7))):
+            for shift in (0, 3):
+                _win_case(N, H, H, heads0 * 2 ** stage, shift, determinism=stage == 0 and shift == 3)
+    _win_case(3, 14, 28, 6, 3)                  # non-square: swapped axes would show
+    _win_case(3, 28, 14, 6, 3)
+    _win_case(4, 7, 14, 12, 3)                  # shifted on x only (H = 7 forces sy = 0)
+    _win_case(2, 14, 14, 6, 0, "dominant")
+    _win_case(2, 14, 14, 6, 0, "constant")
+    for C, H in ((96, 56), (192, 28), (384, 14), (128, 56), (256, 28), (512, 14)):
+        _merge_case(4, H, C, 0.0)
+    _merge_case(3, 14, 96, 50.0)
+    _swin_vs_torchvision("swin_t", 16)
+    dist.init()
+
+    def run(graph, random_drops):
+        torch.manual_seed(0)
+        s = BenchmarkSession("swin_t", 16, True, lr=0.01, momentum=0.9)
+        if not random_drops:        # the eager and the replayed step draw their vectors from different counters
+            for mod in s.model.modules():
+                if hasattr(mod, "sd_prob"):
+                    mod.sd_prob = 0.0
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out
+
+    a, b = run(False, False), run(True, False)
+    rel = max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(a[-4:], b[-4:]))
+    ok = all(x == x for x in a + b) and rel < 5e-2 and a[-1] < a[0]
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] swin_t training without random drops: eager {[round(v, 4) for v in a]} graph "
+          f"replay {[round(v, 4) for v in b]} (largest relative difference of the last 4 {rel:.2e})", flush=True)
+    c = run(True, True)
+    ok = all(x == x and abs(x) < 1e4 for x in c)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] swin_t graph-replayed training with stochastic depth: {[round(v, 4) for v in c]}",
+          flush=True)
+    fp8.reset()
+    fp8.enable(True)
+    try:
+        torch.manual_seed(0)
+        s = BenchmarkSession("swin_t", 16, True, lr=0.01, momentum=0.9)
+        losses = [float(s.step()) for _ in range(4)]
+        torch.cuda.synchronize()
+        s.optimizer.check_errors()
+    finally:
+        fp8.enable(False)
+    n8 = fp8.launches()
+    ok = all(l == l and abs(l) < 1e4 for l in losses) and n8.get("fwd", 0) > 0
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] swin_t fp8 session: losses {[round(v, 3) for v in losses]}, fp8 launches {n8}",
           flush=True)
     del s
     torch.cuda.empty_cache()
