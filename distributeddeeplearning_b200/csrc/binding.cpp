@@ -529,6 +529,43 @@ PYBIND11_MODULE(_C, m) {
           "patch_merge_bwd");
   });
   m.def("patch_merge_bwd_blocks", [](int sms) { return ddl::patch_merge_bwd_blocks(sms); });
+  // ------------------------------------------------------------------ Swin V2: cosine window attention, CPB, merge gather
+  m.def("window_attention_v2_fwd", [](ptr_t qkv, ptr_t table, ptr_t scale, ptr_t qb, ptr_t vb, ptr_t o, ptr_t lse, int N,
+                                      int H, int W, int heads, int C, int sy, int sx, ptr_t stream) {
+    check(ddl::launch_window_attention_v2_fwd(P<const __nv_bfloat16>(qkv), P<const float>(table), P<const float>(scale),
+                                              P<const float>(qb), P<const float>(vb), P<__nv_bfloat16>(o), P<float>(lse),
+                                              N, H, W, heads, C, sy, sx, S(stream)), "window_attention_v2_fwd");
+  });
+  m.def("window_attention_v2_bwd", [](ptr_t qkv, ptr_t table, ptr_t scale, ptr_t qb, ptr_t vb, ptr_t o, ptr_t dout,
+                                      ptr_t lse, ptr_t dqkv, ptr_t dtable, ptr_t dscale, ptr_t dbias, ptr_t scratch, int N,
+                                      int H, int W, int heads, int C, int sy, int sx, bool bias_pad_only,
+                                      ptr_t stream) {
+    check(ddl::launch_window_attention_v2_bwd(P<const __nv_bfloat16>(qkv), P<const float>(table), P<const float>(scale),
+                                              P<const float>(qb), P<const float>(vb), P<const __nv_bfloat16>(o),
+                                              P<const __nv_bfloat16>(dout), P<const float>(lse), P<__nv_bfloat16>(dqkv),
+                                              P<float>(dtable), P<float>(dscale), P<float>(dbias), P<float>(scratch), N, H,
+                                              W, heads, C, sy, sx, bias_pad_only, S(stream)),
+          "window_attention_v2_bwd");
+  });
+  m.def("window_attention_v2_bwd_scratch_floats", [](int N, int H, int heads) {
+    return ddl::window_attention_v2_bwd_scratch_floats(N, H, heads);
+  });
+  m.def("cpb_fwd", [](ptr_t coords, ptr_t w1, ptr_t b1, ptr_t w2, ptr_t table, ptr_t qkv_b, ptr_t qkv_b_eff, int heads,
+                      int C, ptr_t stream) {
+    check(ddl::launch_cpb_fwd(P<const float>(coords), P<const float>(w1), P<const float>(b1), P<const float>(w2),
+                              P<float>(table), P<const float>(qkv_b), P<float>(qkv_b_eff), heads, C, S(stream)), "cpb_fwd");
+  });
+  m.def("cpb_bwd", [](ptr_t coords, ptr_t w1, ptr_t b1, ptr_t w2, ptr_t table, ptr_t dtable, ptr_t dw1, ptr_t db1,
+                      ptr_t dw2, ptr_t scratch, int heads, ptr_t stream) {
+    check(ddl::launch_cpb_bwd(P<const float>(coords), P<const float>(w1), P<const float>(b1), P<const float>(w2),
+                              P<const float>(table), P<const float>(dtable), P<float>(dw1), P<float>(db1), P<float>(dw2),
+                              P<float>(scratch), heads, S(stream)), "cpb_bwd");
+  });
+  m.def("cpb_bwd_scratch_floats", [](int heads) { return ddl::cpb_bwd_scratch_floats(heads); });
+  m.def("merge_gather", [](ptr_t src, ptr_t dst, int N, int H, int W, int C, bool forward, int sms, ptr_t stream) {
+    check(ddl::launch_merge_gather(P<const __nv_bfloat16>(src), P<__nv_bfloat16>(dst), N, H, W, C, forward, sms,
+                                   S(stream)), "merge_gather");
+  });
   // ------------------------------------------------------------------ squeeze-excitation
   m.def("se_scale", [](ptr_t x, ptr_t s, int lds, ptr_t y, int N, int HW, int C, int sms, ptr_t stream) {
     check(ddl::launch_se_scale(P<const __nv_bfloat16>(x), P<const __nv_bfloat16>(s), lds, P<__nv_bfloat16>(y), N, HW, C,

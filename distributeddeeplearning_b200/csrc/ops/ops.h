@@ -179,6 +179,42 @@ cudaError_t launch_window_attention_bwd(const __nv_bfloat16* qkv, const float* t
                                         cudaStream_t stream);
 size_t window_attention_bwd_scratch_floats(int N, int H, int heads);
 
+// ---- Swin V2: scaled-cosine shifted-window attention, window 8, head dim 32 (window_attention_v2.cu) -------------------
+// qkv [N*H*W][3C] bf16 in image order (head h: Q, K, V at columns 32h, C + 32h, 2C + 32h), C = 32 heads, any H, W (the
+// windows tile the padded frame ceil(H/8) 8 x ceil(W/8) 8; a padding token has q = qb, k = 0, v = vb: fp32 [C] or null),
+// shift (sy, sx) in [0, 8) (0 on a side whose padded size is 8).  forward: o [N*H*W][C] and lse [N*H*W][heads] fp32 with
+// logits cos(q, k) exp(min(scale[h], ln 100)) + table[225][heads] + the shifted-window mask.
+cudaError_t launch_window_attention_v2_fwd(const __nv_bfloat16* qkv, const float* table, const float* scale,
+                                           const float* qb, const float* vb, __nv_bfloat16* o, float* lse, int N, int H,
+                                           int W, int heads, int C, int sy, int sx, cudaStream_t stream);
+// backward (three kernels, deterministic): dqkv [N*H*W][3C] in qkv's layout; dtable [225][heads] = the table gradient,
+// dscale [heads] += the logit-scale gradient, dbias [3C] q / v slices += the bias gradients (over every token, padding
+// included, or with bias_pad_only over the padding tokens only; the k slice is not touched), each optional; scratch
+// holds window_attention_v2_bwd_scratch_floats(N, H, heads) fp32
+cudaError_t launch_window_attention_v2_bwd(const __nv_bfloat16* qkv, const float* table, const float* scale,
+                                           const float* qb, const float* vb, const __nv_bfloat16* o,
+                                           const __nv_bfloat16* dout, const float* lse, __nv_bfloat16* dqkv,
+                                           float* dtable, float* dscale, float* dbias, float* scratch, int N, int H,
+                                           int W, int heads, int C, int sy, int sx, bool bias_pad_only,
+                                           cudaStream_t stream);
+size_t window_attention_v2_bwd_scratch_floats(int N, int H, int heads);
+
+// ---- Swin V2: continuous position bias and the patch-merging gather (swin_v2.cu) --------------------------------------
+// table [225][heads] = 16 sigmoid(W2 relu(W1 coords[k] + b1)) (coords [225][2], W1 [512][2], b1 [512], W2 [heads][512],
+// heads <= 32); with qkv_b_eff, also qkv_b_eff [3C] = qkv_b with its k slice zeroed.  One launch.
+cudaError_t launch_cpb_fwd(const float* coords, const float* w1, const float* b1, const float* w2, float* table,
+                           const float* qkv_b, float* qkv_b_eff, int heads, int C, cudaStream_t stream);
+// dw1 [512][2], db1 [512], dw2 [heads][512] += the gradients from dtable [225][heads] and the forward's table (each
+// optional; two launches, fixed order); scratch holds cpb_bwd_scratch_floats(heads) fp32
+cudaError_t launch_cpb_bwd(const float* coords, const float* w1, const float* b1, const float* w2, const float* table,
+                           const float* dtable, float* dw1, float* db1, float* dw2, float* scratch, int heads,
+                           cudaStream_t stream);
+size_t cpb_bwd_scratch_floats(int heads);
+// forward: dst [N * H/2 * W/2][4C] = the 2x2 gather (x0, x1, x2, x3) of src [N][H][W][C]; backward: src [rows][4C] -> dst
+// [N][H][W][C] (H, W even, C % 8 == 0)
+cudaError_t launch_merge_gather(const __nv_bfloat16* src, __nv_bfloat16* dst, int N, int H, int W, int C, bool forward,
+                                int sms, cudaStream_t stream);
+
 // ---- Swin: patch merging (swin.cu) -------------------------------------------------------------------------------------
 // y [N * H/2 * W/2][4C] = LayerNorm over 4C of the 2x2 gather (x0, x1, x2, x3) of the NHWC x [N][H][W][C] (H, W even,
 // C % 8 == 0, C <= 512), saving fp32 mean / rstd [rows]

@@ -6,8 +6,8 @@ Parity: the reference resolves ``--model`` with ``getattr(torchvision.models, na
 AlexNet (SURVEY.md 2.7); ResNet-18/34, the other VGG depths, DenseNet and SqueezeNet (the rest of torchvision
 0.2.1's families) are here too, and the later ResNet family members of torchvision (ResNeXt-50 32x4d, ResNeXt-101
 32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2, MobileNetV3-Large / -Small, EfficientNet-B0 to -B7,
-ConvNeXt-Tiny / -Small / -Base / -Large, the Vision Transformers ViT-B/16, -B/32, -L/16 and -L/32 and the Swin
-Transformers Swin-T, -S and -B.
+ConvNeXt-Tiny / -Small / -Base / -Large, the Vision Transformers ViT-B/16, -B/32, -L/16 and -L/32, the Swin
+Transformers Swin-T, -S and -B and the Swin Transformers V2 Swin-V2-T, -S and -B.
 """
 from __future__ import annotations
 
@@ -24,6 +24,7 @@ from .resnet import (ResNet, resnet18, resnet34, resnet50, resnet101, resnet152,
                      resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2)
 from .squeezenet import SqueezeNet, squeezenet1_0, squeezenet1_1  # noqa: F401
 from .swin import SwinTransformer, swin_b, swin_s, swin_t  # noqa: F401
+from .swin_v2 import INPUT_SIZE as _SWIN_V2_INPUT_SIZE, SwinTransformerV2, swin_v2_b, swin_v2_s, swin_v2_t  # noqa: F401
 from .vgg import VGG, vgg11, vgg11_bn, vgg13, vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn  # noqa: F401
 from .vit import VisionTransformer, vit_b_16, vit_b_32, vit_l_16, vit_l_32  # noqa: F401
 
@@ -35,7 +36,8 @@ _REGISTRY = {
               squeezenet1_0, squeezenet1_1, inception_v3, mobilenet_v2,
               mobilenet_v3_large, mobilenet_v3_small, resnet18, resnet34, resnet50, resnet101, resnet152,
               resnext50_32x4d, resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2, vgg11, vgg11_bn, vgg13,
-              vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn, vit_b_16, vit_b_32, vit_l_16, vit_l_32, swin_t, swin_s, swin_b)
+              vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn, vit_b_16, vit_b_32, vit_l_16, vit_l_32, swin_t, swin_s, swin_b,
+              swin_v2_t, swin_v2_s, swin_v2_b)
 }
 
 
@@ -55,9 +57,12 @@ def get_model(name: str, **kw):
 
 def input_size(model_or_name) -> int:
     """Spatial input size (299 for Inception-v3 — the reference hard-codes 224 and breaks, SURVEY.md Q2; torchvision's
-    crop size for EfficientNet-B0 to -B7, 224 to 600; a Vision Transformer's ``image_size``)."""
+    crop size for EfficientNet-B0 to -B7, 224 to 600, and for Swin-V2-T / -S / -B, 256; a Vision Transformer's
+    ``image_size``)."""
     if isinstance(model_or_name, str):
         if model_or_name in _EFFICIENTNET_INPUT_SIZE:
             return _EFFICIENTNET_INPUT_SIZE[model_or_name]
+        if model_or_name.startswith("swin_v2_"):
+            return _SWIN_V2_INPUT_SIZE
         return 299 if model_or_name.startswith("inception") else 224
     return int(getattr(model_or_name, "input_size", 224))

@@ -887,6 +887,141 @@ def patch_merge_bwd(dy: torch.Tensor, x: torch.Tensor, mean: torch.Tensor, rstd:
 
 
 # ------------------------------------------------------------------------------------------------
+# Swin V2: scaled-cosine window attention (csrc/ops/window_attention_v2.cu), continuous position bias and the
+# patch-merging gather (csrc/ops/swin_v2.cu)
+# ------------------------------------------------------------------------------------------------
+def supports_window_attention_v2(H: int, W: int, window: int, heads: int, head_dim: int) -> bool:
+    """Shapes the cosine window-attention kernels take: window 8, head dim 32, 1 to 32 heads (the CPB kernels' limit),
+    any H and W (padded maps included)."""
+    return window == 8 and head_dim == 32 and 0 < heads <= 32 and H > 0 and W > 0
+
+
+def _win2_check(qkv, table, scale, qb, vb, heads, N, H, W, shift):
+    C = qkv.shape[1] // 3 if qkv.dim() == 2 else 0
+    if C == 0 or C % heads != 0 or not supports_window_attention_v2(H, W, 8, heads, C // heads):
+        raise ValueError(f"window_attention_v2: H={H}, W={W}, {heads} heads of {C // max(heads, 1)} are not supported by "
+                         "the native kernels (window 8, head dim 32, at most 32 heads)")
+    if not 0 <= shift < 8:
+        raise ValueError("window_attention_v2: shift must be in [0, 8)")
+    _check_rows(qkv, N * H * W, 3 * C, "qkv")
+    if table.dtype != torch.float32 or tuple(table.shape) != (225, heads) or not table.is_contiguous():
+        raise ValueError(f"window_attention_v2: table must be a contiguous fp32 [225, {heads}] tensor")
+    _check_f32_vec(scale, heads, "logit_scale")
+    _check_f32_vec(qb, C, "q_bias")
+    _check_f32_vec(vb, C, "v_bias")
+    return C
+
+
+def window_attention_v2_fwd(qkv: torch.Tensor, table: torch.Tensor, scale: torch.Tensor, qb: Optional[torch.Tensor],
+                            vb: Optional[torch.Tensor], heads: int, N: int, H: int, W: int, shift: int):
+    """Scaled-cosine shifted-window attention (window 8, head dim 32) on the image-order qkv rows [N*H*W, 3C] with the
+    position-bias ``table`` [225, heads] and ``logit_scale`` [heads] fp32; padding tokens of a map whose sides are not
+    multiples of 8 have q = ``qb``, k = 0, v = ``vb`` (fp32 [C] or None).  Returns (O [N*H*W, C] in image order, lse
+    fp32 [N*H*W, heads])."""
+    C = _win2_check(qkv, table, scale, qb, vb, heads, N, H, W, shift)
+    sy, sx = window_shift(H, W, 8, shift)
+    o = torch.empty((N * H * W, C), dtype=torch.bfloat16, device=qkv.device)
+    lse = torch.empty((N * H * W, heads), dtype=torch.float32, device=qkv.device)
+    _C().window_attention_v2_fwd(qkv.data_ptr(), table.data_ptr(), scale.data_ptr(), _ptr(qb), _ptr(vb), o.data_ptr(),
+                                 lse.data_ptr(), N, H, W, heads, C, sy, sx, _stream())
+    return o, lse
+
+
+def window_attention_v2_bwd(dout: torch.Tensor, qkv: torch.Tensor, table: torch.Tensor, scale: torch.Tensor,
+                            qb: Optional[torch.Tensor], vb: Optional[torch.Tensor], o: torch.Tensor, lse: torch.Tensor,
+                            heads: int, N: int, H: int, W: int, shift: int, grad_table: Optional[torch.Tensor],
+                            grad_scale: Optional[torch.Tensor], grad_bias: Optional[torch.Tensor],
+                            bias_pad_only: bool = False) -> torch.Tensor:
+    """dqkv [N*H*W, 3C] (qkv's layout) of :func:`window_attention_v2_fwd`.  Optional: grad_table [225, heads] = the
+    table gradient (overwritten), grad_scale [heads] += the logit-scale gradient (0 where the clamp at ln 100 is active),
+    grad_bias [3C] q and v slices += the bias gradients (the k slice is left as it is).  The bias sums cover every token,
+    padding included: the gradient of b_q / b_v when qkv carries [b_q, 0, b_v] on every row.  ``bias_pad_only``: they
+    cover the padding tokens only, the gradient of ``qb`` / ``vb`` as the padding fill of given qkv rows.
+    Deterministic: no atomics."""
+    C = _win2_check(qkv, table, scale, qb, vb, heads, N, H, W, shift)
+    sy, sx = window_shift(H, W, 8, shift)
+    _check_rows(o, N * H * W, C, "o")
+    _check_rows(dout, N * H * W, C, "dout")
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (N * H * W, heads) or not lse.is_contiguous():
+        raise ValueError("window_attention_v2_bwd: lse must be the contiguous fp32 [N*H*W, heads] of the forward")
+    if grad_table is not None and (grad_table.dtype != torch.float32 or tuple(grad_table.shape) != (225, heads)
+                                   or not grad_table.is_contiguous()):
+        raise ValueError("window_attention_v2_bwd: grad_table must be a contiguous fp32 [225, heads] buffer")
+    _check_f32_vec(grad_scale, heads, "grad_scale")
+    _check_f32_vec(grad_bias, 3 * C, "grad_bias")
+    dqkv = torch.empty_like(qkv)
+    scratch = torch.empty(_C().window_attention_v2_bwd_scratch_floats(N, H, heads), dtype=torch.float32,
+                          device=qkv.device)
+    _C().window_attention_v2_bwd(qkv.data_ptr(), table.data_ptr(), scale.data_ptr(), _ptr(qb), _ptr(vb), o.data_ptr(),
+                                 dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(), _ptr(grad_table), _ptr(grad_scale),
+                                 _ptr(grad_bias), scratch.data_ptr(), N, H, W, heads, C, sy, sx, bool(bias_pad_only),
+                                 _stream())
+    return dqkv
+
+
+def _cpb_check(coords, w1, b1, w2, heads):
+    if not 0 < heads <= 32:
+        raise ValueError("cpb: 1 to 32 heads")
+    _check_f32_vec(coords, 450, "relative_coords_table")
+    _check_f32_vec(w1, 1024, "cpb_mlp.0.weight")
+    _check_f32_vec(b1, 512, "cpb_mlp.0.bias")
+    _check_f32_vec(w2, 512 * heads, "cpb_mlp.2.weight")
+
+
+def cpb_fwd(coords: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, heads: int,
+            qkv_b: Optional[torch.Tensor] = None):
+    """The continuous position-bias table [225, heads] fp32 = 16 sigmoid(cpb_mlp(relative_coords_table)); with
+    ``qkv_b`` [3C], also returns it with the k slice zeroed (the bias the qkv linear runs with), else None."""
+    _cpb_check(coords, w1, b1, w2, heads)
+    table = torch.empty((225, heads), dtype=torch.float32, device=coords.device)
+    eff = None
+    if qkv_b is not None:
+        _check_f32_vec(qkv_b, qkv_b.numel(), "qkv_b")
+        eff = torch.empty_like(qkv_b)
+    _C().cpb_fwd(coords.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), table.data_ptr(), _ptr(qkv_b),
+                 _ptr(eff), heads, 0 if qkv_b is None else qkv_b.numel() // 3, _stream())
+    return table, eff
+
+
+def cpb_bwd(coords: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, table: torch.Tensor,
+            grad_table: torch.Tensor, heads: int, grad_w1: Optional[torch.Tensor], grad_b1: Optional[torch.Tensor],
+            grad_w2: Optional[torch.Tensor]) -> None:
+    """grad_w1 [512, 2], grad_b1 [512], grad_w2 [heads, 512] += the CPB MLP's gradients from grad_table [225, heads] and
+    the forward's ``table`` (each optional; fixed order, two kernels)."""
+    _cpb_check(coords, w1, b1, w2, heads)
+    _check_f32_vec(table, 225 * heads, "table")
+    _check_f32_vec(grad_table, 225 * heads, "grad_table")
+    for t, n, name in ((grad_w1, 1024, "grad_w1"), (grad_b1, 512, "grad_b1"), (grad_w2, 512 * heads, "grad_w2")):
+        _check_f32_vec(t, n, name)
+    scratch = torch.empty(_C().cpb_bwd_scratch_floats(heads), dtype=torch.float32, device=coords.device)
+    _C().cpb_bwd(coords.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), table.data_ptr(), grad_table.data_ptr(),
+                 _ptr(grad_w1), _ptr(grad_b1), _ptr(grad_w2), scratch.data_ptr(), heads, _stream())
+
+
+def merge_gather(x: torch.Tensor) -> torch.Tensor:
+    """The 2x2 gather (x[0::2, 0::2], x[1::2, 0::2], x[0::2, 1::2], x[1::2, 1::2]) of the NHWC activation x [N, C, H, W]
+    (H, W even, C % 8 == 0) as rows bf16 [N*H/2*W/2, 4C]."""
+    _check_act(x)
+    _check_aligned(x, "x")
+    N, C, H, W = x.shape
+    if H % 2 or W % 2 or C % 8:
+        raise ValueError(f"merge_gather: an [N, {C}, {H}, {W}] map is not supported (H, W even, C % 8 == 0)")
+    y = torch.empty((N * (H // 2) * (W // 2), 4 * C), dtype=torch.bfloat16, device=x.device)
+    _C().merge_gather(x.data_ptr(), y.data_ptr(), N, H, W, C, True, sm_count(x.device.index or 0), _stream())
+    return y
+
+
+def merge_scatter(dy: torch.Tensor, N: int, C: int, H: int, W: int) -> torch.Tensor:
+    """Backward of :func:`merge_gather`: dx [N, C, H, W] (channels_last) from dy [N*H/2*W/2, 4C]."""
+    if H % 2 or W % 2 or C % 8:
+        raise ValueError(f"merge_scatter: an [N, {C}, {H}, {W}] map is not supported (H, W even, C % 8 == 0)")
+    _check_rows(dy, N * (H // 2) * (W // 2), 4 * C, "dy")
+    dx = torch.empty((N, C, H, W), dtype=torch.bfloat16, device=dy.device, memory_format=torch.channels_last)
+    _C().merge_gather(dy.data_ptr(), dx.data_ptr(), N, H, W, C, False, sm_count(dy.device.index or 0), _stream())
+    return dx
+
+
+# ------------------------------------------------------------------------------------------------
 # squeeze-excitation (csrc/ops/squeeze_excite.cu) and hardswish on [B, F]
 # ------------------------------------------------------------------------------------------------
 def _check_gate(s: torch.Tensor, n: int, c: int) -> None:

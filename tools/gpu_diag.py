@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "swin", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "swin", "swin_v2", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -3452,6 +3452,425 @@ def g_swin():
     ok = all(l == l and abs(l) < 1e4 for l in losses) and n8.get("fwd", 0) > 0
     RESULTS.append(ok)
     print(f"[{'ok' if ok else 'FAIL'}] swin_t fp8 session: losses {[round(v, 3) for v in losses]}, fp8 launches {n8}",
+          flush=True)
+    del s
+    torch.cuda.empty_cache()
+    for kind, r in sorted(WORST.items()):
+        print(f"worst ratio to budget: {kind:24s} {r:.3f}x", flush=True)
+
+
+# ------------------------------------------------------------------------------------------------
+# Swin Transformer V2: scaled-cosine window attention (padded maps native), CPB MLP, PatchMergingV2
+# ------------------------------------------------------------------------------------------------
+# Budgets of the `swin_v2` group as (rtol, atol, arms) of report_abs.  The attention kernels are the V1 kernels'
+# arithmetic at L = 64 (bf16 operands, fp32 accumulation, P and dS rounded to bf16 as A operands, D from the stored bf16
+# O), with the fp32 cosine factors applied to the fp32 accumulator of the raw bf16 q . k.  O, lse and dV take
+# SWIN_BUDGET's entries.  Looser than SWIN_BUDGET, by 2x on both terms:
+# - win2 dq / dk and win2 dtable: the logits are a cosine times s_h = 10 (up to 100) plus a table 16 sigmoid(.) in
+#   [0, 16], against V1's q . k / sqrt(32) plus a table of about +-0.02, so the rows are far more peaked: fewer keys
+#   carry the weight and the bf16 rounding of P and dS (dS scaled by 1/|q| or 1/|k|) is a larger share of rms(ref).  At
+#   SWIN_BUDGET 1 or 2 elements in 10^6 of dq / dk went up to 1.41x, and 1 entry in 3,600 of dT to 1.41x.
+# - win2 dscale: s_h sum(dS o c) over every pair of the head, the same fp32 sums of dS as dT: dT's entry.
+# - win2 dbias: the column sums of dq over the real tokens and of dv over all tokens, padding included, taken before
+#   their bf16 rounding: SWIN_BUDGET's dT entry.
+# - cpb table / grads: fp32 throughout (one MLP of width 512): 2^-16 of |ref| plus 2^-14 of rms(ref).
+# - merge2: the float64 reference takes the reduction GEMM's output rounded to bf16 (as the kernel stores it) into its
+#   LayerNorm, so dgamma / dbeta take VIT_BUDGET's LayerNorm entries.  out takes twice "ln out": the kernel's fp32 GEMM
+#   and the float64 product can round an element of that input to adjacent bf16 values (1 element in 10^6 reached
+#   1.03x of "ln out").  dx is the dgrad GEMM of the bf16-rounded LayerNorm gradient (a sum of 2C products) and dred its
+#   weight gradient: dT's entry.
+SWIN_V2_BUDGET = {"win2 o": SWIN_BUDGET["win o"], "win2 lse": SWIN_BUDGET["win lse"], "win2 dq": (2.0 ** -5, 0.0, 2.0 ** -3),
+                  "win2 dk": (2.0 ** -5, 0.0, 2.0 ** -3), "win2 dv": SWIN_BUDGET["win dv"],
+                  "win2 dtable": (2.0 ** -5, 0.0, 2.0 ** -4), "win2 dscale": (2.0 ** -5, 0.0, 2.0 ** -4),
+                  "win2 dbias": SWIN_BUDGET["win dtable"], "cpb": (2.0 ** -16, 0.0, 2.0 ** -14),
+                  "merge2 out": (2.0 ** -6, 0.0, 2.0 ** -7), "merge2 dx": SWIN_BUDGET["win dtable"],
+                  "merge2 dgamma": VIT_BUDGET["ln dgamma"], "merge2 dbeta": VIT_BUDGET["ln dbeta"],
+                  "merge2 dred": SWIN_BUDGET["win dtable"]}
+
+
+def _swin_v2_check(name, kind, got, ref, atol=None):
+    rtol, atol0, arms = SWIN_V2_BUDGET[kind]
+    report_abs(f"{name} {kind}", got, ref, rtol, atol0 if atol is None else atol, arms, kind=kind)
+
+
+def _win2_lse_ref(qkv, table, ls, qb, vb, heads, N, H, W, shift):
+    """float64 log-sum-exp [N*H*W, heads] of torchvision's V2 logits on the padded map (padding tokens q = qb, k = 0,
+    v = vb), cropped to the real tokens."""
+    import math
+
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native
+    from distributeddeeplearning_b200.ops.swin import relative_position_index
+
+    C = qkv.shape[1] // 3
+    pH, pW = -(-H // 8) * 8, -(-W // 8) * 8
+    sy, sx = native.window_shift(H, W, 8, shift)
+    full = torch.cat([qb, torch.zeros_like(qb), vb]).double().expand(N, pH, pW, 3 * C).clone()
+    full[:, :H, :W] = qkv.double().view(N, H, W, 3 * C)
+    idx = torch.arange(N * pH * pW, device=qkv.device).view(N, pH, pW)
+    reg = torch.zeros(pH, pW, device=qkv.device)
+    if sy + sx > 0:
+        idx = torch.roll(idx, (-sy, -sx), (1, 2))
+        count = 0
+        for h in ((0, -8), (-8, -sy), (-sy, None)):
+            for w in ((0, -8), (-8, -sx), (-sx, None)):
+                reg[h[0]:h[1], w[0]:w[1]] = count
+                count += 1
+    nW = (pH // 8) * (pW // 8)
+    idx = idx.view(N, pH // 8, 8, pW // 8, 8).permute(0, 1, 3, 2, 4).reshape(N * nW, 64)
+    reg = reg.view(pH // 8, 8, pW // 8, 8).permute(0, 2, 1, 3).reshape(nW, 64)
+    mask = ((reg[:, None, :] - reg[:, :, None]) != 0).double() * -100.0
+    t = full.view(-1, 3 * C)[idx].view(N * nW, 64, 3, heads, 32).permute(2, 0, 3, 1, 4)
+    s = F.normalize(t[0], dim=-1) @ F.normalize(t[1], dim=-1).transpose(-2, -1)
+    s = s * torch.clamp(ls.double().view(heads, 1, 1), max=math.log(100.0)).exp()
+    s = s + table.double()[relative_position_index(8).to(qkv.device)].view(64, 64, heads).permute(2, 0, 1)
+    s = (s.view(N, nW, heads, 64, 64) + mask[None, :, None]).view(N * nW, heads, 64, 64)
+    lse = torch.empty(N * pH * pW, heads, dtype=torch.float64, device=qkv.device)
+    lse[idx.reshape(-1)] = torch.logsumexp(s, -1).permute(0, 2, 1).reshape(-1, heads)
+    return lse.view(N, pH, pW, heads)[:, :H, :W].reshape(-1, heads)
+
+
+def _win2_case(N, H, W, heads, shift, special=None, determinism=False):
+    import torch
+
+    from distributeddeeplearning_b200 import ops
+    from distributeddeeplearning_b200.ops import native
+
+    C = 32 * heads
+    qkv = torch.randn(N * H * W, 3 * C, device="cuda")
+    ls = torch.log(10 * torch.ones(heads, 1, 1, device="cuda")) + 0.3 * torch.randn(heads, 1, 1, device="cuda")
+    if special == "dominant":          # token 0 of every head aligned with the token 3 rows below, scale 100
+        for h in range(heads):
+            qkv[0, 32 * h:32 * h + 32] = qkv[3 * W, C + 32 * h:C + 32 * h + 32]
+        ls.fill_(5.0)
+    elif special == "constant":        # every key of image 0 equal (and a zero table): constant score rows
+        qkv[:H * W, C:2 * C] = qkv[:1, C:2 * C]
+    elif special == "zero":            # zero-norm q rows (every 5th token) and k rows (every 7th): c = 0, never NaN
+        qkv[::5, :C] = 0
+        qkv[::7, C:2 * C] = 0
+    elif special == "clamp":           # logit_scale above ln 100 on every other head: gradient 0 there
+        ls[::2] = 5.0
+    qkv = qkv.to(torch.bfloat16)
+    table = torch.rand(225, heads, device="cuda") * (0.0 if special == "constant" else 16.0)
+    qb = torch.randn(C, device="cuda") * 0.5
+    vb = torch.randn(C, device="cuda") * 0.5
+    dout = torch.randn(N * H * W, C, device="cuda").to(torch.bfloat16)
+
+    def bwd():
+        dt, dls, db = torch.empty(225, heads, device="cuda"), torch.zeros(heads, device="cuda"), torch.zeros(
+            3 * C, device="cuda")
+        dqkv = native.window_attention_v2_bwd(dout, qkv, table, ls, qb, vb, o, lse, heads, N, H, W, shift, dt, dls, db)
+        return dqkv, dt, dls, db
+
+    o, lse = native.window_attention_v2_fwd(qkv, table, ls, qb, vb, heads, N, H, W, shift)
+    dqkv, dt, dls, db = bwd()
+    tag = f"window attention v2 N={N} {H}x{W} heads={heads} shift={shift}" + (f" {special}" if special else "")
+    if determinism:
+        again = bwd()
+        ok = all(torch.equal(a, b) for a, b in zip((dqkv, dt, dls, db), again))
+        RESULTS.append(ok)
+        print(f"[{'ok' if ok else 'FAIL'}] {tag} dqkv, dT, dlogit_scale and dbias bitwise equal across two backward "
+              "calls", flush=True)
+    qd, td, lsd = qkv.double().requires_grad_(True), table.double().requires_grad_(True), ls.double().requires_grad_(True)
+    qbd, vbd = qb.double().requires_grad_(True), vb.double().requires_grad_(True)
+    ref = ops.window_attention_v2(qd, td, lsd, qbd, vbd, heads, H, W, 8, shift)   # the float64 composite
+    ref.backward(dout.double())
+    _swin_v2_check(tag, "win2 o", o, ref.detach())
+    _swin_v2_check(tag, "win2 lse", lse, _win2_lse_ref(qkv, table, ls, qb, vb, heads, N, H, W, shift))
+    g = qd.grad
+    floor = 2.0 ** -8 * float(g[:, 2 * C:].pow(2).mean().sqrt())
+    rows = torch.arange(N * H * W, device="cuda")
+    for i, kind in enumerate(("win2 dq", "win2 dk", "win2 dv")):
+        got, want = dqkv[:, i * C:(i + 1) * C], g[:, i * C:(i + 1) * C]
+        if special == "zero" and i < 2:
+            # a zero-norm row's gradient is F.normalize's 1/eps = 1e12 times the others': each set against its own rms
+            zero = rows % (5 if i == 0 else 7) == 0
+            _swin_v2_check(f"{tag} zero-norm rows", kind, got[zero], want[zero])
+            _swin_v2_check(f"{tag} other rows", kind, got[~zero], want[~zero], atol=floor)
+        else:
+            _swin_v2_check(tag, kind, got, want, atol=floor if i < 2 else None)
+    _swin_v2_check(tag, "win2 dtable", dt, td.grad)
+    _swin_v2_check(tag, "win2 dscale", dls, lsd.grad.view(-1))
+    # the bias gradient of qkv = x W^T + [b_q, 0, b_v]: the real tokens' dq / dv plus the padding tokens' (dq = 0 there)
+    pad = [t.grad if t.grad is not None else torch.zeros_like(t) for t in (qbd, vbd)]
+    _swin_v2_check(tag, "win2 dbias", torch.cat([db[:C], db[2 * C:]]),
+                   torch.cat([g[:, :C].sum(0) + pad[0], g[:, 2 * C:].sum(0) + pad[1]]))
+    ok = bool((db[C:2 * C] == 0).all()) and (special != "clamp" or bool((dls[::2] == 0).all()))
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {tag} k-bias gradient exactly 0" + (", clamped heads' dlogit_scale exactly 0"
+                                                                           if special == "clamp" else ""), flush=True)
+
+
+def _win2_functional_case(N, H, W, heads, shift):
+    """ops.window_attention_v2 through autograd on bf16 CUDA rows against the float64 composite: the gradients of qkv,
+    table, logit_scale and of q_bias / v_bias, which fill only the padding tokens (none on an unpadded map)."""
+    import torch
+
+    from distributeddeeplearning_b200 import ops
+
+    C = 32 * heads
+    qkv = torch.randn(N * H * W, 3 * C, device="cuda").to(torch.bfloat16).requires_grad_(True)
+    table = (torch.rand(225, heads, device="cuda") * 16).requires_grad_(True)
+    ls = (torch.log(10 * torch.ones(heads, 1, 1, device="cuda")) + 0.3 * torch.randn(heads, 1, 1, device="cuda"))
+    ls.requires_grad_(True)
+    qb = (torch.randn(C, device="cuda") * 0.5).requires_grad_(True)
+    vb = (torch.randn(C, device="cuda") * 0.5).requires_grad_(True)
+    dout = torch.randn(N * H * W, C, device="cuda").to(torch.bfloat16)
+    out = ops.window_attention_v2(qkv, table, ls, qb, vb, heads, H, W, 8, shift)
+    node = type(out.grad_fn).__name__
+    out.backward(dout)
+    ins = [t.detach().double().requires_grad_(True) for t in (qkv, table, ls, qb, vb)]
+    ref = ops.window_attention_v2(*ins, heads, H, W, 8, shift)
+    ref.backward(dout.double())
+    want = [t.grad if t.grad is not None else torch.zeros_like(t) for t in ins]
+    tag = f"ops.window_attention_v2 autograd N={N} {H}x{W} heads={heads} shift={shift}"
+    ok = node == "_WindowAttentionV2Backward"
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {tag} ran on the native node ({node})", flush=True)
+    _swin_v2_check(tag, "win2 o", out, ref.detach())
+    floor = 2.0 ** -8 * float(want[0][:, 2 * C:].pow(2).mean().sqrt())
+    for i, kind in enumerate(("win2 dq", "win2 dk", "win2 dv")):
+        _swin_v2_check(tag, kind, qkv.grad[:, i * C:(i + 1) * C], want[0][:, i * C:(i + 1) * C],
+                       atol=floor if i < 2 else None)
+    _swin_v2_check(tag, "win2 dtable", table.grad, want[1])
+    _swin_v2_check(tag, "win2 dscale", ls.grad, want[2])
+    _swin_v2_check(f"{tag} q_bias", "win2 dbias", qb.grad, want[3])     # padding queries get dO = 0: exactly 0
+    _swin_v2_check(f"{tag} v_bias", "win2 dbias", vb.grad, want[4])
+    ok = bool((qb.grad == 0).all()) and (H % 8 != 0 or W % 8 != 0 or bool((vb.grad == 0).all()))
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {tag} q_bias gradient exactly 0" +
+          ("" if H % 8 or W % 8 else ", v_bias gradient exactly 0 (no padding)"), flush=True)
+
+
+def _cpb_case(heads):
+    import torch
+
+    from distributeddeeplearning_b200.ops import native
+    from distributeddeeplearning_b200.ops.swin_v2 import cpb_table, relative_coords_table
+
+    coords = relative_coords_table(8).cuda()
+    w1 = torch.randn(512, 2, device="cuda") * 0.5
+    b1 = torch.randn(512, device="cuda") * 0.5
+    w2 = torch.randn(heads, 512, device="cuda") * 0.05
+    C = 32 * heads
+    qkv_b = torch.randn(3 * C, device="cuda")
+    table, eff = native.cpb_fwd(coords, w1, b1, w2, heads, qkv_b)
+    w1d, b1d, w2d = (t.double().requires_grad_(True) for t in (w1, b1, w2))
+    ref = cpb_table(coords.double(), w1d, b1d, w2d, heads)
+    tag = f"cpb heads={heads}"
+    _swin_v2_check(tag, "cpb", table, ref.detach())
+    ok = torch.equal(eff[:C], qkv_b[:C]) and torch.equal(eff[2 * C:], qkv_b[2 * C:]) and bool((eff[C:2 * C] == 0).all())
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {tag} effective qkv bias [b_q, 0, b_v]", flush=True)
+    dT = torch.randn(225, heads, device="cuda")
+    ref.backward(dT.double())
+    outs = [(torch.ones_like(w1), torch.ones_like(b1), torch.ones_like(w2)) for _ in range(2)]
+    for gw1, gb1, gw2 in outs:
+        native.cpb_bwd(coords, w1, b1, w2, table, dT, heads, gw1, gb1, gw2)
+    for name, got, r in (("dW1", outs[0][0], w1d.grad), ("db1", outs[0][1], b1d.grad), ("dW2", outs[0][2], w2d.grad)):
+        _swin_v2_check(f"{tag} {name}", "cpb", got - 1, r)
+    ok = all(torch.equal(a, b) for a, b in zip(outs[0], outs[1]))
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {tag} backward bitwise equal across two calls", flush=True)
+
+
+def _merge2_case(N, H, C, offset):
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import ops
+
+    x = (torch.randn(N, C, H, H, device="cuda") + offset).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    red = (torch.randn(2 * C, 4 * C, device="cuda") * (4 * C) ** -0.5).requires_grad_(True)
+    gamma = (torch.randn(2 * C, device="cuda") * 0.5 + 1.0).requires_grad_(True)
+    beta = (torch.randn(2 * C, device="cuda") * 0.1).requires_grad_(True)
+    xg = x.clone().requires_grad_(True)
+    y = ops.patch_merging_v2(xg, red, gamma, beta, 1e-5)
+    ok = type(y.grad_fn).__name__ == "_PatchMergingV2Backward"
+    xd = x.double().requires_grad_(True)
+    rd, gd, bd = (t.detach().double().requires_grad_(True) for t in (red, gamma, beta))
+    redb = red.detach().to(torch.bfloat16).double()
+    t = xd.permute(0, 2, 3, 1)
+    t = torch.cat([t[:, 0::2, 0::2], t[:, 1::2, 0::2], t[:, 0::2, 1::2], t[:, 1::2, 1::2]], -1)
+    r = F.linear(t, redb + (rd - rd.detach()))          # the bf16 weight's values, rd's gradient
+    r = r + (r.to(torch.bfloat16).double() - r).detach()  # the stored bf16 reduction output, gradient unchanged
+    ref = F.layer_norm(r, (2 * C,), gd, bd, 1e-5).permute(0, 3, 1, 2)
+    tag = f"patch merge v2 N={N} {H}x{H} C={C} offset={offset:g}"
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {tag} ran on the native node", flush=True)
+    _swin_v2_check(tag, "merge2 out", y, ref.detach())
+    dy = torch.randn_like(ref, dtype=torch.float32).to(torch.bfloat16)
+    y.backward(dy)
+    ref.backward(dy.double())
+    _swin_v2_check(tag, "merge2 dx", xg.grad, xd.grad)
+    _swin_v2_check(tag, "merge2 dred", red.grad, rd.grad)
+    _swin_v2_check(tag, "merge2 dgamma", gamma.grad, gd.grad)
+    _swin_v2_check(tag, "merge2 dbeta", beta.grad, bd.grad)
+
+
+def _swin_v2_vs_torchvision(name, bs, size):
+    """A Swin V2 against torchvision fp32 with the same weights (stochastic depth 0) and this repo's bf16 composite;
+    forward hooks check that every block and patch merge ran on the native node."""
+    import torch
+    from torchvision.models.swin_transformer import PatchMergingV2 as TvMerge
+    from torchvision.models.swin_transformer import SwinTransformer as TvSwin
+    from torchvision.models.swin_transformer import SwinTransformerBlockV2 as TvBlock
+
+    from distributeddeeplearning_b200 import models, ops
+    from distributeddeeplearning_b200.models.swin_v2 import _VARIANTS, PatchMergingV2, SwinTransformerBlockV2
+
+    dim, depths, heads, _ = _VARIANTS[name]
+    torch.manual_seed(0)
+    m = models.get_model(name, stochastic_depth_prob=0.0).cuda().train()
+    with torch.no_grad():                  # non-zero q / v biases, so that the padding tokens carry them
+        for mod in m.modules():
+            if isinstance(mod, SwinTransformerBlockV2):
+                mod.attn.qkv.bias.normal_(0.0, 0.02)
+    tv = TvSwin([4, 4], dim, list(depths), list(heads), [8, 8], stochastic_depth_prob=0.0, block=TvBlock,
+                downsample_layer=TvMerge).cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name, stochastic_depth_prob=0.0).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    nodes = []
+    hooks = [mod.register_forward_hook(lambda mod, i, o: nodes.append(type(o.grad_fn).__name__))
+             for mod in m.modules() if isinstance(mod, (SwinTransformerBlockV2, PatchMergingV2))]
+    x = torch.randn(bs, 3, size, size, device="cuda").to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    try:
+        out = m(x)
+        for h in hooks:
+            h.remove()
+        ops.softmax_cross_entropy(out, y, 1000).backward()
+        ro = tv(x)
+        torch.nn.functional.cross_entropy(ro, y).backward()
+        os.environ["DDL_B200_IMPL"] = "torch"
+        co = m2(x)
+        ops.softmax_cross_entropy(co, y, 1000).backward()
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+    want = sum(depths) + len(depths) - 1
+    ok = len(nodes) == want and set(nodes) == {"_SwinV2BlockBackward", "_PatchMergingV2Backward"}
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name} at {size}: {len(nodes)} of {want} blocks / merges ran on "
+          f"{sorted(set(nodes))}", flush=True)
+    c1, c2 = _cos(out, ro), _cos(co, ro)
+    RESULTS.append(c1 > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} at {size} logits cos vs fp32 {c1:.5f}   (bf16 composite {c2:.5f})")
+    gn, gc, tvp = dict(m.named_parameters()), dict(m2.named_parameters()), dict(tv.named_parameters())
+    worst, lag = (1.0, "", 1.0), (-1.0, "")
+    kz = True
+    for k, p in tvp.items():
+        if k.endswith("qkv.bias"):
+            C = p.numel() // 3
+            kz = kz and bool((gn[k].grad[C:2 * C] == 0).all())
+        if float(p.grad.norm()) == 0.0:
+            continue
+        a1, a2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if a1 < worst[0]:
+            worst = (a1, k, a2)
+        if a2 - a1 > lag[0]:
+            lag = (a2 - a1, k)
+    ok = lag[0] <= 0.01 and worst[0] > 0.6 and kz
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name} at {size}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at "
+          f"{worst[1]} (bf16 composite {worst[2]:.4f}); largest deficit vs the bf16 composite = {lag[0]:.4f} at "
+          f"{lag[1]}; k-bias gradients exactly 0: {kz}", flush=True)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        oe, re_ = m(x), tv(x)
+    ce = _cos(oe, re_)
+    RESULTS.append(ce > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} at {size} eval-mode logits cos vs torchvision eval {ce:.5f}",
+          flush=True)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def g_swin_v2():
+    """Swin V2: cosine window attention forward / backward at every stage shape of swin_v2_t and swin_v2_b at 256 and
+    at 224 (padded), shift 0 and 4, non-square and one-axis-shifted maps, a dominant logit, constant score rows,
+    zero-norm rows and a clamped logit scale, bitwise-repeatable backward; ops.window_attention_v2 through autograd on a
+    padded and an unpadded map; the CPB MLP and PatchMergingV2 against float64; swin_v2_t and swin_v2_b against torchvision at 224 and 256, eager vs CUDA-graph training and an fp8
+    session."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.manual_seed(0)
+    for heads0 in (3, 4):                       # swin_v2_t / _s and swin_v2_b
+        for sizes in ((64, 32, 16, 8), (56, 28, 14, 7)):
+            for stage, (N, H) in enumerate(zip((2, 4, 8, 16), sizes)):
+                for shift in (0, 4):
+                    _win2_case(N, H, H, heads0 * 2 ** stage, shift,
+                               determinism=stage == 1 and shift == 4 and heads0 == 3)
+    _win2_case(3, 20, 36, 6, 4)                 # non-square, padded on both axes
+    _win2_case(3, 36, 20, 6, 4)
+    _win2_case(4, 8, 20, 12, 4)                 # shifted on x only (pH = 8 forces sy = 0)
+    _win2_case(2, 14, 14, 6, 4, "dominant")
+    _win2_case(2, 16, 16, 6, 0, "constant")
+    _win2_case(2, 14, 14, 6, 4, "zero")
+    _win2_case(2, 14, 14, 6, 4, "clamp")
+    _win2_functional_case(2, 14, 14, 6, 4)      # padded: q_bias / v_bias fill the padding tokens
+    _win2_functional_case(2, 16, 16, 6, 4)      # unpadded: the output does not depend on them
+    for heads in (3, 24, 32):
+        _cpb_case(heads)
+    for C, H in ((96, 64), (192, 32), (384, 16), (96, 56), (192, 28), (384, 14), (128, 64), (256, 32), (512, 16)):
+        _merge2_case(4, H, C, 0.0)
+    _merge2_case(3, 14, 96, 50.0)
+    for size in (224, 256):
+        _swin_v2_vs_torchvision("swin_v2_t", 8, size)
+        _swin_v2_vs_torchvision("swin_v2_b", 4, size)
+    dist.init()
+
+    def run(graph, random_drops):
+        torch.manual_seed(0)
+        s = BenchmarkSession("swin_v2_t", 16, True, lr=0.01, momentum=0.9)
+        if not random_drops:        # the eager and the replayed step draw their vectors from different counters
+            for mod in s.model.modules():
+                if hasattr(mod, "sd_prob"):
+                    mod.sd_prob = 0.0
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out
+
+    a, b = run(False, False), run(True, False)
+    rel = max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(a[-4:], b[-4:]))
+    ok = all(x == x for x in a + b) and rel < 5e-2 and a[-1] < a[0]
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] swin_v2_t training without random drops: eager {[round(v, 4) for v in a]} graph "
+          f"replay {[round(v, 4) for v in b]} (largest relative difference of the last 4 {rel:.2e})", flush=True)
+    c = run(True, True)
+    ok = all(x == x and abs(x) < 1e4 for x in c)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] swin_v2_t graph-replayed training with stochastic depth: {[round(v, 4) for v in c]}",
+          flush=True)
+    fp8.reset()
+    fp8.enable(True)
+    try:
+        torch.manual_seed(0)
+        s = BenchmarkSession("swin_v2_t", 16, True, lr=0.01, momentum=0.9)
+        losses = [float(s.step()) for _ in range(4)]
+        torch.cuda.synchronize()
+        s.optimizer.check_errors()
+    finally:
+        fp8.enable(False)
+    n8 = fp8.launches()
+    ok = all(l == l and abs(l) < 1e4 for l in losses) and n8.get("fwd", 0) > 0
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] swin_v2_t fp8 session: losses {[round(v, 3) for v in losses]}, fp8 launches {n8}",
           flush=True)
     del s
     torch.cuda.empty_cache()
