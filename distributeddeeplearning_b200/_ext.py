@@ -164,6 +164,7 @@ KERNEL_LAUNCHES = {
     "tokens_fwd": 1, "tokens_bwd": 2,
     "window_attention_fwd": 1, "window_attention_bwd": 3, "patch_merge_fwd": 1, "patch_merge_bwd": 2,
     "window_attention_v2_fwd": 1, "window_attention_v2_bwd": 3, "cpb_fwd": 1, "cpb_bwd": 2, "merge_gather": 1,
+    "grid_attention_fwd": 1, "grid_attention_bwd": 3, "tanh_rows_fwd": 1, "tanh_rows_bwd": 1,
 }
 LAUNCH_COUNT = [0]          # kernels of THIS repo launched so far (bench.py reports the per-region delta)
 

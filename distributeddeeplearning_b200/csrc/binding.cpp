@@ -515,6 +515,23 @@ PYBIND11_MODULE(_C, m) {
   m.def("window_attention_bwd_scratch_floats", [](int N, int H, int heads) {
     return ddl::window_attention_bwd_scratch_floats(N, H, heads);
   });
+  // ------------------------------------------------------------------ MaxViT: partition (grid / window) attention
+  m.def("grid_attention_fwd", [](ptr_t qkv, ptr_t table, ptr_t o, ptr_t lse, int N, int H, int W, int heads, int C,
+                                 bool grid, float scale, ptr_t stream) {
+    check(ddl::launch_grid_attention_fwd(P<const __nv_bfloat16>(qkv), P<const float>(table), P<__nv_bfloat16>(o),
+                                         P<float>(lse), N, H, W, heads, C, grid, scale, S(stream)), "grid_attention_fwd");
+  });
+  m.def("grid_attention_bwd", [](ptr_t qkv, ptr_t table, ptr_t o, ptr_t dout, ptr_t lse, ptr_t dqkv, ptr_t dtable,
+                                 ptr_t scratch, int N, int H, int W, int heads, int C, bool grid, float scale,
+                                 ptr_t stream) {
+    check(ddl::launch_grid_attention_bwd(P<const __nv_bfloat16>(qkv), P<const float>(table), P<const __nv_bfloat16>(o),
+                                         P<const __nv_bfloat16>(dout), P<const float>(lse), P<__nv_bfloat16>(dqkv),
+                                         P<float>(dtable), P<float>(scratch), N, H, W, heads, C, grid, scale,
+                                         S(stream)), "grid_attention_bwd");
+  });
+  m.def("grid_attention_bwd_scratch_floats", [](int N, int H, int heads) {
+    return ddl::grid_attention_bwd_scratch_floats(N, H, heads);
+  });
   m.def("patch_merge_fwd", [](ptr_t x, ptr_t gamma, ptr_t beta, ptr_t y, ptr_t mean, ptr_t rstd, int N, int H, int W,
                               int C, float eps, int sms, ptr_t stream) {
     check(ddl::launch_patch_merge_fwd(P<const __nv_bfloat16>(x), P<const float>(gamma), P<const float>(beta),
@@ -601,6 +618,13 @@ PYBIND11_MODULE(_C, m) {
   });
   m.def("fold_cols_f32", [](ptr_t src, ptr_t dst, int rows, int k, int kp, ptr_t stream) {
     check(ddl::launch_fold_cols_f32(P<const float>(src), P<float>(dst), rows, k, kp, S(stream)), "fold_cols_f32");
+  });
+  m.def("tanh_rows_fwd", [](ptr_t x, ptr_t y, int64_t n, ptr_t stream) {
+    check(ddl::launch_tanh_rows_fwd(P<const __nv_bfloat16>(x), P<__nv_bfloat16>(y), n, S(stream)), "tanh_rows_fwd");
+  });
+  m.def("tanh_rows_bwd", [](ptr_t dy, ptr_t y, ptr_t dx, int64_t n, ptr_t stream) {
+    check(ddl::launch_tanh_rows_bwd(P<const __nv_bfloat16>(dy), P<const __nv_bfloat16>(y), P<__nv_bfloat16>(dx), n,
+                                    S(stream)), "tanh_rows_bwd");
   });
   m.def("silu_rows_fwd", [](ptr_t x, int ldx, ptr_t y, int ldy, int N, ptr_t stream) {
     check(ddl::launch_silu_rows_fwd(P<const __nv_bfloat16>(x), ldx, P<__nv_bfloat16>(y), ldy, N, S(stream)),

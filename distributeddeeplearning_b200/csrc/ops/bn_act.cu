@@ -17,6 +17,8 @@
 //   (bn_hswish_fwd_kernel, sharing the body) and backward mask value; no residual, bit mask or fp8 twin.
 //   SiLU (relu == 4, EfficientNet): z = v * sigmoid(v); the gradient is dz * s * (1 + v * (1 - s)) with s = sigmoid(v),
 //   v recomputed from x.  Own forward kernel (bn_silu_fwd_kernel) and mask value; the same refusals as hardswish.
+//   GELU (relu == 5, MaxViT): z = v * Phi(v), exact (erf); the gradient is dz * (Phi(v) + v * phi(v)), v recomputed from
+//   x.  Own forward kernel (bn_gelu_fwd_kernel) and mask value (9); the same refusals as hardswish.
 //   Stochastic depth (sample_scale, EfficientNet's residual blocks): z = BN(x) * keep[n] + residual with one scale per
 //   sample (row / hw), no activation.  The statistics cover every sample, dropped ones included; backward feeds
 //   dz * keep[n] to the BN and returns dres = dz.  Own forward kernel (bn_sd_fwd_kernel, train only) and mask value.
@@ -35,13 +37,23 @@ namespace {
 
 constexpr int kBnThreads = 256;
 enum { kMaskNone = 0, kMaskZ = 1, kMaskX = 2, kMaskBits = 3, kMaskZ6 = 4, kMaskX6 = 5, kMaskXH = 6, kMaskXS = 7,
-       kMaskSD = 8 };
+       kMaskSD = 8, kMaskXG = 9 };
 constexpr bool mask_from_z(int m) { return m == kMaskZ || m == kMaskZ6; }
-constexpr bool mask_from_x(int m) { return m == kMaskX || m == kMaskX6 || m == kMaskXH || m == kMaskXS; }
+constexpr bool mask_from_x(int m) { return m == kMaskX || m == kMaskX6 || m == kMaskXH || m == kMaskXS || m == kMaskXG; }
 // sigmoid on the MUFU exp and reciprocal (__fdividef, no IEEE division: with `1.f / (...)` the SiLU backward's chunked
 // apply pass spilled at 64 registers).  Relative accuracy holds in the negative tail, where sigmoid(v) is tiny; for
 // v < -87 the denominator overflows to inf and the result is 0.
 DDL_DEVICE float sigmoid(float v) { return __fdividef(1.f, 1.f + __expf(-v)); }
+// Phi(v) and e = exp(-v^2 / 2) from one MUFU exponential: erf by Abramowitz & Stegun 7.1.26 (|error| <= 1.5e-7), with
+// 0.5 erfc(|v| / sqrt 2) formed directly so that the negative tail keeps its relative accuracy.  The GELU backward's
+// apply pass spilled at 64 registers with erff; the forward keeps erff.
+DDL_DEVICE float gelu_cdf(float v, float& e) {
+  const float t = __fdividef(1.f, fmaf(0.3275911f * 0.70710678118654752f, fabsf(v), 1.f));
+  e = __expf(-0.5f * v * v);
+  const float tail = 0.5f * e * t *
+      fmaf(t, fmaf(t, fmaf(t, fmaf(t, 1.061405429f, -1.453152027f), 1.421413741f), -0.284496736f), 0.254829592f);
+  return v >= 0.f ? 1.f - tail : tail;
+}
 // whether the gradient passes the activation at pre-activation (or output) value v
 template <int MASK>
 DDL_DEVICE bool act_passes(float v) {
@@ -55,10 +67,15 @@ DDL_DEVICE float act_bwd(float v, float dz) {
     const float sg = sigmoid(v);
     return dz * sg * fmaf(v, 1.f - sg, 1.f);
   }
+  if (MASK == kMaskXG) {     // Phi(v) + v phi(v), phi(v) = exp(-v^2 / 2) / sqrt(2 pi)
+    float e;
+    const float cdf = gelu_cdf(v, e);
+    return dz * fmaf(v * 0.39894228040143268f, e, cdf);
+  }
   return act_passes<MASK>(v) ? dz : 0.f;
 }
 // forward activations of bn_act_fwd_body
-enum { kActRelu = 0, kActRelu6 = 1, kActHswish = 2, kActSilu = 3, kActSD = 4 };
+enum { kActRelu = 0, kActRelu6 = 1, kActHswish = 2, kActSilu = 3, kActSD = 4, kActGelu = 5 };
 DDL_DEVICE float hardswish(float v) { return v * fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f); }
 
 struct Vec8 {
@@ -123,7 +140,7 @@ DDL_DEVICE void fp8_fold_amax(Fp8Slot* slot, float amax) {
   }
 }
 
-// ACT: kActRelu (ReLU when a.relu, else none), kActRelu6 (when a.relu), kActHswish / kActSilu (always) or kActSD (no
+// ACT: kActRelu (ReLU when a.relu, else none), kActRelu6 (when a.relu), kActHswish / kActSilu / kActGelu (always) or kActSD (no
 // activation; the BN output scaled by the row's sample scale before the residual add)
 template <bool TRAIN, bool CHUNKED, bool FP8, int ACT>
 DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
@@ -191,6 +208,9 @@ DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
     } else if (ACT == kActSilu) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) z[i] *= sigmoid(z[i]);
+    } else if (ACT == kActGelu) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) z[i] *= fmaf(0.5f, erff(z[i] * 0.70710678118654752f), 0.5f);
     } else if (ACT != kActSD && a.relu) {
       if (a.mask) {
         uint32_t bits = 0;
@@ -246,6 +266,11 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_hswish_fwd_kernel(BnFwdArgs 
 template <bool TRAIN, bool CHUNKED>
 __global__ void __launch_bounds__(kBnThreads, 4) bn_silu_fwd_kernel(BnFwdArgs a) {
   bn_act_fwd_body<TRAIN, CHUNKED, false, kActSilu>(a);
+}
+
+template <bool TRAIN, bool CHUNKED>
+__global__ void __launch_bounds__(kBnThreads, 4) bn_gelu_fwd_kernel(BnFwdArgs a) {
+  bn_act_fwd_body<TRAIN, CHUNKED, false, kActGelu>(a);
 }
 
 // stochastic depth is drawn in training only: eval takes the plain residual kernels
@@ -304,8 +329,8 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
   const int last = a.M - 1;
   auto phys = [&](int rr) { return a.reverse ? last - rr : rr; };      // see BnBwdArgs::reverse
   int r = live ? blockIdx.x * 32 + rl : a.M;
-  if constexpr (MASK == kMaskXH || MASK == kMaskXS) {
-    // one row per iteration: the hardswish / SiLU gradient keeps more values live than a mask, and two rows would spill
+  if constexpr (MASK == kMaskXH || MASK == kMaskXS || MASK == kMaskXG) {
+    // one row per iteration: the hardswish / SiLU / GELU gradient keeps more values live than a mask, and two rows would spill
     for (; r < a.M; r += rstep) {
       const size_t off0 = static_cast<size_t>(phys(r)) * a.C + c0;
       accumulate(ld_stream_u4(a.dz + off0), ld_stream_u4(a.x + off0), make_uint4(0, 0, 0, 0));
@@ -326,7 +351,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
       }
     }
   }
-  for (; MASK != kMaskXH && MASK != kMaskXS && MASK != kMaskSD && r + rstep < a.M; r += 2 * rstep) {
+  for (; MASK != kMaskXH && MASK != kMaskXS && MASK != kMaskXG && MASK != kMaskSD && r + rstep < a.M; r += 2 * rstep) {
     const size_t off0 = static_cast<size_t>(phys(r)) * a.C + c0;
     const size_t off1 = static_cast<size_t>(phys(r + rstep)) * a.C + c0;
     const uint4 d0 = ld_stream_u4(a.dz + off0), d1 = ld_stream_u4(a.dz + off1);
@@ -723,7 +748,8 @@ cudaError_t launch_bn_bwd_mask(const BnBwdArgs& a, int sms, cudaStream_t stream,
   const bool f8 = a.dxq != nullptr && a.dxq_slot != nullptr;
   const bool flat = bn_flat_ok(a.C);
   const dim3 grid = flat ? dim3(bn_grid(a.M, a.C, sms)) : rgrid;
-  if constexpr (MASK == kMaskZ6 || MASK == kMaskX6 || MASK == kMaskXH || MASK == kMaskXS || MASK == kMaskSD) {
+  if constexpr (MASK == kMaskZ6 || MASK == kMaskX6 || MASK == kMaskXH || MASK == kMaskXS || MASK == kMaskXG ||
+                MASK == kMaskSD) {
     if (f8) return cudaErrorInvalidValue;
   } else if (f8) {
     return flat ? launch_pdl(bn_act_bwd_apply_kernel<MASK, false, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
@@ -748,8 +774,15 @@ cudaError_t launch_bn_act_fwd(const BnFwdArgs& a_in, bool train, int sms, cudaSt
     return flat ? launch_pdl(bn_sd_fwd_kernel<false>, grid, dim3(kBnThreads), 0, stream, 1, a)
                 : launch_pdl(bn_sd_fwd_kernel<true>, grid, dim3(kBnThreads), 0, stream, 1, a);
   }
-  if (a.relu == 3 || a.relu == 4) {    // hardswish / SiLU: no residual, bit mask or fp8 twin
+  if (a.relu == 3 || a.relu == 4 || a.relu == 5) {    // hardswish / SiLU / GELU: no residual, bit mask or fp8 twin
     if (a.residual != nullptr || a.mask != nullptr || (a.zq != nullptr && a.zq_slot != nullptr)) return cudaErrorInvalidValue;
+    if (a.relu == 5) {
+      if (flat)
+        return train ? launch_pdl(bn_gelu_fwd_kernel<true, false>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                     : launch_pdl(bn_gelu_fwd_kernel<false, false>, grid, dim3(kBnThreads), 0, stream, 1, a);
+      return train ? launch_pdl(bn_gelu_fwd_kernel<true, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                   : launch_pdl(bn_gelu_fwd_kernel<false, true>, grid, dim3(kBnThreads), 0, stream, 1, a);
+    }
     if (a.relu == 4) {
       if (flat)
         return train ? launch_pdl(bn_silu_fwd_kernel<true, false>, grid, dim3(kBnThreads), 0, stream, 1, a)
@@ -784,8 +817,9 @@ cudaError_t launch_bn_act_bwd(const BnBwdArgs& a_in, int sms, cudaStream_t strea
       return cudaErrorInvalidValue;
     return launch_bn_bwd_mask<kMaskSD>(a, sms, stream, false);
   }
-  if (a.relu == 3 || a.relu == 4) {    // hardswish / SiLU: pre-activation recomputed from x only, no residual gradient
-    if (!a.mask_from_x || a.zmask != nullptr || a.dres != nullptr) return cudaErrorInvalidValue;
+  if (a.relu == 3 || a.relu == 4 || a.relu == 5) {    // hardswish / SiLU / GELU: pre-activation recomputed from x only,
+    if (!a.mask_from_x || a.zmask != nullptr || a.dres != nullptr) return cudaErrorInvalidValue;   // no dres
+    if (a.relu == 5) return launch_bn_bwd_mask<kMaskXG>(a, sms, stream, skip_reduce);
     return a.relu == 3 ? launch_bn_bwd_mask<kMaskXH>(a, sms, stream, skip_reduce)
                        : launch_bn_bwd_mask<kMaskXS>(a, sms, stream, skip_reduce);
   }

@@ -666,6 +666,34 @@ __global__ void __launch_bounds__(256) hardswish_bwd_kernel(const __nv_bfloat16*
   }
 }
 
+// tanh on a [B][F] activation (MaxViT's classifier): y = tanh(x), and its backward from the saved output y:
+// dx = dy * (1 - y^2)
+__global__ void __launch_bounds__(256) tanh_rows_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* y,
+                                                            int64_t n8) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    float v[8];
+    unpack8(reinterpret_cast<const uint4*>(x)[i], v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = tanhf(v[k]);
+    reinterpret_cast<uint4*>(y)[i] = pack8(v);
+  }
+}
+
+__global__ void __launch_bounds__(256) tanh_rows_bwd_kernel(const __nv_bfloat16* __restrict__ dy,
+                                                            const __nv_bfloat16* __restrict__ y, __nv_bfloat16* dx,
+                                                            int64_t n8) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    float d[8], v[8];
+    unpack8(reinterpret_cast<const uint4*>(dy)[i], d);
+    unpack8(reinterpret_cast<const uint4*>(y)[i], v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) d[k] *= fmaf(-v[k], v[k], 1.f);
+    reinterpret_cast<uint4*>(dx)[i] = pack8(d);
+  }
+}
+
 // SiLU on the rows of a small bf16 matrix (EfficientNet's squeeze-excitation fc1 output [N][ldx]): y = x * sigmoid(x) into
 // [N][ldy] (ldy <= ldx: the next GEMM's K), and its backward from the saved x into a zero-padded GEMM operand
 // [N][ldx]: dx = dy * s * (1 + x * (1 - s)) for columns < c_valid, 0 beyond.  One thread per 8-column vector.
@@ -901,6 +929,17 @@ cudaError_t launch_hardswish_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* x
                                  cudaStream_t stream) {
   if (n % 8 != 0) return cudaErrorInvalidValue;
   hardswish_bwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>(dy, x, dx, n / 8);
+  return cudaGetLastError();
+}
+cudaError_t launch_tanh_rows_fwd(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, cudaStream_t stream) {
+  if (n % 8 != 0) return cudaErrorInvalidValue;
+  tanh_rows_fwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>(x, y, n / 8);
+  return cudaGetLastError();
+}
+cudaError_t launch_tanh_rows_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* y, __nv_bfloat16* dx, int64_t n,
+                                 cudaStream_t stream) {
+  if (n % 8 != 0) return cudaErrorInvalidValue;
+  tanh_rows_bwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>(dy, y, dx, n / 8);
   return cudaGetLastError();
 }
 cudaError_t launch_silu_rows_fwd(const __nv_bfloat16* x, int ldx, __nv_bfloat16* y, int ldy, int N, cudaStream_t stream) {

@@ -179,6 +179,21 @@ cudaError_t launch_window_attention_bwd(const __nv_bfloat16* qkv, const float* t
                                         cudaStream_t stream);
 size_t window_attention_bwd_scratch_floats(int N, int H, int heads);
 
+// ---- MaxViT: partition attention, 7 x 7 partitions, head dim 32 (grid_attention.cu) ----------------------------------
+// qkv [N*H*W][3C] bf16 in image order (head h: Q, K, V at columns 32h, C + 32h, 2C + 32h), C = 32 heads, H = W a multiple
+// of 7.  grid: the 49 tokens of sequence (i, j) sit at pixels (a H/7 + i, b H/7 + j); else (the window partition) at
+// (7i + a, 7j + b).  forward: o [N*H*W][C] and lse [N*H*W][heads] fp32 with logits q . k * scale + table[169][heads].
+cudaError_t launch_grid_attention_fwd(const __nv_bfloat16* qkv, const float* table, __nv_bfloat16* o, float* lse,
+                                      int N, int H, int W, int heads, int C, bool grid, float scale,
+                                      cudaStream_t stream);
+// backward (three kernels, deterministic): dqkv [N*H*W][3C] in qkv's layout; dtable [169][heads] += the bias gradient
+// (optional); scratch holds grid_attention_bwd_scratch_floats(N, H, heads) fp32
+cudaError_t launch_grid_attention_bwd(const __nv_bfloat16* qkv, const float* table, const __nv_bfloat16* o,
+                                      const __nv_bfloat16* dout, const float* lse, __nv_bfloat16* dqkv, float* dtable,
+                                      float* scratch, int N, int H, int W, int heads, int C, bool grid, float scale,
+                                      cudaStream_t stream);
+size_t grid_attention_bwd_scratch_floats(int N, int H, int heads);
+
 // ---- Swin V2: scaled-cosine shifted-window attention, window 8, head dim 32 (window_attention_v2.cu) -------------------
 // qkv [N*H*W][3C] bf16 in image order (head h: Q, K, V at columns 32h, C + 32h, 2C + 32h), C = 32 heads, any H, W (the
 // windows tile the padded frame ceil(H/8) 8 x ceil(W/8) 8; a padding token has q = qb, k = 0, v = vb: fp32 [C] or null),
@@ -322,6 +337,10 @@ cudaError_t launch_pad_cols_bf16(const __nv_bfloat16* src, __nv_bfloat16* dst, i
 cudaError_t launch_fold_cols_f32(const float* src, float* dst, int rows, int k, int kp, cudaStream_t stream);
 // SiLU on the rows of a bf16 matrix: y [N][ldy] = silu(x [N][ldx]) for columns [0, ldy) (ldy <= ldx, both % 8 == 0), and
 // its backward dx [N][ldx] = dy [N][ldy] * silu'(x) for columns < c_valid, zero elsewhere (a GEMM operand with zero pad)
+// tanh on n bf16 elements (n % 8 == 0), and dx = dy * (1 - y^2) from the saved output y
+cudaError_t launch_tanh_rows_fwd(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, cudaStream_t stream);
+cudaError_t launch_tanh_rows_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* y, __nv_bfloat16* dx, int64_t n,
+                                 cudaStream_t stream);
 cudaError_t launch_silu_rows_fwd(const __nv_bfloat16* x, int ldx, __nv_bfloat16* y, int ldy, int N, cudaStream_t stream);
 cudaError_t launch_silu_rows_bwd(const __nv_bfloat16* dy, int ldy, const __nv_bfloat16* x, int ldx, __nv_bfloat16* dx,
                                  int c_valid, int N, cudaStream_t stream);

@@ -7,7 +7,7 @@ AlexNet (SURVEY.md 2.7); ResNet-18/34, the other VGG depths, DenseNet and Squeez
 0.2.1's families) are here too, and the later ResNet family members of torchvision (ResNeXt-50 32x4d, ResNeXt-101
 32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2, MobileNetV3-Large / -Small, EfficientNet-B0 to -B7,
 ConvNeXt-Tiny / -Small / -Base / -Large, the Vision Transformers ViT-B/16, -B/32, -L/16 and -L/32, the Swin
-Transformers Swin-T, -S and -B and the Swin Transformers V2 Swin-V2-T, -S and -B.
+Transformers Swin-T, -S and -B, the Swin Transformers V2 Swin-V2-T, -S and -B, and MaxViT-T.
 """
 from __future__ import annotations
 
@@ -18,6 +18,7 @@ from .efficientnet import (INPUT_SIZE as _EFFICIENTNET_INPUT_SIZE, EfficientNet,
                            efficientnet_b1, efficientnet_b2, efficientnet_b3, efficientnet_b4, efficientnet_b5,
                            efficientnet_b6, efficientnet_b7)
 from .inception import Inception3, inception_v3  # noqa: F401
+from .maxvit import MaxVit, maxvit_t  # noqa: F401
 from .mobilenet import MobileNetV2, mobilenet_v2  # noqa: F401
 from .mobilenetv3 import MobileNetV3, mobilenet_v3_large, mobilenet_v3_small  # noqa: F401
 from .resnet import (ResNet, resnet18, resnet34, resnet50, resnet101, resnet152, resnext50_32x4d,  # noqa: F401
@@ -37,7 +38,7 @@ _REGISTRY = {
               mobilenet_v3_large, mobilenet_v3_small, resnet18, resnet34, resnet50, resnet101, resnet152,
               resnext50_32x4d, resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2, vgg11, vgg11_bn, vgg13,
               vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn, vit_b_16, vit_b_32, vit_l_16, vit_l_32, swin_t, swin_s, swin_b,
-              swin_v2_t, swin_v2_s, swin_v2_b)
+              swin_v2_t, swin_v2_s, swin_v2_b, maxvit_t)
 }
 
 

@@ -93,9 +93,9 @@ class LayerNorm(nn.Module):
 
 
 def conv_bn(x, conv: Conv2d, bn: BatchNorm2d, relu=True, residual=None, relu6=False, hardswish=False, silu=False,
-            sample_scale=None):
+            sample_scale=None, gelu=False):
     """act(BN(conv(x)) [+ residual]) through the fused op (``relu6``: the activation is ReLU6; ``hardswish``: it is
-    hardswish; ``silu``: it is SiLU).  ``sample_scale``: per-sample scales of stochastic depth applied to the BN output
+    hardswish; ``silu``: it is SiLU; ``gelu``: it is GELU).  ``sample_scale``: per-sample scales of stochastic depth applied to the BN output
     before the residual add (no activation)."""
     return ops.conv_bn_act(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.stride,
                            conv.padding,
@@ -104,6 +104,7 @@ def conv_bn(x, conv: Conv2d, bn: BatchNorm2d, relu=True, residual=None, relu6=Fa
                            **({"relu6": True} if relu6 else {}),
                            **({"hardswish": True} if hardswish else {}),
                            **({"silu": True} if silu else {}),
+                           **({"gelu": True} if gelu else {}),
                            **({"sample_scale": sample_scale} if sample_scale is not None else {}))
 
 

@@ -20,6 +20,7 @@ from .functional import (  # noqa: F401
     topk_correct,
     use_native,
 )
+from .maxvit import grid_attention, maxvit_attention_layer  # noqa: F401
 from .swin import patch_merging, swin_block, window_attention  # noqa: F401
 from .swin_v2 import patch_merging_v2, swin_v2_block, window_attention_v2  # noqa: F401
 from .vit import self_attention, vit_embed, vit_encoder_block  # noqa: F401

@@ -220,22 +220,24 @@ class _ConvBnAct(torch.autograd.Function):
 
 def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad=0, dil=1, eps=1e-5, momentum=0.1,
                 relu=True, residual=None, training=True, groups=1, relu6=False, hardswish=False, silu=False,
-                sample_scale=None):
+                sample_scale=None, gelu=False):
     """z = act(BN(conv(x, weight)) [+ residual])  — the unit every ResNet/Inception layer is made of.  ``groups`` > 1:
     grouped convolution (``weight`` is [Cout, Cin/groups, R, S]); depthwise shapes that ``native.supports_depthwise`` (3x3)
     or ``native.supports_depthwise5`` (5x5) accept run on the depthwise kernels, other shapes outside ``native.supports_grouped`` take the composite path.
     ``relu6``: the activation is ReLU6 (clamp to [0, 6]) instead of ``relu``; ``hardswish``: it is hardswish
     (v * clamp(v + 3, 0, 6) / 6), which takes no ``residual``; ``silu``: it is SiLU (v * sigmoid(v)), which takes no
-    ``residual`` either.  ``sample_scale``: fp32 [N] per-sample scales of stochastic depth (``stochastic_depth_keep``):
+    ``residual`` either; ``gelu``: it is GELU (v * Phi(v), the erf form), with the same restriction.  ``sample_scale``: fp32 [N] per-sample scales of stochastic depth (``stochastic_depth_keep``):
     z = BN(conv(x)) * sample_scale[n] + residual, with a ``residual``, no activation and in training; the batch
     statistics cover every sample, dropped ones included."""
     if hardswish and (relu6 or residual is not None):
         raise ValueError("conv_bn_act: hardswish is neither combined with relu6 nor with a residual")
     if silu and (relu6 or hardswish or residual is not None):
         raise ValueError("conv_bn_act: SiLU is neither combined with relu6 / hardswish nor with a residual")
-    if sample_scale is not None and (residual is None or relu or relu6 or hardswish or silu or not training):
+    if gelu and (relu6 or hardswish or silu or residual is not None):
+        raise ValueError("conv_bn_act: GELU is neither combined with another activation nor with a residual")
+    if sample_scale is not None and (residual is None or relu or relu6 or hardswish or silu or gelu or not training):
         raise ValueError("conv_bn_act: sample_scale needs a residual, no activation and training")
-    act = 4 if silu else (3 if hardswish else (2 if relu6 else relu))
+    act = 5 if gelu else (4 if silu else (3 if hardswish else (2 if relu6 else relu)))
     if use_native(x) and sample_scale is not None:
         if not (native.supports_conv(x.shape[1], weight.shape[0]) and groups == 1 and native.bn_supported(weight.shape[0])
                 and _krsc(weight)):
@@ -261,6 +263,8 @@ def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad
         z = z * sample_scale.to(z.dtype).view(-1, 1, 1, 1)
     if residual is not None:
         z = z + residual
+    if gelu:
+        return F.gelu(z)
     if silu:
         return F.silu(z)
     if hardswish:

@@ -844,6 +844,61 @@ def window_attention_bwd(dout: torch.Tensor, qkv: torch.Tensor, table: torch.Ten
     return dqkv
 
 
+# ------------------------------------------------------------------------------------------------
+# MaxViT: grid / window partition attention (csrc/ops/grid_attention.cu)
+# ------------------------------------------------------------------------------------------------
+def supports_grid_attention(H: int, W: int, partition: int, heads: int, head_dim: int) -> bool:
+    """Shapes the partition-attention kernels take: partition 7, head dim 32, a square map H = W, a multiple of 7."""
+    return (partition == 7 and head_dim == 32 and 0 < heads <= 65535 and H > 0 and H == W and H % 7 == 0
+            and (H // 7) ** 2 <= 65535)
+
+
+def _grid_check(qkv: torch.Tensor, table: torch.Tensor, heads: int, N: int, H: int, W: int):
+    C = qkv.shape[1] // 3 if qkv.dim() == 2 else 0
+    if C == 0 or C % heads != 0 or not supports_grid_attention(H, W, 7, heads, C // heads):
+        raise ValueError(f"grid_attention: H={H}, W={W}, {heads} heads of {C // max(heads, 1)} are not supported by the "
+                         "native kernels (partition 7, head dim 32, H = W a multiple of 7)")
+    _check_rows(qkv, N * H * W, 3 * C, "qkv")
+    if table.dtype != torch.float32 or tuple(table.shape) != (169, heads) or not table.is_contiguous():
+        raise ValueError(f"grid_attention: table must be the contiguous fp32 [169, {heads}] parameter")
+    return C
+
+
+def grid_attention_fwd(qkv: torch.Tensor, table: torch.Tensor, heads: int, N: int, H: int, W: int, scale: float,
+                       grid: bool = True):
+    """MaxViT's partition attention (7 x 7 sequences, head dim 32) on the image-order qkv rows [N*H*W, 3C] with the
+    relative-position bias ``table`` [169, heads] fp32 and logits q . k * ``scale``: the grid partition (sequence (i, j)
+    holds the pixels (a H/7 + i, b H/7 + j)), or with ``grid=False`` the window partition (pixels (7i + a, 7j + b)).
+    Returns (O [N*H*W, C] in image order, lse fp32 [N*H*W, heads])."""
+    C = _grid_check(qkv, table, heads, N, H, W)
+    o = torch.empty((N * H * W, C), dtype=torch.bfloat16, device=qkv.device)
+    lse = torch.empty((N * H * W, heads), dtype=torch.float32, device=qkv.device)
+    _C().grid_attention_fwd(qkv.data_ptr(), table.data_ptr(), o.data_ptr(), lse.data_ptr(), N, H, W, heads, C,
+                            bool(grid), float(scale), _stream())
+    return o, lse
+
+
+def grid_attention_bwd(dout: torch.Tensor, qkv: torch.Tensor, table: torch.Tensor, o: torch.Tensor, lse: torch.Tensor,
+                       heads: int, N: int, H: int, W: int, scale: float, grad_table: Optional[torch.Tensor],
+                       grid: bool = True) -> torch.Tensor:
+    """dqkv [N*H*W, 3C] (qkv's layout) of :func:`grid_attention_fwd`; grad_table [169, heads] += the bias gradient
+    (optional).  Deterministic: no atomics."""
+    C = _grid_check(qkv, table, heads, N, H, W)
+    _check_rows(o, N * H * W, C, "o")
+    _check_rows(dout, N * H * W, C, "dout")
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (N * H * W, heads) or not lse.is_contiguous():
+        raise ValueError("grid_attention_bwd: lse must be the contiguous fp32 [N*H*W, heads] of the forward")
+    if grad_table is not None and (grad_table.dtype != torch.float32 or tuple(grad_table.shape) != (169, heads)
+                                   or not grad_table.is_contiguous()):
+        raise ValueError("grid_attention_bwd: grad_table must be a contiguous fp32 [169, heads] buffer")
+    dqkv = torch.empty_like(qkv)
+    scratch = torch.empty(_C().grid_attention_bwd_scratch_floats(N, H, heads), dtype=torch.float32, device=qkv.device)
+    _C().grid_attention_bwd(qkv.data_ptr(), table.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(),
+                            dqkv.data_ptr(), _ptr(grad_table), scratch.data_ptr(), N, H, W, heads, C, bool(grid),
+                            float(scale), _stream())
+    return dqkv
+
+
 def _merge_check(x: torch.Tensor) -> Tuple[int, int, int, int]:
     _check_act(x)
     _check_aligned(x, "x")
@@ -1168,6 +1223,25 @@ def hardswish_bwd(dy: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
         raise ValueError("hardswish_bwd: dy and x differ in shape")
     dx = torch.empty_like(dy)
     _C().hardswish_bwd(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), x.numel(), _stream())
+    return dx
+
+
+def tanh_rows_fwd(x: torch.Tensor) -> torch.Tensor:
+    """y = tanh(x) elementwise (MaxViT's classifier activation)."""
+    _check_flat(x, "x")
+    y = torch.empty_like(x)
+    _C().tanh_rows_fwd(x.data_ptr(), y.data_ptr(), x.numel(), _stream())
+    return y
+
+
+def tanh_rows_bwd(dy: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+    """dx = dy * (1 - y^2), y being the saved output of :func:`tanh_rows_fwd`."""
+    _check_flat(dy, "dy")
+    _check_flat(y, "y")
+    if dy.shape != y.shape:
+        raise ValueError("tanh_rows_bwd: dy and y differ in shape")
+    dx = torch.empty_like(dy)
+    _C().tanh_rows_bwd(dy.data_ptr(), y.data_ptr(), dx.data_ptr(), y.numel(), _stream())
     return dx
 
 
@@ -1615,12 +1689,12 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
     element telling whether z > 0, which lets the backward of residual layers skip reading z (16x less mask traffic).
     ``relu``: False / True, 2 for ReLU6 (clamp to [0, 6]; not with ``want_mask``) or 3 for hardswish
     (x * clamp(x + 3, 0, 6) / 6; not with ``want_mask`` or ``residual``), 4 for SiLU (x * sigmoid(x); the same
-    refusals).  ``sample_scale``: fp32 [N] (stochastic depth, train only): z = BN(y) * sample_scale[n] + residual, with
+    refusals), 5 for GELU (x * Phi(x), erf form; the same refusals).  ``sample_scale``: fp32 [N] (stochastic depth, train only): z = BN(y) * sample_scale[n] + residual, with
     no activation."""
     C = _C()
     _check_act(y, "y")
-    if int(relu) == 4 and (want_mask or residual is not None):
-        raise ValueError("bn_act_fwd: SiLU takes no residual and has no bit-mask variant")
+    if int(relu) in (4, 5) and (want_mask or residual is not None):
+        raise ValueError("bn_act_fwd: SiLU / GELU take no residual and have no bit-mask variant")
     _check_sample_scale(sample_scale, y, relu, residual, train)
     if int(relu) == 2 and want_mask:
         raise ValueError("bn_act_fwd: ReLU6 has no bit-mask variant")
@@ -1641,7 +1715,7 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
         zq = slot = None
         key = ("act", gamma.data_ptr(), N, H, W)
         # emit the e4m3 twin only when an fp8 convolution consumed this layer's output in an earlier step
-        twin = _fp8.enabled() and int(relu) not in (2, 3, 4) and sample_scale is None and Ch % 128 == 0 and M >= 2048 \
+        twin = _fp8.enabled() and int(relu) not in (2, 3, 4, 5) and sample_scale is None and Ch % 128 == 0 and M >= 2048 \
             and _fp8.note_producer(z, key)
         if twin:
             idx, fused = _fp8.producer_slot(key, y.device, z)
@@ -1702,13 +1776,14 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
         raise ValueError("bn_act_bwd: need z or zmask for the ReLU mask of a residual layer")
     if int(relu) == 2 and not mask_from_x and zmask is not None:
         raise ValueError("bn_act_bwd: ReLU6 has no bit-mask variant (pass z)")
-    if int(relu) in (3, 4) and (not mask_from_x or want_dres):
-        raise ValueError("bn_act_bwd: hardswish / SiLU recompute their input from y (pass beta, had_residual=False)")
+    if int(relu) in (3, 4, 5) and (not mask_from_x or want_dres):
+        raise ValueError("bn_act_bwd: hardswish / SiLU / GELU recompute their input from y (pass beta, "
+                         "had_residual=False)")
     from . import fp8 as _fp8
 
     dyq = slot = None
     key = ("grad", gamma.data_ptr(), N, H, W)
-    twin = _fp8.enabled() and int(relu) not in (2, 3, 4) and sample_scale is None and Ch % 128 == 0 and M >= 2048 \
+    twin = _fp8.enabled() and int(relu) not in (2, 3, 4, 5) and sample_scale is None and Ch % 128 == 0 and M >= 2048 \
         and _fp8.note_producer(dy, key)                           # an fp8 dgrad consumed it before
     if twin:
         idx, fused = _fp8.producer_slot(key, y.device, dy, e5m2=True)

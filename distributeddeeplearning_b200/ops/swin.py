@@ -155,17 +155,32 @@ def _act4(rows: torch.Tensor, N: int, H: int, W: int) -> torch.Tensor:
     return rows.view(N, H, W, rows.shape[1]).permute(0, 3, 1, 2)
 
 
+def _attn_fwd(qkv, table, heads, N, H, W, shift, part):
+    if part is None:
+        return native.window_attention_fwd(qkv, table, heads, N, H, W, shift)
+    return native.grid_attention_fwd(qkv, table, heads, N, H, W, part[1], grid=part[0])
+
+
+def _attn_bwd(do, qkv, table, o, lse, heads, N, H, W, shift, part, grad_table):
+    if part is None:
+        return native.window_attention_bwd(do, qkv, table, o, lse, heads, N, H, W, shift, grad_table)
+    return native.grid_attention_bwd(do, qkv, table, o, lse, heads, N, H, W, part[1], grad_table, grid=part[0])
+
+
 class _SwinBlock(torch.autograd.Function):
+    """``part`` None: Swin's shifted-window attention (window_attention.cu).  ``part`` (grid, scale): MaxViT's
+    partition attention (grid_attention.cu), grid or window partition, logits scaled by ``scale``, no shift."""
+
     @staticmethod
-    def forward(ctx, x, keep1, keep2, heads, shift, eps, train, n1_w, n1_b, qkv_w, qkv_b, proj_w, proj_b, table, n2_w,
-                n2_b, w1, b1, w2, b2):
+    def forward(ctx, x, keep1, keep2, heads, shift, part, eps, train, n1_w, n1_b, qkv_w, qkv_b, proj_w, proj_b, table,
+                n2_w, n2_b, w1, b1, w2, b2):
         N, C, H, W = x.shape
         x2 = _rows4(x)
         wq, wp, w1b, w2b = weight_bf16(qkv_w), weight_bf16(proj_w), weight_bf16(w1), weight_bf16(w2)
         ones = _ones(C, x.device)
         t1, mean1, rstd1 = native.layer_norm_fwd(x2, n1_w, n1_b, eps)
         qkv = _lin(t1, wq, qkv_b, 3 * C, N)
-        o, lse = native.window_attention_fwd(qkv, table, heads, N, H, W, shift)
+        o, lse = _attn_fwd(qkv, table, heads, N, H, W, shift, part)
         a = _lin(o, wp, proj_b, C, N)
         x1 = native.layer_scale_fwd(_act4(a, N, H, W), ones, keep1, x)
         x1r = _rows4(x1)
@@ -175,7 +190,7 @@ class _SwinBlock(torch.autograd.Function):
         y = _lin(g, w2b, b2, C, N)
         z = native.layer_scale_fwd(_act4(y, N, H, W), ones, keep2, x1)
         ctx.params = (n1_w, n1_b, qkv_w, qkv_b, proj_w, proj_b, table, n2_w, n2_b, w1, b1, w2, b2)
-        ctx.dims = (N, C, H, W, heads, shift)
+        ctx.dims = (N, C, H, W, heads, shift, part)
         ctx.keep = (keep1, keep2)
         if train:
             ctx.wb = (wq, wp, w1b, w2b)   # views of the bf16 weight arena: see functional._ConvBnAct
@@ -187,7 +202,7 @@ class _SwinBlock(torch.autograd.Function):
         n1_w, n1_b, qkv_w, qkv_b, proj_w, proj_b, table, n2_w, n2_b, w1, b1, w2, b2 = ctx.params
         x2, t1, mean1, rstd1, qkv, o, lse, x1r, t2, mean2, rstd2, h, g = ctx.saved_tensors
         wq, wp, w1b, w2b = ctx.wb
-        N, C, H, W, heads, shift = ctx.dims
+        N, C, H, W, heads, shift, part = ctx.dims
         keep1, keep2 = ctx.keep
         ones = _ones(C, dz.device)
         if not dz.is_contiguous(memory_format=CL):
@@ -204,7 +219,7 @@ class _SwinBlock(torch.autograd.Function):
         da = _rows4(native.layer_scale_bwd(dx1_4, dx1_4, ones, keep1, None, _gb(proj_b)))
         do = _dgrad(da, wp, C, N)
         _wgrad(proj_w, o, da, N)
-        dqkv = native.window_attention_bwd(do, qkv, table, o, lse, heads, N, H, W, shift, _gb(table))
+        dqkv = _attn_bwd(do, qkv, table, o, lse, heads, N, H, W, shift, part, _gb(table))
         if qkv_b.requires_grad:
             native.bias_relu_bwd(dqkv, dqkv, grad_buffer(qkv_b), False)
         dx = None
@@ -215,7 +230,7 @@ class _SwinBlock(torch.autograd.Function):
         for p in (b2, w2, b1, w1, n2_w, n2_b, proj_b, proj_w, table, qkv_b, qkv_w, n1_w, n1_b):   # LAST
             if p.requires_grad:
                 notify_ready(p)
-        return (dx if ctx.needs_input_grad[0] else None,) + (None,) * 19
+        return (dx if ctx.needs_input_grad[0] else None,) + (None,) * 20
 
 
 def swin_block_native(x: torch.Tensor, heads: int, window: int, w1: torch.Tensor) -> bool:
@@ -238,7 +253,7 @@ def swin_block(x: torch.Tensor, heads: int, window: int, shift: int, eps: float,
     params = (n1_w, n1_b, qkv_w, qkv_b, proj_w, proj_b, table, n2_w, n2_b, w1, b1, w2, b2)
     if swin_block_native(x, heads, window, w1):
         train = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
-        return _SwinBlock.apply(x, keep1, keep2, heads, shift, eps, train, *params)
+        return _SwinBlock.apply(x, keep1, keep2, heads, shift, None, eps, train, *params)
     dt = x.dtype if x.is_cuda else n1_w.dtype
     c = (lambda p: p.to(dt)) if x.is_cuda else (lambda p: p)
     N, C, H, W = x.shape

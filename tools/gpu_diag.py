@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "swin", "swin_v2", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "swin", "swin_v2", "maxvit", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -4345,6 +4345,307 @@ def g_classic():
     dist.init()
     _graph_replay("inception_v3", 8)
     _graph_replay("densenet121", 16)
+    for kind, r in sorted(WORST.items()):
+        print(f"worst ratio to budget: {kind:24s} {r:.3f}x", flush=True)
+
+
+# ------------------------------------------------------------------------------------------------
+# MaxViT: grid / window partition attention, GELU in the fused BN, tanh on [B, F]
+# ------------------------------------------------------------------------------------------------
+# The partition-attention kernels are window_attention.cu's arithmetic (bf16 operands, fp32 accumulation, P and dS
+# rounded to bf16 as A operands, D from the stored bf16 O) with a 1/sqrt(C) scale instead of 1/sqrt(32): the logits
+# are flatter than Swin's, so SWIN_BUDGET's entries apply unchanged.  BN-GELU takes the SiLU BN's budgets (one fp32
+# row computation rounded to bf16; fp32 sums for dgamma / dbeta).  The tanh pair: one bf16 rounding of an fp32
+# elementwise result, 2^-7 of |ref| (the backward reads the bf16-rounded y, which the float64 reference also does).
+def _part_lse_ref(qkv, table, heads, N, H, grid):
+    """float64 log-sum-exp [N*H*W, heads] of torchvision's logits q . k / sqrt(C) + bias of the grid / window map."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import maxvit as mx
+
+    C = qkv.shape[1] // 3
+    idx = mx._to_seq(torch.arange(N * H * H, device=qkv.device, dtype=torch.float64).view(N, H, H, 1), grid)
+    idx = idx.reshape(-1, 49).long()
+    t = qkv.double()[idx].view(-1, 49, 3, heads, C // heads).permute(2, 0, 3, 1, 4)
+    s = t[0] @ (t[1] * C ** -0.5).transpose(-2, -1) + mx.relative_position_bias(table.double())
+    lse = torch.empty(N * H * H, heads, dtype=torch.float64, device=qkv.device)
+    lse[idx.reshape(-1)] = torch.logsumexp(s, -1).permute(0, 2, 1).reshape(-1, heads)
+    return lse
+
+
+def _grid_case(N, H, heads, grid, special=None, determinism=False):
+    import torch
+
+    from distributeddeeplearning_b200.ops import maxvit as mx
+    from distributeddeeplearning_b200.ops import native
+
+    C = 32 * heads
+    scale = C ** -0.5
+    qkv = torch.randn(N * H * H, 3 * C, device="cuda")
+    if special == "dominant":          # token 0 of every head aligned with one key of its sequence, scaled
+        p = H // 7 if grid else 1
+        for h in range(heads):
+            qkv[0, 32 * h:32 * h + 32] = 6.0 * qkv[3 * p * H, C + 32 * h:C + 32 * h + 32]
+    elif special == "constant":        # every key of image 0 equal (and a zero table): constant score rows
+        qkv[:H * H, C:2 * C] = qkv[:1, C:2 * C]
+    qkv = qkv.to(torch.bfloat16)
+    table = torch.randn(169, heads, device="cuda") * (0.0 if special == "constant" else 0.5)
+    dout = torch.randn(N * H * H, C, device="cuda").to(torch.bfloat16)
+    o, lse = native.grid_attention_fwd(qkv, table, heads, N, H, H, scale, grid=grid)
+    dt = torch.zeros(169, heads, device="cuda")
+    dqkv = native.grid_attention_bwd(dout, qkv, table, o, lse, heads, N, H, H, scale, dt, grid=grid)
+    tag = f"{'grid' if grid else 'window'} attention N={N} {H}x{H} heads={heads}" + (f" {special}" if special else "")
+    if determinism:
+        dt2 = torch.zeros(169, heads, device="cuda")
+        dqkv2 = native.grid_attention_bwd(dout, qkv, table, o, lse, heads, N, H, H, scale, dt2, grid=grid)
+        ok = torch.equal(dqkv, dqkv2) and torch.equal(dt, dt2)
+        RESULTS.append(ok)
+        print(f"[{'ok' if ok else 'FAIL'}] {tag} dqkv and dtable bitwise equal across two backward calls", flush=True)
+    qd, td = qkv.double().requires_grad_(True), table.double().requires_grad_(True)
+    ref = mx._attend_map(qd.view(N, H, H, 3 * C), td, heads, grid).reshape(N * H * H, C)   # torchvision's maths
+    ref.backward(dout.double())
+    _swin_check(tag, "win o", o, ref.detach())
+    _swin_check(tag, "win lse", lse, _part_lse_ref(qkv, table, heads, N, H, grid))
+    g = qd.grad
+    floor = 2.0 ** -8 * float(g[:, 2 * C:].pow(2).mean().sqrt())
+    for i, kind in enumerate(("win dq", "win dk", "win dv")):
+        _swin_check(tag, kind, dqkv[:, i * C:(i + 1) * C], g[:, i * C:(i + 1) * C], atol=floor if i < 2 else None)
+    _swin_check(tag, "win dtable", dt, td.grad)
+
+
+def _gelu_bn(C):
+    """GELU in the fused BN kernels: train forward (z, running statistics), eval forward and backward (pre-activation
+    recomputed from y), on inputs straddling 0."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    y = cl(bf(torch.randn(4, C, 9, 9, device="cuda") * 3))
+    g = torch.rand(C, device="cuda") * 2 + 0.5
+    b = torch.randn(C, device="cuda") * 2
+    rm, rv = torch.randn(C, device="cuda") * 0.1, torch.rand(C, device="cuda") + 0.5
+    rm2, rv2 = rm.double(), rv.double()
+    z, save = nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.01, 5, None, True)
+    v = F.batch_norm(y.double(), rm2, rv2, g.double(), b.double(), True, 0.01, 1e-3)
+    report_abs(f"gelu bn fwd C={C}", z, F.gelu(v), 2.0 ** -7, 2.0 ** -6)
+    report_abs(f"gelu bn running_mean C={C}", rm, rm2, 2.0 ** -8, 1e-5)
+    report_abs(f"gelu bn running_var  C={C}", rv, rv2, 2.0 ** -8, 1e-5)
+    ze, _ = nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.01, 5, None, False)
+    report_abs(f"gelu bn eval fwd C={C}", ze,
+               F.gelu(F.batch_norm(y.double(), rm.double(), rv.double(), g.double(), b.double(), False, 0.01, 1e-3)),
+               2.0 ** -7, 2.0 ** -6)
+    dz = cl(bf(torch.randn(y.shape, device="cuda")))
+    gg, bg = torch.zeros(C, device="cuda"), torch.zeros(C, device="cuda")
+    dy, _, _ = nv.bn_act_bwd(dz, None, y, save, g, 5, False, gg, bg, beta=b, had_residual=False)
+    yr = y.double().requires_grad_(True)
+    gr, br = g.double().requires_grad_(True), b.double().requires_grad_(True)
+    F.gelu(F.batch_norm(yr, None, None, gr, br, True, 0.01, 1e-3)).backward(dz.double())
+    report_abs(f"gelu bn bwd dx C={C}", dy, yr.grad, 2.0 ** -6, 0.0, arms=2.0 ** -7)
+    report_abs(f"gelu bn bwd dgamma C={C}", gg, gr.grad, 2.0 ** -8, 0.0, arms=2.0 ** -8)
+    report_abs(f"gelu bn bwd dbeta C={C}", bg, br.grad, 2.0 ** -8, 0.0, arms=2.0 ** -8)
+    refused = []
+    for kw in ({"want_mask": True}, {"residual": y}):
+        try:
+            nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.01, 5, kw.get("residual"), True, kw.get("want_mask", False))
+            refused.append(False)
+        except ValueError:
+            refused.append(True)
+    RESULTS.append(all(refused))
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] bn_act_fwd refuses GELU with the bit mask / a residual {refused}")
+
+
+def _gelu_conv_case(cin, cout, k, stride, groups, train):
+    """conv_bn_act(..., gelu=True) on the 1x1 (_ConvBnAct) and depthwise 3x3 (_DwConvBnAct) paths against float64 of
+    the same bf16 operands, forward and (train) backward."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import ops
+
+    torch.manual_seed(cin + k + stride)
+    x = cl(bf(torch.randn(4, cin, 28, 28, device="cuda")))
+    w = cl(bf(torch.randn(cout, cin // groups, k, k, device="cuda") * (cin // groups * k * k) ** -0.5)).float()
+    g, b = torch.rand(cout, device="cuda") + 0.5, torch.randn(cout, device="cuda") * 0.5
+    rm, rv = torch.zeros(cout, device="cuda"), torch.ones(cout, device="cuda")
+    xs = x.clone().requires_grad_(train)
+    ws, gs, bs = w.clone().requires_grad_(train), g.clone().requires_grad_(train), b.clone().requires_grad_(train)
+    z = ops.conv_bn_act(xs, ws, gs, bs, rm.clone(), rv.clone(), stride, (k - 1) // 2, 1, 1e-3, 0.01, False, None,
+                        train, groups, gelu=True)
+    xd, wd = x.double().requires_grad_(train), w.double().requires_grad_(train)
+    gd, bd = g.double().requires_grad_(train), b.double().requires_grad_(train)
+    zr = F.gelu(F.batch_norm(F.conv2d(xd, wd, None, stride, (k - 1) // 2, 1, groups), rm.double(), rv.double(), gd, bd,
+                             train, 0.01, 1e-3))
+    tag = f"conv{k}x{k}/s{stride} groups={groups} + BN-GELU {'train' if train else 'eval'}"
+    report(f"{tag} z", z, zr, 2e-2)
+    if train:
+        dz = cl(bf(torch.randn(z.shape, device="cuda")))
+        z.backward(dz)
+        zr.backward(dz.double())
+        for n, a, r in (("dx", xs, xd), ("dw", ws, wd), ("dgamma", gs, gd), ("dbeta", bs, bd)):
+            report(f"{tag} {n}", a.grad, r.grad, 3e-2)
+
+
+def _tanh_case():
+    import torch
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    x = bf(torch.randn(64, 512, device="cuda") * 2)
+    y = nv.tanh_rows_fwd(x)
+    report_abs("tanh rows fwd [64, 512]", y, torch.tanh(x.double()), 2.0 ** -7, 2.0 ** -12)
+    dy = bf(torch.randn(64, 512, device="cuda"))
+    dx = nv.tanh_rows_bwd(dy, y)
+    report_abs("tanh rows bwd [64, 512]", dx, dy.double() * (1 - y.double() ** 2), 2.0 ** -7, 2.0 ** -12)
+
+
+def _maxvit_vs_torchvision(bs, size):
+    """maxvit_t against torchvision fp32 with the same weights (stochastic depth 0) and this repo's bf16 composite;
+    forward hooks check that every attention layer ran on the native node."""
+    import torch
+    from torchvision.models.maxvit import MaxVit as TvMaxVit
+
+    from distributeddeeplearning_b200 import models, ops
+    from distributeddeeplearning_b200.models.maxvit import PartitionAttentionLayer
+
+    torch.manual_seed(0)
+    m = models.get_model("maxvit_t", stochastic_depth_prob=0.0, input_size=size).cuda().train()
+    tv = TvMaxVit((size, size), 64, 7, [64, 128, 256, 512], [2, 2, 5, 2], 32, 0.0).cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model("maxvit_t", stochastic_depth_prob=0.0, input_size=size).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    nodes = []
+    hooks = [mod.register_forward_hook(lambda mod, i, o: nodes.append(type(o.grad_fn).__name__))
+             for mod in m.modules() if isinstance(mod, PartitionAttentionLayer)]
+    x = torch.randn(bs, 3, size, size, device="cuda").to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    try:
+        out = m(x)
+        for h in hooks:
+            h.remove()
+        ops.softmax_cross_entropy(out, y, 1000).backward()
+        ro = tv(x)
+        torch.nn.functional.cross_entropy(ro, y).backward()
+        os.environ["DDL_B200_IMPL"] = "torch"
+        co = m2(x)
+        ops.softmax_cross_entropy(co, y, 1000).backward()
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+    ok = len(nodes) == 22 and set(nodes) == {"_SwinBlockBackward"}
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] maxvit_t {size}: {len(nodes)} of 22 attention layers ran on {sorted(set(nodes))}",
+          flush=True)
+    c1, c2 = _cos(out, ro), _cos(co, ro)
+    RESULTS.append(c1 > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] maxvit_t {size} logits cos vs fp32 {c1:.5f}   (bf16 composite {c2:.5f})")
+    gn, gc, tvp = dict(m.named_parameters()), dict(m2.named_parameters()), dict(tv.named_parameters())
+    worst, lag = (1.0, "", 1.0), (-1.0, "")
+    for k, p in tvp.items():
+        # the MBConv pre-norm biases: zero gradient in exact arithmetic (a train-mode BN follows the 1x1 conv), so
+        # every implementation's value is rounding noise and its cosine says nothing
+        if float(p.grad.norm()) == 0.0 or k.endswith("pre_norm.bias"):
+            continue
+        a1, a2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if a1 < worst[0]:
+            worst = (a1, k, a2)
+        if a2 - a1 > lag[0]:
+            lag = (a2 - a1, k)
+    ok = lag[0] <= 0.01 and worst[0] > 0.6
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] maxvit_t {size}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at "
+          f"{worst[1]} (bf16 composite {worst[2]:.4f}); largest deficit vs the bf16 composite = {lag[0]:.4f} at "
+          f"{lag[1]}", flush=True)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        oe, re_ = m(x), tv(x)
+    ce = _cos(oe, re_)
+    RESULTS.append(ce > 0.99)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] maxvit_t {size} eval-mode logits cos vs torchvision eval {ce:.5f}",
+          flush=True)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def g_maxvit():
+    """MaxViT: grid and window partition attention forward / backward at every maxvit_t stage shape at 224 and 448, a
+    dominant logit and constant score rows, bitwise-repeatable backward; Swin's window kernel at shift 0 at MaxViT's
+    shapes; BN-GELU in train and eval on the BN kernels and the 1x1 / depthwise conv paths; the tanh pair; maxvit_t
+    against torchvision, eager vs CUDA-graph training and an fp8 session."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.manual_seed(0)
+    for size in (224, 448):
+        for stage, (N, heads) in enumerate(((2, 2), (4, 4), (4, 8), (8, 16))):
+            H = size // 4 // 2 ** stage
+            for grid in (True, False):
+                _grid_case(N, H, heads, grid, determinism=stage == 0 and size == 224)
+            if size == 224:
+                _win_case(N, H, H, heads, 0)
+    for grid in (True, False):
+        _grid_case(2, 28, 4, grid, "dominant")
+        _grid_case(2, 28, 4, grid, "constant")
+    for C in (64, 256, 1024, 96):
+        _gelu_bn(C)
+    for train in (True, False):
+        _gelu_conv_case(64, 256, 1, 1, 1, train)
+        _gelu_conv_case(256, 256, 3, 1, 256, train)
+        _gelu_conv_case(256, 256, 3, 2, 256, train)
+    _tanh_case()
+    _maxvit_vs_torchvision(8, 224)
+    dist.init()
+
+    def run(graph, random_drops):
+        torch.manual_seed(0)
+        s = BenchmarkSession("maxvit_t", 16, True, lr=0.01, momentum=0.9)
+        if not random_drops:        # the eager and the replayed step draw their vectors from different counters
+            for mod in s.model.modules():
+                if hasattr(mod, "sd_prob"):
+                    mod.sd_prob = 0.0
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out
+
+    a, b = run(False, False), run(True, False)
+    rel = max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(a[-4:], b[-4:]))
+    ok = all(x == x for x in a + b) and rel < 5e-2 and a[-1] < a[0]
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] maxvit_t training without random drops: eager {[round(v, 4) for v in a]} graph "
+          f"replay {[round(v, 4) for v in b]} (largest relative difference of the last 4 {rel:.2e})", flush=True)
+    c = run(True, True)
+    ok = all(x == x and abs(x) < 1e4 for x in c)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] maxvit_t graph-replayed training with stochastic depth: "
+          f"{[round(v, 4) for v in c]}", flush=True)
+    fp8.reset()
+    fp8.enable(True)
+    try:
+        torch.manual_seed(0)
+        s = BenchmarkSession("maxvit_t", 16, True, lr=0.01, momentum=0.9)
+        losses = [float(s.step()) for _ in range(4)]
+        torch.cuda.synchronize()
+        s.optimizer.check_errors()
+    finally:
+        fp8.enable(False)
+    n8 = fp8.launches()
+    ok = all(l == l and abs(l) < 1e4 for l in losses) and n8.get("fwd", 0) > 0
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] maxvit_t fp8 session: losses {[round(v, 3) for v in losses]}, fp8 launches {n8}",
+          flush=True)
+    del s
+    torch.cuda.empty_cache()
     for kind, r in sorted(WORST.items()):
         print(f"worst ratio to budget: {kind:24s} {r:.3f}x", flush=True)
 
