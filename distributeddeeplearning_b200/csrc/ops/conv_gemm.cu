@@ -92,6 +92,12 @@ constexpr bool mode_b_mn(int mode) { return mode == kConvDgrad || mode == kConvT
 constexpr bool mode_tile(int mode) { return mode == kConvTileFwd || mode == kConvTileDgrad || mode == kConvStemTma; }
 constexpr bool mode_stem(int mode) { return mode == kConvStem || mode == kConvStemTma; }
 
+// grouped convolution: first source channel of the bundle that owns the 64-wide N tile at expanded row n0 (one tile
+// per bundle, T = 1, needs no division)
+DDL_DEVICE int grp_src0(const ConvArgs& a, int n0) {
+  return (a.cchunks == 1 ? (n0 >> 6) : (n0 >> 6) / a.cchunks) * a.grouped;
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // epilogue building blocks
@@ -308,8 +314,9 @@ DDL_DEVICE void epi_stats_accum(uint32_t stg, uint32_t ybuf, int etid, const Con
 // Publish `acc` (sums of tile column acc.n0) and clear it.  Contains one named barrier: must be reached by all
 // kEpiThreads epilogue threads together; `red` = [epi warps][2][BLOCK_N] floats of scratch.  A later flush may rewrite
 // the scratch only after another barrier of the same group (every caller has one per tile / chunk in between).
+// Channels >= n_end (a grouped tile's overhang into the next bundle) are left out.
 template <int BLOCK_N>
-DDL_DEVICE void epi_stats_flush(uint32_t red, int etid, int ew, const ConvArgs& a, StatAcc& acc) {
+DDL_DEVICE void epi_stats_flush(uint32_t red, int etid, int ew, const ConvArgs& a, StatAcc& acc, int n_end) {
   constexpr int kColGroups = BLOCK_N / 8;
   if (a.variant & kDbgNoStats) { acc.clear(); return; }
   const int cg = etid % kColGroups;
@@ -343,7 +350,7 @@ DDL_DEVICE void epi_stats_flush(uint32_t red, int etid, int ew, const ConvArgs& 
       float v = 0.f;
 #pragma unroll
       for (int wq = 0; wq < kEpiThreads / 32; ++wq) v += lds_f32(red + ((wq * 2 + which) * BLOCK_N + col) * 4);
-      if (n0 + col < a.n_valid) atomicAdd((which ? a.sumsq : a.sum) + n0 + col, v);
+      if (n0 + col < min(a.n_valid, n_end)) atomicAdd((which ? a.sumsq : a.sum) + n0 + col, v);
     }
   } else {
     for (int col = etid; col < BLOCK_N; col += kEpiThreads) {      // dbeta += S1, dgamma += invstd * (S2 - mean * S1)
@@ -363,16 +370,17 @@ DDL_DEVICE void epi_stats_flush(uint32_t red, int etid, int ew, const ConvArgs& 
 }
 
 // The coalesced 16-byte global stores of the staged tile (optional `+= add`, optional zero-fill of the three stride-2
-// siblings): thread = (16-byte column chunk, row phase); a tile row is BLOCK_N*2 contiguous bytes.
+// siblings): thread = (16-byte column chunk, row phase); a tile row is BLOCK_N*2 contiguous bytes.  Channels >= n_end
+// are not stored.
 template <int BLOCK_N, bool TILE>
-DDL_DEVICE void epi_store(uint32_t stg, int etid, const ConvArgs& a, int n0, int m0) {
+DDL_DEVICE void epi_store(uint32_t stg, int etid, const ConvArgs& a, int n0, int m0, int n_end) {
   constexpr int kPitch = BLOCK_N * 2 + 16;
   constexpr int kVecPerRow = BLOCK_N / 8;
   constexpr int kRowStep = kEpiThreads / kVecPerRow;
   constexpr int kIters = kBlockM / kRowStep;
   const int ch = etid % kVecPerRow;
   const int r0 = etid / kVecPerRow;
-  if (n0 + ch * 8 >= a.ldc) return;                       // channel padding of the last N tile (ldc = row width)
+  if (n0 + ch * 8 >= min(a.ldc, n_end)) return;          // channel padding of the last N tile (ldc = row width)
   if (a.variant & kDbgNoStore) return;
   uint32_t sp = stg + r0 * kPitch + ch * 16;
   const size_t coff = static_cast<size_t>(n0 + ch * 8);
@@ -421,18 +429,18 @@ DDL_DEVICE void epi_store(uint32_t stg, int etid, const ConvArgs& a, int n0, int
   }
 }
 
-// One tile: accumulate, publish, store.
+// One tile: accumulate, publish, store (channels [n0, n_end)).
 template <int BLOCK_N, bool STATS, bool TILE>
 DDL_DEVICE void epi_stats_store(uint32_t stg, uint32_t red, uint32_t ybuf, int etid, int ew, const ConvArgs& a, int n0,
-                                int m0) {
+                                int m0, int n_end) {
   if (STATS) {
     StatAcc acc;
     acc.clear();
     epi_stats_accum<BLOCK_N, TILE>(stg, ybuf, etid, a, n0, m0, acc);
     acc.n0 = n0;
-    epi_stats_flush<BLOCK_N>(red, etid, ew, a, acc);
+    epi_stats_flush<BLOCK_N>(red, etid, ew, a, acc, n_end);
   }
-  epi_store<BLOCK_N, TILE>(stg, etid, a, n0, m0);
+  epi_store<BLOCK_N, TILE>(stg, etid, a, n0, m0, n_end);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -463,6 +471,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
   constexpr bool kATma = mode_a_tma(MODE);
   constexpr bool kBMn = mode_b_mn(MODE) && FP8 == 0;   // fp8 data gradients read a transposed, K-major weight copy
   constexpr bool kTile = mode_tile(MODE);
+  // the instantiations the launcher may run grouped (bf16, 64-wide tiles, window forward / data gradient)
+  constexpr bool kGrp = BLOCK_N == 64 && FP8 == 0 &&
+                        (MODE == kConvFwd || MODE == kConvDgrad || MODE == kConvTileFwd || MODE == kConvTileDgrad);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nstages = a.stages;
@@ -535,6 +546,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
       const uint32_t row_off = row * 128u;
       const uint32_t sw = row & 7u;
       int tap_r = 0, tap_s = 0, cc = 0;   // incremental decode of kb -> (r, s, channel chunk)
+      const int src0 = kGrp && a.grouped ? grp_src0(a, n0) : 0;     // grouped: the tile's bundle
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = 0; kb < KB; ++kb) {
@@ -574,7 +586,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
             sh = hb + tap_r * a.dil; swd = wb + tap_s * a.dil;
             ok = row_ok && sh >= 0 && sh < a.srcH && swd >= 0 && swd < a.srcW;
           }
-          const int c0 = (a.grouped ? n0 : 0) + cc * 64;     // grouped: the tile's own 64 source channels
+          const int c0 = src0 + cc * 64;
           const __nv_bfloat16* src =
               ok ? img_base + (static_cast<size_t>(sh) * a.srcW + swd) * a.srcC + c0 : a.src;
           const int crem = a.srcC - c0;           // channels left in this tap (last k-block of a tap may be partial)
@@ -605,6 +617,15 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
       for (int item = unit; item < items; item += units) {
         decode(item);
         int tap = 0, cc = 0, tap_r = 0, tap_s = 0;
+        // grouped, per tile: the bundle's first source channel; for the data gradient the expanded weight box origin
+        // (column of slice t in tap 0, first row of the bundle)
+        int src0 = 0, bcol = 0, brow = 0;
+        if (kGrp && a.grouped) {
+          const int nt = n0 >> 6, t = a.cchunks == 1 ? 0 : nt % a.cchunks;
+          src0 = grp_src0(a, n0);
+          bcol = t * 64;
+          brow = (nt - t) * 64;
+        }
         const uint32_t a_bytes = kTile ? static_cast<uint32_t>(a.tw * a.th * a.tn) * 128u : kATileBytes;
         for (int kb = 0; kb < KB; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1u, 17);
@@ -634,9 +655,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
                                     n0 + static_cast<int>(rank) * (BLOCK_N / 2), &full[stage], 0x3);
             }
           } else if (kBMn) {
-            if (a.grouped) {
-              // expanded grouped weights [Cout][(tap, 64)]: K rows = output channels [n0, n0 + 64), N = tap's columns
-              tma_load_2d(sB, &tmB, widx * 64, n0, &full[stage]);
+            if (kGrp && a.grouped) {
+              // expanded grouped weights: K rows = the bundle's 64 output channels of k-block cc, N = the columns of
+              // this tile's slice t of the bundle in the tap
+              tma_load_2d(sB, &tmB, widx * a.kstride + bcol, brow + cc * 64, &full[stage]);
             } else {
               // weights W[co][(r,s,ci)]: K rows = 64 output channels, N = input channels (contiguous)
 #pragma unroll
@@ -651,8 +673,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
           } else if (MODE == kConvStemTma) {
             tma_load_5d(smem_u32(sA), &tmA, 0, kb, tq0, tp0, tn0, &full[stage]);
           } else if (kTile) {
-            tma_load_4d(smem_u32(sA), &tmAs.m[mapi], (a.grouped ? n0 : 0) + cc * kcol, tq0 + dw, tp0 + dh, tn0,
-                        &full[stage]);
+            tma_load_4d(smem_u32(sA), &tmAs.m[mapi], src0 + cc * kcol, tq0 + dw, tp0 + dh, tn0, &full[stage]);
           }
           if (++cc == a.cchunks) { cc = 0; ++tap; if (++tap_s == a.S) { tap_s = 0; ++tap_r; } }
           if (++stage == nstages) { stage = 0; phase ^= 1u; }
@@ -738,7 +759,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant_
       // the row's destination index rides in the pad bytes of its staging row (pitch = 2*BLOCK_N + 16)
       if (kTile && etid < kBlockM) sts32(stg + etid * Cfg::kPitch + BLOCK_N * 2, static_cast<uint32_t>(dest_row(etid)));
       named_bar_sync(1, kEpiThreads);
-      epi_stats_store<BLOCK_N, STATS, kTile>(stg, smem_u32(full) + 256, ybuf, etid, warp, a, n0, m0);
+      // grouped: slice t of bundle b covers output channels from b*Wb + 64 t up to the bundle's end
+      int nc0 = n0, n_end = 0x7fffffff;
+      if (kGrp && a.grouped) {
+        const int s0 = grp_src0(a, n0);
+        nc0 = a.cchunks == 1 ? s0 : s0 + (n0 >> 6) % a.cchunks * 64;
+        n_end = s0 + a.grouped;
+      }
+      epi_stats_store<BLOCK_N, STATS, kTile>(stg, smem_u32(full) + 256, ybuf, etid, warp, a, nc0, m0, n_end);
     }
   }
   if (CL) cluster_sync_all();          // no CTA leaves while its peer may still multicast into it or arrive on it
@@ -774,7 +802,14 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   const int warp = threadIdx.x >> 5;
   const int col0 = blockIdx.x * 128;          // first k column of this tile
   constexpr int kCoTile = SWAP ? 64 : 128;
-  const int co0 = blockIdx.y * kCoTile;       // first output channel of this tile
+  int co0 = blockIdx.y * kCoTile;             // first output channel of this tile
+  int cs0 = co0, cs_end = a.Cout;             // grouped: first input channel of the tile's bundle, end of the bundle
+  if (a.group_width) {                        // tile = slice t of bundle b (ConvArgs::grouped), T = Cpad / 64
+    const int gw = a.group_width, T = a.Cpad >> 6;
+    cs0 = static_cast<int>(blockIdx.y) / T * (gw < 64 ? 64 / gw * gw : gw);
+    co0 = cs0 + static_cast<int>(blockIdx.y) % T * 64;
+    cs_end = min(cs0 + (gw < 64 ? 64 / gw * gw : gw), a.Cout);
+  }
   const int kb_begin = blockIdx.z * a.kb_per_split;
   const int kb_end = min(kb_begin + a.kb_per_split, a.total_kb);
   const int KB = kb_end - kb_begin;
@@ -817,7 +852,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
         c_off = colc - tap * a.Cpad;
         tap_r = tap / a.S;
         tap_s = tap - tap_r * a.S;
-        if (a.group_width) c_off += co0;        // grouped: the input channels of this tile's 64 output channels
+        if (a.group_width) c_off += cs0;        // grouped: the input channels of this tile's bundle
       }
       const int crem = a.C - c_off;             // real channels left in this tap
       const uint32_t row_off = 16384u + chunk * 8192u + row * 128u;
@@ -885,7 +920,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
         for (int j = 0; j < 2; ++j) {
           const int colc = col0 + j * 64;
           const int tap = colc / a.Cpad;
-          tc0[j] = colc - tap * a.Cpad + (a.group_width ? co0 : 0);
+          tc0[j] = colc - tap * a.Cpad + (a.group_width ? cs0 : 0);
           const int r = tap / a.S, sx = tap - r * a.S;
           const int oh = r * a.dil - a.pad, ow = sx * a.dil - a.pad_w;
           if (a.stride == 1) {
@@ -993,14 +1028,15 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     const int vtap = vc / a.Cpad;
     const int vch = vc - vtap * a.Cpad;
     if (a.group_width) {
-      // grouped (SWAP, Cpad = 64): row r pairs with input channel co0 + vch; only the diagonal group x group blocks
-      // exist.  group_width % 4 == 0, so this lane's 4 columns lie in one group and land as one 16-byte vector
+      // grouped (SWAP, Cpad = 64 T): row r is output channel co0 + r, column vch input channel cs0 + vch of the
+      // bundle; only the diagonal group x group blocks exist.  group_width % 4 == 0, so this lane's 4 columns lie in
+      // one group and land as one 16-byte vector
       const int gw = a.group_width;
       if (vc < a.ncols) {
         const int c = vtap * gw + vch % gw;
         for (int r = warp; r < kCoTile; r += kEpiThreads / 32) {
           const int co = co0 + r;
-          if (co < a.Cout && r / gw == vch / gw) {
+          if (co < cs_end && (co - cs0) / gw == vch / gw) {
             const float4 val = *reinterpret_cast<const float4*>(stg + r * kWgPitch + lane * 4);
             red_add_f32x4(a.dw + static_cast<size_t>(co) * a.ldw + c, val.x, val.y, val.z, val.w);
           }
@@ -1289,11 +1325,15 @@ cudaError_t launch_conv_gemm(int mode, const ConvArgs& a_in, const void* w, int 
   const int bn = (n_total % 128 == 0 && !a.grouped) ? 128 : 64;
   if (n_total % 64 != 0) return cudaErrorInvalidValue;
   if (a.grouped) {
-    // block-diagonal tiles: bf16 window convolutions (forward or data gradient, tile or gather modes) on the expanded
-    // weights, one k-block per tap; the shortcut add and the fused BN-backward reduction are not offered
+    // group bundles: bf16 window convolutions (forward or data gradient, tile or gather modes) on the expanded
+    // weights, T = cchunks k-blocks per tap; bias / ReLU, the shortcut add and the fused BN-backward reduction are not
+    // offered
     const bool ok_mode = mode == kConvFwd || mode == kConvTileFwd || mode == kConvDgrad || mode == kConvTileDgrad;
-    if (!ok_mode || a.fp8 || a.add != nullptr || a.add_mask != nullptr || a.bnr_y != nullptr || a.cchunks != 1 ||
-        a.kstride != 64 || w_cols != a.R * a.S * 64 || w_rows != n_total || a.srcC != n_total || a.ldc != n_total)
+    const int wb = a.grouped, T = (wb + 63) / 64;
+    if (!ok_mode || a.fp8 || a.add != nullptr || a.add_mask != nullptr || a.bnr_y != nullptr || a.bias != nullptr ||
+        a.relu || wb % 8 != 0 || a.ldc % 8 != 0 || a.cchunks != T || a.kstride != T * 64 ||
+        w_cols != a.R * a.S * T * 64 || w_rows != n_total || n_total != (a.ldc + wb - 1) / wb * T * 64 ||
+        a.srcC != a.ldc)
       return cudaErrorInvalidValue;
   }
   const int es = a.fp8 ? 1 : 2;                   // operand element size (bytes)
@@ -1428,12 +1468,15 @@ cudaError_t launch_conv_wgrad(const WgradArgs& a_in, const void* dy, const void*
   WgradArgs a = a_in;
   CUtensorMap tmDy;
   TmaSet tmX;
+  int co_tiles = 0;             // grouped: T 64-channel tiles per bundle
   if (a.group_width) {
-    // grouped: window modes only, 64-channel tiles in the (tap, 64) column space, 16-byte in-group vectors
+    // grouped: window modes only, 64-channel tiles in the (tap, 64 T) column space, 16-byte in-group vectors
     const int gw = a.group_width;
-    if ((a.mode != kConvFwd && a.mode != kConvTileFwd) || gw % 4 != 0 || 64 % gw != 0 || a.Cout % 64 != 0 ||
-        a.C != a.Cout || a.Cpad != 64 || a.ncols != a.R * a.S * 64 || a.ldw != a.R * a.S * gw)
+    const int wb = gw < 64 ? 64 / gw * gw : gw, T = (wb + 63) / 64;
+    if ((a.mode != kConvFwd && a.mode != kConvTileFwd) || gw % 4 != 0 || a.Cout % 8 != 0 || a.Cout % gw != 0 ||
+        a.C != a.Cout || a.Cpad != T * 64 || a.ncols != a.R * a.S * T * 64 || a.ldw != a.R * a.S * gw)
       return cudaErrorInvalidValue;
+    co_tiles = (a.Cout + wb - 1) / wb * T;
   }
   if (a.mode == kConvTileFwd || a.mode == kConvStemTma) {
     if (a.tw * a.th * a.tn > 64 || a.tw < 1 || a.th < 1 || a.tn < 1) return cudaErrorInvalidValue;
@@ -1485,7 +1528,7 @@ cudaError_t launch_conv_wgrad(const WgradArgs& a_in, const void* dy, const void*
   // narrow outputs (the last 128-channel tile would be at most half full): swap operand roles, 64-channel tiles
   const int co_rem = a.Cout % 128;
   const bool swap = a.group_width != 0 || (g_wgrad_swap && co_rem > 0 && co_rem <= 64);   // grouped: 64-wide tiles
-  dim3 grid((a.ncols + 127) / 128, swap ? (a.Cout + 63) / 64 : (a.Cout + 127) / 128, splits);
+  dim3 grid((a.ncols + 127) / 128, co_tiles ? co_tiles : (swap ? (a.Cout + 63) / 64 : (a.Cout + 127) / 128), splits);
   static bool configured[16] = {};
 #define DDL_WG(MODE)                                                                                          \
   do {                                                                                                        \
@@ -1510,33 +1553,40 @@ cudaError_t launch_conv_wgrad(const WgradArgs& a_in, const void* dy, const void*
   return cudaGetLastError();
 }
 
-// Expanded grouped weights: compact w[co][tap * gw + j] (KRSC of a [Cout, gw, R, S] weight) -> [Cout][taps * 64] with
-// row co holding its gw input channels of each tap at columns tap * 64 + (co % 64 - co % gw) + j and zeros elsewhere:
-// the B operand of the block-diagonal 64-channel tiles.  One thread per 8 output columns (one 16-byte store).
+// Expanded grouped weights: compact w[co][tap * gw + j] (KRSC of a [Cout, gw, R, S] weight) -> the bundle operand
+// [nbundles * T * 64][taps * T * 64] of the grouped tiles (ConvArgs::grouped: bundles of wb channels, T = ceil(wb / 64)).
+// Row b*T*64 + l (l < wb: output channel co = b*wb + l < Cout) holds co's gw input channels of each tap at columns
+// tap * T * 64 + (l - l % gw) + j; everything else is zero, rows l >= wb included, so that the data gradient's K
+// overhang past a bundle meets zero rows.  At wb = 64 this is [Cout][taps * 64] with columns tap * 64 + (co % 64 -
+// co % gw) + j.  One thread per 8 output columns (one 16-byte store).
 __global__ void expand_grouped_weight_kernel(const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ out,
-                                             int cout, int taps, int gw) {
+                                             int cout, int taps, int gw, int wb, int T, int rows) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int vec_per_row = taps * 8;
-  if (i >= static_cast<long long>(cout) * vec_per_row) return;
-  const int co = static_cast<int>(i / vec_per_row);
-  const int v = static_cast<int>(i - static_cast<long long>(co) * vec_per_row);
-  const int tap = v >> 3, c0 = (v & 7) * 8;             // first of the 8 columns inside the tap's 64
-  const int g0 = (co & 63) - (co & 63) % gw;             // first column of co's group inside the tap
+  const int vec_per_row = taps * T * 8;
+  if (i >= static_cast<long long>(rows) * vec_per_row) return;
+  const int row = static_cast<int>(i / vec_per_row);
+  const int v = static_cast<int>(i - static_cast<long long>(row) * vec_per_row);
+  const int l = row % (T * 64), co = row / (T * 64) * wb + l;
+  const int tap = v / (T * 8), c0 = (v - tap * T * 8) * 8;   // first of the 8 columns inside the tap's 64 T
+  const int g0 = l - l % gw;                                  // first column of co's group inside the tap
+  const bool live = l < wb && co < cout;
   __align__(16) __nv_bfloat16 vals[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int c = c0 + j - g0;
-    vals[j] = (c >= 0 && c < gw) ? w[static_cast<size_t>(co) * taps * gw + tap * gw + c] : __float2bfloat16(0.f);
+    vals[j] = (live && c >= 0 && c < gw) ? w[static_cast<size_t>(co) * taps * gw + tap * gw + c] : __float2bfloat16(0.f);
   }
-  *reinterpret_cast<uint4*>(out + static_cast<size_t>(co) * taps * 64 + tap * 64 + c0) =
+  *reinterpret_cast<uint4*>(out + static_cast<size_t>(row) * taps * T * 64 + tap * T * 64 + c0) =
       *reinterpret_cast<const uint4*>(vals);
 }
 
 cudaError_t launch_expand_grouped_weight(const void* w, void* out, int cout, int taps, int gw, cudaStream_t stream) {
-  if (cout <= 0 || taps <= 0 || gw <= 0 || 64 % gw != 0) return cudaErrorInvalidValue;
-  const long long n = static_cast<long long>(cout) * taps * 8;
+  if (cout <= 0 || taps <= 0 || gw <= 0 || cout % gw != 0 || (64 % gw != 0 && gw % 8 != 0)) return cudaErrorInvalidValue;
+  const int wb = gw < 64 ? 64 / gw * gw : gw, T = (wb + 63) / 64;
+  const int rows = (cout + wb - 1) / wb * T * 64;
+  const long long n = static_cast<long long>(rows) * taps * T * 8;
   expand_grouped_weight_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
-      static_cast<const __nv_bfloat16*>(w), static_cast<__nv_bfloat16*>(out), cout, taps, gw);
+      static_cast<const __nv_bfloat16*>(w), static_cast<__nv_bfloat16*>(out), cout, taps, gw, wb, T, rows);
   return cudaGetLastError();
 }
 

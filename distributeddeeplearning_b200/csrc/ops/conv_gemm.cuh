@@ -84,10 +84,12 @@ struct ConvArgs {
   // in the source map, which of the 4 source maps to read, and the weight tap index r*S+s
   int ntaps;
   signed char tap_dh[16], tap_dw[16], tap_map[16], tap_widx[16];
-  // grouped convolution (Cin = Cout, group width dividing 64): N tiles are 64 wide and block-diagonal.  The tile of
-  // channels [n0, n0 + 64) reads only source channels [n0, n0 + 64), one k-block per filter tap (KB = R*S taps,
-  // cchunks = 1), and the weights are the expanded matrix [Cout][R*S*64] (expand_grouped_weight): K-major with
-  // kstride = 64 in the forward, MN-major rows [n0, n0 + 64) x columns tap*64 in the data gradient.
+  // grouped convolution (Cin = Cout = C): 0 = dense, else the bundle width Wb.  A bundle is max(1, 64 / cg)
+  // consecutive groups (Wb channels) and spans T = ceil(Wb / 64) = cchunks N tiles of 64 and T k-blocks per filter tap
+  // (KB = R*S*T).  N tile nt (expanded row n0 = 64 nt) is slice t = nt % T of bundle b = nt / T: it writes channels
+  // [b*Wb + 64 t, min(b*Wb + 64 t + 64, (b + 1)*Wb, C)) and reads source channels b*Wb + [0, 64 T).  The weights are
+  // the expanded matrix [nbundles*T*64][R*S*T*64] (expand_grouped_weight), zero outside each bundle's groups: K-major
+  // with kstride = 64 T in the forward, MN-major rows (b*T + cc)*64 x columns (tap*T + t)*64 in the data gradient.
   int grouped;
 };
 
@@ -116,8 +118,9 @@ struct WgradArgs {
   int stages;
   int batch, tw, th, tn, tiles_w, tiles_h;   // tile mode: a pixel block is a tw x th x tn box (<= 64 pixels)
   int group_width;            // grouped convolution: input channels per group (0 = dense).  Tiles are 64 output
-                              //   channels x (tap, the same 64 input channels) (Cpad = 64); only the in-group entries
-                              //   are added, to dw column tap * group_width + ci % group_width
+                              //   channels (slice t of a bundle, see ConvArgs::grouped) x (tap, the bundle's 64 T input
+                              //   channels) (Cpad = 64 T); only the in-group entries are added, to dw column
+                              //   tap * group_width + ci % group_width
 };
 
 }  // namespace ddl

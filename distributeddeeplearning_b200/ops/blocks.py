@@ -14,6 +14,10 @@ produced exactly once.  It also trims Python/autograd overhead (1 node instead o
               dx = dgrad_1(dy_1) + (dres | dgrad_d(bn_bwd(dres)))          <- the '+' is the dgrad epilogue
     where dgrad_1 is a 1x1 conv, its epilogue also takes the previous block's bn_L sums over dx (``_Bn3Handoff``)
 
+An optional squeeze-excitation (RegNetY) sits between the last two layers: h_{L-1} <- h_{L-1} * sigmoid(fc2(relu(
+fc1(mean_hw(h_{L-1}))))).  The last dgrad then produces the gradient at the SE output, so it does not take BN_{L-1}'s
+reduction (that needs the gradient at the SE input, formed by ``se_apply``).
+
 Reference parity: the maths is exactly torchvision's BasicBlock/Bottleneck (SURVEY.md 2.7); this only changes how
 the backward is scheduled.
 """
@@ -25,6 +29,45 @@ import torch
 
 from . import native
 from .functional import CL, grad_buffer, notify_ready, run_wgrad, weight_bf16
+
+
+def _se_fwd(x, w1, b1, w2, b2):
+    """x * sigmoid(fc2(relu(fc1(mean_hw(x))))) on the squeeze-excitation kernels; fc1 / fc2 are the 1x1 convs
+    [C', C, 1, 1] / [C, C', 1, 1] with biases.  fc1's output h keeps C' rounded up to 64 columns (the pad is zero) and
+    is fc2's operand as it stands, against fc2's weight padded with zero columns to match (made here, so a captured
+    graph rebuilds it every replay).  Returns y and what :func:`_se_bwd` needs."""
+    w1b, w2b = weight_bf16(w1), weight_bf16(w2, stem=False)      # [C', C], [C, C']
+    pooled = native.global_avgpool_fwd(x)                         # [N, C]
+    h = native.linear_fwd(pooled, w1b, b1, relu=True)             # [N, C' rounded up to 64]
+    w2p = w2b if h.shape[1] == w2b.shape[1] else native.pad_cols_bf16(w2b, h.shape[1])
+    s = native.linear_fwd(h, w2p, b2)                             # [N, C rounded up to 64]: the gate logits
+    return native.se_scale(x, s, gate="sigmoid"), (x, pooled, h, s, w1b, w2p)
+
+
+def _se_bwd(dy, saved, w1, b1, w2, b2):
+    """Input gradient of :func:`_se_fwd` (both paths in one ``se_apply`` pass); accumulates the fc1 / fc2 gradients of
+    the parameters that need them."""
+    x, pooled, h, s, w1b, w2p = saved
+    cs, c = w1.shape[0], w1.shape[1]
+    ds = native.se_reduce(dy, x, s, gate="sigmoid")               # [N, C rounded up to 64], pad columns 0
+    if b2.requires_grad:
+        native.bias_relu_bwd(ds, ds, grad_buffer(b2), False, c_valid=c)
+    dh = native.linear_dgrad(ds, w2p)                             # [N, C' rounded up to 64], pad columns 0
+    if w2.requires_grad:
+        if w2p.shape[1] == cs:
+            native.linear_wgrad(h, ds, grad_buffer(w2))
+        else:
+            gw = native.zeros_f32((c, w2p.shape[1]), ds.device)
+            native.linear_wgrad(h, ds, gw)
+            native.fold_cols_f32(gw, grad_buffer(w2))
+    dh = native.bias_relu_bwd(dh, h, grad_buffer(b1) if b1.requires_grad else None, True, c_valid=cs)
+    dx = native.se_apply(dy, s, native.linear_dgrad(dh, w1b), gate="sigmoid")
+    if w1.requires_grad:
+        native.linear_wgrad(pooled, dh, grad_buffer(w1))
+    for p in (b2, w2, b1, w1):
+        if p.requires_grad:
+            notify_ready(p)
+    return dx
 
 
 class _Bn3Handoff:
@@ -54,9 +97,12 @@ class _ResidualBlock(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, cfg, *params):
         """cfg: tuple of per-layer (stride, pad, dil, eps, momentum) for the L main convs [+ downsample last];
-        params: per layer (weight, gamma, beta, running_mean, running_var), downsample (if any) last."""
+        params: per layer (weight, gamma, beta, running_mean, running_var), downsample (if any) last, then the SE's
+        (fc1 weight, fc1 bias, fc2 weight, fc2 bias) if ``cfg["has_se"]``."""
         n_main, has_ds = cfg["n_main"], cfg["has_ds"]
         layers = [params[5 * i: 5 * i + 5] for i in range(n_main + (1 if has_ds else 0))]
+        se = params[5 * len(layers):] if cfg["has_se"] else None
+        se_saved = None
         saved = []
         wbs = []
         h = x
@@ -83,6 +129,8 @@ class _ResidualBlock(torch.autograd.Function):
                 cfg["bn3_out"].bn = (y, save, g, b, zmask)
             else:
                 z, save = native.bn_act_fwd(y, stats, g, b, rm, rv, eps, mom, True, None, True)
+                if se is not None and i == n_main - 2:
+                    z, se_saved = _se_fwd(z, *se)
             saved += [h, y, save]
             wbs.append(wb)
             h = z
@@ -90,6 +138,7 @@ class _ResidualBlock(torch.autograd.Function):
         ctx.layers = layers
         ctx.wbs = wbs
         ctx.ds_pack = ds_pack if has_ds else None
+        ctx.se = (se, se_saved) if se is not None else None
         ctx.save_for_backward(x, zmask, *saved)
         return h
 
@@ -134,11 +183,14 @@ class _ResidualBlock(torch.autograd.Function):
                 # in its epilogue (it holds the gradient tile anyway and only has to read the y tile, which it fetches
                 # while its MMAs run): BN_{i-1}'s backward is then one pass over (d_{i-1}, y) instead of two
                 gp, bp = layers[i - 1][1], layers[i - 1][2]
-                fuse = groups == 1 and native.dgrad_fuses_bn_reduce(kernel, st, pad)
+                se_here = ctx.se is not None and i == n_main - 1     # d is then the gradient at the SE output
+                fuse = groups == 1 and not se_here and native.dgrad_fuses_bn_reduce(kernel, st, pad)
                 pre = native.zeros_f32((2, h_in.shape[1]), h_in.device) if fuse else None
                 d = native.conv_dgrad(dy, ctx.wbs[i], h_in.shape, kernel, st, pad, dil,
                                       bn_reduce=(saved[3 * (i - 1) + 1], gp, bp, saved[3 * (i - 1) + 2], pre)
                                       if fuse else None, groups=groups)
+                if se_here:
+                    d = _se_bwd(d, ctx.se[1], *ctx.se[0])
             elif need_dx:
                 add = dres
                 if has_ds:
@@ -195,12 +247,14 @@ class _ResidualBlock(torch.autograd.Function):
             for p in (gd, bd, wd):
                 if p.requires_grad:
                     notify_ready(p)
-        return (dx, None) + (None,) * (5 * len(layers))
+        return (dx, None) + (None,) * (5 * len(layers) + (4 if ctx.se is not None else 0))
 
 
-def residual_block_supported(x: torch.Tensor, convs: Sequence, bns: Sequence, downsample) -> bool:
+def residual_block_supported(x: torch.Tensor, convs: Sequence, bns: Sequence, downsample, se=None) -> bool:
     from .functional import use_native
 
+    if se is not None and (len(convs) < 2 or se.fc1.weight.shape[1] != convs[-2].out_channels):
+        return False
     if not use_native(x) or not torch.is_grad_enabled():
         return False
     mods = list(zip(convs, bns)) + ([tuple(downsample)] if downsample is not None else [])
@@ -211,7 +265,7 @@ def residual_block_supported(x: torch.Tensor, convs: Sequence, bns: Sequence, do
         if not native.supports_conv(conv.in_channels, conv.out_channels) or not native.bn_supported(conv.out_channels):
             return False
         groups = getattr(conv, "groups", 1)
-        if groups > 1 and (not native.supports_grouped(conv.in_channels, conv.out_channels, groups) or
+        if groups > 1 and (not native.grouped_conv_native(conv.in_channels, conv.out_channels, groups) or
                            (downsample is not None and conv is downsample[0])):     # main-path convs only
             return False
         if conv.in_channels <= 4 or not conv.weight.is_contiguous(memory_format=CL) and conv.weight.dim() == 4 and \
@@ -220,19 +274,23 @@ def residual_block_supported(x: torch.Tensor, convs: Sequence, bns: Sequence, do
     return cin % 8 == 0
 
 
-def residual_block(x: torch.Tensor, convs: Sequence, bns: Sequence, downsample=None) -> torch.Tensor:
+def residual_block(x: torch.Tensor, convs: Sequence, bns: Sequence, downsample=None, se=None) -> torch.Tensor:
     """convs/bns: the main-path layer containers (``models.layers.Conv2d`` / ``BatchNorm2d``) in order;
-    downsample: optional (conv, bn) pair of the projection shortcut."""
+    downsample: optional (conv, bn) pair of the projection shortcut; se: optional squeeze-excitation with ``fc1`` /
+    ``fc2`` 1x1 convs (with biases), a ReLU inner activation and a sigmoid gate, applied to the input of the last conv
+    (torchvision's RegNetY ``SqueezeExcitation``)."""
     mods = list(zip(convs, bns)) + ([tuple(downsample)] if downsample is not None else [])
     # a block output carries its BN3 handoff; the first block to consume it takes it (a second consumer finds none)
     prev = x.__dict__.pop("_ddl_bn3", None)
     cfg = {"n_main": len(convs), "has_ds": downsample is not None,
            "layers": [(c.stride, c.padding, c.dilation, b.eps, b.momentum) for c, b in mods],
-           "groups": [getattr(c, "groups", 1) for c, _ in mods],
+           "groups": [getattr(c, "groups", 1) for c, _ in mods], "has_se": se is not None,
            "bn3_in": prev, "bn3_out": _Bn3Handoff()}
     params = []
     for c, b in mods:
         params += [c.weight, b.weight, b.bias, b.running_mean, b.running_var]
+    if se is not None:
+        params += [se.fc1.weight, se.fc1.bias, se.fc2.weight, se.fc2.bias]
     out = _ResidualBlock.apply(x, cfg, *params)
     out._ddl_bn3 = cfg["bn3_out"]
     return out

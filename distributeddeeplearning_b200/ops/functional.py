@@ -223,7 +223,7 @@ def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad
                 sample_scale=None, gelu=False):
     """z = act(BN(conv(x, weight)) [+ residual])  — the unit every ResNet/Inception layer is made of.  ``groups`` > 1:
     grouped convolution (``weight`` is [Cout, Cin/groups, R, S]); depthwise shapes that ``native.supports_depthwise`` (3x3)
-    or ``native.supports_depthwise5`` (5x5) accept run on the depthwise kernels, other shapes outside ``native.supports_grouped`` take the composite path.
+    or ``native.supports_depthwise5`` (5x5) accept run on the depthwise kernels, other shapes outside ``native.grouped_conv_native`` take the composite path.
     ``relu6``: the activation is ReLU6 (clamp to [0, 6]) instead of ``relu``; ``hardswish``: it is hardswish
     (v * clamp(v + 3, 0, 6) / 6), which takes no ``residual``; ``silu``: it is SiLU (v * sigmoid(v)), which takes no
     ``residual`` either; ``gelu``: it is GELU (v * Phi(v), the erf form), with the same restriction.  ``sample_scale``: fp32 [N] per-sample scales of stochastic depth (``stochastic_depth_keep``):
@@ -251,7 +251,7 @@ def conv_bn_act(x, weight, gamma, beta, running_mean, running_var, stride=1, pad
         return _DwConvBnAct.apply(x, residual, weight, gamma, beta, running_mean, running_var, stride, eps, momentum,
                                   act, training)
     if use_native(x) and native.supports_conv(x.shape[1], weight.shape[0]) \
-            and (groups == 1 or native.supports_grouped(x.shape[1], weight.shape[0], groups)) \
+            and (groups == 1 or native.grouped_conv_native(x.shape[1], weight.shape[0], groups)) \
             and native.bn_supported(weight.shape[0]) and _krsc(weight):
         return _ConvBnAct.apply(x, residual, weight, gamma, beta, running_mean, running_var, stride, pad, dil, eps,
                                 momentum, act, training, groups)
@@ -655,6 +655,12 @@ def squeeze_excite(x, w1, b1, w2, b2, gate="hardsigmoid", act="relu"):
     if native_act and cs % 8 == 0:
         train = torch.is_grad_enabled() and any(t.requires_grad for t in (x, w1, b1, w2, b2))
         return _SqueezeExcite.apply(x, w1, b1, w2, b2, train)
+    return squeeze_excite_composite(x, w1, b1, w2, b2, gate, act)
+
+
+def squeeze_excite_composite(x, w1, b1, w2, b2, gate, act):
+    """The torch composite of :func:`squeeze_excite` for any (gate, act) pair: the CPU path and, for RegNetY's
+    (sigmoid, relu) unit, the path of a residual block outside the native node."""
     dt = x.dtype if x.is_cuda else w1.dtype
     xi = x.to(dt)
     sc = xi.float().mean((2, 3), keepdim=True).to(dt) if x.is_cuda else xi.mean((2, 3), keepdim=True)

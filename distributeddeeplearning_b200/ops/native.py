@@ -340,15 +340,39 @@ def supports_conv(cin: int, cout: int) -> bool:
 
 
 def supports_grouped(cin: int, cout: int, groups: int) -> bool:
-    """Grouped convolutions the block-diagonal kernels handle: ``cin == cout``, a multiple of 64, split into groups whose
-    width divides 64 (a 64-channel tile then holds whole groups) and is a multiple of 4 (each 16-byte weight-gradient
-    vector lies in one group).  Other grouped shapes (depthwise among them) take the composite path."""
+    """The whole-groups-per-tile subset of the grouped convolutions: ``cin == cout``, a multiple of 64, split into groups
+    whose width divides 64 (a 64-channel tile then holds whole groups) and is a multiple of 4 (each 16-byte
+    weight-gradient vector lies in one group).  :func:`grouped_conv_native` is what the kernels take."""
     if groups <= 1:
         return supports_conv(cin, cout)
     if cin != cout or cin % groups != 0 or cin % 64 != 0:
         return False
     cg = cin // groups
     return 64 % cg == 0 and cg % 4 == 0
+
+
+def grouped_conv_native(cin: int, cout: int, groups: int) -> bool:
+    """Grouped convolutions (``groups`` > 1) the conv kernels run natively: :func:`supports_grouped`, or ``cin == cout``
+    a multiple of 8 in groups of a width ``cg`` that is a multiple of 8 (group bundles, :func:`grouped_bundle`).
+    Depthwise convolutions (``cg == 1``) are not among them; other shapes take the composite path."""
+    if groups <= 1:
+        return False
+    if supports_grouped(cin, cout, groups):
+        return True
+    return cin == cout and cin % groups == 0 and cin % 8 == 0 and (cin // groups) % 8 == 0
+
+
+def grouped_bundle(cg: int) -> Tuple[int, int]:
+    """(Wb, T) of the grouped kernels for group width ``cg``: a bundle is ``max(1, 64 // cg)`` consecutive groups, Wb
+    channels wide, and spans T = ceil(Wb / 64) N tiles of 64 channels and T k-blocks of 64 channels per filter tap."""
+    wb = max(1, 64 // cg) * cg
+    return wb, _ceil_div(wb, 64)
+
+
+def grouped_expanded_shape(c: int, taps: int, groups: int) -> Tuple[int, int]:
+    """Shape [nbundles * T * 64, taps * T * 64] of :func:`expand_grouped_weight`'s result."""
+    wb, t = grouped_bundle(c // groups)
+    return _ceil_div(c, wb) * t * 64, taps * t * 64
 
 
 def _depthwise_ok(k_want: int, c: int, kernel, stride: int, pad, dil: int, groups: int) -> bool:
@@ -1246,37 +1270,60 @@ def tanh_rows_bwd(dy: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
 
 
 def expand_grouped_weight(w_bf16: torch.Tensor, taps: int, groups: int) -> torch.Tensor:
-    """Compact grouped weights ``[Cout, taps * cg]`` bf16 (KRSC of ``[Cout, cg, R, S]``) -> the block-diagonal operand
-    ``[Cout, taps * 64]`` of the grouped kernels: row ``co`` holds its ``cg`` input channels of each tap at columns
-    ``tap * 64 + (co % 64 - co % cg) + j``, zeros elsewhere.  Made once per step, in forward (so that a captured graph
-    re-derives it from the weights every replay), and kept for that step's data gradient."""
+    """Compact grouped weights ``[Cout, taps * cg]`` bf16 (KRSC of ``[Cout, cg, R, S]``) -> the operand of the grouped
+    kernels, laid out per group bundle (:func:`grouped_bundle`: Wb channels, T tiles):
+    ``[nbundles * T * 64, taps * T * 64]``.  Row ``b * T * 64 + l`` (``l < Wb``) belongs to output channel
+    ``co = b * Wb + l`` and holds its ``cg`` input channels of each tap at columns ``tap * T * 64 + (l - l % cg) + j``;
+    everything else is zero, including the rows ``l >= Wb`` that the data gradient's K overhang reads.  At Wb = 64 this
+    is ``[Cout, taps * 64]`` with columns ``tap * 64 + (co % 64 - co % cg) + j``.  Made once per step, in forward (so
+    that a captured graph re-derives it from the weights every replay), and kept for that step's data gradient."""
     cout = w_bf16.shape[0]
     cg = cout // groups
     if w_bf16.dtype != torch.bfloat16 or w_bf16.numel() != cout * taps * cg or not w_bf16.is_contiguous():
         raise ValueError("expand_grouped_weight: expected contiguous bf16 [Cout, taps * Cout / groups] weights")
-    out = torch.empty((cout, taps * 64), dtype=torch.bfloat16, device=w_bf16.device)
+    out = torch.empty(grouped_expanded_shape(cout, taps, groups), dtype=torch.bfloat16, device=w_bf16.device)
     _C().expand_grouped_weight(w_bf16.data_ptr(), out.data_ptr(), cout, taps, cg, _stream())
     return out
 
 
+def expand_grouped_weight_ref(w: torch.Tensor, taps: int, groups: int) -> torch.Tensor:
+    """Torch twin of :func:`expand_grouped_weight` (any device and dtype), index by index from the bundle layout: the
+    reference the kernel is checked against."""
+    cout = w.shape[0]
+    cg = cout // groups
+    wb, t = grouped_bundle(cg)
+    out = w.new_zeros(grouped_expanded_shape(cout, taps, groups))
+    wc = w.reshape(cout, taps, cg)
+    co = torch.arange(cout, device=w.device)
+    l = co % wb                                       # position in the bundle
+    row = co // wb * t * 64 + l
+    col0 = l - l % cg                                 # first column of co's group inside a tap's 64 T
+    for tap in range(taps):
+        for j in range(cg):
+            out[row, tap * t * 64 + col0 + j] = wc[:, tap, j]
+    return out
+
+
 def _check_grouped(cin: int, cout: int, groups: int, w_bf16: torch.Tensor, taps: int) -> None:
-    if not supports_grouped(cin, cout, groups):
+    if not grouped_conv_native(cin, cout, groups):
         raise ValueError(f"grouped conv {cin} -> {cout} in {groups} groups is not supported by the native kernels")
-    if tuple(w_bf16.shape) != (cout, taps * 64):
-        raise ValueError("grouped conv: pass the expanded weights of expand_grouped_weight ([Cout, R*S*64])")
+    if tuple(w_bf16.shape) != grouped_expanded_shape(cout, taps, groups):
+        raise ValueError("grouped conv: pass the expanded weights of expand_grouped_weight")
 
 
 def _conv_grouped(mode: int, src: torch.Tensor, out: torch.Tensor, w_bf16: torch.Tensor, C: int, M: int, srcHW, dstHW,
-                  kernel, stride: int, ph: int, pw: int, dil: int, s_ptr: int = 0, ss_ptr: int = 0, batch: int = 0,
-                  tile=(0, 0, 0), zfill: int = 0, variant: int = 0) -> None:
-    """One launch of the block-diagonal grouped kernels (forward: tile / gather fwd; data gradient: tile / gather dgrad)
-    with one 64-channel k-block per tap."""
+                  kernel, stride: int, ph: int, pw: int, dil: int, groups: int, s_ptr: int = 0, ss_ptr: int = 0,
+                  batch: int = 0, tile=(0, 0, 0), zfill: int = 0, variant: int = 0) -> None:
+    """One launch of the grouped kernels (forward: tile / gather fwd; data gradient: tile / gather dgrad) with T
+    64-channel k-blocks per tap (:func:`grouped_bundle`)."""
     R, S = kernel
+    wb, t = grouped_bundle(C // groups)
+    rows, cols = w_bf16.shape
     tma = mode in (_C().CONV_TILE_FWD, _C().CONV_TILE_DGRAD)
-    _C().conv_gemm(mode, 0 if tma else src.data_ptr(), out.data_ptr(), 0, 0, s_ptr, ss_ptr, M, R * S, C, srcHW[0],
-                   srcHW[1], C, dstHW[0], dstHW[1], R, S, stride, ph, dil, 1, 0, C, w_bf16.data_ptr(), C, R * S * 64, C,
+    _C().conv_gemm(mode, 0 if tma else src.data_ptr(), out.data_ptr(), 0, 0, s_ptr, ss_ptr, M, R * S * t, C, srcHW[0],
+                   srcHW[1], C, dstHW[0], dstHW[1], R, S, stride, ph, dil, t, 0, C, w_bf16.data_ptr(), rows, cols, rows,
                    src.data_ptr() if tma else 0, C if tma else 0, batch, tile[0], tile[1], tile[2], zfill, _stream(), pw,
-                   64, variant=variant, grouped=1)
+                   t * 64, variant=variant, grouped=wb)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1289,15 +1336,15 @@ def conv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, kernel: Tuple[int, int], str
     ``prepadded``: result of :func:`stem_prepare` for this (x, geometry) — skips the internal padding copy.
 
     ``w_bf16``: [Cout, R*S*Cin] bf16 (or the packed stem matrix [Cout, KB*64]); ``pad``: int or (pad_h, pad_w).
-    ``groups`` > 1: a grouped convolution (:func:`supports_grouped`); ``w_bf16`` is then the expanded
-    [Cout, R*S*64] matrix of :func:`expand_grouped_weight`; no bias / ReLU.
+    ``groups`` > 1: a grouped convolution (:func:`grouped_conv_native`); ``w_bf16`` is then the expanded matrix of
+    :func:`expand_grouped_weight`; no bias / ReLU.
     """
     C = _C()
     _check_act(x)
     N, Cin, H, W = x.shape
     R, S = kernel
     ph, pw = _pad2(pad)
-    Cout = cout if cout is not None else w_bf16.shape[0]
+    Cout = cout if cout is not None else (Cin if groups > 1 else w_bf16.shape[0])   # grouped: Cin = Cout
     if Cout % 8 != 0:
         raise ValueError("conv_fwd: Cout must be a multiple of 8")
     P, Q = conv_out_hw(H, W, kernel, stride, (ph, pw), dil)
@@ -1309,12 +1356,13 @@ def conv_fwd(x: torch.Tensor, w_bf16: torch.Tensor, kernel: Tuple[int, int], str
         _check_grouped(Cin, Cout, groups, w_bf16, R * S)
         if bias is not None or relu:
             raise ValueError("conv_fwd: grouped convolutions take no bias / ReLU epilogue")
-        geo = dict(srcHW=(H, W), dstHW=(P, Q), kernel=kernel, stride=stride, ph=ph, pw=pw, dil=dil, s_ptr=s_ptr,
-                   ss_ptr=ss_ptr, batch=N)
+        geo = dict(srcHW=(H, W), dstHW=(P, Q), kernel=kernel, stride=stride, ph=ph, pw=pw, dil=dil, groups=groups,
+                   s_ptr=s_ptr, ss_ptr=ss_ptr, batch=N)
         if USE_TILE_TMA and (stride == 1 or (stride == 2 and R * S <= 16 and USE_TILE_S2)):
             tile = tile_geometry(P, Q, N, 128)
+            t = grouped_bundle(Cin // groups)[1]
             _tuned(("fwd_g", N, H, W, Cin, Cout, R, S, stride, ph, pw, dil, stats, groups),
-                   conv_variants(Cout, M, R * S, False, grouped=True),
+                   conv_variants(w_bf16.shape[0], M, R * S * t, False, grouped=True),
                    lambda v: _conv_grouped(C.CONV_TILE_FWD, x, y, w_bf16, Cout, M, tile=tile, variant=v, **geo),
                    (st,) if stats else ())
         else:
@@ -1401,7 +1449,7 @@ def conv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, kernel: Tuple[in
                dil: int = 1, add: Optional[torch.Tensor] = None, add_mask: Optional[torch.Tensor] = None,
                bn_reduce: Optional[tuple] = None, groups: int = 1) -> torch.Tensor:
     """dx = conv_transpose(dy, w) (+ add [gated by the bit mask ``add_mask``: uint8 [M, Cin/8]]).
-    ``w_bf16`` is the forward matrix [Cout, R*S*Cin] (``groups`` > 1: the expanded [Cout, R*S*64] matrix of the forward).
+    ``w_bf16`` is the forward matrix [Cout, R*S*Cin] (``groups`` > 1: the forward's :func:`expand_grouped_weight`).
 
     ``bn_reduce = (y, gamma, beta, save, scratch[, zmask])``: dx is the output gradient of a BN+ReLU layer whose saved
     input is ``y``; the kernel's epilogue then also accumulates that BN's dbeta / dgamma sums into ``scratch`` (fp32
@@ -1430,22 +1478,24 @@ def conv_dgrad(dy: torch.Tensor, w_bf16: torch.Tensor, x_shape, kernel: Tuple[in
         elif R < 2 or S < 2 or not (covered_h and covered_w):
             dx.zero_()
     if groups > 1:
-        # block-diagonal tiles: the N tile of input channels [n0, n0 + 64) reads dy channels [n0, n0 + 64) and the
-        # expanded weights MN-major; the shortcut add and the BN-backward reduction are not fused here
+        # group bundles: an N tile of input channels of a bundle reads that bundle's dy channels and the expanded
+        # weights MN-major; the shortcut add and the BN-backward reduction are not fused here
         _check_grouped(Cin, Cout, groups, w_bf16, R * S)
         if add is not None or add_mask is not None or bn_reduce is not None:
             raise ValueError("conv_dgrad: grouped convolutions take no add / add_mask / bn_reduce")
-        geo = dict(srcHW=(P, Q), dstHW=(H, W), kernel=kernel, stride=stride, ph=ph, pw=pw, dil=dil, batch=N)
+        geo = dict(srcHW=(P, Q), dstHW=(H, W), kernel=kernel, stride=stride, ph=ph, pw=pw, dil=dil, groups=groups,
+                   batch=N)
+        nt, t = w_bf16.shape[0], grouped_bundle(Cin // groups)[1]
         if stride == 1 and USE_TILE_TMA:
             tile = tile_geometry(H, W, N, 128)
             _tuned(("dgrad_g", N, H, W, Cin, Cout, R, S, 1, ph, pw, dil, groups),
-                   conv_variants(Cin, N * H * W, R * S, True, grouped=True),
+                   conv_variants(nt, N * H * W, R * S * t, True, grouped=True),
                    lambda v: _conv_grouped(C.CONV_TILE_DGRAD, dy, dx, w_bf16, Cin, N * H * W, tile=tile, variant=v,
                                            **geo))
         elif s2_tile:
             tile = tile_geometry((H + 1) // 2, (W + 1) // 2, N, 128)
             _tuned(("dgrad_s2_g", N, H, W, Cin, Cout, R, S, 2, ph, pw, dil, zfill, groups),
-                   conv_variants(Cin, N * ((H + 1) // 2) * ((W + 1) // 2), max(1, (R * S) // 4), True, grouped=True),
+                   conv_variants(nt, N * ((H + 1) // 2) * ((W + 1) // 2), max(1, (R * S * t) // 4), True, grouped=True),
                    lambda v: _conv_grouped(C.CONV_TILE_DGRAD, dy, dx, w_bf16, Cin, N * H * W, tile=tile, zfill=zfill,
                                            variant=v, **geo))
         else:
@@ -1570,21 +1620,23 @@ def conv_wgrad(x: torch.Tensor, dy: torch.Tensor, grad_w: torch.Tensor, kernel: 
     if grad_w.dtype != torch.float32:
         raise TypeError("grad_w must be fp32")
     if groups > 1:
-        # tiles of 64 output channels x (tap, the same 64 input channels); the epilogue adds the in-group entries
-        if not supports_grouped(Cin, Cout, groups):
+        # tiles of 64 output channels of a bundle x (tap, the bundle's 64 T input channels); the epilogue adds the
+        # in-group entries
+        if not grouped_conv_native(Cin, Cout, groups):
             raise ValueError(f"grouped conv {Cin} -> {Cout} in {groups} groups is not supported by the native kernels")
         cg = Cin // groups
         if grad_w.numel() != Cout * R * S * cg:
             raise ValueError("conv_wgrad: grad_w does not match the grouped weight [Cout, Cin/groups, R, S]")
-        ncols = R * S * 64
+        wb, t = grouped_bundle(cg)
+        ncols = R * S * t * 64
         if USE_TILE_TMA and (stride == 1 or (stride == 2 and USE_TILE_S2)):
             mode, (tw, th, tn) = C.CONV_TILE_FWD, tile_geometry(P, Q, N, 64)
             total_kb = -(-Q // tw) * -(-P // th) * -(-N // tn)
         else:
             mode, (tw, th, tn), total_kb = C.CONV_FWD, (0, 0, 0), (M + 63) // 64
-        splits = _wgrad_splits(((ncols + 127) // 128) * (Cout // 64), total_kb, dev)
+        splits = _wgrad_splits(((ncols + 127) // 128) * (_ceil_div(Cout, wb) * t), total_kb, dev)
         C.conv_wgrad(mode, x.data_ptr(), dy.data_ptr(), grad_w.data_ptr(), M, Cout, Cout, R * S * cg, ncols, H, W, Cin,
-                     P, Q, R, S, stride, ph, dil, 0, splits, N, tw, th, tn, _stream(), pw, 64, cg, group_width=cg)
+                     P, Q, R, S, stride, ph, dil, 0, splits, N, tw, th, tn, _stream(), pw, t * 64, cg, group_width=cg)
         return
     if Cin <= 4:
         SP, RPK, KB, RP = stem_geometry(R, S)

@@ -1,0 +1,65 @@
+"""GPU tests (H100) of RegNetX / RegNetY and the group-bundle mode of the grouped conv kernels: the `regnet` group of
+tools/gpu_diag.py (one subprocess per run, as in test_grouped_gpu.py), its layer checks under the forced persistent /
+CTA-pair kernels, the `grouped` group's ResNeXt checks untouched, the benchmark entry point and the ImageNet trainer
+on regnet_y_400mf."""
+import json
+import os
+import subprocess
+import sys
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+pytestmark = pytest.mark.gpu
+
+
+def _group(name, timeout=1800, env=None):
+    e = dict(os.environ)
+    e.update(env or {})
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "gpu_diag.py"), "--group", name], cwd=ROOT,
+                       capture_output=True, text=True, timeout=timeout, env=e)
+    out = r.stdout + r.stderr
+    tail = "\n".join(l for l in out.splitlines() if "FAIL" in l or "Error" in l)[:3000] + "\n...\n" + out[-3000:]
+    assert r.returncode == 0, tail
+    assert "FAIL" not in r.stdout, tail
+
+
+def test_regnet_group():
+    """Default configuration: every grouped RegNet layer, the blocks, four models against torchvision, graph replay,
+    fp8 and regnet_y_128gf."""
+    _group("regnet")
+
+
+def test_regnet_layers_persistent_forced():
+    _group("regnet_layers", env={"DDL_CONV_PERSISTENT": "2", "DDL_CONV_DEEP": "0", "DDL_CONV_AUTOTUNE": "0"})
+
+
+def test_regnet_layers_cluster_pairs():
+    """CTA pairs forced wherever they apply (the grouped forward; MN-major 64-wide grouped data gradients have none)."""
+    _group("regnet_layers", env={"DDL_CONV_CLUSTER": "1", "DDL_CONV_PERSISTENT": "2"})
+
+
+def test_bench_regnet_y_400mf():
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--model", "regnet_y_400mf", "--steps", "3",
+                        "--warmup", "3", "--batch-size", "32"], cwd=ROOT, capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0, (r.stdout + r.stderr)[-3000:]
+    out = json.loads([l for l in r.stdout.splitlines() if l.startswith("{")][-1])
+    for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
+                "vs_baseline", "dtype", "data", "config", "clocks", "e2e", "gpu_launches"):
+        assert key in out, key
+    assert out["value"] > 0 and out["gpu_launches"] > 0 and out["e2e"]["value"] > 0
+
+
+def test_imagenet_trainer_regnet_y_400mf(tmp_path):
+    sys.path.insert(0, ROOT)
+    import io
+
+    from distributeddeeplearning_b200.cli import launcher
+
+    out, err = io.StringIO(), io.StringIO()
+    res = launcher.launch("distributeddeeplearning_b200.workloads.imagenet",
+                          ["--epochs", "1", "--batch_size", "16", "--model", "regnet_y_400mf",
+                           "--save_filepath", str(tmp_path / "ck-{epoch}.pt")], gpus=1, record=False, stdout=out,
+                          stderr=err, timeout=900, env={"PYTHONPATH": ROOT, "FAKE_DATA_LENGTH": "64"})
+    assert res.returncode == 0, (out.getvalue() + err.getvalue())[-3000:]
+    assert "Training epoch 0 took" in out.getvalue()

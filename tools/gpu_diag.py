@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "swin", "swin_v2", "maxvit", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -1417,17 +1417,22 @@ def _rx(inp, planes, stride=1, proj=False, groups=32, width=4):
     return Bottleneck(inp, planes, stride, ds, groups, width)
 
 
-def _model_vs_torchvision(name, bs, hooks_on=None):
+def _model_vs_torchvision(name, bs, hooks_on=None, zero_init=None):
     """zero_init_residual model vs torchvision fp32 with the same weights (and this repo's bf16 composite): logits cosine
     and per-parameter gradient cosines, under g_model's bounds.  ``hooks_on``: module type whose forward outputs must
-    come from the native residual-block node."""
+    come from the native residual-block node.  ``zero_init``: for models without ``zero_init_residual``, a function
+    that zeroes their residual BN gammas instead."""
     import torch
     import torchvision
 
     from distributeddeeplearning_b200 import models, ops
 
     torch.manual_seed(0)
-    m = models.get_model(name, zero_init_residual=True).cuda().train()
+    if zero_init is None:
+        m = models.get_model(name, zero_init_residual=True).cuda().train()
+    else:
+        m = models.get_model(name).cuda().train()
+        zero_init(m)
     tv = getattr(torchvision.models, name)().cuda().train()
     tv.load_state_dict(m.state_dict())
     m2 = models.get_model(name).cuda().train()
@@ -4648,6 +4653,214 @@ def g_maxvit():
     torch.cuda.empty_cache()
     for kind, r in sorted(WORST.items()):
         print(f"worst ratio to budget: {kind:24s} {r:.3f}x", flush=True)
+
+
+def regnet_grouped_shapes(size=224):
+    from distributeddeeplearning_b200.models import regnet
+
+    return regnet.grouped_shapes(size=size)
+
+
+def _regnet_block(win, wout, stride, cg, se):
+    from distributeddeeplearning_b200.models.regnet import ResBottleneckBlock
+
+    return ResBottleneckBlock(win, wout, stride, cg, 0.25 if se else None)
+
+
+def _regnet_block_case(label, blk, xshape, frozen=()):
+    """One RegNet block on the native residual-block node against torchvision's ``ResBottleneckBlock`` in float64 with
+    the same weights: the output, the input gradient and every parameter gradient must have a cosine to float64 of at
+    least ``floor`` and no more than 0.01 below the repo's bf16 composite's (the float64 twin does not follow the bf16
+    ReLU ties, so element-wise budgets measure those flips, in both implementations alike); frozen parameters keep
+    ``grad is None``."""
+    import copy
+
+    import torch
+    from torchvision.models.regnet import ResBottleneckBlock as TvBlock
+
+    print(f"-- regnet block: {label}", flush=True)
+    blk = blk.cuda().train()
+    _randomize_bn([blk])
+    for n, p in blk.named_parameters():
+        if n in frozen:
+            p.requires_grad_(False)
+    comp = copy.deepcopy(blk)
+    f = blk.f
+    se = hasattr(f, "se")
+    tv = TvBlock(f.a[0].in_channels, f.c[0].out_channels, f.b[0].stride, torch.nn.BatchNorm2d,
+                 torch.nn.ReLU, f.b[0].in_channels // f.b[0].groups, 1.0, 0.25 if se else None)
+    tv.load_state_dict(blk.state_dict())
+    tv = tv.to(device="cuda", dtype=torch.float64).train()
+    for n, p in tv.named_parameters():
+        p.requires_grad_(n not in frozen)
+    x = cl(bf(torch.randn(*xshape, device="cuda")))
+    outs = {}
+    for impl, m in (("native", blk), ("torch", comp)):
+        os.environ["DDL_B200_IMPL"] = impl
+        try:
+            xin = x.clone().requires_grad_(True)
+            o = m(xin)
+            if impl == "native":
+                RESULTS.append(type(o.grad_fn).__name__ == "_ResidualBlockBackward")
+                print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] native residual_block node: {type(o.grad_fn).__name__}")
+                g = cl(bf(torch.randn(o.shape, device="cuda")))
+            o.backward(g.to(o.dtype))
+            outs[impl] = (o, xin.grad)
+        finally:
+            os.environ["DDL_B200_IMPL"] = "native"
+    xr = x.double().requires_grad_(True)
+    orf = tv(xr)
+    orf.backward(g.double())
+    (on, dxn), (oc, dxc) = outs["native"], outs["torch"]
+
+    def check(name, got, comp_, ref, floor):
+        cn, cc = _cos(got, ref), _cos(comp_, ref)
+        RESULTS.append(cn >= floor and cn >= cc - 0.01)
+        print(f"[{'ok' if RESULTS[-1] else 'FAIL'}]    {label} {name:28s} cos(native, f64) {cn:.5f}  "
+              f"cos(bf16 composite, f64) {cc:.5f}", flush=True)
+
+    check("output", on, oc, orf, 0.999)
+    check("dx", dxn, dxc, xr.grad, 0.99)
+    pn, pc = dict(blk.named_parameters()), dict(comp.named_parameters())
+    for n, p in tv.named_parameters():
+        if n in frozen:
+            RESULTS.append(pn[n].grad is None and pc[n].grad is None)
+            print(f"[{'ok' if RESULTS[-1] else 'FAIL'}]    {n} frozen: grad stays None", flush=True)
+            continue
+        check(f"{n} grad", pn[n].grad, pc[n].grad, p.grad, 0.99)
+
+
+def _zero_regnet_final_bn(m):
+    import torch
+
+    with torch.no_grad():
+        for n, p in m.named_parameters():
+            if n.endswith("f.c.1.weight"):
+                p.zero_()
+
+
+def g_regnet_layers():
+    """The group-bundle mode of the grouped conv kernels on every RegNet grouped 3x3 layer, plus edge cases, and the
+    expanded operand against its torch twin."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    torch.manual_seed(0)
+    shapes = regnet_grouped_shapes()
+    RESULTS.append(len(shapes) == 101)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {len(shapes)} distinct RegNet grouped shapes at 224", flush=True)
+    # a 13x13 stride-2 map, C < 64, a partial last bundle, and cg = 264 with five k-blocks per tap
+    extra = [(96, 13, 2, 24), (48, 9, 1, 8), (48, 13, 2, 8), (72, 9, 1, 24), (72, 13, 2, 24), (528, 7, 1, 264),
+             (528, 13, 2, 264)]
+    for C, hw, stride, cg in shapes + extra:
+        _conv_layer(C, C, (3, 3), stride, (1, 1), hw, hw, 3 if hw <= 14 else 2, groups=C // cg)
+    for C, cg in [(c, g) for c, _, _, g in shapes] + [(72, 24), (48, 8), (528, 264)] + \
+            [(c, g) for c, _, _, g in GROUPED_SHAPES]:
+        w = bf(torch.randn(C, 9 * cg, device="cuda"))
+        got, ref = nv.expand_grouped_weight(w, 9, C // cg), nv.expand_grouped_weight_ref(w, 9, C // cg)
+        if not torch.equal(got, ref):
+            RESULTS.append(False)
+            print(f"[FAIL] expand_grouped_weight C={C} cg={cg} differs from its twin", flush=True)
+    RESULTS.append(all(tuple(nv.expand_grouped_weight(bf(torch.randn(C, 9 * cg, device="cuda")), 9, C // cg).shape)
+                       == (C, 9 * 64) for C, _, _, cg in GROUPED_SHAPES))
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] expand_grouped_weight bit-equal to its twin; ResNeXt shapes keep "
+          f"[Cout, taps * 64]", flush=True)
+    # residual blocks (M = 2*7*7 = 98 etc.: none a multiple of 128)
+    _regnet_block_case("X identity (C = 48, cg = 16)", _regnet_block(48, 48, 1, 16, False), (2, 48, 9, 9))
+    _regnet_block_case("X projection stride 2 (72, cg = 24)", _regnet_block(48, 72, 2, 24, False), (2, 48, 13, 13))
+    _regnet_block_case("Y, SE squeeze 12 (48 -> 48, cg = 8)", _regnet_block(48, 48, 1, 8, True), (2, 48, 9, 9))
+    _regnet_block_case("Y projection, cg = 232 (232 -> 464)", _regnet_block(232, 464, 2, 232, True), (2, 232, 13, 13))
+    _regnet_block_case("Y, frozen grouped weight and SE", _regnet_block(104, 104, 1, 8, True), (3, 104, 7, 7),
+                       frozen=("f.b.0.weight", "f.se.fc1.weight", "f.se.fc1.bias", "f.se.fc2.weight",
+                               "f.se.fc2.bias"))
+
+
+def g_regnet():
+    """RegNetX / RegNetY: g_regnet_layers, whole models against torchvision, CUDA-graph replay, an fp8 session and
+    one regnet_y_128gf training step."""
+    import torch
+
+    from distributeddeeplearning_b200.models.regnet import ResBottleneckBlock
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.ops import native as nv
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    g_regnet_layers()
+    for name in ("regnet_y_400mf", "regnet_x_1_6gf", "regnet_y_16gf", "regnet_x_32gf"):
+        _model_vs_torchvision(name, 16, ResBottleneckBlock, zero_init=_zero_regnet_final_bn)
+
+    dist.init()
+
+    def run(graph):
+        torch.manual_seed(0)
+        s = BenchmarkSession("regnet_y_400mf", 16, True, lr=0.01, momentum=0.9)
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out[-4:]
+
+    a, b = run(False), run(True)
+    ok = all(x == x for x in a + b) and all(abs(x - y) < 5e-2 * max(1.0, abs(x)) for x, y in zip(a, b))
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] regnet_y_400mf training: eager {[round(v, 4) for v in a]} "
+          f"graph replay {[round(v, 4) for v in b]}", flush=True)
+
+    # fp8: the 128-multiple dense layers take fp8; grouped and SE layers stay bf16
+    fp8.reset()
+    fp8.enable(True)
+    calls, se_fp8 = [], []
+    fwd, dgrad, lin = nv.conv_fwd, nv.conv_dgrad, nv.linear_fwd
+
+    def spy(fn, kind):
+        def f(*a, **k):
+            before = fp8.launches()[kind]
+            r = fn(*a, **k)
+            if k.get("groups", 1) > 1:
+                calls.append(fp8.launches()[kind] - before)
+            return r
+        return f
+
+    def spy_lin(*a, **k):
+        before = sum(fp8.launches().values())
+        r = lin(*a, **k)
+        se_fp8.append(sum(fp8.launches().values()) - before)
+        return r
+
+    nv.conv_fwd, nv.conv_dgrad, nv.linear_fwd = spy(fwd, "fwd"), spy(dgrad, "dgrad"), spy_lin
+    try:
+        torch.manual_seed(0)
+        s = BenchmarkSession("regnet_y_8gf", 16, True, lr=0.01, momentum=0.9)     # 896-channel stage: fp8
+        losses = [float(s.step()) for _ in range(3)]
+        torch.cuda.synchronize()
+    finally:
+        nv.conv_fwd, nv.conv_dgrad, nv.linear_fwd = fwd, dgrad, lin
+        fp8.enable(False)
+    n = fp8.launches()
+    ok = all(l == l for l in losses) and n["fwd"] > 0 and len(calls) > 0 and not any(calls) and not any(se_fp8)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] regnet_y_8gf fp8: losses {[round(v, 3) for v in losses]}, fp8 launches {n}, "
+          f"grouped launches {len(calls)} of which fp8 {sum(calls)}, SE/fc GEMMs in fp8 {sum(se_fp8)}", flush=True)
+    del s
+    torch.cuda.empty_cache()
+
+    # the largest model: one training step at a small batch
+    torch.cuda.reset_peak_memory_stats()
+    torch.manual_seed(0)
+    s = BenchmarkSession("regnet_y_128gf", 8, True, lr=0.01, momentum=0.9)
+    loss = float(s.step())
+    torch.cuda.synchronize()
+    s.optimizer.check_errors()
+    RESULTS.append(loss == loss)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] regnet_y_128gf batch 8 step: loss {loss:.4f}, peak memory "
+          f"{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB", flush=True)
 
 
 def run_group(name):

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Per-layer timing of the grouped 3x3 convolutions of ResNeXt-50 32x4d: native block-diagonal kernels (forward with
-BN statistics, data gradient, weight gradient, and the per-step weight expansion) against cuDNN's bf16 channels_last
-grouped convolution (torch.nn.functional.conv2d and its autograd backward), CUDA events, L2 flushed before every run.
+"""Per-layer timing of the grouped 3x3 convolutions of ResNeXt-50 32x4d (default) or of one RegNet (``--model
+regnet_*``: its distinct grouped layers at 224): native group-bundle kernels (forward with BN statistics, data
+gradient, weight gradient, and the per-step weight expansion) against cuDNN's bf16 channels_last grouped convolution
+(torch.nn.functional.conv2d and its autograd backward), CUDA events, L2 flushed before every run.
 
-    python tools/grouped_bench.py [--batch 256] [--iters 20]
+    python tools/grouped_bench.py [--model regnet_y_16gf] [--batch 256] [--iters 20]
 """
 import argparse
 import json
@@ -38,20 +39,26 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--model", default=None, help="a regnet_* name: time its grouped layers instead of ResNeXt-50's")
     a = ap.parse_args()
     import torch
     import torch.nn.functional as F
 
+    from distributeddeeplearning_b200.models import regnet
     from distributeddeeplearning_b200.ops import native as nv
+
+    if a.model is not None and a.model not in regnet._PARAMS:
+        ap.error(f"--model must be one of {sorted(regnet._PARAMS)}")
+    shapes = SHAPES if a.model is None else regnet.grouped_shapes(a.model)
 
     torch.backends.cudnn.benchmark = True
     dev = torch.device("cuda")
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    print(f"# {torch.cuda.get_device_name(0)}, batch {a.batch}, median of {a.iters} (us)")
+    print(f"# {torch.cuda.get_device_name(0)}, {a.model or 'resnext50_32x4d'}, batch {a.batch}, median of {a.iters} (us)")
     print(f"{'C':>5} {'HW':>3} {'s':>1} {'cg':>3} | {'fwd':>8} {'cudnn':>8} | {'dgrad':>8} {'cudnn':>8} | {'wgrad':>8} "
           f"{'cudnn':>8} | {'expand':>6}")
     rows = []
-    for C, hw, s, cg in SHAPES:
+    for C, hw, s, cg in shapes:
         g = C // cg
         x = torch.randn(a.batch, C, hw, hw, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
         w = (torch.randn(C, cg, 3, 3, device=dev) * 0.1).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
@@ -75,7 +82,8 @@ def main():
               f"{r['dgrad_cudnn']:8.1f} | {r['wgrad']:8.1f} {r['wgrad_cudnn']:8.1f} | {r['expand']:6.1f}", flush=True)
     tot = {k: sum(r[k] for r in rows) for k in ("fwd", "fwd_cudnn", "dgrad", "dgrad_cudnn", "wgrad", "wgrad_cudnn")}
     print("total  " + "  ".join(f"{k}={v:.0f}" for k, v in tot.items()))
-    print("JSON " + json.dumps({"device": torch.cuda.get_device_name(0), "batch": a.batch, "rows": rows}))
+    print("JSON " + json.dumps({"device": torch.cuda.get_device_name(0), "model": a.model or "resnext50_32x4d",
+                                "batch": a.batch, "rows": rows}))
 
 
 if __name__ == "__main__":
