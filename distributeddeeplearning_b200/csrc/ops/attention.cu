@@ -29,12 +29,15 @@
 
 #include "../common.cuh"
 #include "ops.h"
+#include "mma_tile.cuh"
 #include "tc_utils.cuh"
 #include "../launch.h"
 
 namespace ddl {
 
 namespace {
+
+using namespace mma_tile;
 
 constexpr int kD = 64;           // head dim
 constexpr int kTile = 64;        // rows per CTA and per streamed block
@@ -52,66 +55,6 @@ struct AttnArgs {
   float* delta;                  // [N][H][L]  (backward: D, written by the dQ kernel, read by the dK/dV kernel)
   int L, H, C;
 };
-
-DDL_DEVICE void mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-               "{%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-DDL_DEVICE void ldsm4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-DDL_DEVICE void ldsm4_t(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-
-// Lane addresses of the three ldmatrix forms on a [64][kLd] tile (lane l feeds row l % 8 of matrix l / 8):
-// A fragment of rows m0.., columns k0.. (row-major A)  and  B of a [k][n]-stored operand (trans): offsets ((i&1)*8, (i>>1)*8)
-DDL_DEVICE uint32_t lane_addr_a(uint32_t tile, int r0, int c0, int lane) {
-  const int i = lane >> 3, r = lane & 7;
-  return tile + static_cast<uint32_t>(((r0 + (i & 1) * 8 + r) * kLd + c0 + (i >> 1) * 8) * 2);
-}
-// B of an [n][k]-stored operand (non-trans): matrices (n0, k0), (n0, k0+8), (n0+8, k0), (n0+8, k0+8)
-DDL_DEVICE uint32_t lane_addr_bn(uint32_t tile, int n0, int k0, int lane) {
-  const int i = lane >> 3, r = lane & 7;
-  return tile + static_cast<uint32_t>(((n0 + (i >> 1) * 8 + r) * kLd + k0 + (i & 1) * 8) * 2);
-}
-
-// S[16 x 64] = A[16 x 64] * B^T with B a [64 rows = n][64 = k] tile (K in S = Q K^T, dO in dP^T = V dO^T, ...)
-DDL_DEVICE void mm_abt(float (&s)[8][4], const uint32_t (&a)[4][4], uint32_t tile, int lane) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-    for (int jp = 0; jp < 4; ++jp) {
-      uint32_t b[4];
-      ldsm4(lane_addr_bn(tile, 16 * jp, 16 * kk, lane), b);
-      mma_bf16(s[2 * jp], a[kk], b[0], b[1]);
-      mma_bf16(s[2 * jp + 1], a[kk], b[2], b[3]);
-    }
-  }
-}
-// acc[16 x 64] += P[16 x 64] * B with B a [64 rows = k][64 = n] tile (V in O += P V, K in dQ += dS K, ...); P given as
-// the accumulator-layout fp32 tile, rounded to bf16 here
-DDL_DEVICE void mm_pb(float (&acc)[8][4], const float (&p)[8][4], uint32_t tile, int lane) {
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-    const uint32_t a[4] = {pack_bf16x2(p[2 * kk][0], p[2 * kk][1]), pack_bf16x2(p[2 * kk][2], p[2 * kk][3]),
-                           pack_bf16x2(p[2 * kk + 1][0], p[2 * kk + 1][1]),
-                           pack_bf16x2(p[2 * kk + 1][2], p[2 * kk + 1][3])};
-#pragma unroll
-    for (int jp = 0; jp < 4; ++jp) {
-      uint32_t b[4];
-      ldsm4_t(lane_addr_a(tile, 16 * kk, 16 * jp, lane), b);
-      mma_bf16(acc[2 * jp], a, b[0], b[1]);
-      mma_bf16(acc[2 * jp + 1], a, b[2], b[3]);
-    }
-  }
-}
 
 // 64 rows x 64 bf16 of a row-major matrix (row stride ld) from row r0 (rows >= rows_valid are zero-filled) into a tile
 DDL_DEVICE void load_tile(uint32_t tile, const __nv_bfloat16* base, int ld, int r0, int col, int rows_valid, int tid) {
@@ -175,10 +118,10 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(AttnArgs a) {
     __syncthreads();
     if (kb == 0) {
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) ldsm4(lane_addr_a(q_s, 16 * warp, 16 * kk, lane), qf[kk]);
+      for (int kk = 0; kk < 4; ++kk) ldsm4(addr_a<kLd>(q_s, 16 * warp, 16 * kk, lane), qf[kk]);
     }
     float s[8][4];
-    mm_abt(s, qf, k_s + cur * kStage, lane);
+    mm_abt<kLd>(s, qf, k_s + cur * kStage, lane);
     const int key0 = kb * kTile + 2 * t;
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -211,7 +154,7 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(AttnArgs a) {
       }
       l[r] = l[r] * corr + ls;
     }
-    mm_pb(acc, s, v_s + cur * kStage, lane);
+    mm_pb<kLd>(acc, s, v_s + cur * kStage, lane);
     __syncthreads();                           // everyone is done with stage cur before it is refilled
   }
   const size_t head = (static_cast<size_t>(n) * a.H + h) * L;
@@ -294,8 +237,8 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(AttnArgs a) {
     }
     __syncthreads();                           // (also publishes sD on the first pass)
     float p[8][4], dp[8][4];
-    mm_abt(p, qf, k_s + cur * kStage, lane);
-    mm_abt(dp, df, v_s + cur * kStage, lane);
+    mm_abt<kLd>(p, qf, k_s + cur * kStage, lane);
+    mm_abt<kLd>(dp, df, v_s + cur * kStage, lane);
     const int key0 = kb * kTile + 2 * t;
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -310,7 +253,7 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(AttnArgs a) {
         }
       }
     }
-    mm_pb(dq, p, k_s + cur * kStage, lane);
+    mm_pb<kLd>(dq, p, k_s + cur * kStage, lane);
     __syncthreads();
   }
 #pragma unroll
@@ -365,7 +308,7 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(AttnArgs a) {
     }
     __syncthreads();
     float p[8][4];
-    mm_abt(p, kf, q_s + cur * kStage, lane);             // S^T = K Q^T
+    mm_abt<kLd>(p, kf, q_s + cur * kStage, lane);        // S^T = K Q^T
     const int qc0 = qb * kTile + 2 * t;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -375,15 +318,15 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(AttnArgs a) {
         p[j][i] = qc0 + 8 * j + (i & 1) < L ? exp2f(fmaf(p[j][i], sl2, -sL[cur][c])) : 0.f;
       }
     }
-    mm_pb(dv, p, o_s + cur * kStage, lane);              // dV += P^T dO
+    mm_pb<kLd>(dv, p, o_s + cur * kStage, lane);         // dV += P^T dO
     float dp[8][4];
-    mm_abt(dp, vf, o_s + cur * kStage, lane);            // dP^T = V dO^T
+    mm_abt<kLd>(dp, vf, o_s + cur * kStage, lane);       // dP^T = V dO^T
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) p[j][i] *= dp[j][i] - sD[cur][8 * j + 2 * t + (i & 1)];
     }
-    mm_pb(dk, p, q_s + cur * kStage, lane);              // dK += dS^T Q
+    mm_pb<kLd>(dk, p, q_s + cur * kStage, lane);         // dK += dS^T Q
     __syncthreads();
   }
 #pragma unroll

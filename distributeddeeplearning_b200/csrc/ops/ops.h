@@ -179,7 +179,7 @@ cudaError_t launch_window_attention_bwd(const __nv_bfloat16* qkv, const float* t
                                         cudaStream_t stream);
 size_t window_attention_bwd_scratch_floats(int N, int H, int heads);
 
-// ---- MaxViT: partition attention, 7 x 7 partitions, head dim 32 (grid_attention.cu) ----------------------------------
+// ---- MaxViT: partition attention, 7 x 7 partitions, head dim 32 (window_attention.cu) --------------------------------
 // qkv [N*H*W][3C] bf16 in image order (head h: Q, K, V at columns 32h, C + 32h, 2C + 32h), C = 32 heads, H = W a multiple
 // of 7.  grid: the 49 tokens of sequence (i, j) sit at pixels (a H/7 + i, b H/7 + j); else (the window partition) at
 // (7i + a, 7j + b).  forward: o [N*H*W][C] and lse [N*H*W][heads] fp32 with logits q . k * scale + table[169][heads].

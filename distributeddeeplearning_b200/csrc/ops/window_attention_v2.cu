@@ -39,12 +39,15 @@
 
 #include "../common.cuh"
 #include "ops.h"
+#include "mma_tile.cuh"
 #include "tc_utils.cuh"
 #include "../launch.h"
 
 namespace ddl {
 
 namespace {
+
+using namespace mma_tile;
 
 constexpr int kWin = 8;
 constexpr int kL = kWin * kWin;   // 64 tokens per window = the tile rows
@@ -83,89 +86,6 @@ struct BwdSmem {
   float d[kL], rq[kL], rk[kL], fq[kL], fk[kL];
   float bq[4][kD], bv[4][kD], dsc[4];
 };
-
-DDL_DEVICE void mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-               "{%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-DDL_DEVICE void ldsm4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-DDL_DEVICE void ldsm4_t(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-
-// lane addresses of ldmatrix on a tile of row stride LD (lane l feeds row l % 8 of matrix l / 8):
-// A fragment of rows m0.., columns k0.. (row-major A), and B of a [k][n]-stored operand (trans)
-template <int LD>
-DDL_DEVICE uint32_t addr_a(uint32_t tile, int r0, int c0, int lane) {
-  const int i = lane >> 3, r = lane & 7;
-  return tile + static_cast<uint32_t>(((r0 + (i & 1) * 8 + r) * LD + c0 + (i >> 1) * 8) * 2);
-}
-// B of an [n][k]-stored operand (non-trans)
-template <int LD>
-DDL_DEVICE uint32_t addr_bn(uint32_t tile, int n0, int k0, int lane) {
-  const int i = lane >> 3, r = lane & 7;
-  return tile + static_cast<uint32_t>(((n0 + (i >> 1) * 8 + r) * LD + k0 + (i & 1) * 8) * 2);
-}
-// A fragment of the transpose of a row-major [k][m] tile (trans): A rows m0.., columns k0..
-template <int LD>
-DDL_DEVICE uint32_t addr_at(uint32_t tile, int m0, int k0, int lane) {
-  const int i = lane >> 3, r = lane & 7;
-  return tile + static_cast<uint32_t>(((k0 + (i >> 1) * 8 + r) * LD + m0 + (i & 1) * 8) * 2);
-}
-
-// S[16 x 64] = A[16 x 32] B^T with B a [64 = n][32 = k] tile of stride kLd
-DDL_DEVICE void mm_abt(float (&s)[8][4], const uint32_t (&a)[2][4], uint32_t tile, int lane) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-#pragma unroll
-  for (int kk = 0; kk < 2; ++kk) {
-#pragma unroll
-    for (int jp = 0; jp < 4; ++jp) {
-      uint32_t b[4];
-      ldsm4(addr_bn<kLd>(tile, 16 * jp, 16 * kk, lane), b);
-      mma_bf16(s[2 * jp], a[kk], b[0], b[1]);
-      mma_bf16(s[2 * jp + 1], a[kk], b[2], b[3]);
-    }
-  }
-}
-// acc[16 x 32] += P[16 x 64] B with B a [64 = k][32 = n] tile of stride kLd; P in the accumulator layout (fp32)
-DDL_DEVICE void mm_pb(float (&acc)[4][4], const float (&p)[8][4], uint32_t tile, int lane) {
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-    const uint32_t a[4] = {pack_bf16x2(p[2 * kk][0], p[2 * kk][1]), pack_bf16x2(p[2 * kk][2], p[2 * kk][3]),
-                           pack_bf16x2(p[2 * kk + 1][0], p[2 * kk + 1][1]),
-                           pack_bf16x2(p[2 * kk + 1][2], p[2 * kk + 1][3])};
-#pragma unroll
-    for (int jp = 0; jp < 2; ++jp) {
-      uint32_t b[4];
-      ldsm4_t(addr_a<kLd>(tile, 16 * kk, 16 * jp, lane), b);
-      mma_bf16(acc[2 * jp], a, b[0], b[1]);
-      mma_bf16(acc[2 * jp + 1], a, b[2], b[3]);
-    }
-  }
-}
-// acc[16 x 32] += A^T[16 x 64] B with A^T the transpose of the rows m0.. of a [64 = k][64 = m] tile of stride kLdP and
-// B a [64 = k][32 = n] tile of stride kLd  (dV = P^T dO, G' = (rq o dS)^T Q)
-DDL_DEVICE void mm_atb(float (&acc)[4][4], uint32_t at, int m0, uint32_t tile, int lane) {
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-    uint32_t a[4];
-    ldsm4_t(addr_at<kLdP>(at, m0, 16 * kk, lane), a);
-#pragma unroll
-    for (int jp = 0; jp < 2; ++jp) {
-      uint32_t b[4];
-      ldsm4_t(addr_a<kLd>(tile, 16 * kk, 16 * jp, lane), b);
-      mma_bf16(acc[2 * jp], a, b[0], b[1]);
-      mma_bf16(acc[2 * jp + 1], a, b[2], b[3]);
-    }
-  }
-}
 
 // image-order row of token i of window (wy, wx) of image n, or -1 for a virtual (padding) token
 DDL_DEVICE long long token_row(const WinArgs& a, int n, int wy, int wx, int i) {
@@ -236,16 +156,6 @@ DDL_DEVICE void inv_norms(const __nv_bfloat16* sQ, const __nv_bfloat16* sK, floa
   if (fq != nullptr) (tid < kL ? fq : fk)[r] = nrm >= kEps ? 1.f : 0.f;
 }
 
-// sum of dS over the pairs (i, j) of relative index k = (iy - jy + 7) * 15 + (ix - jx + 7), in row-major order of i
-DDL_DEVICE float rel_sum(const float* dsf, int k) {
-  const int dy = k / 15 - 7, dx = k - (k / 15) * 15 - 7;
-  float s = 0.f;
-  for (int iy = dy > 0 ? dy : 0; iy < (dy < 0 ? kWin + dy : kWin); ++iy)
-    for (int ix = dx > 0 ? dx : 0; ix < (dx < 0 ? kWin + dx : kWin); ++ix)
-      s += dsf[(iy * kWin + ix) * kLdF + (iy - dy) * kWin + ix - dx];
-  return s;
-}
-
 DDL_DEVICE float logit_scale(const WinArgs& a, int h) { return expf(fminf(__ldg(a.scale + h), kLn100)); }
 
 __global__ void __launch_bounds__(kThreads) win2_attn_fwd_kernel(WinArgs a) {
@@ -273,7 +183,7 @@ __global__ void __launch_bounds__(kThreads) win2_attn_fwd_kernel(WinArgs a) {
 #pragma unroll
   for (int kk = 0; kk < 2; ++kk) ldsm4(addr_a<kLd>(q_s, 16 * warp, 16 * kk, lane), qf[kk]);
   float s[8][4];
-  mm_abt(s, qf, k_s, lane);
+  mm_abt<kLd>(s, qf, k_s, lane);
   float m[2], l[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -311,7 +221,7 @@ __global__ void __launch_bounds__(kThreads) win2_attn_fwd_kernel(WinArgs a) {
   float acc[4][4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
-  mm_pb(acc, s, v_s, lane);
+  mm_pb<kLd>(acc, s, v_s, lane);
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const long long row = token_row(a, n, wy, wx, 16 * warp + g + 8 * r);
@@ -431,8 +341,8 @@ __global__ void __launch_bounds__(kThreads) win2_attn_bwd_kernel(WinArgs a) {
         ldsm4(addr_a<kLd>(o_s, 16 * warp, 16 * kk, lane), df[kk]);
       }
       float p[8][4], dp[8][4];
-      mm_abt(p, qf, k_s, lane);
-      mm_abt(dp, df, v_s, lane);
+      mm_abt<kLd>(p, qf, k_s, lane);
+      mm_abt<kLd>(dp, df, v_s, lane);
       float dsc = 0.f;
       bool real[2];
 #pragma unroll
@@ -476,7 +386,7 @@ __global__ void __launch_bounds__(kThreads) win2_attn_bwd_kernel(WinArgs a) {
       float dq[4][4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) dq[j][0] = dq[j][1] = dq[j][2] = dq[j][3] = 0.f;
-      mm_pb(dq, dp, k_s, lane);                                      // G = (dS o rk) K
+      mm_pb<kLd>(dq, dp, k_s, lane);                                 // G = (dS o rk) K
       norm_grad(dq, sm.q, sm.rq, sm.fq, 16 * warp, sh, lane);
       const bool qu[2] = {real[0] != (a.bias_pad_only != 0), real[1] != (a.bias_pad_only != 0)};
       col_sums(dq, qu, sm.bq[warp], lane);
@@ -494,8 +404,8 @@ __global__ void __launch_bounds__(kThreads) win2_attn_bwd_kernel(WinArgs a) {
       float dk[4][4], dv[4][4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) dk[j][0] = dk[j][1] = dk[j][2] = dk[j][3] = dv[j][0] = dv[j][1] = dv[j][2] = dv[j][3] = 0.f;
-      mm_atb(dv, p_s, 16 * warp, o_s, lane);                         // dV = P^T dO
-      mm_atb(dk, s_s, 16 * warp, q_s, lane);                         // G' = (rq o dS)^T Q
+      mm_atb<kLdP, kLd>(dv, p_s, 16 * warp, o_s, lane);              // dV = P^T dO
+      mm_atb<kLdP, kLd>(dk, s_s, 16 * warp, q_s, lane);              // G' = (rq o dS)^T Q
       norm_grad(dk, sm.k, sm.rk, sm.fk, 16 * warp, sh, lane);
       long long rows[2];
       bool vu[2];
@@ -517,8 +427,8 @@ __global__ void __launch_bounds__(kThreads) win2_attn_bwd_kernel(WinArgs a) {
         }
       }
     }
-    if (tid < kTab) dt_sum += rel_sum(sm.dsf, tid);
-    if (tid + kThreads < kTab) dt_sum2 += rel_sum(sm.dsf, tid + kThreads);
+    if (tid < kTab) dt_sum += rel_sum<kWin, kLdF>(sm.dsf, tid);
+    if (tid + kThreads < kTab) dt_sum2 += rel_sum<kWin, kLdF>(sm.dsf, tid + kThreads);
     if (tid == kThreads - 1) aux += ((sm.dsc[0] + sm.dsc[1]) + sm.dsc[2]) + sm.dsc[3];
     __syncthreads();                              // the tiles and sums are refilled by the next window
     if (tid < 2 * kD) {
@@ -532,21 +442,6 @@ __global__ void __launch_bounds__(kThreads) win2_attn_bwd_kernel(WinArgs a) {
   if (tid + kThreads < kTab) part[tid + kThreads] = dt_sum2;
   if (tid == kThreads - 1) part[kTab] = aux;
   if (tid < 2 * kD) part[kTab + 1 + tid] = aux;
-}
-
-// first level: chunk c of the P = N * nWy partials, summed in order, for every (head, k) -> chunk [kChunks][heads*kPer]
-__global__ void __launch_bounds__(kThreads) win2_grad_chunk_kernel(const float* __restrict__ part,
-                                                                   float* __restrict__ chunk, int P, int per) {
-  pdl_trigger();
-  pdl_wait();
-  const int e = blockIdx.x * kThreads + threadIdx.x, c = blockIdx.y;
-  if (e >= per) return;
-  const int p0 = static_cast<int>(static_cast<int64_t>(P) * c / kChunks);
-  const int p1 = static_cast<int>(static_cast<int64_t>(P) * (c + 1) / kChunks);
-  float s = 0.f;
-#pragma unroll 8
-  for (int p = p0; p < p1; ++p) s += part[static_cast<size_t>(p) * per + e];
-  chunk[static_cast<size_t>(c) * per + e] = s;
 }
 
 // second level: the chunks in order -> dtable[k][h] (written), dscale[h] += s_h sum(dS o c) unless clamped, dbias q / v
@@ -622,8 +517,8 @@ cudaError_t launch_window_attention_v2_bwd(const __nv_bfloat16* qkv, const float
   if (e != cudaSuccess) return e;
   const int P = N * a.nwy, per = heads * kPer;
   float* chunk = scratch + static_cast<size_t>(P) * per;
-  e = launch_pdl(win2_grad_chunk_kernel, dim3((per + kThreads - 1) / kThreads, kChunks), dim3(kThreads), 0, stream, 1,
-                 static_cast<const float*>(scratch), chunk, P, per);
+  e = launch_pdl(grad_chunk_kernel<kThreads, kChunks>, dim3((per + kThreads - 1) / kThreads, kChunks), dim3(kThreads),
+                 0, stream, 1, static_cast<const float*>(scratch), chunk, P, per);
   if (e != cudaSuccess) return e;
   return launch_pdl(win2_grad_final_kernel, dim3((per + kThreads - 1) / kThreads), dim3(kThreads), 0, stream, 1,
                     static_cast<const float*>(chunk), scale, dtable, dscale, dbias, heads, C);

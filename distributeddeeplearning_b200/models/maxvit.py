@@ -8,7 +8,7 @@ grid-partition attention layer:
   sigmoid / SiLU squeeze-excitation, 1x1 conv + bias; the shortcut is the identity, or 3x3/s2 average pooling + a 1x1
   conv + bias.  Stochastic depth + residual is one kernel in each direction (``ops.maxvit.stochastic_depth_add``).
 * Each attention layer is one autograd node (``ops.maxvit_attention_layer``), the Swin block's node with the partition
-  attention kernels (csrc/ops/grid_attention.cu).  Two independent stochastic-depth draws per layer, one per residual.
+  attention kernels (csrc/ops/window_attention.cu).  Two independent stochastic-depth draws per layer, one per residual.
 
 The classifier is global average pooling, LayerNorm, Linear, tanh and a bias-free Linear: torchvision's order.
 """

@@ -7,7 +7,7 @@ with the partition-attention kernels), stochastic depth + residual for MBConv, a
 
 torchvision partitions the map first and runs every op on the partitioned tensor.  LayerNorm, the linears and the
 per-sample stochastic depth act on one token at a time, so they commute with the partition: the native node runs them on
-the image-order rows and the attention kernels (csrc/ops/grid_attention.cu) gather each sequence from qkv with index
+the image-order rows and the attention kernels (csrc/ops/window_attention.cu) gather each sequence from qkv with index
 arithmetic.  The window partition puts token t = 7a + b of sequence (i, j) at pixel (7i + a, 7j + b), the grid partition
 (WindowPartition(H/7) + SwapAxes) at (a H/7 + i, b H/7 + j).
 

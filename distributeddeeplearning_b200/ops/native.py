@@ -869,7 +869,7 @@ def window_attention_bwd(dout: torch.Tensor, qkv: torch.Tensor, table: torch.Ten
 
 
 # ------------------------------------------------------------------------------------------------
-# MaxViT: grid / window partition attention (csrc/ops/grid_attention.cu)
+# MaxViT: grid / window partition attention (csrc/ops/window_attention.cu)
 # ------------------------------------------------------------------------------------------------
 def supports_grid_attention(H: int, W: int, partition: int, heads: int, head_dim: int) -> bool:
     """Shapes the partition-attention kernels take: partition 7, head dim 32, a square map H = W, a multiple of 7."""

@@ -169,7 +169,7 @@ def _attn_bwd(do, qkv, table, o, lse, heads, N, H, W, shift, part, grad_table):
 
 class _SwinBlock(torch.autograd.Function):
     """``part`` None: Swin's shifted-window attention (window_attention.cu).  ``part`` (grid, scale): MaxViT's
-    partition attention (grid_attention.cu), grid or window partition, logits scaled by ``scale``, no shift."""
+    partition attention (the same file's kernels), grid or window partition, logits scaled by ``scale``, no shift."""
 
     @staticmethod
     def forward(ctx, x, keep1, keep2, heads, shift, part, eps, train, n1_w, n1_b, qkv_w, qkv_b, proj_w, proj_b, table,

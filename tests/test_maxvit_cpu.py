@@ -258,10 +258,13 @@ def test_predicates_and_refusals():
 
 @pytest.mark.skipif(not _NVCC, reason="needs nvcc and c++filt")
 def test_new_kernels_compile_without_spills_and_fit_their_launch_bounds():
-    ga = _ptxas("grid_attention.cu")
-    assert sorted(ga) == ["part_attn_bwd_kernel<false>", "part_attn_bwd_kernel<true>", "part_attn_fwd_kernel<false>",
-                          "part_attn_fwd_kernel<true>", "part_bias_grad_chunk_kernel",
-                          "part_bias_grad_final_kernel"], sorted(ga)
+    ga = _ptxas("window_attention.cu")
+    # nvcc 12.9 register counts of the grid (true) and window (false) partition instances; Swin's instances and the
+    # shared bias-gradient reduction are pinned in test_swin_cpu.py
+    used = {n: v[0] for n, v in ga.items() if "Partition" in n}
+    assert used == {"win_attn_fwd_kernel<ddl::Partition<true> >": 70, "win_attn_fwd_kernel<ddl::Partition<false> >": 66,
+                    "win_attn_bwd_kernel<ddl::Partition<true> >": 168,
+                    "win_attn_bwd_kernel<ddl::Partition<false> >": 168}, used
     for n, (regs, st, ld, stack) in ga.items():
         assert st == 0 and ld == 0 and stack == 0 and regs <= 255, (n, regs, st, ld, stack)   # 128 threads
     bn = _ptxas("bn_act.cu")

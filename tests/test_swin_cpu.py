@@ -262,8 +262,11 @@ def test_predicates():
 @pytest.mark.skipif(not _NVCC, reason="needs nvcc and c++filt")
 def test_new_kernels_compile_without_spills_and_fit_their_launch_bounds():
     wa = _ptxas("window_attention.cu")
-    assert sorted(wa) == ["win_attn_bwd_kernel", "win_attn_fwd_kernel", "win_bias_grad_chunk_kernel",
-                          "win_bias_grad_final_kernel"], sorted(wa)
+    # nvcc 12.9 register counts of Swin's instances and the bias-gradient reduction; MaxViT's (Partition) are pinned
+    # in test_maxvit_cpu.py
+    used = {n: v[0] for n, v in wa.items() if "Partition" not in n}
+    assert used == {"win_attn_fwd_kernel<ddl::ShiftedWindow>": 80, "win_attn_bwd_kernel<ddl::ShiftedWindow>": 255,
+                    "mma_tile::grad_chunk_kernel<128, 64>": 26, "win_bias_grad_final_kernel": 25}, used
     for n, (regs, st, ld, stack) in wa.items():
         assert st == 0 and ld == 0 and stack == 0 and regs <= 255, (n, regs, st, ld, stack)   # 128 threads
     sw = _ptxas("swin.cu")

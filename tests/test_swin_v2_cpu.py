@@ -291,8 +291,9 @@ def test_predicates():
 @pytest.mark.skipif(not _NVCC, reason="needs nvcc and c++filt")
 def test_new_kernels_compile_without_spills_and_fit_their_launch_bounds():
     wa = _ptxas("window_attention_v2.cu")
-    assert sorted(wa) == ["win2_attn_bwd_kernel", "win2_attn_fwd_kernel", "win2_grad_chunk_kernel",
-                          "win2_grad_final_kernel"], sorted(wa)
+    used = {n: v[0] for n, v in wa.items()}     # nvcc 12.9
+    assert used == {"win2_attn_fwd_kernel": 80, "win2_attn_bwd_kernel": 166, "mma_tile::grad_chunk_kernel<128, 64>": 26,
+                    "win2_grad_final_kernel": 26}, used
     for n, (regs, st, ld, stack) in wa.items():
         assert st == 0 and ld == 0 and stack == 0 and regs <= 255, (n, regs, st, ld, stack)   # 128 threads
     sw = _ptxas("swin_v2.cu")

@@ -185,7 +185,8 @@ _NVCC = shutil.which("c++filt") and os.path.isfile(os.path.join(_ext.CUDA_HOME, 
 @pytest.mark.skipif(not _NVCC, reason="needs nvcc and c++filt")
 def test_new_kernels_compile_without_spills_and_fit_their_launch_bounds():
     at = _ptxas("attention.cu")
-    assert sorted(at) == ["attn_bwd_dkv_kernel", "attn_bwd_dq_kernel", "attn_fwd_kernel"], sorted(at)
+    used = {n: v[0] for n, v in at.items()}     # nvcc 12.9: a change in a count is a change in the kernel's code
+    assert used == {"attn_fwd_kernel": 128, "attn_bwd_dq_kernel": 166, "attn_bwd_dkv_kernel": 232}, used
     for n, (regs, st, ld, stack) in at.items():
         assert st == 0 and ld == 0 and stack == 0 and regs <= 255, (n, regs, st, ld, stack)   # 128 threads
     vt = _ptxas("vit.cu")

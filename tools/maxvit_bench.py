@@ -2,7 +2,7 @@
 """Timing of MaxViT's kernels at the stage shapes of maxvit_t (224: 56/2, 28/4, 14/8, 7/16 map / heads), batch 256,
 on the same bf16 operands, and of maxvit_t's training step.
 
-- Grid and window partition attention (csrc/ops/grid_attention.cu) against ``F.scaled_dot_product_attention`` on
+- Grid and window partition attention (csrc/ops/window_attention.cu) against ``F.scaled_dot_product_attention`` on
   pre-partitioned sequences [N, G * heads, 49, 32] with the relative-position bias as a bf16 ``attn_mask`` (the
   partition itself is not timed), and Swin's window kernel at shift 0 (whose scale is 1/sqrt(32), not MaxViT's
   1/sqrt(C): timed for comparison only).  Forward: O (and the native log-sum-exp); backward: dQ, dK, dV (and the native
