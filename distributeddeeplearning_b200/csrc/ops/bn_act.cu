@@ -22,6 +22,10 @@
 //   Stochastic depth (sample_scale, EfficientNet's residual blocks): z = BN(x) * keep[n] + residual with one scale per
 //   sample (row / hw), no activation.  The statistics cover every sample, dropped ones included; backward feeds
 //   dz * keep[n] to the BN and returns dres = dz.  Own forward kernel (bn_sd_fwd_kernel, train only) and mask value.
+//   SiLU before the residual (relu == 6, EfficientNetV2's Fused-MBConv): z = silu(BN(x)) * keep[n] + residual, keep
+//   optional (scale 1 without it; never in eval).  The gradient is dz * keep[n] * silu'(v), v recomputed from x in both
+//   passes; the residual's gradient is dz itself, so no dres is written.  Own forward kernel (bn_silu_res_fwd_kernel) and
+//   mask value (10); no bit mask, pre-reduced sums or fp8 twin.
 //
 // Thread mapping: a thread owns 8 consecutive channels (one 16-byte vector) of a FIXED channel
 // group and walks rows with a grid stride, so per-channel constants live in registers.  The loops
@@ -37,9 +41,11 @@ namespace {
 
 constexpr int kBnThreads = 256;
 enum { kMaskNone = 0, kMaskZ = 1, kMaskX = 2, kMaskBits = 3, kMaskZ6 = 4, kMaskX6 = 5, kMaskXH = 6, kMaskXS = 7,
-       kMaskSD = 8, kMaskXG = 9 };
+       kMaskSD = 8, kMaskXG = 9, kMaskXSR = 10 };
 constexpr bool mask_from_z(int m) { return m == kMaskZ || m == kMaskZ6; }
-constexpr bool mask_from_x(int m) { return m == kMaskX || m == kMaskX6 || m == kMaskXH || m == kMaskXS || m == kMaskXG; }
+constexpr bool mask_from_x(int m) {
+  return m == kMaskX || m == kMaskX6 || m == kMaskXH || m == kMaskXS || m == kMaskXG || m == kMaskXSR;
+}
 // sigmoid on the MUFU exp and reciprocal (__fdividef, no IEEE division: with `1.f / (...)` the SiLU backward's chunked
 // apply pass spilled at 64 registers).  Relative accuracy holds in the negative tail, where sigmoid(v) is tiny; for
 // v < -87 the denominator overflows to inf and the result is 0.
@@ -63,7 +69,7 @@ DDL_DEVICE bool act_passes(float v) {
 template <int MASK>
 DDL_DEVICE float act_bwd(float v, float dz) {
   if (MASK == kMaskXH) return v <= -3.f ? 0.f : (v >= 3.f ? dz : dz * fmaf(v, 1.f / 3.f, 0.5f));
-  if (MASK == kMaskXS) {
+  if (MASK == kMaskXS || MASK == kMaskXSR) {
     const float sg = sigmoid(v);
     return dz * sg * fmaf(v, 1.f - sg, 1.f);
   }
@@ -75,7 +81,7 @@ DDL_DEVICE float act_bwd(float v, float dz) {
   return act_passes<MASK>(v) ? dz : 0.f;
 }
 // forward activations of bn_act_fwd_body
-enum { kActRelu = 0, kActRelu6 = 1, kActHswish = 2, kActSilu = 3, kActSD = 4, kActGelu = 5 };
+enum { kActRelu = 0, kActRelu6 = 1, kActHswish = 2, kActSilu = 3, kActSD = 4, kActGelu = 5, kActSiluRes = 6 };
 DDL_DEVICE float hardswish(float v) { return v * fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f); }
 
 struct Vec8 {
@@ -140,8 +146,9 @@ DDL_DEVICE void fp8_fold_amax(Fp8Slot* slot, float amax) {
   }
 }
 
-// ACT: kActRelu (ReLU when a.relu, else none), kActRelu6 (when a.relu), kActHswish / kActSilu / kActGelu (always) or kActSD (no
-// activation; the BN output scaled by the row's sample scale before the residual add)
+// ACT: kActRelu (ReLU when a.relu, else none), kActRelu6 (when a.relu), kActHswish / kActSilu / kActGelu (always), kActSD (no
+// activation; the BN output scaled by the row's sample scale before the residual add) or kActSiluRes (SiLU, then the optional
+// sample scale and the residual add)
 template <bool TRAIN, bool CHUNKED, bool FP8, int ACT>
 DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
   pdl_trigger();
@@ -193,6 +200,16 @@ DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
       const float ks = a.sample_scale[off / (static_cast<size_t>(a.hw) * a.C)];
 #pragma unroll
       for (int i = 0; i < 8; ++i) z[i] = fmaf(fmaf(x[i], scale[i], shift[i]), ks, res[i]);
+    } else if (ACT == kActSiluRes) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float v = fmaf(x[i], scale[i], shift[i]);
+        z[i] = v * sigmoid(v);
+      }
+      const float ks = a.sample_scale ? a.sample_scale[off / (static_cast<size_t>(a.hw) * a.C)] : 1.f;
+      const float2 r01 = unpack_bf16x2(ur.x), r23 = unpack_bf16x2(ur.y), r45 = unpack_bf16x2(ur.z), r67 = unpack_bf16x2(ur.w);
+      z[0] = fmaf(z[0], ks, r01.x); z[1] = fmaf(z[1], ks, r01.y); z[2] = fmaf(z[2], ks, r23.x); z[3] = fmaf(z[3], ks, r23.y);
+      z[4] = fmaf(z[4], ks, r45.x); z[5] = fmaf(z[5], ks, r45.y); z[6] = fmaf(z[6], ks, r67.x); z[7] = fmaf(z[7], ks, r67.y);
     } else if (a.residual) {
       float res[8];
       unpack8(ur, res);
@@ -211,7 +228,7 @@ DDL_DEVICE void bn_act_fwd_body(const BnFwdArgs& a) {
     } else if (ACT == kActGelu) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) z[i] *= fmaf(0.5f, erff(z[i] * 0.70710678118654752f), 0.5f);
-    } else if (ACT != kActSD && a.relu) {
+    } else if (ACT != kActSD && ACT != kActSiluRes && a.relu) {
       if (a.mask) {
         uint32_t bits = 0;
 #pragma unroll
@@ -279,6 +296,11 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_sd_fwd_kernel(BnFwdArgs a) {
   bn_act_fwd_body<true, CHUNKED, false, kActSD>(a);
 }
 
+template <bool TRAIN, bool CHUNKED>
+__global__ void __launch_bounds__(kBnThreads, 4) bn_silu_res_fwd_kernel(BnFwdArgs a) {
+  bn_act_fwd_body<TRAIN, CHUNKED, false, kActSiluRes>(a);
+}
+
 // ---- backward pass 1: per-channel reductions ----------------------------------------------------
 // accumulates S1 = sum dy and S2 = sum dy * x (raw x); dbeta = S1, dgamma = invstd * (S2 - mean * S1).
 // Mapping: a block owns ONE 64-channel chunk (blockIdx.y) and 32 row lanes (thread = 8 channels x 1 row lane),
@@ -336,6 +358,22 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
       accumulate(ld_stream_u4(a.dz + off0), ld_stream_u4(a.x + off0), make_uint4(0, 0, 0, 0));
     }
   }
+  if constexpr (MASK == kMaskXSR) {       // one row per iteration, as SiLU; the BN sees dz * keep[sample] * silu'(v)
+    for (; r < a.M; r += rstep) {
+      const int pr = phys(r);
+      const size_t off0 = static_cast<size_t>(pr) * a.C + c0;
+      const float ks = a.sample_scale ? a.sample_scale[pr / a.hw] : 1.f;
+      float dz[8], x[8];
+      unpack8(ld_stream_u4(a.dz + off0), dz);
+      unpack8(ld_stream_u4(a.x + off0), x);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float d = act_bwd<MASK>(fmaf(x[i], msc[i], msh[i]), dz[i] * ks);
+        s1[i] += d;
+        s2[i] = fmaf(d, x[i], s2[i]);
+      }
+    }
+  }
   if constexpr (MASK == kMaskSD) {        // the BN sees dz * keep[sample]
     for (; r < a.M; r += rstep) {
       const int pr = phys(r);
@@ -351,7 +389,8 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_reduce_kernel(BnBwdA
       }
     }
   }
-  for (; MASK != kMaskXH && MASK != kMaskXS && MASK != kMaskXG && MASK != kMaskSD && r + rstep < a.M; r += 2 * rstep) {
+  for (; MASK != kMaskXH && MASK != kMaskXS && MASK != kMaskXG && MASK != kMaskSD && MASK != kMaskXSR && r + rstep < a.M;
+       r += 2 * rstep) {
     const size_t off0 = static_cast<size_t>(phys(r)) * a.C + c0;
     const size_t off1 = static_cast<size_t>(phys(r + rstep)) * a.C + c0;
     const uint4 d0 = ld_stream_u4(a.dz + off0), d1 = ld_stream_u4(a.dz + off1);
@@ -443,6 +482,11 @@ __global__ void __launch_bounds__(kBnThreads, 4) bn_act_bwd_apply_kernel(BnBwdAr
     float dz[8], x[8];
     unpack8(ld_stream_u4(a.dz + off), dz);
     unpack8(ld_stream_u4(a.x + off), x);
+    if constexpr (MASK == kMaskXSR) {
+      const float ks = a.sample_scale ? a.sample_scale[r / a.hw] : 1.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) dz[i] *= ks;
+    }
     if (mask_from_z(MASK)) {
       float z[8];
       unpack8(ld_stream_u4(a.z + off), z);
@@ -749,7 +793,7 @@ cudaError_t launch_bn_bwd_mask(const BnBwdArgs& a, int sms, cudaStream_t stream,
   const bool flat = bn_flat_ok(a.C);
   const dim3 grid = flat ? dim3(bn_grid(a.M, a.C, sms)) : rgrid;
   if constexpr (MASK == kMaskZ6 || MASK == kMaskX6 || MASK == kMaskXH || MASK == kMaskXS || MASK == kMaskXG ||
-                MASK == kMaskSD) {
+                MASK == kMaskSD || MASK == kMaskXSR) {
     if (f8) return cudaErrorInvalidValue;
   } else if (f8) {
     return flat ? launch_pdl(bn_act_bwd_apply_kernel<MASK, false, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
@@ -767,6 +811,16 @@ cudaError_t launch_bn_act_fwd(const BnFwdArgs& a_in, bool train, int sms, cudaSt
   if (a.C % 8 != 0 || a.C <= 0) return cudaErrorInvalidValue;
   const bool flat = bn_flat_ok(a.C);
   const dim3 grid = flat ? dim3(bn_grid(a.M, a.C, sms)) : bn_chunk_grid(a.M, a.C, sms);
+  if (a.relu == 6) {        // SiLU, then the optional per-sample scale (train only) and the residual add
+    if (a.residual == nullptr || a.mask != nullptr || (a.zq != nullptr && a.zq_slot != nullptr) ||
+        (a.sample_scale != nullptr && (!train || a.hw <= 0 || a.M % a.hw != 0)))
+      return cudaErrorInvalidValue;
+    if (flat)
+      return train ? launch_pdl(bn_silu_res_fwd_kernel<true, false>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                   : launch_pdl(bn_silu_res_fwd_kernel<false, false>, grid, dim3(kBnThreads), 0, stream, 1, a);
+    return train ? launch_pdl(bn_silu_res_fwd_kernel<true, true>, grid, dim3(kBnThreads), 0, stream, 1, a)
+                 : launch_pdl(bn_silu_res_fwd_kernel<false, true>, grid, dim3(kBnThreads), 0, stream, 1, a);
+  }
   if (a.sample_scale != nullptr) {     // stochastic depth: train only, a residual, no activation, bit mask or fp8 twin
     if (!train || a.relu != 0 || a.residual == nullptr || a.mask != nullptr || (a.zq != nullptr && a.zq_slot != nullptr) ||
         a.hw <= 0 || a.M % a.hw != 0)
@@ -811,6 +865,12 @@ cudaError_t launch_bn_act_bwd(const BnBwdArgs& a_in, int sms, cudaStream_t strea
   BnBwdArgs a = a_in;
   a.reverse = g_bn_reverse;
   if (a.C % 8 != 0 || a.C <= 0) return cudaErrorInvalidValue;
+  if (a.relu == 6) {        // SiLU before the residual: v recomputed from x, dres is dz itself (not written)
+    if (!a.mask_from_x || a.zmask != nullptr || a.dres != nullptr || skip_reduce ||
+        (a.sample_scale != nullptr && (a.hw <= 0 || a.M % a.hw != 0)))
+      return cudaErrorInvalidValue;
+    return launch_bn_bwd_mask<kMaskXSR>(a, sms, stream, false);
+  }
   if (a.sample_scale != nullptr) {     // stochastic depth: no activation, no fp8 twin, sums not pre-reduced
     if (a.relu != 0 || a.zmask != nullptr || skip_reduce || (a.dxq != nullptr && a.dxq_slot != nullptr) || a.hw <= 0 ||
         a.M % a.hw != 0)

@@ -34,7 +34,8 @@ struct BnFwdArgs {
   int reverse;                    // walk the rows from the END: the producing conv wrote x front to back, so the tail of a
                                   //   tensor larger than L2 is what is still cached (set by the launcher: set_bn_reverse)
   const float* sample_scale;      // optional [M / hw] per-sample scale of the BN output before the residual add
-  int hw;                         //   (stochastic depth: z = BN(x) * sample_scale[row / hw] + residual; no activation)
+  int hw;                         //   (stochastic depth: z = BN(x) * sample_scale[row / hw] + residual; no activation,
+                                  //   or relu == 6: z = silu(BN(x)) * sample_scale[row / hw] + residual)
 };
 
 struct BnBwdArgs {
@@ -59,7 +60,7 @@ struct BnBwdArgs {
   int reverse;                    // the REDUCE pass walks the rows from the end (dz was just written front to back; the apply
                                   //   pass then walks forward and finds the rows the reduce pass read last)
   const float* sample_scale;      // optional, as in BnFwdArgs: BN sees dz * sample_scale[row / hw], dres = dz
-  int hw;
+  int hw;                         //   (relu == 6: the SiLU's input sees dz * sample_scale[row / hw] * silu'(v))
 };
 
 cudaError_t launch_bn_act_fwd(const BnFwdArgs& a, bool train, int sms, cudaStream_t stream);

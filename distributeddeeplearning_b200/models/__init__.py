@@ -19,6 +19,8 @@ from .densenet import DenseNet, densenet121, densenet161, densenet169, densenet2
 from .efficientnet import (INPUT_SIZE as _EFFICIENTNET_INPUT_SIZE, EfficientNet, efficientnet_b0,  # noqa: F401
                            efficientnet_b1, efficientnet_b2, efficientnet_b3, efficientnet_b4, efficientnet_b5,
                            efficientnet_b6, efficientnet_b7)
+from .efficientnet_v2 import (INPUT_SIZE as _EFFICIENTNET_V2_INPUT_SIZE, EfficientNetV2,  # noqa: F401
+                              efficientnet_v2_l, efficientnet_v2_m, efficientnet_v2_s)
 from .inception import Inception3, inception_v3  # noqa: F401
 from .maxvit import MaxVit, maxvit_t  # noqa: F401
 from .mobilenet import MobileNetV2, mobilenet_v2  # noqa: F401
@@ -38,7 +40,8 @@ _REGISTRY = {
     f.__name__: f
     for f in (alexnet, convnext_tiny, convnext_small, convnext_base, convnext_large, densenet121, densenet161,
               densenet169, densenet201, efficientnet_b0, efficientnet_b1, efficientnet_b2, efficientnet_b3,
-              efficientnet_b4, efficientnet_b5, efficientnet_b6, efficientnet_b7,
+              efficientnet_b4, efficientnet_b5, efficientnet_b6, efficientnet_b7, efficientnet_v2_s,
+              efficientnet_v2_m, efficientnet_v2_l,
               squeezenet1_0, squeezenet1_1, inception_v3, mobilenet_v2,
               mobilenet_v3_large, mobilenet_v3_small, resnet18, resnet34, resnet50, resnet101, resnet152,
               resnext50_32x4d, resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2, vgg11, vgg11_bn, vgg13,
@@ -65,11 +68,13 @@ def get_model(name: str, **kw):
 
 def input_size(model_or_name) -> int:
     """Spatial input size (299 for Inception-v3 — the reference hard-codes 224 and breaks, SURVEY.md Q2; torchvision's
-    crop size for EfficientNet-B0 to -B7, 224 to 600, and for Swin-V2-T / -S / -B, 256; a Vision Transformer's
-    ``image_size``)."""
+    crop size for EfficientNet-B0 to -B7, 224 to 600, for EfficientNetV2-S / -M / -L, 384 / 480 / 480, and for
+    Swin-V2-T / -S / -B, 256; a Vision Transformer's ``image_size``)."""
     if isinstance(model_or_name, str):
         if model_or_name in _EFFICIENTNET_INPUT_SIZE:
             return _EFFICIENTNET_INPUT_SIZE[model_or_name]
+        if model_or_name in _EFFICIENTNET_V2_INPUT_SIZE:
+            return _EFFICIENTNET_V2_INPUT_SIZE[model_or_name]
         if model_or_name.startswith("swin_v2_"):
             return _SWIN_V2_INPUT_SIZE
         return 299 if model_or_name.startswith("inception") else 224

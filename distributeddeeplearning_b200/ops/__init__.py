@@ -1,5 +1,6 @@
 """Fused ops: hand-written sm_90a kernels on CUDA, PyTorch composites on CPU (see functional.py)."""
 from .convnext import convnext_block, layer_norm_channels  # noqa: F401
+from .efficientnet_v2 import fused_mbconv, fused_mbconv_supported  # noqa: F401
 from .functional import (  # noqa: F401
     advance_dropout_step,
     avg_pool2d,

@@ -1741,12 +1741,15 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
     element telling whether z > 0, which lets the backward of residual layers skip reading z (16x less mask traffic).
     ``relu``: False / True, 2 for ReLU6 (clamp to [0, 6]; not with ``want_mask``) or 3 for hardswish
     (x * clamp(x + 3, 0, 6) / 6; not with ``want_mask`` or ``residual``), 4 for SiLU (x * sigmoid(x); the same
-    refusals), 5 for GELU (x * Phi(x), erf form; the same refusals).  ``sample_scale``: fp32 [N] (stochastic depth, train only): z = BN(y) * sample_scale[n] + residual, with
-    no activation."""
+    refusals), 5 for GELU (x * Phi(x), erf form; the same refusals), 6 for SiLU before a ``residual`` (required):
+    z = silu(BN(y)) [* sample_scale[n]] + residual (no bit mask).  ``sample_scale``: fp32 [N] (stochastic depth, train
+    only): z = BN(y) * sample_scale[n] + residual, with no activation, or with code 6 as above."""
     C = _C()
     _check_act(y, "y")
     if int(relu) in (4, 5) and (want_mask or residual is not None):
         raise ValueError("bn_act_fwd: SiLU / GELU take no residual and have no bit-mask variant")
+    if int(relu) == 6 and (want_mask or residual is None):
+        raise ValueError("bn_act_fwd: SiLU before the residual (6) needs a residual and has no bit-mask variant")
     _check_sample_scale(sample_scale, y, relu, residual, train)
     if int(relu) == 2 and want_mask:
         raise ValueError("bn_act_fwd: ReLU6 has no bit-mask variant")
@@ -1767,8 +1770,8 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
         zq = slot = None
         key = ("act", gamma.data_ptr(), N, H, W)
         # emit the e4m3 twin only when an fp8 convolution consumed this layer's output in an earlier step
-        twin = _fp8.enabled() and int(relu) not in (2, 3, 4, 5) and sample_scale is None and Ch % 128 == 0 and M >= 2048 \
-            and _fp8.note_producer(z, key)
+        twin = _fp8.enabled() and int(relu) not in (2, 3, 4, 5, 6) and sample_scale is None and Ch % 128 == 0 \
+            and M >= 2048 and _fp8.note_producer(z, key)
         if twin:
             idx, fused = _fp8.producer_slot(key, y.device, z)
             if fused:       # the e4m3 twin rides in this kernel's pass (+1 B/element) instead of a 3 B/element pass
@@ -1792,8 +1795,9 @@ def bn_act_fwd(y: torch.Tensor, stats: Optional[torch.Tensor], gamma, beta, runn
 def _check_sample_scale(sample_scale, y, relu, residual, train) -> None:
     if sample_scale is None:
         return
-    if int(relu) != 0 or residual is None or not train:
-        raise ValueError("bn: a per-sample scale (stochastic depth) needs training, a residual and no activation")
+    if int(relu) not in (0, 6) or residual is None or not train:
+        raise ValueError("bn: a per-sample scale (stochastic depth) needs training, a residual and no activation "
+                         "(or SiLU before the residual, 6)")
     if sample_scale.dtype != torch.float32 or not sample_scale.is_cuda or sample_scale.dim() != 1 \
             or sample_scale.shape[0] != y.shape[0] or not sample_scale.is_contiguous():
         raise ValueError(f"bn: sample_scale must be a contiguous CUDA fp32 [{y.shape[0]}] tensor")
@@ -1809,19 +1813,24 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
 
     ReLU mask source: recomputed from y when the layer had no residual (``beta`` given), else the bit mask written by
     the forward (``zmask``), else the saved output ``z``.  ``sample_scale``: the forward's per-sample scale (stochastic
-    depth): the BN sees dz * sample_scale[n] while dres = dz."""
+    depth): the BN sees dz * sample_scale[n] while dres = dz.  ``relu`` 6 (SiLU before the residual): the SiLU's input
+    is recomputed from y (``beta`` required, ``had_residual`` ignored) and sees dz [* sample_scale[n]]; the residual's
+    gradient is dz itself, returned as dres without a copy."""
     C = _C()
     _check_act(dz, "dz")
     if sample_scale is not None:
         _check_sample_scale(sample_scale, y, relu, True, True)
         if pre_reduced is not None or zmask is not None:
             raise ValueError("bn_act_bwd: a per-sample scale takes neither pre-reduced sums nor a bit mask")
+    if int(relu) == 6 and (beta is None or zmask is not None or pre_reduced is not None):
+        raise ValueError("bn_act_bwd: SiLU before the residual (6) recomputes its input from y (pass beta) and takes "
+                         "neither a bit mask nor pre-reduced sums")
     N, Ch, H, W = y.shape
     M = N * H * W
     dy = torch.empty_like(y)
-    dres = torch.empty_like(y) if want_dres else None
+    dres = torch.empty_like(y) if (want_dres and int(relu) != 6) else None
     scratch = pre_reduced if pre_reduced is not None else zeros_f32((2, Ch), y.device)
-    mask_from_x = bool(relu and beta is not None and not had_residual)     # z is not read at all in that case
+    mask_from_x = bool(relu and beta is not None and (not had_residual or int(relu) == 6))   # z is then never read
     if pre_reduced is not None and not (mask_from_x or (relu and zmask is not None)):
         raise ValueError("pre_reduced sums are only defined for BN+ReLU layers (mask from y or from the bit mask)")
     if relu and not mask_from_x and zmask is None and z is None:
@@ -1835,8 +1844,8 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
 
     dyq = slot = None
     key = ("grad", gamma.data_ptr(), N, H, W)
-    twin = _fp8.enabled() and int(relu) not in (2, 3, 4, 5) and sample_scale is None and Ch % 128 == 0 and M >= 2048 \
-        and _fp8.note_producer(dy, key)                           # an fp8 dgrad consumed it before
+    twin = _fp8.enabled() and int(relu) not in (2, 3, 4, 5, 6) and sample_scale is None and Ch % 128 == 0 \
+        and M >= 2048 and _fp8.note_producer(dy, key)             # an fp8 dgrad consumed it before
     if twin:
         idx, fused = _fp8.producer_slot(key, y.device, dy, e5m2=True)
         if fused:
@@ -1851,6 +1860,8 @@ def bn_act_bwd(dz: torch.Tensor, z: Optional[torch.Tensor], y: torch.Tensor, sav
             _fp8.attach_twin(dy, dyq, idx)
         else:
             _fp8.attach_by_quantize(dy, key, e5m2=True)
+    if want_dres and int(relu) == 6:
+        dres = dz
     return dy, dres, scratch
 
 

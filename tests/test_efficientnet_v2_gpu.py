@@ -1,0 +1,63 @@
+"""GPU tests (H100) of EfficientNetV2 and the SiLU-before-residual BN: the `efficientnet_v2` group of tools/gpu_diag.py
+(BN code 6 on both thread mappings, the one-node Fused-MBConv at every residual Fused shape of -S / -M / -L against
+float64, efficientnet_v2_s against torchvision, graph replay, fp8), its layer checks under the forced persistent /
+CTA-pair conv kernels, the benchmark entry point under graph capture and the ImageNet trainer on efficientnet_v2_s."""
+import json
+import os
+import subprocess
+import sys
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+pytestmark = pytest.mark.gpu
+
+
+def _group(name, timeout=1800, env=None):
+    e = dict(os.environ)
+    e.update(env or {})
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "gpu_diag.py"), "--group", name], cwd=ROOT,
+                       capture_output=True, text=True, timeout=timeout, env=e)
+    out = r.stdout + r.stderr
+    tail = "\n".join(l for l in out.splitlines() if "FAIL" in l or "Error" in l)[:3000] + "\n...\n" + out[-3000:]
+    assert r.returncode == 0, tail
+    assert "FAIL" not in r.stdout, tail
+
+
+def test_efficientnet_v2_group():
+    _group("efficientnet_v2")
+
+
+def test_efficientnet_v2_layers_persistent_forced():
+    _group("efficientnet_v2_layers", env={"DDL_CONV_PERSISTENT": "2", "DDL_CONV_DEEP": "0", "DDL_CONV_AUTOTUNE": "0"})
+
+
+def test_efficientnet_v2_layers_cluster_pairs():
+    _group("efficientnet_v2_layers", env={"DDL_CONV_CLUSTER": "1", "DDL_CONV_PERSISTENT": "2"})
+
+
+def test_bench_efficientnet_v2_s():
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--model", "efficientnet_v2_s", "--steps", "3",
+                        "--warmup", "3", "--batch-size", "16"], cwd=ROOT, capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0, (r.stdout + r.stderr)[-3000:]
+    out = json.loads([l for l in r.stdout.splitlines() if l.startswith("{")][-1])
+    for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
+                "vs_baseline", "dtype", "data", "config", "clocks", "e2e", "gpu_launches"):
+        assert key in out, key
+    assert out["value"] > 0 and out["gpu_launches"] > 0 and out["e2e"]["value"] > 0
+    assert out["config"]["cuda_graph"] is True and out["config"]["model"] == "efficientnet_v2_s"
+
+
+def test_imagenet_trainer_efficientnet_v2_s(tmp_path):
+    sys.path.insert(0, ROOT)
+    import io
+
+    from distributeddeeplearning_b200.cli import launcher
+
+    out, err = io.StringIO(), io.StringIO()
+    res = launcher.launch("distributeddeeplearning_b200.workloads.imagenet",
+                          ["--epochs", "1", "--batch_size", "16", "--model", "efficientnet_v2_s",
+                           "--save_filepath", str(tmp_path / "ck-{epoch}.pt")], gpus=1, record=False, stdout=out,
+                          stderr=err, timeout=900, env={"PYTHONPATH": ROOT, "FAKE_DATA_LENGTH": "64"})
+    assert res.returncode == 0, (out.getvalue() + err.getvalue())[-3000:]
+    assert "Training epoch 0 took" in out.getvalue()

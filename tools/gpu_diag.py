@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -2464,6 +2464,10 @@ def _efficientnet_vs_torchvision(name, bs, size, judge_lag=True):
              for mod in m.modules() if isinstance(mod, effnet.ConvBNAct) and mod[0].groups > 1]
     hooks += [mod.register_forward_hook(lambda mod, i, o: se.append(type(o.grad_fn).__name__))
               for mod in m.modules() if isinstance(mod, effnet.SqueezeExcitation)]
+    fused = []          # EfficientNetV2: the residual Fused-MBConv blocks run on their one-node form
+    hooks += [mod.register_forward_hook(lambda mod, i, o: fused.append(type(o.grad_fn).__name__))
+              for mod in m.modules() if type(mod).__name__ == "FusedMBConv" and mod.use_res_connect]
+    n_fused = sum(1 for mod in m.modules() if type(mod).__name__ == "FusedMBConv" and mod.use_res_connect)
     x = torch.randn(bs, 3, size, size, device="cuda").to(torch.bfloat16).float()
     y = torch.randint(0, 1000, (bs,), device="cuda")
     try:
@@ -2487,10 +2491,12 @@ def _efficientnet_vs_torchvision(name, bs, size, judge_lag=True):
     n_blocks = sum(1 for mod in m.modules() if isinstance(mod, effnet.MBConv))
     dropped = sum(int((k == 0).sum()) for k in keeps)
     ok = len(dw) == n_blocks and set(dw) == {"_DwConvBnActBackward"} and len(se) == n_blocks \
-        and set(se) == {"_SqueezeExciteSiLUBackward"} and dropped > 0
+        and set(se) == {"_SqueezeExciteSiLUBackward"} and dropped > 0 and len(fused) == n_fused \
+        and set(fused) <= {"_FusedMBConvBackward"}
     RESULTS.append(ok)
     print(f"[{'ok' if ok else 'FAIL'}] {name} at {size}: {len(dw)} depthwise layers, nodes {sorted(set(dw))}; {len(se)} SE "
-          f"units, nodes {sorted(set(se))}; {len(keeps)} stochastic-depth draws, {dropped} dropped samples")
+          f"units, nodes {sorted(set(se))}; {len(keeps)} stochastic-depth draws, {dropped} dropped samples"
+          + (f"; {len(fused)} residual Fused-MBConv blocks, nodes {sorted(set(fused))}" if n_fused else ""))
     c1, c2 = _cos(out, ro), _cos(out, co)
     RESULTS.append(c1 > 0.98)
     print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} logits cos vs fp32 {c1:.5f}   vs bf16-composite {c2:.5f}")
@@ -2504,6 +2510,8 @@ def _efficientnet_vs_torchvision(name, bs, size, judge_lag=True):
             zero.add(f"{k}.block.{len(mod.block) - 1}.1.bias")
             if mod.block[0][0].groups == 1:
                 cancel |= {f"{k}.block.0.1.weight", f"{k}.block.0.1.bias"}
+        elif type(mod).__name__ == "FusedMBConv" and len(mod.block) == 2:
+            zero.add(f"{k}.block.1.1.bias")          # the linear projection's BN, as the MBConv projection's
     print(f"   projection-BN beta gradients (analytically zero), max |grad| native "
           f"{max(float(gn[k].grad.abs().max()) for k in zero):.2e}, fp32 {max(float(tvp[k].grad.abs().max()) for k in zero):.2e}")
     cc = sorted((_cos(gn[k].grad, tvp[k].grad), _cos(gc[k].grad, tvp[k].grad), k) for k in cancel)
@@ -2609,6 +2617,248 @@ def g_efficientnet():
     ok = all(l == l and abs(l) < 1e4 for l in losses)
     RESULTS.append(ok)
     print(f"[{'ok' if ok else 'FAIL'}] efficientnet_b0 fp8 session: losses {[round(v, 3) for v in losses]}, "
+          f"fp8 launches {fp8.launches()}", flush=True)
+    del s
+    torch.cuda.empty_cache()
+
+
+def _silu_res_bn(C):
+    """BN code 6 (SiLU before the residual) in the fused BN kernels against float64: train forward with a keep vector
+    containing zeros and without one (z, running statistics), eval forward, backward (dx, dgamma, dbeta; the residual's
+    gradient is dz itself), and the refusals around it."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    n = 4
+    y = cl(bf(torch.randn(n, C, 9, 9, device="cuda") * 3))
+    r = cl(bf(torch.randn(n, C, 9, 9, device="cuda")))
+    g = torch.rand(C, device="cuda") * 2 + 0.5
+    b = torch.randn(C, device="cuda") * 2
+    keep = torch.tensor([1.25, 0.0, 1.25, 1.25], device="cuda")
+    for kname, k in (("keep with a zero", keep), ("no keep", None)):
+        rm, rv = torch.randn(C, device="cuda") * 0.1, torch.rand(C, device="cuda") + 0.5
+        rm2, rv2 = rm.double(), rv.double()
+        z, save = nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.1, 6, r, True, sample_scale=k)
+        v = F.batch_norm(y.double(), rm2, rv2, g.double(), b.double(), True, 0.1, 1e-3)
+        kk = k.double().view(-1, 1, 1, 1) if k is not None else 1.0
+        tag = f"C={C} {kname}"
+        report_abs(f"silu-res bn fwd {tag}", z, F.silu(v) * kk + r.double(), 2.0 ** -7, 0.0, arms=2.0 ** -8)
+        if k is not None:
+            RESULTS.append(torch.equal(z[1], r[1]))
+            print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] silu-res bn {tag}: the dropped sample is its residual")
+        report_abs(f"silu-res bn running_mean {tag}", rm, rm2, 2.0 ** -8, 1e-5)
+        report_abs(f"silu-res bn running_var  {tag}", rv, rv2, 2.0 ** -8, 1e-5)
+        dz = cl(bf(torch.randn(y.shape, device="cuda")))
+        gg, bg = torch.zeros(C, device="cuda"), torch.zeros(C, device="cuda")
+        dy, dres, _ = nv.bn_act_bwd(dz, None, y, save, g, 6, True, gg, bg, beta=b, sample_scale=k)
+        RESULTS.append(dres is dz)
+        print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] silu-res bn bwd {tag}: dres is dz itself (no copy)")
+        yr = y.double().requires_grad_(True)
+        gr, br = g.double().requires_grad_(True), b.double().requires_grad_(True)
+        (F.silu(F.batch_norm(yr, None, None, gr, br, True, 0.1, 1e-3)) * kk).backward(dz.double())
+        report_abs(f"silu-res bn bwd dx {tag}", dy, yr.grad, 2.0 ** -6, 0.0, arms=2.0 ** -7)
+        report_abs(f"silu-res bn bwd dgamma {tag}", gg, gr.grad, 2.0 ** -8, 0.0, arms=2.0 ** -8)
+        report_abs(f"silu-res bn bwd dbeta {tag}", bg, br.grad, 2.0 ** -8, 0.0, arms=2.0 ** -8)
+    ze, _ = nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.1, 6, r, False)
+    ref = F.silu(F.batch_norm(y.double(), rm.double(), rv.double(), g.double(), b.double(), False, 0.1, 1e-3))
+    report_abs(f"silu-res bn eval fwd C={C}", ze, ref + r.double(), 2.0 ** -7, 0.0, arms=2.0 ** -8)
+    refusals = {
+        "code 6 without a residual": lambda: nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.1, 6, None, True),
+        "code 6 with the bit mask": lambda: nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.1, 6, r, True, True),
+        "code 6 keep in eval": lambda: nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.1, 6, r, False, sample_scale=keep),
+        "SiLU (4) with a residual": lambda: nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.1, 4, r, True),
+        "keep with SiLU (4)": lambda: nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.1, 4, r, True, sample_scale=keep),
+        "keep with ReLU": lambda: nv.bn_act_fwd(y, None, g, b, rm, rv, 1e-3, 0.1, True, r, True, sample_scale=keep),
+        "code 6 backward without beta": lambda: nv.bn_act_bwd(dz, None, y, save, g, 6, False, None, None),
+        "code 6 backward with pre-reduced sums": lambda: nv.bn_act_bwd(dz, None, y, save, g, 6, False, None, None,
+                                                                       beta=b, pre_reduced=torch.zeros(2, C,
+                                                                                                       device="cuda")),
+    }
+    failed = []
+    for what, fn in refusals.items():
+        try:
+            fn()
+            failed.append(what)
+        except ValueError:
+            pass
+    RESULTS.append(not failed)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] bn refusals around code 6 C={C} (accepted: {failed})", flush=True)
+
+
+# residual Fused-MBConv blocks as (C, expand, H=W, batch, model): every one of EfficientNetV2-S / -M / -L at its input size
+V2_FUSED_CASES = [(24, 1, 192, 2, "S"), (48, 4, 96, 2, "S"), (64, 4, 48, 4, "S"), (24, 1, 240, 2, "M"),
+                  (48, 4, 120, 2, "M"), (80, 4, 60, 4, "M"), (32, 1, 240, 2, "L"), (64, 4, 120, 2, "L"),
+                  (96, 4, 60, 4, "L")]
+
+
+def _fused_mbconv_case(C, expand, hw, n, label, keep=True, frozen=()):
+    """ops.fused_mbconv on its native node against the float64 composite with the same (bf16) input and weights: z, dx,
+    every trainable parameter's gradient and the running statistics, then the eval forward; frozen parameters keep
+    ``grad is None``.  The bf16 per-layer composition (``fused_mbconv_layers`` under the torch implementation) is
+    printed alongside, and every bound is one that composition meets too: z carries up to three bf16 roundings of
+    values as large as rms(z) (y, and with an expansion h and y2), so its bound is 2^-5 rms(z); the 1x1 projection's
+    weight gradient feeds a BN, so it is orthogonal to its weight row and its elements are small differences of large
+    sums: 2^-4 rms (the composition reaches 1.7x of 2^-5 rms on one shape, the node 1.2x on another)."""
+    import copy
+
+    import torch
+
+    from distributeddeeplearning_b200 import ops
+    from distributeddeeplearning_b200.models.efficientnet_v2 import _BN, FusedMBConv
+    from distributeddeeplearning_b200.ops.efficientnet_v2 import fused_mbconv_composite
+
+    torch.manual_seed(C * 1000 + hw)
+    blk = FusedMBConv(expand, 3, 1, C, C, 0.0, _BN).cuda().train()
+    with torch.no_grad():
+        for mod in blk.modules():
+            if hasattr(mod, "running_var"):
+                mod.weight.uniform_(0.5, 1.5)
+                mod.bias.normal_(0.0, 0.5)
+                mod.running_mean.normal_(0.0, 0.1)
+                mod.running_var.uniform_(0.5, 1.5)
+            elif hasattr(mod, "weight"):
+                mod.weight.copy_(bf(mod.weight).float())            # the kernels' bf16 operand, exactly
+    names = dict(blk.named_parameters())
+    for nm in frozen:
+        names[nm].requires_grad_(False)
+    comp = copy.deepcopy(blk)
+    ref_p = {k: v.detach().double().requires_grad_(k not in frozen) for k, v in names.items()}
+    ref_b = {k: v.double() for k, v in blk.named_buffers() if "running" in k}
+    x = cl(bf(torch.randn(n, C, hw, hw, device="cuda")))
+    kv = None
+    if keep:
+        kv = torch.full((n,), 1.0 / 0.75, device="cuda")
+        kv[1] = 0.0
+    tag = f"{label}: C={C} expand {expand} {hw}x{hw} N={n}{' keep' if keep else ''}{' frozen' if frozen else ''}"
+    print(f"-- fused-mbconv {tag}", flush=True)
+    mods = [(blk.block[i][0], blk.block[i][1]) for i in range(len(blk.block))]
+    cmods = [(comp.block[i][0], comp.block[i][1]) for i in range(len(comp.block))]
+    xn = x.clone().requires_grad_(True)
+    z = ops.fused_mbconv(xn, *[m for pair in mods for m in pair], keep=kv)
+    RESULTS.append(type(z.grad_fn).__name__ == "_FusedMBConvBackward")
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {tag} on the native node: {type(z.grad_fn).__name__}")
+    dz = cl(bf(torch.randn(z.shape, device="cuda")))
+    z.backward(dz)
+    os.environ["DDL_B200_IMPL"] = "torch"
+    try:
+        xc = x.clone().requires_grad_(True)
+        zc = ops.fused_mbconv(xc, *[m for pair in cmods for m in pair], keep=kv)
+        zc.backward(dz)
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+    two = ()
+    if expand > 1:
+        two = (ref_p["block.1.0.weight"], ref_p["block.1.1.weight"], ref_p["block.1.1.bias"],
+               ref_b["block.1.1.running_mean"], ref_b["block.1.1.running_var"], 1e-3, 0.1)
+    xr = x.double().requires_grad_(True)
+    zr = fused_mbconv_composite(xr, ref_p["block.0.0.weight"], ref_p["block.0.1.weight"], ref_p["block.0.1.bias"],
+                                ref_b["block.0.1.running_mean"], ref_b["block.0.1.running_var"], 1e-3, 0.1, True, *two,
+                                keep=kv.double() if kv is not None else None)
+    zr.backward(dz.double())
+    report_abs(f"fused-mbconv z {tag}", z, zr, 2.0 ** -6, 0.0, arms=2.0 ** -5, also=(zc, zr))
+    if keep:
+        RESULTS.append(torch.equal(z[1], x[1]))
+        print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {tag}: the dropped sample is its input")
+    report_abs(f"fused-mbconv dx {tag}", xn.grad, xr.grad, 2.0 ** -5, 0.0, arms=2.0 ** -5, also=(xc.grad, xr.grad))
+    cp = dict(comp.named_parameters())
+    for k, p in names.items():
+        if k in frozen:
+            RESULTS.append(p.grad is None and cp[k].grad is None)
+            print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {tag} {k} frozen: grad stays None", flush=True)
+            continue
+        arms = 2.0 ** -4 if k == "block.1.0.weight" else 2.0 ** -5
+        report_abs(f"fused-mbconv d{k} {tag}", p.grad, ref_p[k].grad, 2.0 ** -5, 0.0, arms=arms,
+                   also=(cp[k].grad, ref_p[k].grad))
+    bufs = dict(blk.named_buffers())
+    for k, v in ref_b.items():
+        report_abs(f"fused-mbconv {k} {tag}", bufs[k], v, 2.0 ** -8, 1e-5)
+    blk.eval()
+    with torch.no_grad():
+        ze = ops.fused_mbconv(x, *[m for pair in mods for m in pair])
+        eb = {k: v.double() for k, v in blk.named_buffers() if "running" in k}
+        two = () if expand == 1 else (ref_p["block.1.0.weight"], ref_p["block.1.1.weight"], ref_p["block.1.1.bias"],
+                                      eb["block.1.1.running_mean"], eb["block.1.1.running_var"], 1e-3, 0.1)
+        zre = fused_mbconv_composite(x.double(), ref_p["block.0.0.weight"], ref_p["block.0.1.weight"],
+                                     ref_p["block.0.1.bias"], eb["block.0.1.running_mean"], eb["block.0.1.running_var"],
+                                     1e-3, 0.1, False, *two)
+    report_abs(f"fused-mbconv eval z {tag}", ze, zre, 2.0 ** -6, 0.0, arms=2.0 ** -5)
+    del blk, comp
+    torch.cuda.empty_cache()
+
+
+def g_efficientnet_v2_layers():
+    """BN code 6 on the flat (C = 64, 128) and 64-channel-chunk (C = 24, 48, 80, 96) mappings, and the one-node
+    Fused-MBConv at every residual Fused-MBConv shape of EfficientNetV2-S / -M / -L, plus frozen parameters."""
+    import torch
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    for C in (64, 128, 24, 48, 80, 96):
+        _silu_res_bn(C)
+    for i, (C, e, hw, n, model) in enumerate(V2_FUSED_CASES):
+        _fused_mbconv_case(C, e, hw, n, model, keep=i not in (0, 4))       # two shapes without a keep vector
+    _fused_mbconv_case(24, 1, 48, 3, "frozen", frozen=("block.0.0.weight", "block.0.1.weight", "block.0.1.bias"))
+    _fused_mbconv_case(48, 4, 24, 3, "frozen", frozen=("block.1.0.weight", "block.0.1.weight", "block.0.1.bias"))
+
+
+def g_efficientnet_v2():
+    """EfficientNetV2: g_efficientnet_v2_layers, efficientnet_v2_s against torchvision at 384, eager vs CUDA-graph
+    training and an fp8 session."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import fp8
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    g_efficientnet_v2_layers()
+    _efficientnet_vs_torchvision("efficientnet_v2_s", 8, 384)
+    dist.init()
+
+    def run(graph, random_drops):
+        torch.manual_seed(0)
+        s = BenchmarkSession("efficientnet_v2_s", 16, True, lr=0.01, momentum=0.9)
+        if not random_drops:        # the eager and the replayed step draw their masks from different counters
+            s.model.classifier[0].p = 0.0
+            for mod in s.model.modules():
+                if hasattr(mod, "sd_prob"):
+                    mod.sd_prob = 0.0
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out[-4:]
+
+    a, b = run(False, False), run(True, False)
+    rel = max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(a, b))
+    ok = all(x == x for x in a + b) and rel < 5e-2
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] efficientnet_v2_s training without random drops: eager {[round(v, 4) for v in a]} "
+          f"graph replay {[round(v, 4) for v in b]} (largest relative difference {rel:.2e})", flush=True)
+    c = run(True, True)
+    ok = all(x == x and abs(x) < 1e4 for x in c)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] efficientnet_v2_s graph-replayed training with stochastic depth and dropout: "
+          f"{[round(v, 4) for v in c]}", flush=True)
+    fp8.reset()
+    fp8.enable(True)
+    try:
+        torch.manual_seed(0)
+        s = BenchmarkSession("efficientnet_v2_s", 16, True, lr=0.01, momentum=0.9)
+        losses = [float(s.step()) for _ in range(4)]
+        torch.cuda.synchronize()
+        s.optimizer.check_errors()
+    finally:
+        fp8.enable(False)
+    ok = all(l == l and abs(l) < 1e4 for l in losses)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] efficientnet_v2_s fp8 session: losses {[round(v, 3) for v in losses]}, "
           f"fp8 launches {fp8.launches()}", flush=True)
     del s
     torch.cuda.empty_cache()
