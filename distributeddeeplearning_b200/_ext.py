@@ -156,8 +156,8 @@ KERNEL_LAUNCHES = {
     "nhwc_u8_to_nhwc4": 1, "cast_f32_bf16": 1, "pack_stem_weight": 1, "unpack_stem_grad": 1, "bias_relu_bwd": 1,
     "dropout": 1, "add_bf16": 1, "fp8_quantize": 1, "fp8_quantize_mx": 1, "fp8_transpose_taps": 1, "fp8_amax": 1, "fp8_update_scales": 1, "pad_nhwc4": 1, "expand_grouped_weight": 1, "concat_channels": 1, "bn_relu_maxpool_fwd": 1, "bn_pool_bwd": 2,
     "dwconv_fwd": 1, "dwconv_dgrad": 1, "dwconv_wgrad": 1, "se_scale": 1, "se_reduce": 1, "se_apply": 1,
-    "hardswish_fwd": 1, "hardswish_bwd": 1, "se_sig_scale": 1, "se_sig_reduce": 1, "se_sig_apply": 1, "pad_cols_bf16": 1,
-    "fold_cols_f32": 1, "silu_rows_fwd": 1, "silu_rows_bwd": 1, "stochastic_depth_keep": 1,
+    "hardswish_fwd": 1, "hardswish_bwd": 1, "se_sig_scale": 1, "se_sig_reduce": 1, "se_sig_apply": 1, "pad_cols": 1,
+    "fold_cols": 1, "silu_rows_fwd": 1, "silu_rows_bwd": 1, "stochastic_depth_keep": 1,
     "dwconv7_fwd": 1, "dwconv7_dgrad": 1, "dwconv7_wgrad": 1, "layer_norm_fwd": 1, "layer_norm_bwd": 1, "gelu_fwd": 1,
     "gelu_bwd": 1, "layer_scale_fwd": 1, "layer_scale_bwd": 1,
     "attention_fwd": 1, "attention_bwd": 2, "add_layer_norm_fwd": 1, "layer_norm_bwd_add": 1, "patchify": 1,
@@ -165,6 +165,7 @@ KERNEL_LAUNCHES = {
     "window_attention_fwd": 1, "window_attention_bwd": 3, "patch_merge_fwd": 1, "patch_merge_bwd": 2,
     "window_attention_v2_fwd": 1, "window_attention_v2_bwd": 3, "cpb_fwd": 1, "cpb_bwd": 2, "merge_gather": 1,
     "grid_attention_fwd": 1, "grid_attention_bwd": 3, "tanh_rows_fwd": 1, "tanh_rows_bwd": 1,
+    "shuffle_fwd": 1, "shuffle_bwd": 2,
 }
 LAUNCH_COUNT = [0]          # kernels of THIS repo launched so far (bench.py reports the per-region delta)
 

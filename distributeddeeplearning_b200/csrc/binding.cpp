@@ -12,6 +12,8 @@
 
 #include <stdexcept>
 #include <string>
+#include <tuple>
+#include <vector>
 
 #include "comm/comm.h"
 #include "ops/conv_gemm.cuh"
@@ -612,12 +614,56 @@ PYBIND11_MODULE(_C, m) {
                                    P<const __nv_bfloat16>(dpooled), P<__nv_bfloat16>(dx), N, HW, C, sms, S(stream)),
           "se_sig_apply");
   });
-  m.def("pad_cols_bf16", [](ptr_t src, ptr_t dst, int rows, int k, int kp, ptr_t stream) {
-    check(ddl::launch_pad_cols_bf16(P<const __nv_bfloat16>(src), P<__nv_bfloat16>(dst), rows, k, kp, S(stream)),
-          "pad_cols_bf16");
+  // bn_*: (sum, sumsq, gamma, beta, mean, invstd, running_mean, running_var, dgamma, dbeta, gamma_grad, beta_grad,
+  // eps, momentum) as pointers (0 = none) and two floats; see ShuffleArgs
+  using ShBn = std::tuple<ptr_t, ptr_t, ptr_t, ptr_t, ptr_t, ptr_t, ptr_t, ptr_t, ptr_t, ptr_t, ptr_t, ptr_t, float, float>;
+  auto sh_bn = [](const ShBn& t) {
+    return ddl::ShuffleBn{P<const float>(std::get<0>(t)), P<const float>(std::get<1>(t)), P<const float>(std::get<2>(t)),
+                          P<const float>(std::get<3>(t)), P<float>(std::get<4>(t)), P<float>(std::get<5>(t)),
+                          P<float>(std::get<6>(t)), P<float>(std::get<7>(t)), std::get<12>(t), std::get<13>(t),
+                          P<float>(std::get<8>(t)), P<float>(std::get<9>(t)), P<float>(std::get<10>(t)),
+                          P<float>(std::get<11>(t))};
+  };
+  m.def("shuffle_fwd", [sh_bn](ptr_t a, ptr_t b, ptr_t s0, ptr_t s1, int M, int half, int ld_ab, int ld_s, int split,
+                               int a_bn, int train, const ShBn& bn_a, const ShBn& bn_b, int sms, ptr_t stream) {
+    ddl::ShuffleArgs p{};
+    p.a = P<const __nv_bfloat16>(a); p.b = P<const __nv_bfloat16>(b); p.s0 = P<__nv_bfloat16>(s0); p.s1 = P<__nv_bfloat16>(s1);
+    p.M = M; p.half = half; p.ld_ab = ld_ab; p.ld_s = ld_s; p.split = split; p.a_bn = a_bn; p.train = train;
+    p.bn_a = sh_bn(bn_a); p.bn_b = sh_bn(bn_b);
+    check(ddl::launch_shuffle_fwd(p, sms, S(stream)), "shuffle_fwd");
   });
-  m.def("fold_cols_f32", [](ptr_t src, ptr_t dst, int rows, int k, int kp, ptr_t stream) {
-    check(ddl::launch_fold_cols_f32(P<const float>(src), P<float>(dst), rows, k, kp, S(stream)), "fold_cols_f32");
+  m.def("shuffle_bwd", [sh_bn](ptr_t ds0, ptr_t ds1, ptr_t a, ptr_t b, ptr_t da, ptr_t db, int M, int half, int ld_ab,
+                               int ld_s, int split, int a_bn, const ShBn& bn_a, const ShBn& bn_b, int sms, ptr_t stream) {
+    ddl::ShuffleArgs p{};
+    p.ds0 = P<const __nv_bfloat16>(ds0); p.ds1 = P<const __nv_bfloat16>(ds1); p.a = P<const __nv_bfloat16>(a);
+    p.b = P<const __nv_bfloat16>(b); p.da = P<__nv_bfloat16>(da); p.db = P<__nv_bfloat16>(db);
+    p.M = M; p.half = half; p.ld_ab = ld_ab; p.ld_s = ld_s; p.split = split; p.a_bn = a_bn; p.train = 1;
+    p.bn_a = sh_bn(bn_a); p.bn_b = sh_bn(bn_b);
+    check(ddl::launch_shuffle_bwd(p, sms, S(stream)), "shuffle_bwd");
+  });
+  // mats: [(src, dst, rows, k, prows, kp, element bytes)]
+  m.def("pad_cols", [](const std::vector<std::tuple<ptr_t, ptr_t, int, int, int, int, int>>& mats, ptr_t stream) {
+    if (mats.empty() || mats.size() > static_cast<size_t>(ddl::kPadMax)) throw std::runtime_error("pad_cols: 1..kPadMax matrices");
+    ddl::PadBatch b{};
+    b.n = static_cast<int>(mats.size());
+    for (int i = 0; i < b.n; ++i) {
+      const auto& t = mats[i];
+      b.m[i] = ddl::PadMatrix{P<const void>(std::get<0>(t)), P<void>(std::get<1>(t)), std::get<2>(t), std::get<3>(t),
+                              std::get<4>(t), std::get<5>(t), std::get<6>(t)};
+    }
+    check(ddl::launch_pad_cols(b, S(stream)), "pad_cols");
+  });
+  // mats: [(src, dst, rows, k, kp, add)]
+  m.def("fold_cols", [](const std::vector<std::tuple<ptr_t, ptr_t, int, int, int, int>>& mats, ptr_t stream) {
+    if (mats.empty() || mats.size() > static_cast<size_t>(ddl::kPadMax)) throw std::runtime_error("fold_cols: 1..kPadMax matrices");
+    ddl::FoldBatch b{};
+    b.n = static_cast<int>(mats.size());
+    for (int i = 0; i < b.n; ++i) {
+      const auto& t = mats[i];
+      b.m[i] = ddl::FoldMatrix{P<const void>(std::get<0>(t)), P<void>(std::get<1>(t)), std::get<2>(t), std::get<3>(t),
+                               std::get<4>(t), std::get<5>(t)};
+    }
+    check(ddl::launch_fold_cols(b, S(stream)), "fold_cols");
   });
   m.def("tanh_rows_fwd", [](ptr_t x, ptr_t y, int64_t n, ptr_t stream) {
     check(ddl::launch_tanh_rows_fwd(P<const __nv_bfloat16>(x), P<__nv_bfloat16>(y), n, S(stream)), "tanh_rows_fwd");

@@ -332,10 +332,31 @@ cudaError_t launch_se_sig_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* x
                                  __nv_bfloat16* ds, int ldd, int N, int HW, int C, cudaStream_t stream);
 cudaError_t launch_se_sig_apply(const __nv_bfloat16* dy, const __nv_bfloat16* s, int lds, const __nv_bfloat16* dpooled,
                                 __nv_bfloat16* dx, int N, int HW, int C, int sms, cudaStream_t stream);
-// bf16 [rows][k] -> [rows][kp] with zero columns [k, kp) (the squeeze dimension of fc2's weight padded to 8)
-cudaError_t launch_pad_cols_bf16(const __nv_bfloat16* src, __nv_bfloat16* dst, int rows, int k, int kp, cudaStream_t stream);
-// fp32 dst [rows][k] += src [rows][kp] columns [0, k)  (fc2's weight gradient folded into its compact slot)
-cudaError_t launch_fold_cols_f32(const float* src, float* dst, int rows, int k, int kp, cudaStream_t stream);
+// Batched zero padding: each matrix src [rows][k] (bf16 or fp32: esize 2 / 4) -> dst [prows][kp] with src in the
+// top-left corner and zeros elsewhere (fc2's squeeze dimension padded to 8; ShuffleNetV2's operands padded to 8 in both
+// dimensions), one launch for up to kPadMax matrices
+constexpr int kPadMax = 24;
+struct PadMatrix {
+  const void* src;
+  void* dst;
+  int rows, k, prows, kp, esize;
+};
+struct PadBatch {
+  PadMatrix m[kPadMax];
+  int n;
+};
+cudaError_t launch_pad_cols(const PadBatch& b, cudaStream_t stream);
+// Batched fold: fp32 dst [rows][k] += src [>= rows][kp] columns [0, k) (add), or = (copy: running statistics)
+struct FoldMatrix {
+  const void* src;
+  void* dst;
+  int rows, k, kp, add;
+};
+struct FoldBatch {
+  FoldMatrix m[kPadMax];
+  int n;
+};
+cudaError_t launch_fold_cols(const FoldBatch& b, cudaStream_t stream);
 // SiLU on the rows of a bf16 matrix: y [N][ldy] = silu(x [N][ldx]) for columns [0, ldy) (ldy <= ldx, both % 8 == 0), and
 // its backward dx [N][ldx] = dy [N][ldy] * silu'(x) for columns < c_valid, zero elsewhere (a GEMM operand with zero pad)
 // tanh on n bf16 elements (n % 8 == 0), and dx = dy * (1 - y^2) from the saved output y
@@ -367,6 +388,42 @@ struct CatArgs {
 cudaError_t launch_concat_channels(const CatArgs& a, bool scatter, cudaStream_t stream);
 cudaError_t launch_add_bf16(const __nv_bfloat16* a, const __nv_bfloat16* b, __nv_bfloat16* y, int64_t n,
                             cudaStream_t stream);
+
+// ---- ShuffleNetV2: channel shuffle fused into the branch BatchNorm (shufflenet.cu) ----------------------------------
+// s[2i] = a[i] (stride 1: the pass-through, a bit copy) or relu(BN_a(a[i])) (stride 2), s[2i+1] = relu(BN_b(b[i])),
+// i < half (even).  a, b and the backward outputs da, db: [M][ld_ab]; s whole [M][ld_s] or its halves lo = s[:, :half],
+// hi = s[:, half:] ([M][ld_ab] each, split).  Channels past the real width are written as zeros.
+struct ShuffleBn {
+  const float* sum;          // train forward: per-channel sum / sum of squares of the conv output (conv epilogue)
+  const float* sumsq;
+  const float* gamma;        // [half]
+  const float* beta;
+  float* mean;               // [half]: written by a train forward, read by backward
+  float* invstd;
+  float* running_mean;       // [half]: updated by a train forward (may be null), read in eval
+  float* running_var;
+  float eps, momentum;
+  float* dgamma;             // backward: [half] zeroed scratch receiving the sums
+  float* dbeta;
+  float* gamma_grad;         // backward, optional: accumulate targets
+  float* beta_grad;
+};
+struct ShuffleArgs {
+  const __nv_bfloat16* a;    // forward input / backward saved conv output (a_bn only)
+  const __nv_bfloat16* b;
+  __nv_bfloat16* s0;         // forward output: s, or lo
+  __nv_bfloat16* s1;         //   hi (split)
+  const __nv_bfloat16* ds0;  // backward input: ds, or dlo
+  const __nv_bfloat16* ds1;  //   dhi (split)
+  __nv_bfloat16* da;         // backward output: the pass-through gradient (stride 1) or BN_a's input gradient
+  __nv_bfloat16* db;         //   BN_b's input gradient
+  int M, half, ld_ab, ld_s;  // ld_s: row pitch of s, or of lo / hi (= ld_ab)
+  int split, a_bn, train;
+  ShuffleBn bn_a, bn_b;
+};
+cudaError_t launch_shuffle_fwd(const ShuffleArgs& p, int sms, cudaStream_t stream);
+// two launches: the reduce pass (and the pass-through copy), then the apply pass
+cudaError_t launch_shuffle_bwd(const ShuffleArgs& p, int sms, cudaStream_t stream);
 
 // ---- FP8 operand preparation (fp8.cu) ----------------------------------------------------------------
 cudaError_t launch_fp8_quantize(const __nv_bfloat16* x, uint8_t* out, int64_t n, Fp8Slot* slot, bool e5m2, int sms,

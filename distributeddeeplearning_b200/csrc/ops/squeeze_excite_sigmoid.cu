@@ -9,10 +9,15 @@
 //
 // EfficientNet's squeeze widths C' = C_in / 4 (4, 6, 10, 12, 14, ...) are not multiples of 8, so fc2's K = C' cannot be
 // a TMA operand (row pitch not a multiple of 16 bytes).  The squeeze dimension is padded to C'8 = C' rounded up to 8 with
-// zero columns: pad_cols_bf16 builds the padded bf16 fc2 weight [C][C'8] each forward (graph capture records it), and
-// fold_cols_f32 adds the padded fp32 weight gradient [C][C'8] into the compact slot [C][C'].
+// zero columns: pad_cols builds the padded bf16 fc2 weight [C][C'8] each forward (graph capture records it), and
+// fold_cols adds the padded fp32 weight gradient [C][C'8] into the compact slot [C][C'].
+// Both take a batch of up to kPadMax matrices per launch, each padded in rows and columns: ShuffleNetV2's units pad
+// every operand of a unit whose widths are not multiples of 8 (bf16 weights, fp32 BN parameters and running
+// statistics) in one launch, and fold the padded gradients (or copy the running statistics) back in one more.
 #include "../common.cuh"
 #include "ops.h"
+
+#include <algorithm>
 
 namespace ddl {
 
@@ -125,23 +130,33 @@ __global__ void __launch_bounds__(kSgThreads) sesig_apply_kernel(const __nv_bflo
   }
 }
 
-__global__ void __launch_bounds__(kSgThreads) pad_cols_bf16_kernel(const __nv_bfloat16* __restrict__ src,
-                                                                   __nv_bfloat16* __restrict__ dst, int rows, int k,
-                                                                   int kp) {
-  const int64_t total = static_cast<int64_t>(rows) * kp;
+// blockIdx.y = matrix: dst [prows][kp] = src [rows][k] in its top-left corner, zeros elsewhere (2- or 4-byte elements)
+__global__ void __launch_bounds__(kSgThreads) pad_cols_kernel(PadBatch b) {
+  const PadMatrix& m = b.m[blockIdx.y];
+  const int64_t total = static_cast<int64_t>(m.prows) * m.kp;
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(i % kp);
-    dst[i] = c < k ? src[(i / kp) * k + c] : __float2bfloat16_rn(0.f);
+    const int r = static_cast<int>(i / m.kp), c = static_cast<int>(i % m.kp);
+    const bool in = r < m.rows && c < m.k;
+    const int64_t s = static_cast<int64_t>(r) * m.k + c;
+    if (m.esize == 4)
+      static_cast<uint32_t*>(m.dst)[i] = in ? static_cast<const uint32_t*>(m.src)[s] : 0u;
+    else
+      static_cast<uint16_t*>(m.dst)[i] = in ? static_cast<const uint16_t*>(m.src)[s] : static_cast<uint16_t>(0);
   }
 }
 
-__global__ void __launch_bounds__(kSgThreads) fold_cols_f32_kernel(const float* __restrict__ src, float* __restrict__ dst,
-                                                                   int rows, int k, int kp) {
-  const int64_t total = static_cast<int64_t>(rows) * k;
+// blockIdx.y = matrix: fp32 dst [rows][k] (+)= src [>= rows][kp] columns [0, k)
+__global__ void __launch_bounds__(kSgThreads) fold_cols_kernel(FoldBatch b) {
+  const FoldMatrix& m = b.m[blockIdx.y];
+  const int64_t total = static_cast<int64_t>(m.rows) * m.k;
+  const float* src = static_cast<const float*>(m.src);
+  float* dst = static_cast<float*>(m.dst);
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
-       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
-    dst[i] += src[(i / k) * kp + i % k];
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const float v = src[(i / m.k) * m.kp + i % m.k];
+    dst[i] = m.add ? dst[i] + v : v;
+  }
 }
 
 // 16 blocks of 256 threads per SM at most (grid-stride beyond that)
@@ -182,16 +197,27 @@ cudaError_t launch_se_sig_apply(const __nv_bfloat16* dy, const __nv_bfloat16* s,
   return cudaGetLastError();
 }
 
-cudaError_t launch_pad_cols_bf16(const __nv_bfloat16* src, __nv_bfloat16* dst, int rows, int k, int kp,
-                                 cudaStream_t stream) {
-  if (rows <= 0 || k <= 0 || kp < k) return cudaErrorInvalidValue;
-  pad_cols_bf16_kernel<<<sg_grid(static_cast<int64_t>(rows) * kp, 132), kSgThreads, 0, stream>>>(src, dst, rows, k, kp);
+cudaError_t launch_pad_cols(const PadBatch& b, cudaStream_t stream) {
+  if (b.n <= 0 || b.n > kPadMax) return cudaErrorInvalidValue;
+  int64_t most = 0;
+  for (int i = 0; i < b.n; ++i) {
+    const PadMatrix& m = b.m[i];
+    if (m.rows <= 0 || m.k <= 0 || m.prows < m.rows || m.kp < m.k || (m.esize != 2 && m.esize != 4)) return cudaErrorInvalidValue;
+    most = std::max(most, static_cast<int64_t>(m.prows) * m.kp);
+  }
+  pad_cols_kernel<<<dim3(sg_grid(most, 132), b.n), kSgThreads, 0, stream>>>(b);
   return cudaGetLastError();
 }
 
-cudaError_t launch_fold_cols_f32(const float* src, float* dst, int rows, int k, int kp, cudaStream_t stream) {
-  if (rows <= 0 || k <= 0 || kp < k) return cudaErrorInvalidValue;
-  fold_cols_f32_kernel<<<sg_grid(static_cast<int64_t>(rows) * k, 132), kSgThreads, 0, stream>>>(src, dst, rows, k, kp);
+cudaError_t launch_fold_cols(const FoldBatch& b, cudaStream_t stream) {
+  if (b.n <= 0 || b.n > kPadMax) return cudaErrorInvalidValue;
+  int64_t most = 0;
+  for (int i = 0; i < b.n; ++i) {
+    const FoldMatrix& m = b.m[i];
+    if (m.rows <= 0 || m.k <= 0 || m.kp < m.k) return cudaErrorInvalidValue;
+    most = std::max(most, static_cast<int64_t>(m.rows) * m.k);
+  }
+  fold_cols_kernel<<<dim3(sg_grid(most, 132), b.n), kSgThreads, 0, stream>>>(b);
   return cudaGetLastError();
 }
 

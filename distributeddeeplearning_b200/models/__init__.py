@@ -7,9 +7,9 @@ AlexNet (SURVEY.md 2.7); ResNet-18/34, the other VGG depths, DenseNet and Squeez
 0.2.1's families) are here too, and the later ResNet family members of torchvision (ResNeXt-50 32x4d, ResNeXt-101
 32x8d / 64x4d, Wide ResNet-50-2 / 101-2), MobileNetV2, MobileNetV3-Large / -Small, EfficientNet-B0 to -B7,
 ConvNeXt-Tiny / -Small / -Base / -Large, the Vision Transformers ViT-B/16, -B/32, -L/16 and -L/32, the Swin
-Transformers Swin-T, -S and -B, the Swin Transformers V2 Swin-V2-T, -S and -B, MaxViT-T, and the RegNets:
+Transformers Swin-T, -S and -B, the Swin Transformers V2 Swin-V2-T, -S and -B, MaxViT-T, the RegNets:
 RegNetX-400MF, -800MF, -1.6GF, -3.2GF, -8GF, -16GF and -32GF, and RegNetY-400MF, -800MF, -1.6GF, -3.2GF, -8GF, -16GF,
--32GF and -128GF.
+-32GF and -128GF, and ShuffleNetV2 x0.5, x1.0, x1.5 and x2.0.
 """
 from __future__ import annotations
 
@@ -30,6 +30,8 @@ from .regnet import (RegNet, regnet_x_1_6gf, regnet_x_3_2gf, regnet_x_8gf, regne
                      regnet_y_32gf, regnet_y_128gf, regnet_y_400mf, regnet_y_800mf)
 from .resnet import (ResNet, resnet18, resnet34, resnet50, resnet101, resnet152, resnext50_32x4d,  # noqa: F401
                      resnext101_32x8d, resnext101_64x4d, wide_resnet50_2, wide_resnet101_2)
+from .shufflenetv2 import (ShuffleNetV2, shufflenet_v2_x0_5, shufflenet_v2_x1_0,  # noqa: F401
+                           shufflenet_v2_x1_5, shufflenet_v2_x2_0)
 from .squeezenet import SqueezeNet, squeezenet1_0, squeezenet1_1  # noqa: F401
 from .swin import SwinTransformer, swin_b, swin_s, swin_t  # noqa: F401
 from .swin_v2 import INPUT_SIZE as _SWIN_V2_INPUT_SIZE, SwinTransformerV2, swin_v2_b, swin_v2_s, swin_v2_t  # noqa: F401
@@ -48,7 +50,8 @@ _REGISTRY = {
               vgg13_bn, vgg16, vgg16_bn, vgg19, vgg19_bn, vit_b_16, vit_b_32, vit_l_16, vit_l_32, swin_t, swin_s, swin_b,
               swin_v2_t, swin_v2_s, swin_v2_b, maxvit_t, regnet_x_400mf, regnet_x_800mf, regnet_x_1_6gf,
               regnet_x_3_2gf, regnet_x_8gf, regnet_x_16gf, regnet_x_32gf, regnet_y_400mf, regnet_y_800mf,
-              regnet_y_1_6gf, regnet_y_3_2gf, regnet_y_8gf, regnet_y_16gf, regnet_y_32gf, regnet_y_128gf)
+              regnet_y_1_6gf, regnet_y_3_2gf, regnet_y_8gf, regnet_y_16gf, regnet_y_32gf, regnet_y_128gf,
+              shufflenet_v2_x0_5, shufflenet_v2_x1_0, shufflenet_v2_x1_5, shufflenet_v2_x2_0)
 }
 
 

@@ -1176,20 +1176,51 @@ def se_apply(dy: torch.Tensor, s: torch.Tensor, dpooled: torch.Tensor, gate: str
 def pad_cols_bf16(w: torch.Tensor, kp: int) -> torch.Tensor:
     """bf16 [rows, k] -> [rows, kp] with zero columns [k, kp): fc2's weight with its squeeze dimension padded to a
     multiple of 8, so that its rows are 16-byte GEMM operand rows."""
-    if w.dtype != torch.bfloat16 or not w.is_cuda or w.dim() != 2 or not w.is_contiguous() or kp < w.shape[1]:
+    if w.dtype != torch.bfloat16 or w.dim() != 2 or kp < w.shape[1]:
         raise ValueError(f"pad_cols_bf16: expected a contiguous CUDA bf16 matrix with at most {kp} columns")
-    out = torch.empty((w.shape[0], kp), dtype=torch.bfloat16, device=w.device)
-    _C().pad_cols_bf16(w.data_ptr(), out.data_ptr(), w.shape[0], w.shape[1], kp, _stream())
+    return pad_cols([(w, w.shape[0], kp)])[0]
+
+
+def pad_cols(mats) -> list:
+    """Zero-padded copies of up to 24 matrices in ONE launch: ``mats`` = [(src, prows, kp)] with ``src`` a contiguous
+    CUDA bf16 or fp32 tensor viewed as [rows, k] (its first dimension, the rest flattened; a vector is one row), and the
+    result for each a new [prows, kp] tensor of the same dtype holding ``src`` in its top-left corner, zeros elsewhere."""
+    out, desc = [], []
+    for src, prows, kp in mats:
+        rows, k = (1, src.numel()) if src.dim() == 1 else (src.shape[0], src.numel() // max(1, src.shape[0]))
+        if src.dtype not in (torch.bfloat16, torch.float32) or not src.is_cuda or not src.is_contiguous() \
+                or prows < rows or kp < k or rows <= 0 or k <= 0:
+            raise ValueError(f"pad_cols: expected contiguous CUDA bf16 / fp32 matrices of at most [{prows}, {kp}], got "
+                             f"{tuple(src.shape)} {src.dtype}")
+        dst = torch.empty((prows, kp), dtype=src.dtype, device=src.device)
+        out.append(dst)
+        desc.append((src.data_ptr(), dst.data_ptr(), rows, k, prows, kp, src.element_size()))
+    if not 0 < len(desc) <= 24:
+        raise ValueError("pad_cols: 1 to 24 matrices per launch")
+    _C().pad_cols(desc, _stream())
     return out
 
 
 def fold_cols_f32(src: torch.Tensor, dst: torch.Tensor) -> None:
     """dst [rows, k] (fp32, any contiguous shape of rows * k elements) += src [rows, kp][:, :k]."""
-    rows, kp = src.shape
-    if src.dtype != torch.float32 or dst.dtype != torch.float32 or not src.is_contiguous() or not dst.is_contiguous() \
-            or dst.numel() % rows != 0 or dst.numel() // rows > kp:
-        raise ValueError("fold_cols_f32: expected contiguous fp32 src [rows, kp] and dst [rows, k <= kp]")
-    _C().fold_cols_f32(src.data_ptr(), dst.data_ptr(), rows, dst.numel() // rows, kp, _stream())
+    fold_cols([(src, dst, src.shape[0])])
+
+
+def fold_cols(mats, add: bool = True) -> None:
+    """ONE launch over up to 24 pairs ``(src [prows, kp], dst, rows)``: fp32 ``dst`` (contiguous, rows * k elements)
+    += ``src[:rows, :k]`` (``add``), or = it (the running statistics of a padded BatchNorm)."""
+    desc = []
+    for src, dst, rows in mats:
+        if src.dim() == 1:
+            src = src.view(1, -1)
+        if src.dtype != torch.float32 or dst.dtype != torch.float32 or not src.is_contiguous() \
+                or not dst.is_contiguous() or rows <= 0 or rows > src.shape[0] or dst.numel() % rows != 0 \
+                or dst.numel() // rows > src.shape[1]:
+            raise ValueError("fold_cols: expected contiguous fp32 src [prows, kp] and dst [rows <= prows, k <= kp]")
+        desc.append((src.data_ptr(), dst.data_ptr(), rows, dst.numel() // rows, src.shape[1], int(add)))
+    if not 0 < len(desc) <= 24:
+        raise ValueError("fold_cols: 1 to 24 matrices per launch")
+    _C().fold_cols(desc, _stream())
 
 
 def silu_rows_fwd(x: torch.Tensor, cols: int) -> torch.Tensor:
@@ -2080,6 +2111,77 @@ def dgrad_fuses_bn_reduce(kernel: Tuple[int, int], stride: int, pad) -> bool:
     GEMMs; the y tile is fetched under the MMAs), no for window convolutions, where the statistics epilogue of their many
     short tiles costs more than the reduction pass it replaces."""
     return tuple(kernel) == (1, 1) and stride == 1 and _pad2(pad) == (0, 0)
+
+
+# ------------------------------------------------------------------------------------------------
+# ShuffleNetV2: channel shuffle fused into the branch BatchNorm (csrc/ops/shufflenet.cu)
+# ------------------------------------------------------------------------------------------------
+def _sh_bn(bn) -> tuple:
+    """(sum, sumsq, gamma, beta, mean, invstd, running_mean, running_var, dgamma, dbeta, gamma_grad, beta_grad, eps,
+    momentum) of the binding from a dict of tensors (missing entries: none)."""
+    if bn is None:
+        return (0,) * 12 + (0.0, 0.0)
+    keys = ("sum", "sumsq", "gamma", "beta", "mean", "invstd", "running_mean", "running_var", "dgamma", "dbeta",
+            "gamma_grad", "beta_grad")
+    for k in keys:
+        t = bn.get(k)
+        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous()):
+            raise ValueError(f"shuffle: BN {k} must be a contiguous CUDA fp32 vector")
+    return tuple(_ptr(bn.get(k)) for k in keys) + (float(bn.get("eps", 0.0)), float(bn.get("momentum", 0.0)))
+
+
+def _sh_geometry(ab: torch.Tensor, half: int):
+    _check_act(ab, "a / b")
+    N, ld_ab, H, W = ab.shape
+    if half <= 0 or half % 2 != 0 or ld_ab != _ceil_div(half, 8) * 8:
+        raise ValueError(f"shuffle: half = {half} must be even and the branch tensors {ld_ab} = half rounded up to 8 wide")
+    return N, ld_ab, H, W
+
+
+def shuffle_fwd(a: torch.Tensor, b: torch.Tensor, half: int, split: bool, train: bool, bn_b: dict,
+                bn_a: Optional[dict] = None):
+    """s[2i] = a[i] (a bit copy; with ``bn_a``: relu(BN_a(a[i]))), s[2i+1] = relu(BN_b(b[i])) for i < ``half``.
+    ``a``, ``b``: NHWC bf16 [N, p(half), H, W] with p(c) = c rounded up to 8, zero beyond ``half``.  Returns (lo, hi) =
+    (s[:, :half], s[:, half:]) as two [N, p(half), H, W] tensors (``split``) or s as one [N, p(2 half), H, W] tensor,
+    zero in the pad channels.  ``bn_*``: dicts of fp32 vectors: gamma, beta, running_mean, running_var, eps, momentum;
+    in training also the conv epilogue's sum / sumsq and the mean / invstd outputs the backward reads."""
+    N, ld, H, W = _sh_geometry(b, half)
+    if tuple(a.shape) != tuple(b.shape):
+        raise ValueError("shuffle_fwd: a and b must have the same shape")
+    _check_act(a, "a")
+    if split:
+        s0, s1 = empty_act(N, ld, H, W, b.device), empty_act(N, ld, H, W, b.device)
+        ld_s = ld
+    else:
+        ld_s = _ceil_div(2 * half, 8) * 8
+        s0, s1 = empty_act(N, ld_s, H, W, b.device), None
+    _C().shuffle_fwd(a.data_ptr(), b.data_ptr(), s0.data_ptr(), _ptr(s1), N * H * W, half, ld, ld_s, int(split),
+                     int(bn_a is not None), int(train), _sh_bn(bn_a), _sh_bn(bn_b), sm_count(b.device.index or 0),
+                     _stream())
+    return (s0, s1) if split else s0
+
+
+def shuffle_bwd(ds, b: torch.Tensor, half: int, bn_b: dict, a: Optional[torch.Tensor] = None,
+                bn_a: Optional[dict] = None):
+    """Backward of :func:`shuffle_fwd` in training: ``ds`` the gradient of s, or the pair (dlo, dhi).  Returns (da, db):
+    the pass-through gradient (a bit copy) or, with ``bn_a``, the gradient of branch1's conv output ``a``, and the
+    gradient of ``b``, both [N, p(half), H, W] with zero pad channels.  ``bn_*`` as in the forward plus dgamma / dbeta
+    (zeroed fp32 scratch) and the optional gamma_grad / beta_grad accumulators.  Two launches: reduce, apply."""
+    N, ld, H, W = _sh_geometry(b, half)
+    split = isinstance(ds, (tuple, list))
+    parts = list(ds) if split else [ds]
+    ld_s = ld if split else _ceil_div(2 * half, 8) * 8
+    for t in parts:
+        _check_act(t, "ds")
+        if tuple(t.shape) != (N, ld_s, H, W):
+            raise ValueError(f"shuffle_bwd: gradient of shape {tuple(t.shape)}, expected {(N, ld_s, H, W)}")
+    if (bn_a is None) != (a is None):
+        raise ValueError("shuffle_bwd: a and bn_a go together")
+    da, db = empty_act(N, ld, H, W, b.device), empty_act(N, ld, H, W, b.device)
+    _C().shuffle_bwd(parts[0].data_ptr(), parts[1].data_ptr() if split else 0, _ptr(a), b.data_ptr(), da.data_ptr(),
+                     db.data_ptr(), N * H * W, half, ld, ld_s, int(split), int(bn_a is not None), _sh_bn(bn_a),
+                     _sh_bn(bn_b), sm_count(b.device.index or 0), _stream())
+    return da, db
 
 
 # ------------------------------------------------------------------------------------------------

@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "shufflenet", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -5111,6 +5111,477 @@ def g_regnet():
     RESULTS.append(loss == loss)
     print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] regnet_y_128gf batch 8 step: loss {loss:.4f}, peak memory "
           f"{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB", flush=True)
+
+
+# ShuffleNetV2 units as (inp, oup, stride, input H = W) of x0.5 / x1.0 / x1.5 / x2.0 at 224; a stride-1 shape is run with
+# the split (lo, hi) output of a unit inside a stage and with the whole output of a stage's last unit
+def shufflenet_unit_shapes():
+    from distributeddeeplearning_b200.models.shufflenetv2 import _WIDTHS
+
+    out = []
+    for name, w in _WIDTHS.items():
+        inp, hw = w[0], 56
+        for oup in w[1:4]:
+            out.append((name, inp, oup, 2, hw))
+            hw //= 2
+            out.append((name, oup, oup, 1, hw))
+            inp = oup
+    return out
+
+
+def _p8(c):
+    return (c + 7) // 8 * 8
+
+
+def _pad_zero(name, t, real):
+    ok = t.shape[1] == _p8(real) and bool((t[:, real:] == 0).all().item())
+    RESULTS.append(ok)
+    if not ok:
+        print(f"[FAIL] {name}: pad channels [{real}, {t.shape[1]}) not exactly zero", flush=True)
+    return ok
+
+
+def _padded_act(n, c, hw, scale=1.0):
+    import torch
+
+    t = torch.zeros(n, _p8(c), hw, hw, device="cuda")
+    t[:, :c] = torch.randn(n, c, hw, hw, device="cuda") * scale
+    return cl(bf(t))
+
+
+def _shuffle_kernels():
+    """shuffle_fwd / shuffle_bwd against float64 in train and eval, split and whole, with and without branch1's BN: the
+    pass-through half bit for bit, the BN halves under the bn group's budget, the pad channels exactly zero; pad_cols and
+    fold_cols bit for bit."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    n, hw = 4, 9
+    for half, split, abn in ((58, True, False), (58, False, True), (122, False, False), (48, True, True),
+                             (24, False, False)):
+        torch.manual_seed(half)
+        pb = _p8(half)
+        a, b = _padded_act(n, half, hw, 2.0), _padded_act(n, half, hw, 2.0)
+        tag = f"half={half} {'split' if split else 'whole'}{' bn_a' if abn else ''}"
+
+        def params():
+            return dict(gamma=torch.rand(half, device="cuda") + 0.5, beta=torch.randn(half, device="cuda"),
+                        running_mean=torch.randn(half, device="cuda") * 0.1,
+                        running_var=torch.rand(half, device="cuda") + 0.5, eps=1e-5, momentum=0.1)
+
+        pa, pbn = params(), params()
+        refs = {}
+        for side, t, p in (("a", a, pa), ("b", b, pbn)):
+            refs[side] = (p["running_mean"].double().clone(), p["running_var"].double().clone())
+            st = torch.stack([t[:, :half].float().sum((0, 2, 3)), t[:, :half].float().pow(2).sum((0, 2, 3))])
+            p.update(sum=st[0].contiguous(), sumsq=st[1].contiguous(), mean=torch.empty(half, device="cuda"),
+                     invstd=torch.empty(half, device="cuda"))
+        out = nv.shuffle_fwd(a, b, half, split, True, pbn, pa if abn else None)
+        s = torch.cat([out[0][:, :half], out[1][:, :half]], 1) if split else out[:, :2 * half]
+        for t in (out if split else (out,)):
+            _pad_zero(f"shuffle fwd {tag} pad", t, half if split else 2 * half)
+
+        def ref_bn(t, p, side, train=True):
+            rm, rv = refs[side]
+            return F.relu(F.batch_norm(t[:, :half].double(), rm, rv, p["gamma"].double(), p["beta"].double(), train,
+                                       0.1, 1e-5))
+
+        rb = ref_bn(b, pbn, "b")
+        ra = ref_bn(a, pa, "a") if abn else a[:, :half].double()
+        report_abs(f"shuffle fwd odd channels {tag}", s[:, 1::2], rb, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+        if abn:
+            report_abs(f"shuffle fwd even channels (BN_a) {tag}", s[:, 0::2], ra, 2.0 ** -7, 0.0, arms=2.0 ** -8)
+        else:
+            _exact(f"shuffle fwd pass-through half bit for bit {tag}", torch.equal(s[:, 0::2], a[:, :half]))
+        report_abs(f"shuffle fwd running_mean {tag}", pbn["running_mean"], refs["b"][0], 2.0 ** -8, 1e-5)
+        report_abs(f"shuffle fwd running_var {tag}", pbn["running_var"], refs["b"][1], 2.0 ** -8, 1e-5)
+        # backward
+        ds = [_padded_act(n, half, hw), _padded_act(n, half, hw)] if split else [_padded_act(n, 2 * half, hw)]
+        dsr = torch.cat([d[:, :half] for d in ds], 1) if split else ds[0][:, :2 * half]
+        for p in (pa, pbn):
+            scr = torch.zeros(2, half, device="cuda")
+            p.update(dgamma=scr[0], dbeta=scr[1], gamma_grad=torch.zeros(half, device="cuda"),
+                     beta_grad=torch.zeros(half, device="cuda"))
+        da, db = nv.shuffle_bwd(tuple(ds) if split else ds[0], b, half, pbn, a=a if abn else None,
+                                bn_a=pa if abn else None)
+        _pad_zero(f"shuffle bwd {tag} da pad", da, half)
+        _pad_zero(f"shuffle bwd {tag} db pad", db, half)
+        for side, t, p, dt, g in (("b", b, pbn, db, dsr[:, 1::2]), ("a", a, pa, da, dsr[:, 0::2])):
+            if side == "a" and not abn:
+                _exact(f"shuffle bwd pass-through gradient bit for bit {tag}", torch.equal(da[:, :half], g))
+                continue
+            tr = t[:, :half].double().requires_grad_(True)
+            gr = p["gamma"].double().requires_grad_(True)
+            br = p["beta"].double().requires_grad_(True)
+            F.relu(F.batch_norm(tr, None, None, gr, br, True, 0.1, 1e-5)).backward(g.double())
+            report_abs(f"shuffle bwd d{side} {tag}", dt[:, :half], tr.grad, 2.0 ** -6, 0.0, arms=2.0 ** -7)
+            report_abs(f"shuffle bwd dgamma_{side} {tag}", p["gamma_grad"], gr.grad, 2.0 ** -8, 0.0, arms=2.0 ** -8)
+            report_abs(f"shuffle bwd dbeta_{side} {tag}", p["beta_grad"], br.grad, 2.0 ** -8, 0.0, arms=2.0 ** -8)
+        # eval
+        out = nv.shuffle_fwd(a, b, half, split, False, pbn, pa if abn else None)
+        s = torch.cat([out[0][:, :half], out[1][:, :half]], 1) if split else out[:, :2 * half]
+        def eval_bn(t, p):
+            return F.relu(F.batch_norm(t[:, :half].double(), p["running_mean"].double(), p["running_var"].double(),
+                                       p["gamma"].double(), p["beta"].double(), False, 0.1, 1e-5))
+
+        report_abs(f"shuffle eval fwd odd channels {tag}", s[:, 1::2], eval_bn(b, pbn), 2.0 ** -7, 0.0, arms=2.0 ** -8)
+        if abn:
+            report_abs(f"shuffle eval fwd even channels (BN_a) {tag}", s[:, 0::2], eval_bn(a, pa), 2.0 ** -7, 0.0,
+                       arms=2.0 ** -8)
+        else:
+            _exact(f"shuffle eval fwd pass-through bit for bit {tag}", torch.equal(s[:, 0::2], a[:, :half]))
+    # pad / fold: bf16 and fp32 matrices in one launch each
+    w = bf(torch.randn(58, 116, device="cuda"))
+    dw = bf(torch.randn(58, 9, device="cuda"))
+    g = torch.randn(122, device="cuda")
+    pw, pdw, pg = nv.pad_cols([(w, 64, 120), (dw, 64, 9), (g, 1, 128)])
+    ok = torch.equal(pw[:58, :116], w) and bool((pw[58:] == 0).all()) and bool((pw[:, 116:] == 0).all()) \
+        and torch.equal(pdw[:58], dw) and bool((pdw[58:] == 0).all()) and torch.equal(pg[0, :122], g) \
+        and bool((pg[0, 122:] == 0).all())
+    _exact("pad_cols: bf16 and fp32 matrices, bit for bit, zero pad", ok)
+    src, dst = torch.randn(64, 120, device="cuda"), torch.randn(58, 116, 1, 1, device="cuda")
+    src2, dst2 = torch.randn(1, 128, device="cuda"), torch.randn(122, device="cuda")
+    ref = dst.view(58, 116) + src[:58, :116]
+    nv.fold_cols([(src, dst, 58)])
+    nv.fold_cols([(src2, dst2, 1)], add=False)
+    _exact("fold_cols: add and copy, bit for bit", torch.equal(dst.view(58, 116), ref) and torch.equal(dst2, src2[0, :122]))
+
+
+# The gamma / beta gradients of branch2's first BN, whose output reaches the loss only through ReLU, the depthwise conv
+# and BN2 (the BN-feeding-a-depthwise-layer case of _check_ir_tensor), have their own budget, set from the worst ratio
+# the bf16 composite reaches on the 45 unit cases of shufflenet_layers: 0.27 to 0.36 rms for gamma between runs on an
+# H100 (4.4x to 5.8x the block budget's 2^-4 rms; the sums' atomic order varies), 0.1 rms for beta.  Every other tensor
+# of the unit stays within BLOCK_BUDGET.  Checked strictly: no fallback to the composite's ratio.
+SHUFFLE_BN1_BUDGET = {"branch2.1.weight": (2.0 ** -1, 2.0 ** -7), "branch2.1.bias": (2.0 ** -1, 2.0 ** -7)}
+
+
+def _check_shuffle_bn1(name, kind, got, ref, got_c, ref_c):
+    a, r = SHUFFLE_BN1_BUDGET[name.rsplit(" ", 1)[1]]
+    bad, w_n, finite = _bound_ratio(got, ref, r, 0.0, a)
+    w_c = _bound_ratio(got_c, ref_c, r, 0.0, a)[1]
+    ok = finite and bad == 0
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}]    {name + ' (' + kind + ')':55s} worst={w_n:.3f}x (bf16 composite {w_c:.3f}x) of "
+          f"({a:g}*rms(ref) + rtol {r:g}*|ref|), violations={bad}/{got.numel()}", flush=True)
+
+
+def _shuffle_unit_case(name, inp, oup, stride, hw, n, whole):
+    """One unit on the native node against its float64 twin (``shuffle_unit_composite`` in float64 with the same bf16
+    input and weights, its ReLUs taking the native side within BLOCK_TIE of zero), under BLOCK_BUDGET as the depthwise
+    group's inverted-residual blocks are checked (``_check_ir_tensor``, the bf16 composite against its own twin printed
+    alongside): the output, the input gradient(s), every parameter gradient and the running statistics, then the eval
+    forward; the pass-through gradient bit for bit; every pad channel of the output, the input gradients and every
+    saved activation exactly zero."""
+    import copy
+
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.models.shufflenetv2 import InvertedResidual
+    from distributeddeeplearning_b200.ops.shufflenet import shuffle_unit_composite
+
+    torch.manual_seed(inp * 7 + oup + hw)
+    u = InvertedResidual(inp, oup, stride, whole_output=whole).cuda().train()
+    with torch.no_grad():
+        for mod in u.modules():
+            if hasattr(mod, "running_var"):
+                mod.weight.uniform_(0.5, 1.5)
+                mod.bias.normal_(0.0, 0.5)
+                mod.running_mean.normal_(0.0, 0.1)
+                mod.running_var.uniform_(0.5, 1.5)
+            elif hasattr(mod, "weight"):
+                mod.weight.copy_(bf(mod.weight).float())
+    comp = copy.deepcopy(u)
+    init_p = {k: v.detach().double() for k, v in u.named_parameters()}
+    init_b = {k: v.detach().double().clone() for k, v in u.named_buffers() if "running" in k}
+    bf_ = oup // 2
+    tag = f"{name} {inp}->{oup} s{stride} {hw}x{hw} N={n}{' whole' if whole else ' split'}"
+    print(f"-- shuffle unit {tag}", flush=True)
+
+    def branches(params, bufs):
+        def bn(prefix):
+            return (params[prefix + ".weight"], params[prefix + ".bias"], bufs[prefix + ".running_mean"],
+                    bufs[prefix + ".running_var"], 1e-5, 0.1)
+
+        b2 = (params["branch2.0.weight"], bn("branch2.1"), params["branch2.3.weight"], bn("branch2.4"),
+              params["branch2.5.weight"], bn("branch2.6"))
+        b1 = None if stride == 1 else (params["branch1.0.weight"], bn("branch1.1"), params["branch1.2.weight"],
+                                       bn("branch1.3"))
+        return b2, b1
+
+    def twin(x64, dz64, ties):
+        """float64 twin from the unit's initial state; ties: the tested implementation's ReLU outputs > 0 after
+        branch2's first BN, branch2's last BN and branch1's last BN."""
+        params = {k: v.clone().requires_grad_(True) for k, v in init_p.items()}
+        bufs = {k: v.clone() for k, v in init_b.items()}
+        xt = x64.detach().requires_grad_(True)
+        relus = [lambda v, t=t: _tie_relu(v, t) for t in ties]
+        zt = shuffle_unit_composite(xt, *branches(params, bufs), True, relus=relus)
+        zt.backward(dz64)
+        return xt, zt, params, bufs
+
+    if stride == 2:
+        x = _padded_act(n, inp, hw).requires_grad_(True)
+        xin, x64 = x, x[:, :inp].double()
+    else:
+        lo, hi = _padded_act(n, bf_, hw).requires_grad_(True), _padded_act(n, bf_, hw).requires_grad_(True)
+        xin, x64 = (lo, hi), torch.cat([lo[:, :bf_], hi[:, :bf_]], 1).double()
+    out = u(xin)
+    node = (out if whole else out[0]).grad_fn
+    RESULTS.append(type(node).__name__ == "_ShuffleUnitBackward")
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {tag} on the native node")
+    for t in (out if isinstance(out, tuple) else (out,)):
+        _pad_zero(f"{tag} output pad", t, oup if whole else bf_)
+    saved = node.saved_tensors
+    for t in saved:
+        if t.dim() == 4:
+            real = inp if (stride == 2 and t.shape[1] == _p8(inp) and t.shape[1] != _p8(bf_)) else bf_
+            _pad_zero(f"{tag} saved activation pad", t, real)
+    h1 = saved[-6][:, :bf_].detach()            # relu(BN1(y1)) as the node stored it
+    if whole:
+        dz = _padded_act(n, oup, out.shape[2])
+        dz64 = dz[:, :oup].double()
+        out.backward(dz)
+        got = out[:, :oup].detach()
+    else:
+        dz = (_padded_act(n, bf_, out[0].shape[2]), _padded_act(n, bf_, out[0].shape[2]))
+        dz64 = torch.cat([d[:, :bf_] for d in dz], 1).double()
+        torch.autograd.backward(out, dz)
+        got = torch.cat([o[:, :bf_] for o in out], 1).detach()
+    xr, zr, rp, rb = twin(x64, dz64, (h1 > 0, got[:, 1::2] > 0, got[:, 0::2] > 0))
+    # the bf16 composite on a copy of the unit, recording its ReLU outputs for its own twin
+    acts = [None, None, None]
+
+    def rec(i):
+        def relu(v):
+            acts[i] = F.relu(v)
+            return acts[i]
+        return relu
+
+    cp = dict(comp.named_parameters())
+    cb = {k: v for k, v in comp.named_buffers() if "running" in k}
+    xc = cl(bf(x64.detach())).requires_grad_(True)
+    zc = shuffle_unit_composite(xc, *branches(cp, cb), True, relus=[rec(0), rec(1), rec(2)])
+    zc.backward(cl(bf(dz64)))
+    xrc, zrc, rpc, rbc = twin(x64, dz64, [a > 0 if a is not None else None for a in acts])
+    _check_ir_tensor(f"{tag} output", "out", got, zr, zc, zrc)
+    if stride == 2:
+        _pad_zero(f"{tag} dx pad", x.grad, inp)
+        _check_ir_tensor(f"{tag} input", "dx", x.grad[:, :inp], xr.grad, xc.grad, xrc.grad)
+    else:
+        _pad_zero(f"{tag} dlo pad", lo.grad, bf_)
+        _pad_zero(f"{tag} dhi pad", hi.grad, bf_)
+        _exact(f"{tag} pass-through gradient bit for bit", torch.equal(lo.grad[:, :bf_].double(), xr.grad[:, :bf_]))
+        _check_ir_tensor(f"{tag} input (hi)", "dx", hi.grad[:, :bf_], xr.grad[:, bf_:], xc.grad[:, bf_:],
+                         xrc.grad[:, bf_:])
+    # the beta of a BN without an activation whose output feeds a 1x1 conv + BN has an analytically zero gradient
+    zero = {"branch2.4.bias", "branch1.1.bias"}
+    for k, p in u.named_parameters():
+        if k in zero:
+            print(f"   d{k} (analytically zero): max |grad| native {float(p.grad.abs().max()):.2e}, composite "
+                  f"{float(cp[k].grad.abs().max()):.2e}")
+            continue
+        kind = "conv weight grad" if p.dim() == 4 else ("gamma grad" if k.endswith("weight") else "beta grad")
+        if k in SHUFFLE_BN1_BUDGET:
+            _check_shuffle_bn1(f"{tag} {k}", kind, p.grad, rp[k].grad, cp[k].grad, rpc[k].grad)
+        else:
+            _check_ir_tensor(f"{tag} {k}", kind, p.grad, rp[k].grad, cp[k].grad, rpc[k].grad)
+    bufs = dict(u.named_buffers())
+    for k, v in rb.items():
+        _check_ir_tensor(f"{tag} {k}", k.rsplit(".", 1)[1], bufs[k], v, cb[k], rbc[k])
+    u.eval()
+    with torch.no_grad():
+        oe = u(xin)
+        ge = oe[:, :oup] if whole else torch.cat([o[:, :bf_] for o in oe], 1)
+        eb = {k: v.double() for k, v in u.named_buffers() if "running" in k}
+        ep = {k: v.detach().double() for k, v in u.named_parameters()}
+        zre = shuffle_unit_composite(x64, *branches(ep, eb), False)
+    report_abs(f"shuffle unit eval z {tag}", ge, zre, 2.0 ** -6, 0.0, arms=2.0 ** -5)
+    del u, comp
+    torch.cuda.empty_cache()
+
+
+def g_shufflenet_layers():
+    """The shuffle kernels against float64, and the one-node unit at every distinct unit shape of the four models."""
+    import torch
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    _shuffle_kernels()
+    for name, inp, oup, stride, hw in shufflenet_unit_shapes():
+        for whole in ((False,) if stride == 2 else (False, True)):
+            _shuffle_unit_case(name, inp, oup, stride, hw, 32, whole)
+
+
+def _shufflenet_native_step(name):
+    """One training step with F.conv2d / F.batch_norm patched to raise, counting the pad / fold launches."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import _ext, models, ops
+    from distributeddeeplearning_b200.ops import native as nv
+
+    C = nv._C()
+    counts = {"pad_cols": 0, "fold_cols": 0}
+    orig = {k: getattr(C, k) for k in counts}
+
+    def counter(k):
+        def call(*a, **kw):
+            counts[k] += 1
+            return orig[k](*a, **kw)
+        return call
+
+    saved = (F.conv2d, F.batch_norm)
+
+    def refuse(*a, **k):
+        raise AssertionError("a torch composite ran on the native path")
+
+    m = models.get_model(name).cuda().train()
+    x = torch.randn(8, 3, 224, 224, device="cuda")
+    y = torch.randint(0, 1000, (8,), device="cuda")
+    F.conv2d, F.batch_norm = refuse, refuse
+    for k in counts:
+        setattr(C, k, counter(k))
+    try:
+        n0 = _ext.launch_count()
+        ops.softmax_cross_entropy(m(x), y, 1000).backward()
+        torch.cuda.synchronize()
+        ok = True
+    except AssertionError as e:
+        ok, n0 = False, str(e)
+    finally:
+        F.conv2d, F.batch_norm = saved
+        for k in counts:
+            setattr(C, k, orig[k])
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: a training step with F.conv2d / F.batch_norm refusing "
+          f"({_ext.launch_count() - n0 if ok else n0} native launches)", flush=True)
+    padded = name in ("shufflenet_v2_x1_0", "shufflenet_v2_x2_0")
+    ok = all(k in _ext.KERNEL_LAUNCHES for k in counts) and ((min(counts.values()) > 0) if padded
+                                                             else sum(counts.values()) == 0)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: pad / fold launches in one step {counts} "
+          f"({'padded widths' if padded else 'multiples of 8: none expected'})", flush=True)
+    del m
+    torch.cuda.empty_cache()
+
+
+def _shufflenet_vs_torchvision(name, bs):
+    """name vs torchvision fp32 with the same weights (and this repo's bf16 composite), under _mobilenet_vs_torchvision's
+    bounds: logits cosine, gradient cosines with no deficit against the bf16 composite, eval-mode logits."""
+    import torch
+    import torchvision
+
+    from distributeddeeplearning_b200 import models, ops
+
+    torch.manual_seed(0)
+    m = models.get_model(name).cuda().train()
+    tv = getattr(torchvision.models, name)().cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    x = torch.randn(bs, 3, 224, 224, device="cuda").to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    out = m(x)
+    ops.softmax_cross_entropy(out, y, 1000).backward()
+    ro = tv(x)
+    torch.nn.functional.cross_entropy(ro, y).backward()
+    os.environ["DDL_B200_IMPL"] = "torch"
+    try:
+        co = m2(x)
+        ops.softmax_cross_entropy(co, y, 1000).backward()
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+    c = _cos(out, ro)
+    RESULTS.append(c > 0.98)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} logits cos vs fp32 {c:.5f}   vs bf16-composite {_cos(out, co):.5f}")
+    gn, gc = dict(m.named_parameters()), dict(m2.named_parameters())
+    # Two classes of gradients are cancellation-dominated at random init, in bf16 for the composite as much as for the
+    # node, and are not held to the floor (their cosines, native and composite, are printed):
+    # * the gamma / beta of every BN inside the stages and of the stem: each such BN's output reaches the loss only
+    #   through a 1x1 or depthwise conv and another BN (directly, or through the pass-through halves into a later
+    #   unit's depthwise layer), as mobilenet_v2's BNs that feed a depthwise layer do;
+    # * the depthwise weights: BN2 follows each depthwise conv directly, so each channel's 9-tap gradient is what remains
+    #   of large sums after the component along that channel's own 9 weights cancels (BN is invariant to their scale).
+    # The depthwise weights are still held to no deficit against the bf16 composite.  The units' BNs and depthwise
+    # weights are checked element-wise against float64 in shufflenet_layers.
+    def cls(k, p):
+        if p.dim() == 1 and not k.startswith(("fc", "conv5")):
+            return "bn"
+        return "dw" if p.dim() == 4 and p.shape[1] == 1 else "judged"
+
+    for c in ("bn", "dw"):
+        cc = sorted((_cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad), k) for k, p in tv.named_parameters()
+                    if cls(k, p) == c and float(p.grad.norm()) > 0)
+        print(f"   {'BN gamma / beta' if c == 'bn' else 'depthwise weights'} (no floor): lowest cos native "
+              f"{cc[0][0]:.3f} at {cc[0][2]}, bf16 composite {min(x[1] for x in cc):.3f}")
+    worst, worst_c, lag = (1.0, ""), 1.0, (0.0, "")
+    for k, p in tv.named_parameters():
+        if float(p.grad.norm()) == 0.0 or cls(k, p) == "bn":
+            continue
+        c1, c2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if c2 - c1 > lag[0]:
+            lag = (c2 - c1, k)
+        if cls(k, p) == "dw":
+            continue
+        worst_c = min(worst_c, c2)
+        if c1 < worst[0]:
+            worst = (c1, k)
+    # _mobilenet_vs_torchvision's deficit bound against the bf16 composite.  Its 0.60 floor is not met by the bf16
+    # composite itself here (every conv of ShuffleNetV2 feeds a BN directly; the composite's worst cosine, printed next
+    # to native's, is near 0.37 at random init), so the floor only catches a broken kernel: cosine near 0.
+    ok = worst[0] > 0.25 and lag[0] < 0.08
+    print(f"[{'ok' if ok else 'FAIL'}] {name}: worst cosine(native grad, fp32 grad) of the 1x1 / stem / conv5 / fc "
+          f"weights and conv5's BN = {worst[0]:.4f} at {worst[1]} (bf16 composite {worst_c:.4f}); largest deficit vs "
+          f"the bf16 composite (those and the depthwise weights) = {lag[0]:.4f} at {lag[1]}", flush=True)
+    RESULTS.append(ok)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        oe, re_ = m(x), tv(x)
+    ce = _cos(oe, re_)
+    RESULTS.append(ce > 0.98)
+    print(f"[{'ok' if RESULTS[-1] else 'FAIL'}] {name} eval-mode logits cos vs torchvision eval {ce:.5f}", flush=True)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def g_shufflenet():
+    """ShuffleNetV2: g_shufflenet_layers, a native-only training step of each model with the pad / fold launch counts,
+    x1.0 and x2.0 against torchvision, and eager vs CUDA-graph training of x1.0."""
+    import torch
+
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    g_shufflenet_layers()
+    for name in ("shufflenet_v2_x0_5", "shufflenet_v2_x1_0", "shufflenet_v2_x1_5", "shufflenet_v2_x2_0"):
+        _shufflenet_native_step(name)
+    _shufflenet_vs_torchvision("shufflenet_v2_x1_0", 16)
+    _shufflenet_vs_torchvision("shufflenet_v2_x2_0", 16)
+    dist.init()
+
+    def run(graph):
+        torch.manual_seed(0)
+        s = BenchmarkSession("shufflenet_v2_x1_0", 32, True, lr=0.01, momentum=0.9)
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            assert s.enable_graph(warmup=1), "capture failed"
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out[-4:]
+
+    a, b = run(False), run(True)
+    rel = max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(a, b))
+    ok = all(x == x for x in a + b) and rel < 5e-2
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}] shufflenet_v2_x1_0 training: eager {[round(v, 4) for v in a]} graph replay "
+          f"{[round(v, 4) for v in b]} (largest relative difference {rel:.2e})", flush=True)
 
 
 def run_group(name):
