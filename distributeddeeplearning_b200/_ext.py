@@ -166,6 +166,7 @@ KERNEL_LAUNCHES = {
     "window_attention_v2_fwd": 1, "window_attention_v2_bwd": 3, "cpb_fwd": 1, "cpb_bwd": 2, "merge_gather": 1,
     "grid_attention_fwd": 1, "grid_attention_bwd": 3, "tanh_rows_fwd": 1, "tanh_rows_bwd": 1,
     "shuffle_fwd": 1, "shuffle_bwd": 2,
+    "bn_seg_fwd": 1, "bn_seg_bwd": 2, "adaptive_avgpool_fwd": 1, "adaptive_avgpool_bwd": 1, "transpose_rows": 1,
 }
 LAUNCH_COUNT = [0]          # kernels of THIS repo launched so far (bench.py reports the per-region delta)
 

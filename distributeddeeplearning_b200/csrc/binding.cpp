@@ -641,8 +641,59 @@ PYBIND11_MODULE(_C, m) {
     p.bn_a = sh_bn(bn_a); p.bn_b = sh_bn(bn_b);
     check(ddl::launch_shuffle_bwd(p, sms, S(stream)), "shuffle_bwd");
   });
+  // GoogLeNet (inception.cu).  segs: per segment 25 integers (x, z, dz, dx, ldx, colx, ldz, colz, lddz, coldz, lddx,
+  // coldx, C, sum, sumsq, gamma, beta, mean, invstd, running_mean, running_var, dgamma, dbeta, gamma_grad, beta_grad;
+  // pointers 0 = none) and (eps, momentum); see BnSeg
+  auto bn_seg = [](const std::vector<std::vector<int64_t>>& segs, const std::vector<std::pair<float, float>>& em, int M) {
+    if (segs.empty() || segs.size() > static_cast<size_t>(ddl::kSegMax) || em.size() != segs.size())
+      throw std::runtime_error("bn_seg: 1..kSegMax segments");
+    ddl::BnSegArgs a{};
+    a.n = static_cast<int>(segs.size());
+    a.M = M;
+    for (int i = 0; i < a.n; ++i) {
+      const auto& v = segs[i];
+      if (v.size() != 25) throw std::runtime_error("bn_seg: 25 fields per segment");
+      ddl::BnSeg& g = a.s[i];
+      g.x = P<const __nv_bfloat16>(v[0]); g.z = P<__nv_bfloat16>(v[1]); g.dz = P<const __nv_bfloat16>(v[2]);
+      g.dx = P<__nv_bfloat16>(v[3]);
+      g.ldx = static_cast<int>(v[4]); g.colx = static_cast<int>(v[5]); g.ldz = static_cast<int>(v[6]);
+      g.colz = static_cast<int>(v[7]); g.lddz = static_cast<int>(v[8]); g.coldz = static_cast<int>(v[9]);
+      g.lddx = static_cast<int>(v[10]); g.coldx = static_cast<int>(v[11]); g.C = static_cast<int>(v[12]);
+      g.sum = P<const float>(v[13]); g.sumsq = P<const float>(v[14]); g.gamma = P<const float>(v[15]);
+      g.beta = P<const float>(v[16]); g.mean = P<float>(v[17]); g.invstd = P<float>(v[18]);
+      g.running_mean = P<float>(v[19]); g.running_var = P<float>(v[20]); g.dgamma = P<float>(v[21]);
+      g.dbeta = P<float>(v[22]); g.gamma_grad = P<float>(v[23]); g.beta_grad = P<float>(v[24]);
+      g.eps = em[i].first; g.momentum = em[i].second;
+    }
+    return a;
+  };
+  m.def("bn_seg_grid_x", [](int M, int chunks, int sms) { return ddl::bn_seg_grid_x(M, chunks, sms); });
+  m.def("bn_seg_fwd", [bn_seg](const std::vector<std::vector<int64_t>>& segs,
+                               const std::vector<std::pair<float, float>>& em, int M, int train, int sms, ptr_t stream) {
+    check(ddl::launch_bn_seg_fwd(bn_seg(segs, em, M), train != 0, sms, S(stream)), "bn_seg_fwd");
+  });
+  m.def("bn_seg_bwd", [bn_seg](const std::vector<std::vector<int64_t>>& segs,
+                               const std::vector<std::pair<float, float>>& em, int M, ptr_t partial, ptr_t done,
+                               int grid_x, ptr_t stream) {
+    ddl::BnSegArgs a = bn_seg(segs, em, M);
+    a.partial = P<float>(partial);
+    a.done = P<unsigned int>(done);
+    check(ddl::launch_bn_seg_bwd(a, grid_x, S(stream)), "bn_seg_bwd");
+  });
+  m.def("adaptive_avgpool_fwd", [](ptr_t x, ptr_t y, int N, int H, int W, int C, int Pq, int Q, int sms, ptr_t stream) {
+    check(ddl::launch_adaptive_avgpool_fwd(P<const __nv_bfloat16>(x), P<__nv_bfloat16>(y), N, H, W, C, Pq, Q, sms,
+                                           S(stream)), "adaptive_avgpool_fwd");
+  });
+  m.def("adaptive_avgpool_bwd", [](ptr_t dy, ptr_t dx, int N, int H, int W, int C, int Pq, int Q, int sms, ptr_t stream) {
+    check(ddl::launch_adaptive_avgpool_bwd(P<const __nv_bfloat16>(dy), P<__nv_bfloat16>(dx), N, H, W, C, Pq, Q, sms,
+                                           S(stream)), "adaptive_avgpool_bwd");
+  });
+  m.def("transpose_rows", [](ptr_t in, ptr_t out, int N, int A, int B, int sms, ptr_t stream) {
+    check(ddl::launch_transpose_rows(P<const __nv_bfloat16>(in), P<__nv_bfloat16>(out), N, A, B, sms, S(stream)),
+          "transpose_rows");
+  });
   // mats: [(src, dst, rows, k, prows, kp, element bytes)]
-  m.def("pad_cols", [](const std::vector<std::tuple<ptr_t, ptr_t, int, int, int, int, int>>& mats, ptr_t stream) {
+  m.def("pad_cols",[](const std::vector<std::tuple<ptr_t, ptr_t, int, int, int, int, int>>& mats, ptr_t stream) {
     if (mats.empty() || mats.size() > static_cast<size_t>(ddl::kPadMax)) throw std::runtime_error("pad_cols: 1..kPadMax matrices");
     ddl::PadBatch b{};
     b.n = static_cast<int>(mats.size());

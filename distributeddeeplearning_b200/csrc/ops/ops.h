@@ -425,6 +425,55 @@ cudaError_t launch_shuffle_fwd(const ShuffleArgs& p, int sms, cudaStream_t strea
 // two launches: the reduce pass (and the pass-through copy), then the apply pass
 cudaError_t launch_shuffle_bwd(const ShuffleArgs& p, int sms, cudaStream_t stream);
 
+// ---- GoogLeNet: segmented BatchNorm + ReLU, adaptive average pooling, row transpose (inception.cu) ---------------
+// One launch applies up to kSegMax BatchNorm + ReLU layers, each to a channel segment of C (% 8 == 0) channels read
+// from x[r * ldx + colx + c] and written to z[r * ldz + colz + c] (forward), or with the gradient read from
+// dz[r * lddz + coldz + c] and written to dx[r * lddx + coldx + c] (backward, x the saved pre-BN input).  Pitches and
+// column offsets are multiples of 8; channels of a destination outside its segment are not touched.
+constexpr int kSegMax = 4;
+struct BnSeg {
+  const __nv_bfloat16* x;
+  __nv_bfloat16* z;
+  const __nv_bfloat16* dz;
+  __nv_bfloat16* dx;
+  int ldx, colx, ldz, colz, lddz, coldz, lddx, coldx;
+  int C;
+  const float* sum;          // train forward: the conv epilogue's per-channel sum / sum of squares
+  const float* sumsq;
+  const float* gamma;
+  const float* beta;
+  float* mean;               // written by a train forward, read by backward
+  float* invstd;
+  float* running_mean;       // updated by a train forward (may be null), read in eval
+  float* running_var;
+  float eps, momentum;
+  float* dgamma;             // backward: this step's dgamma / dbeta (written by the reduce pass, read by the apply pass)
+  float* dbeta;
+  float* gamma_grad;         // backward, optional: accumulate targets (the .grad slots)
+  float* beta_grad;
+};
+struct BnSegArgs {
+  BnSeg s[kSegMax];
+  int n, M;
+  int chunk0[kSegMax + 1];   // first 64-channel chunk of each segment (set by the launchers)
+  float* partial;            // backward: [chunks][grid_x][128] per-block sums
+  unsigned int* done;        // backward: [chunks] zeroed counters (left zeroed)
+};
+// blocks along the rows of the segmented kernels for `chunks` 64-channel chunks (the backward's partial buffer holds
+// chunks * bn_seg_grid_x(...) * 128 floats)
+int bn_seg_grid_x(int M, int chunks, int sms);
+cudaError_t launch_bn_seg_fwd(BnSegArgs a, bool train, int sms, cudaStream_t stream);
+// two launches: the reduce pass (dgamma / dbeta, deterministic), then the apply pass
+cudaError_t launch_bn_seg_bwd(BnSegArgs a, int grid_x, cudaStream_t stream);
+// NHWC [N][H][W][C] <-> [N][P][Q][C] with torch's adaptive windows; C % 8 == 0
+cudaError_t launch_adaptive_avgpool_fwd(const __nv_bfloat16* x, __nv_bfloat16* y, int N, int H, int W, int C, int P,
+                                        int Q, int sms, cudaStream_t stream);
+cudaError_t launch_adaptive_avgpool_bwd(const __nv_bfloat16* dy, __nv_bfloat16* dx, int N, int H, int W, int C, int P,
+                                        int Q, int sms, cudaStream_t stream);
+// out[n][b][a] = in[n][a][b], A % 8 == 0
+cudaError_t launch_transpose_rows(const __nv_bfloat16* in, __nv_bfloat16* out, int N, int A, int B, int sms,
+                                  cudaStream_t stream);
+
 // ---- FP8 operand preparation (fp8.cu) ----------------------------------------------------------------
 cudaError_t launch_fp8_quantize(const __nv_bfloat16* x, uint8_t* out, int64_t n, Fp8Slot* slot, bool e5m2, int sms,
                                 cudaStream_t stream);

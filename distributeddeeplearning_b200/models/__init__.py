@@ -9,7 +9,7 @@ AlexNet (SURVEY.md 2.7); ResNet-18/34, the other VGG depths, DenseNet and Squeez
 ConvNeXt-Tiny / -Small / -Base / -Large, the Vision Transformers ViT-B/16, -B/32, -L/16 and -L/32, the Swin
 Transformers Swin-T, -S and -B, the Swin Transformers V2 Swin-V2-T, -S and -B, MaxViT-T, the RegNets:
 RegNetX-400MF, -800MF, -1.6GF, -3.2GF, -8GF, -16GF and -32GF, and RegNetY-400MF, -800MF, -1.6GF, -3.2GF, -8GF, -16GF,
--32GF and -128GF, and ShuffleNetV2 x0.5, x1.0, x1.5 and x2.0.
+-32GF and -128GF, ShuffleNetV2 x0.5, x1.0, x1.5 and x2.0, GoogLeNet, and MNASNet 0.5, 0.75, 1.0 and 1.3.
 """
 from __future__ import annotations
 
@@ -21,9 +21,11 @@ from .efficientnet import (INPUT_SIZE as _EFFICIENTNET_INPUT_SIZE, EfficientNet,
                            efficientnet_b6, efficientnet_b7)
 from .efficientnet_v2 import (INPUT_SIZE as _EFFICIENTNET_V2_INPUT_SIZE, EfficientNetV2,  # noqa: F401
                               efficientnet_v2_l, efficientnet_v2_m, efficientnet_v2_s)
+from .googlenet import GoogLeNet, googlenet  # noqa: F401
 from .inception import Inception3, inception_v3  # noqa: F401
 from .maxvit import MaxVit, maxvit_t  # noqa: F401
 from .mobilenet import MobileNetV2, mobilenet_v2  # noqa: F401
+from .mnasnet import MNASNet, mnasnet0_5, mnasnet0_75, mnasnet1_0, mnasnet1_3  # noqa: F401
 from .mobilenetv3 import MobileNetV3, mobilenet_v3_large, mobilenet_v3_small  # noqa: F401
 from .regnet import (RegNet, regnet_x_1_6gf, regnet_x_3_2gf, regnet_x_8gf, regnet_x_16gf, regnet_x_32gf,  # noqa: F401
                      regnet_x_400mf, regnet_x_800mf, regnet_y_1_6gf, regnet_y_3_2gf, regnet_y_8gf, regnet_y_16gf,
@@ -51,7 +53,8 @@ _REGISTRY = {
               swin_v2_t, swin_v2_s, swin_v2_b, maxvit_t, regnet_x_400mf, regnet_x_800mf, regnet_x_1_6gf,
               regnet_x_3_2gf, regnet_x_8gf, regnet_x_16gf, regnet_x_32gf, regnet_y_400mf, regnet_y_800mf,
               regnet_y_1_6gf, regnet_y_3_2gf, regnet_y_8gf, regnet_y_16gf, regnet_y_32gf, regnet_y_128gf,
-              shufflenet_v2_x0_5, shufflenet_v2_x1_0, shufflenet_v2_x1_5, shufflenet_v2_x2_0)
+              shufflenet_v2_x0_5, shufflenet_v2_x1_0, shufflenet_v2_x1_5, shufflenet_v2_x2_0, googlenet, mnasnet0_5,
+              mnasnet0_75, mnasnet1_0, mnasnet1_3)
 }
 
 

@@ -147,6 +147,7 @@ class InceptionAux(nn.Module):
 
 class Inception3(nn.Module):
     input_size = 299
+    aux_loss_weight = 0.4          # the auxiliary head's weight in the training loss (ops.aux_classification_loss)
 
     def __init__(self, num_classes=1000, aux_logits=True, dropout=0.5):
         super().__init__()

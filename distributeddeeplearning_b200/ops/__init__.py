@@ -3,6 +3,7 @@ from .convnext import convnext_block, layer_norm_channels  # noqa: F401
 from .efficientnet_v2 import fused_mbconv, fused_mbconv_supported  # noqa: F401
 from .functional import (  # noqa: F401
     advance_dropout_step,
+    aux_classification_loss,
     avg_pool2d,
     batch_norm_act,
     concat_channels,
@@ -21,6 +22,7 @@ from .functional import (  # noqa: F401
     topk_correct,
     use_native,
 )
+from .googlenet import adaptive_avg_pool2d, flatten_nchw, inception_module  # noqa: F401
 from .maxvit import grid_attention, maxvit_attention_layer  # noqa: F401
 from .shufflenet import shuffle_unit  # noqa: F401
 from .swin import patch_merging, swin_block, window_attention  # noqa: F401

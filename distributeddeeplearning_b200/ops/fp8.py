@@ -16,6 +16,7 @@ classifier stay in bf16 — the usual "first and last layer in higher precision"
 """
 from __future__ import annotations
 
+import contextlib
 import os
 from typing import Dict, Optional, Tuple
 
@@ -34,6 +35,18 @@ def enable(on: bool = True) -> None:
 
 def enabled() -> bool:
     return bool(_STATE["enabled"])
+
+
+@contextlib.contextmanager
+def bf16_only():
+    """The convolutions launched inside take bf16 operands whatever the session's precision (a node whose widths do
+    not all meet the fp8 path's multiple-of-128 rule keeps one precision throughout)."""
+    was = _STATE["enabled"]
+    _STATE["enabled"] = False
+    try:
+        yield
+    finally:
+        _STATE["enabled"] = was
 
 
 def launches() -> Dict[str, int]:

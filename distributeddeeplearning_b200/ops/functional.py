@@ -858,6 +858,22 @@ def softmax_cross_entropy(logits, labels, classes: Optional[int] = None):
     return F.cross_entropy(logits[:, :classes].float(), labels)
 
 
+def aux_classification_loss(output, labels, classes: Optional[int], aux_weight: Optional[float]):
+    """The training loss of a classifier's output: the mean cross-entropy of a logits tensor, or, for a tuple
+    (logits, aux_1, ..., aux_k) of a model with auxiliary heads (Inception-v3, GoogLeNet), that of the logits plus
+    ``aux_weight`` times that of every auxiliary output that is not None.  ``aux_weight`` is the model's
+    ``aux_loss_weight`` (0.4 for Inception-v3, 0.3 for GoogLeNet)."""
+    if not isinstance(output, tuple):
+        return softmax_cross_entropy(output, labels, classes)
+    if aux_weight is None:
+        raise ValueError("aux_classification_loss: a model with auxiliary outputs must define aux_loss_weight")
+    loss = softmax_cross_entropy(output[0], labels, classes)
+    for aux in output[1:]:
+        if aux is not None:
+            loss = loss + aux_weight * softmax_cross_entropy(aux, labels, classes)
+    return loss
+
+
 def topk_correct(logits, labels, classes: Optional[int] = None):
     """int32[2] = (#top-1 hits, #top-5 hits) without a host sync."""
     classes = classes or logits.shape[1]

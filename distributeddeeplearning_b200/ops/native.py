@@ -1184,15 +1184,22 @@ def pad_cols_bf16(w: torch.Tensor, kp: int) -> torch.Tensor:
 def pad_cols(mats) -> list:
     """Zero-padded copies of up to 24 matrices in ONE launch: ``mats`` = [(src, prows, kp)] with ``src`` a contiguous
     CUDA bf16 or fp32 tensor viewed as [rows, k] (its first dimension, the rest flattened; a vector is one row), and the
-    result for each a new [prows, kp] tensor of the same dtype holding ``src`` in its top-left corner, zeros elsewhere."""
+    result for each a new [prows, kp] tensor of the same dtype holding ``src`` in its top-left corner, zeros elsewhere.
+    An entry (src, prows, kp, dst) writes into ``dst`` instead (a contiguous [prows, kp] tensor, for instance a row
+    slice of a stacked matrix), which is also the result."""
     out, desc = [], []
-    for src, prows, kp in mats:
+    for entry in mats:
+        src, prows, kp = entry[:3]
+        dst = entry[3] if len(entry) > 3 else None
         rows, k = (1, src.numel()) if src.dim() == 1 else (src.shape[0], src.numel() // max(1, src.shape[0]))
         if src.dtype not in (torch.bfloat16, torch.float32) or not src.is_cuda or not src.is_contiguous() \
                 or prows < rows or kp < k or rows <= 0 or k <= 0:
             raise ValueError(f"pad_cols: expected contiguous CUDA bf16 / fp32 matrices of at most [{prows}, {kp}], got "
                              f"{tuple(src.shape)} {src.dtype}")
-        dst = torch.empty((prows, kp), dtype=src.dtype, device=src.device)
+        if dst is None:
+            dst = torch.empty((prows, kp), dtype=src.dtype, device=src.device)
+        elif dst.dtype != src.dtype or not dst.is_contiguous() or dst.numel() != prows * kp or dst.device != src.device:
+            raise ValueError(f"pad_cols: the destination must be a contiguous {src.dtype} tensor of {prows} x {kp}")
         out.append(dst)
         desc.append((src.data_ptr(), dst.data_ptr(), rows, k, prows, kp, src.element_size()))
     if not 0 < len(desc) <= 24:
@@ -2182,6 +2189,117 @@ def shuffle_bwd(ds, b: torch.Tensor, half: int, bn_b: dict, a: Optional[torch.Te
                      db.data_ptr(), N * H * W, half, ld, ld_s, int(split), int(bn_a is not None), _sh_bn(bn_a),
                      _sh_bn(bn_b), sm_count(b.device.index or 0), _stream())
     return da, db
+
+
+# ------------------------------------------------------------------------------------------------
+# GoogLeNet: segmented BatchNorm + ReLU, adaptive average pooling, row transpose (csrc/ops/inception.cu)
+# ------------------------------------------------------------------------------------------------
+def _seg_slice(t: torch.Tensor, col: int, c: int, M: int, name: str) -> Tuple[int, int, int]:
+    """(data_ptr, row pitch, column offset) of channels [col, col + c) of an NHWC bf16 activation with M rows."""
+    _check_act(t, name)
+    ld = t.shape[1]
+    if t.numel() != M * ld or col % 8 or ld % 8 or col < 0 or col + c > ld:
+        raise ValueError(f"bn_seg: {name} must hold {M} rows and channels [{col}, {col + c}) at offsets of 8, "
+                         f"got {tuple(t.shape)}")
+    return t.data_ptr(), ld, col
+
+
+def _seg_vec(t: Optional[torch.Tensor], c: int, name: str) -> int:
+    if t is None:
+        return 0
+    if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous() or t.numel() != c:
+        raise ValueError(f"bn_seg: {name} must be a contiguous CUDA fp32 vector of {c}")
+    return t.data_ptr()
+
+
+def _seg_M(t: torch.Tensor) -> int:
+    return t.numel() // t.shape[1]
+
+
+def bn_seg_fwd(segs, train: bool) -> None:
+    """relu(BN(.)) of up to 4 channel segments in ONE launch.  ``segs``: dicts with ``x`` / ``z`` = (tensor, column
+    offset) (NHWC bf16 activations of the same rows; a segment reads channels [col, col + c) of x and writes them to z),
+    ``c`` (a multiple of 8), fp32 ``gamma`` / ``beta`` / ``running_mean`` / ``running_var`` vectors of c, ``eps``,
+    ``momentum``; in training also the conv epilogue's ``sum`` / ``sumsq`` and the ``mean`` / ``invstd`` outputs.
+    Channels of z outside the segments are not written."""
+    rows, em, M = [], [], None
+    for s in segs:
+        c = int(s["c"])
+        M = _seg_M(s["x"][0]) if M is None else M
+        xp, ldx, colx = _seg_slice(s["x"][0], s["x"][1], c, M, "x")
+        zp, ldz, colz = _seg_slice(s["z"][0], s["z"][1], c, M, "z")
+        v = {k: _seg_vec(s.get(k), c, k) for k in ("sum", "sumsq", "gamma", "beta", "mean", "invstd", "running_mean",
+                                                   "running_var")}
+        if train and not all(v[k] for k in ("sum", "sumsq", "mean", "invstd")):
+            raise ValueError("bn_seg_fwd: training needs sum, sumsq, mean and invstd")
+        rows.append([xp, zp, 0, 0, ldx, colx, ldz, colz, 0, 0, 0, 0, c, v["sum"], v["sumsq"], v["gamma"], v["beta"],
+                     v["mean"], v["invstd"], v["running_mean"], v["running_var"], 0, 0, 0, 0])
+        em.append((float(s["eps"]), float(s["momentum"])))
+    dev = segs[0]["x"][0].device
+    _C().bn_seg_fwd(rows, em, M, int(train), sm_count(dev.index or 0), _stream())
+
+
+def bn_seg_bwd(segs) -> None:
+    """Backward of :func:`bn_seg_fwd` (training) in two launches: a deterministic reduce pass and the apply pass.
+    ``segs``: dicts with ``dz`` / ``x`` / ``dx`` = (tensor, column offset): the output gradient, the saved pre-BN input
+    and the input gradient's destination, ``c``, fp32 ``gamma`` / ``beta`` / ``mean`` / ``invstd`` and the optional
+    ``gamma_grad`` / ``beta_grad`` accumulators (the ``.grad`` slots, += dgamma / dbeta)."""
+    rows, em, M, chunks = [], [], None, 0
+    dev = segs[0]["x"][0].device
+    # this step's dgamma / dbeta of every segment (written by the reduce pass, read by the apply pass): one buffer, so
+    # that no segment's slice is freed, and handed to the next segment, before the kernels run
+    sums = torch.empty((2, sum(int(s["c"]) for s in segs)), dtype=torch.float32, device=dev)
+    off = 0
+    for s in segs:
+        c = int(s["c"])
+        M = _seg_M(s["x"][0]) if M is None else M
+        xp, ldx, colx = _seg_slice(s["x"][0], s["x"][1], c, M, "x")
+        dzp, lddz, coldz = _seg_slice(s["dz"][0], s["dz"][1], c, M, "dz")
+        dxp, lddx, coldx = _seg_slice(s["dx"][0], s["dx"][1], c, M, "dx")
+        v = {k: _seg_vec(s.get(k), c, k) for k in ("gamma", "beta", "mean", "invstd", "gamma_grad", "beta_grad")}
+        rows.append([xp, 0, dzp, dxp, ldx, colx, 0, 0, lddz, coldz, lddx, coldx, c, 0, 0, v["gamma"], v["beta"],
+                     v["mean"], v["invstd"], 0, 0, sums[0, off].data_ptr(), sums[1, off].data_ptr(), v["gamma_grad"],
+                     v["beta_grad"]])
+        off += c
+        em.append((0.0, 0.0))
+        chunks += _ceil_div(c, 64)
+    C = _C()
+    gx = C.bn_seg_grid_x(M, chunks, sm_count(dev.index or 0))
+    partial = torch.empty(chunks * gx * 128, dtype=torch.float32, device=dev)
+    done = zeros_f32((chunks,), dev)           # counters: zero bits; the kernel leaves them zero
+    C.bn_seg_bwd(rows, em, M, partial.data_ptr(), done.data_ptr(), gx, _stream())
+
+
+def adaptive_avgpool_fwd(x: torch.Tensor, out_hw: Tuple[int, int]) -> torch.Tensor:
+    _check_act(x)
+    N, Ch, H, W = x.shape
+    P, Q = out_hw
+    y = empty_act(N, Ch, P, Q, x.device)
+    _C().adaptive_avgpool_fwd(x.data_ptr(), y.data_ptr(), N, H, W, Ch, P, Q, sm_count(x.device.index or 0), _stream())
+    return y
+
+
+def adaptive_avgpool_bwd(dy: torch.Tensor, x_shape) -> torch.Tensor:
+    _check_act(dy, "dy")
+    N, Ch, H, W = x_shape
+    dx = empty_act(N, Ch, H, W, dy.device)
+    _C().adaptive_avgpool_bwd(dy.data_ptr(), dx.data_ptr(), N, H, W, Ch, dy.shape[2], dy.shape[3],
+                              sm_count(dy.device.index or 0), _stream())
+    return dx
+
+
+def transpose_rows(x: torch.Tensor, a: int, b: int) -> torch.Tensor:
+    """out[n][j][i] = x[n][i][j] for a contiguous bf16 tensor of N * a * b elements, as a [N, b * a] matrix (a % 8 == 0).
+    An NHWC activation [N, C, H, W] with (a, b) = (H * W, C) comes out flattened in NCHW order (``torch.flatten``);
+    (a, b) = (C, H * W) is the inverse."""
+    if x.dtype != torch.bfloat16 or not x.is_cuda or a % 8 != 0 or x.numel() % (a * b) != 0:
+        raise ValueError("transpose_rows: expected a CUDA bf16 tensor of N * a * b elements with a % 8 == 0")
+    if not (x.is_contiguous() or x.is_contiguous(memory_format=CL)):
+        raise ValueError("transpose_rows: expected dense memory")
+    n = x.numel() // (a * b)
+    out = torch.empty((n, a * b), dtype=torch.bfloat16, device=x.device)
+    _C().transpose_rows(x.data_ptr(), out.data_ptr(), n, a, b, sm_count(x.device.index or 0), _stream())
+    return out
 
 
 # ------------------------------------------------------------------------------------------------

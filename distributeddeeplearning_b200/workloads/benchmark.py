@@ -102,11 +102,8 @@ class BenchmarkSession:
         self._graph = None
 
     def loss_fn(self, output, target):
-        if isinstance(output, tuple):           # Inception-v3 in train mode: (logits, aux)
-            main, aux = output
-            return ops.softmax_cross_entropy(main, target, self.num_classes) + 0.4 * ops.softmax_cross_entropy(
-                aux, target, self.num_classes)
-        return ops.softmax_cross_entropy(output, target, self.num_classes)
+        return ops.aux_classification_loss(output, target, self.num_classes,
+                                           getattr(self.model, "aux_loss_weight", None))
 
     # ---- CUDA-graph replay of the whole step (launch-bound regimes: small per-GPU batches) -------------------------
     def enable_graph(self, warmup: int = 3) -> bool:

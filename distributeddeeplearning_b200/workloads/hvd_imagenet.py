@@ -133,10 +133,7 @@ def main(argv=None) -> int:
         dist.broadcast_optimizer_state(optimizer, root_rank=0)
 
     def criterion(output, target):
-        if isinstance(output, tuple):
-            return ops.softmax_cross_entropy(output[0], target, classes) + 0.4 * ops.softmax_cross_entropy(
-                output[1], target, classes)
-        return ops.softmax_cross_entropy(output, target, classes)
+        return ops.aux_classification_loss(output, target, classes, getattr(net, "aux_loss_weight", None))
 
     carry = hasattr(optimizer, "piggyback")
 

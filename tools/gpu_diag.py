@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "shufflenet", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "shufflenet", "googlenet", "mnasnet", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -5582,6 +5582,456 @@ def g_shufflenet():
     RESULTS.append(ok)
     print(f"[{'ok' if ok else 'FAIL'}] shufflenet_v2_x1_0 training: eager {[round(v, 4) for v in a]} graph replay "
           f"{[round(v, 4) for v in b]} (largest relative difference {rel:.2e})", flush=True)
+
+
+# ------------------------------------------------------------------------------------------------
+# GoogLeNet and MNASNet
+# ------------------------------------------------------------------------------------------------
+# (cin, c1, c2r, c2, c3r, c3, c4, spatial size) of GoogLeNet's nine Inception modules
+GOOGLENET_MODULES = [(192, 64, 96, 128, 16, 32, 32, 28), (256, 128, 128, 192, 32, 96, 64, 28),
+                     (480, 192, 96, 208, 16, 48, 64, 14), (512, 160, 112, 224, 24, 64, 64, 14),
+                     (512, 128, 128, 256, 24, 64, 64, 14), (512, 112, 144, 288, 32, 64, 64, 14),
+                     (528, 256, 160, 320, 32, 128, 128, 14), (832, 256, 160, 320, 32, 128, 128, 7),
+                     (832, 384, 192, 384, 48, 128, 128, 7)]
+
+
+def _seg_bn_params(c, seed):
+    import torch
+
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    return dict(gamma=torch.rand(c, device="cuda", generator=g) + 0.5, beta=torch.randn(c, device="cuda", generator=g),
+                running_mean=torch.randn(c, device="cuda", generator=g) * 0.1,
+                running_var=torch.rand(c, device="cuda", generator=g) + 0.5, eps=1e-3, momentum=0.1)
+
+
+def _bn_seg_kernels():
+    """bn_seg_fwd / bn_seg_bwd: bit-equal to bn_act_fwd on one contiguous segment (train and eval, with the saved
+    statistics and the running statistics); three / four strided segments against float64 in train and eval, with
+    the destination channels outside the segments exactly unchanged; the backward deterministic."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    # one contiguous segment against bn_act_fwd, bit for bit
+    for c, n, hw in ((64, 8, 28), (208, 4, 14), (24, 16, 7)):
+        torch.manual_seed(c)
+        y = cl(bf(torch.randn(n, c, hw, hw, device="cuda") * 2 + 0.5))
+        st = torch.stack([y.float().sum((0, 2, 3)), y.float().pow(2).sum((0, 2, 3))]).contiguous()
+        p1, p2 = _seg_bn_params(c, c), _seg_bn_params(c, c)
+        z1, save1 = nv.bn_act_fwd(y, st, p1["gamma"], p1["beta"], p1["running_mean"], p1["running_var"], 1e-3, 0.1,
+                                  True, None, True)
+        z2 = torch.empty_like(y)
+        save2 = torch.empty(2, c, device="cuda")
+        nv.bn_seg_fwd([dict(x=(y, 0), z=(z2, 0), c=c, sum=st[0], sumsq=st[1], mean=save2[0], invstd=save2[1], **p2)],
+                      True)
+        _exact(f"bn_seg_fwd train C={c}: output, mean / invstd and running statistics bit-equal to bn_act_fwd",
+               torch.equal(z1, z2) and torch.equal(save1, save2) and torch.equal(p1["running_mean"], p2["running_mean"])
+               and torch.equal(p1["running_var"], p2["running_var"]))
+        z1, _ = nv.bn_act_fwd(y, None, p1["gamma"], p1["beta"], p1["running_mean"], p1["running_var"], 1e-3, 0.1, True,
+                              None, False)
+        nv.bn_seg_fwd([dict(x=(y, 0), z=(z2, 0), c=c, **p2)], False)
+        _exact(f"bn_seg_fwd eval C={c}: output bit-equal to bn_act_fwd", torch.equal(z1, z2))
+    # strided segments: R [M, 96 + 16 + 32] -> out[:, 0:96] and two contiguous tensors; then three sources -> out
+    n, hw = 8, 14
+    torch.manual_seed(5)
+    R = cl(bf(torch.randn(n, 144, hw, hw, device="cuda") * 1.5 + 0.3))
+    out = cl(bf(torch.randn(n, 200, hw, hw, device="cuda")))
+    t2, t3 = cl(bf(torch.randn(n, 16, hw, hw, device="cuda"))), cl(bf(torch.randn(n, 32, hw, hw, device="cuda")))
+    out0 = out.clone()
+    layout = [(0, 96, out, 64), (96, 16, t2, 0), (112, 32, t3, 0)]    # (column in R, c, destination, its column)
+    for train in (True, False):
+        ps = [_seg_bn_params(c, 10 + i) for i, (_, c, _, _) in enumerate(layout)]
+        refs = [(p["running_mean"].double().clone(), p["running_var"].double().clone()) for p in ps]
+        saves = [torch.empty(2, c, device="cuda") for _, c, _, _ in layout]
+        segs = []
+        for (col, c, dst, dcol), p, sv in zip(layout, ps, saves):
+            d = dict(x=(R, col), z=(dst, dcol), c=c, **p)
+            if train:
+                sl = R[:, col:col + c].float()
+                d.update(sum=sl.sum((0, 2, 3)).contiguous(), sumsq=sl.pow(2).sum((0, 2, 3)).contiguous(), mean=sv[0],
+                         invstd=sv[1])
+            segs.append(d)
+        nv.bn_seg_fwd(segs, train)
+        mode = "train" if train else "eval"
+        _exact(f"bn_seg_fwd {mode}: out channels outside the segment unchanged",
+               torch.equal(out[:, :64], out0[:, :64]) and torch.equal(out[:, 160:], out0[:, 160:]))
+        for (col, c, dst, dcol), p, (rm, rv) in zip(layout, ps, refs):
+            ref = F.relu(F.batch_norm(R[:, col:col + c].double(), rm, rv, p["gamma"].double(), p["beta"].double(),
+                                      train, 0.1, 1e-3))
+            _classic("bn out", f"bn_seg_fwd {mode} segment R[{col}:{col + c}]", dst[:, dcol:dcol + c], ref)
+            if train:
+                _classic("bn running_mean", f"bn_seg_fwd running_mean R[{col}:{col + c}]", p["running_mean"], rm)
+                _classic("bn running_var", f"bn_seg_fwd running_var R[{col}:{col + c}]", p["running_var"], rv)
+        if not train:
+            continue
+        # backward: the gradient is a strided slice of one tensor, the destinations a slice of dR and contiguous tensors
+        dout = cl(bf(torch.randn(n, 200, hw, hw, device="cuda")))
+        dR = cl(bf(torch.randn(n, 144, hw, hw, device="cuda")))
+        d2 = cl(bf(torch.randn(n, 16, hw, hw, device="cuda")))
+        d3 = cl(bf(torch.randn(n, 32, hw, hw, device="cuda")))
+        dR0 = dR.clone()
+        gg = [torch.zeros(c, device="cuda") for _, c, _, _ in layout]
+        bg = [torch.zeros(c, device="cuda") for _, c, _, _ in layout]
+        dz_cols = [(dout, 64), (dout, 8), (dout, 168)]
+        dsts = [(dR, 0), (d2, 0), (d3, 0)]
+
+        def bwd_segs():
+            return [dict(dz=dz, x=(R, col), dx=dx, c=c, gamma=p["gamma"], beta=p["beta"], mean=sv[0], invstd=sv[1],
+                         gamma_grad=g1, beta_grad=b1)
+                    for (col, c, _, _), p, sv, dz, dx, g1, b1 in zip(layout, ps, saves, dz_cols, dsts, gg, bg)]
+
+        nv.bn_seg_bwd(bwd_segs())
+        _exact("bn_seg_bwd: dR channels outside the segments unchanged", torch.equal(dR[:, 96:], dR0[:, 96:]))
+        first = (dR[:, :96].clone(), d2.clone(), d3.clone(), [t.clone() for t in gg], [t.clone() for t in bg])
+        for (col, c, _, _), p, (dz, dc), (dx, xc), g1, b1 in zip(layout, ps, dz_cols, dsts, gg, bg):
+            tr = R[:, col:col + c].double().requires_grad_(True)
+            gr, br = p["gamma"].double().requires_grad_(True), p["beta"].double().requires_grad_(True)
+            F.relu(F.batch_norm(tr, None, None, gr, br, True, 0.1, 1e-3)).backward(dz[:, dc:dc + c].double())
+            _classic("bn dx", f"bn_seg_bwd dx segment R[{col}:{col + c}]", dx[:, xc:xc + c], tr.grad)
+            _classic("bn dgamma", f"bn_seg_bwd dgamma segment R[{col}:{col + c}]", g1, gr.grad)
+            _classic("bn dbeta", f"bn_seg_bwd dbeta segment R[{col}:{col + c}]", b1, br.grad)
+        for t in gg + bg:
+            t.zero_()
+        nv.bn_seg_bwd(bwd_segs())
+        _exact("bn_seg_bwd deterministic: a second run is bit-equal (dx and dgamma / dbeta)",
+               torch.equal(first[0], dR[:, :96]) and torch.equal(first[1], d2) and torch.equal(first[2], d3)
+               and all(torch.equal(a, b) for a, b in zip(first[3] + first[4], gg + bg)))
+
+
+def _adaptive_pool_and_flatten():
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import ops
+
+    for (h, w), out, c in (((14, 14), (4, 4), 512), ((14, 14), (4, 4), 528), ((7, 9), (3, 4), 64), ((17, 14), (6, 4), 16),
+                           ((7, 7), (7, 7), 8)):
+        torch.manual_seed(h * w + c)
+        x = cl(bf(torch.randn(4, c, h, w, device="cuda"))).requires_grad_(True)
+        y = ops.adaptive_avg_pool2d(x, out)
+        xr = x.detach().double().requires_grad_(True)
+        yr = F.adaptive_avg_pool2d(xr, out)
+        _classic("pool out", f"adaptive_avg_pool2d {h}x{w}->{out} C={c}", y, yr)
+        dy = cl(bf(torch.randn_like(yr.float())))
+        y.backward(dy)
+        yr.backward(dy.double())
+        _classic("pool grad", f"adaptive_avg_pool2d grad {h}x{w}->{out} C={c}", x.grad, xr.grad)
+        _exact(f"adaptive_avg_pool2d {h}x{w}->{out} on the native node", type(y.grad_fn).__name__ == "_AdaptiveAvgPoolBackward")
+    x = cl(bf(torch.randn(8, 128, 4, 4, device="cuda"))).requires_grad_(True)
+    f = ops.flatten_nchw(x)
+    g = bf(torch.randn(8, 2048, device="cuda"))
+    f.backward(g)
+    _exact("flatten_nchw: torchvision's NCHW order bit for bit, forward and backward",
+           torch.equal(f, torch.flatten(x.detach().contiguous(), 1)) and torch.equal(x.grad, g.view(8, 128, 4, 4))
+           and type(f.grad_fn).__name__ == "_FlattenNCHWBackward")
+
+
+def _inception_case(shape, n):
+    """One module on the native node against its float64 twin (``inception_module_composite`` in float64 with the same
+    bf16 input and weights, its ReLUs taking the native side within BLOCK_TIE of zero), under BLOCK_BUDGET by the
+    inverted-residual rule (``_check_ir_tensor``, the bf16 composite against its own twin printed alongside): the
+    output, the input gradient, every parameter gradient and the running statistics; then the eval forward and the
+    refusal of a backward through eval-mode BNs."""
+    import copy
+
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200.models.googlenet import Inception
+    from distributeddeeplearning_b200.ops.googlenet import inception_module_composite
+
+    cin, c1, c2r, c2, c3r, c3, c4, hw = shape
+    torch.manual_seed(cin + c1 + c2)
+    u = Inception(cin, c1, c2r, c2, c3r, c3, c4).cuda().train()
+    with torch.no_grad():
+        for mod in u.modules():
+            if hasattr(mod, "running_var"):
+                mod.weight.uniform_(0.5, 1.5)
+                mod.bias.normal_(0.0, 0.5)
+                mod.running_mean.normal_(0.0, 0.1)
+                mod.running_var.uniform_(0.5, 1.5)
+            elif hasattr(mod, "weight") and mod.weight is not None:
+                mod.weight.normal_(0.0, 1.0 / (mod.weight[0].numel() ** 0.5))
+                mod.weight.copy_(bf(mod.weight).float())
+    comp = copy.deepcopy(u)
+    names = ["branch1", "branch2.0", "branch2.1", "branch3.0", "branch3.1", "branch4.1"]
+    init_p = {k: v.detach().double() for k, v in u.named_parameters()}
+    init_b = {k: v.detach().double().clone() for k, v in u.named_buffers() if "running" in k}
+    tag = f"inception {cin}->{c1}/{c2r}-{c2}/{c3r}-{c3}/{c4} {hw}x{hw} N={n}"
+    print(f"-- {tag}", flush=True)
+
+    def layers(params, bufs):
+        return [(params[f"{m}.conv.weight"], (params[f"{m}.bn.weight"], params[f"{m}.bn.bias"],
+                                               bufs[f"{m}.bn.running_mean"], bufs[f"{m}.bn.running_var"], 1e-3, 0.1))
+                for m in names]
+
+    def twin(x64, dz64, ties):
+        params = {k: v.clone().requires_grad_(True) for k, v in init_p.items()}
+        bufs = {k: v.clone() for k, v in init_b.items()}
+        xt = x64.detach().requires_grad_(True)
+        relus = [lambda v, t=t: _tie_relu(v, t) for t in ties]
+        zt = inception_module_composite(xt, layers(params, bufs), True, relus=relus)
+        zt.backward(dz64)
+        return xt, zt, params, bufs
+
+    x = cl(bf(torch.randn(n, cin, hw, hw, device="cuda"))).requires_grad_(True)
+    out = u(x)
+    node = out.grad_fn
+    _exact(f"{tag} on the native node", type(node).__name__ == "_InceptionBackward")
+    saved = node.saved_tensors
+    t2, t3 = saved[4].detach(), saved[5].detach()
+    dz = cl(bf(torch.randn_like(out.float())))
+    out.backward(dz)
+    got = out.detach()
+    x64, dz64 = x.detach().double(), dz.double()
+    o = [0, c1, c1 + c2, c1 + c2 + c3, c1 + c2 + c3 + c4]
+    ties = [got[:, o[0]:o[1]] > 0, t2 > 0, got[:, o[1]:o[2]] > 0, t3 > 0, got[:, o[2]:o[3]] > 0, got[:, o[3]:o[4]] > 0]
+    xr, zr, rp, rb = twin(x64, dz64, ties)
+    acts = [None] * 6
+
+    def rec(i):
+        def relu(v):
+            acts[i] = F.relu(v)
+            return acts[i]
+        return relu
+
+    cp = dict(comp.named_parameters())
+    cb = {k: v for k, v in comp.named_buffers() if "running" in k}
+    xc = cl(bf(x64)).requires_grad_(True)
+    zc = inception_module_composite(xc, layers(cp, cb), True, relus=[rec(i) for i in range(6)])
+    zc.backward(cl(bf(dz64)))
+    xrc, zrc, rpc, rbc = twin(x64, dz64, [a > 0 for a in acts])
+    _check_ir_tensor(f"{tag} output", "out", got, zr, zc, zrc)
+    _check_ir_tensor(f"{tag} input", "dx", x.grad, xr.grad, xc.grad, xrc.grad)
+    for k, p in u.named_parameters():
+        kind = "conv weight grad" if p.dim() == 4 else ("gamma grad" if k.endswith("weight") else "beta grad")
+        _check_ir_tensor(f"{tag} {k}", kind, p.grad, rp[k].grad, cp[k].grad, rpc[k].grad)
+    bufs = dict(u.named_buffers())
+    for k, v in rb.items():
+        _check_ir_tensor(f"{tag} {k}", k.rsplit(".", 1)[1], bufs[k], v, cb[k], rbc[k])
+    u.eval()
+    with torch.no_grad():
+        oe = u(x.detach())
+        eb = {k: v.double() for k, v in u.named_buffers() if "running" in k}
+        ep = {k: v.detach().double() for k, v in u.named_parameters()}
+        zre = inception_module_composite(x64, layers(ep, eb), False)
+    report_abs(f"inception eval z {tag}", oe, zre, 2.0 ** -6, 0.0, arms=2.0 ** -5)
+    try:
+        u(x).sum().backward()
+        refused = False
+    except RuntimeError as e:
+        refused = "eval mode" in str(e)
+    _exact(f"{tag}: backward through eval-mode BNs raises RuntimeError", refused)
+    del u, comp
+    torch.cuda.empty_cache()
+
+
+def g_googlenet_layers():
+    """The segmented BN, adaptive pool and flatten kernels against float64, and the one-node Inception module at all
+    nine module shapes at batch 32."""
+    import torch
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    _bn_seg_kernels()
+    _adaptive_pool_and_flatten()
+    for shape in GOOGLENET_MODULES:
+        _inception_case(shape, 32)
+
+
+def _native_step(name, bs=8):
+    """One training step with F.conv2d / F.batch_norm patched to raise, and no torch-composite node in its graph."""
+    import torch
+    import torch.nn.functional as F
+
+    from distributeddeeplearning_b200 import _ext, models, ops
+
+    saved = (F.conv2d, F.batch_norm)
+
+    def refuse(*a, **k):
+        raise AssertionError("a torch composite ran on the native path")
+
+    m = models.get_model(name).cuda().train()
+    x = torch.randn(bs, 3, 224, 224, device="cuda")
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    F.conv2d, F.batch_norm = refuse, refuse
+    try:
+        n0 = _ext.launch_count()
+        loss = ops.aux_classification_loss(m(x), y, 1000, getattr(m, "aux_loss_weight", None))
+        nodes = _graph_nodes(loss)
+        loss.backward()
+        torch.cuda.synchronize()
+        ok, msg = True, f"{_ext.launch_count() - n0} native launches"
+    except AssertionError as e:
+        ok, msg, nodes = False, str(e), {}
+    finally:
+        F.conv2d, F.batch_norm = saved
+    fallback = {k: nodes[k] for k in FALLBACK_NODES if nodes.get(k)}
+    _exact(f"{name}: a training step with F.conv2d / F.batch_norm refusing ({msg}); composite nodes {fallback}",
+           ok and not fallback)
+    del m
+    torch.cuda.empty_cache()
+
+
+def _zoo_vs_torchvision(name, bs):
+    """name (dropout 0) against torchvision fp32 with the same weights and this repo's bf16 composite: logits (and aux
+    logits) cosine above 0.98 or within 0.01 of the composite's, parameter gradients with no deficit over 0.08 against
+    the composite where the composite resolves them, eval-mode logits."""
+    import torch
+    import torch.nn.functional as F
+    import torchvision
+
+    from distributeddeeplearning_b200 import models, ops
+
+    torch.manual_seed(0)
+    kw = dict(dropout=0.0, **({"dropout_aux": 0.0} if name == "googlenet" else {}))
+    m = models.get_model(name, **kw).cuda().train()
+    tv = getattr(torchvision.models, name)(**kw, **({"init_weights": True} if name == "googlenet" else {}))
+    tv = tv.cuda().train()
+    tv.load_state_dict(m.state_dict())
+    m2 = models.get_model(name, **kw).cuda().train()
+    m2.load_state_dict(m.state_dict())
+    contrast = torch.linspace(0.25, 2.0, bs, device="cuda").view(-1, 1, 1, 1)
+    x = (torch.randn(bs, 3, 224, 224, device="cuda") * contrast).to(torch.bfloat16).float()
+    y = torch.randint(0, 1000, (bs,), device="cuda")
+    w = getattr(m, "aux_loss_weight", None)
+
+    def heads(o):
+        return [t[:, :1000] for t in o] if isinstance(o, tuple) else [o[:, :1000]]
+
+    out = m(x)
+    ops.aux_classification_loss(out, y, 1000, w).backward()
+    ro = tv(x)
+    (sum(((1.0,) + (w,) * (len(ro) - 1))[i] * F.cross_entropy(o, y) for i, o in enumerate(ro))
+     if isinstance(ro, tuple) else F.cross_entropy(ro, y)).backward()
+    os.environ["DDL_B200_IMPL"] = "torch"
+    try:
+        co = m2(x)
+        ops.aux_classification_loss(co, y, 1000, w).backward()
+    finally:
+        os.environ["DDL_B200_IMPL"] = "native"
+    for head, a, r, c in zip(("logits", "aux logits 2", "aux logits 1"), heads(out), heads(ro), heads(co)):
+        c1, c2 = _cos(a, r), _cos(c, r)
+        _exact(f"{name} {head} cos vs fp32 {c1:.5f} (bf16 composite {c2:.5f})", c1 > 0.98 or c1 > c2 - 0.01)
+    gn, gc = dict(m.named_parameters()), dict(m2.named_parameters())
+    worst, lag, noise = (1.0, "", 1.0), (0.0, ""), 0
+    for k, p in tv.named_parameters():
+        if float(p.grad.norm()) == 0.0:
+            continue
+        c1, c2 = _cos(gn[k].grad, p.grad), _cos(gc[k].grad, p.grad)
+        if c2 < CLASSIC_RESOLVED:
+            noise += 1
+            continue
+        if c1 < worst[0]:
+            worst = (c1, k, c2)
+        if c2 - c1 > lag[0]:
+            lag = (c2 - c1, k)
+    _exact(f"{name}: worst cosine(native grad, fp32 grad) = {worst[0]:.4f} at {worst[1]} (bf16 composite "
+           f"{worst[2]:.4f}); largest deficit vs the bf16 composite = {lag[0]:.4f} at {lag[1]}; {noise} gradients the "
+           f"composite does not resolve", lag[0] < 0.08)
+    m.eval(), tv.eval()
+    with torch.no_grad():
+        ce = _cos(m(x)[:, :1000], tv(x))
+    _exact(f"{name} eval-mode logits cos vs torchvision eval {ce:.5f}", ce > 0.98)
+    del m, m2, tv
+    torch.cuda.empty_cache()
+
+
+def _replay(name, bs):
+    """Training with the fused engine, eager then CUDA-graph replay, every dropout off: the capture succeeds and the
+    replayed losses track the eager ones (5 % or twice the drift between two eager runs)."""
+    import torch
+
+    from distributeddeeplearning_b200.parallel import dist
+    from distributeddeeplearning_b200.workloads.benchmark import BenchmarkSession
+
+    dist.init()
+    captured = []
+
+    def run(graph):
+        torch.manual_seed(0)
+        s = BenchmarkSession(name, bs, True, lr=0.01)
+        for mod in s.model.modules():
+            if hasattr(mod, "p"):
+                mod.p = 0.0
+        out = [float(s.step()) for _ in range(3)]
+        if graph:
+            captured.append(s.enable_graph(warmup=1))
+        else:
+            out.append(float(s.step()))
+        out += [float(s.step()) for _ in range(4)]
+        s.optimizer.check_errors()
+        del s
+        torch.cuda.empty_cache()
+        return out[-4:]
+
+    def drift(u, v):
+        return max(abs(x - y) / max(1.0, abs(x)) for x, y in zip(u, v))
+
+    a, a2, b = run(False), run(False), run(True)
+    rel, noise = drift(a, b), drift(a, a2)
+    _exact(f"{name} training: captured={captured[0]} eager {[round(v, 4) for v in a]} graph replay "
+           f"{[round(v, 4) for v in b]} (largest relative difference {rel:.2e}; between two eager runs {noise:.2e})",
+           captured[0] and all(x == x for x in a + b) and rel < max(5e-2, 2 * noise))
+
+
+def _inception_fp8_session():
+    """In an fp8 session the node keeps bf16 operands: no fp8 forward or data-gradient launch, the same output as in a
+    bf16 session.  inception3b's 3x3 (128 -> 192) and pool projection (256 -> 64) would meet the fp8 rule on their own."""
+    import torch
+
+    from distributeddeeplearning_b200.models.googlenet import Inception
+    from distributeddeeplearning_b200.ops import fp8
+
+    torch.manual_seed(3)
+    u = Inception(256, 128, 128, 192, 32, 96, 64).cuda().train()
+    x = cl(bf(torch.randn(64, 256, 28, 28, device="cuda")))
+    dz = cl(bf(torch.randn(64, 480, 28, 28, device="cuda")))
+
+    def run():
+        xi = x.detach().requires_grad_(True)
+        out = u(xi)
+        out.backward(dz)
+        return out.detach(), xi.grad
+
+    ref = run()
+    fp8.enable(True)
+    try:
+        before = fp8.launches()
+        got = run()
+        after = fp8.launches()
+    finally:
+        fp8.enable(False)
+    # the conv epilogues' BN sums are atomics: two bf16 runs agree to rounding, not bit for bit
+    close = all(float((g.float() - r.float()).abs().max()) <= 2.0 ** -5 * float(r.float().abs().max())
+                for g, r in zip(got, ref))
+    _exact(f"inception module in an fp8 session: fp8 launches {before} -> {after}, output and dx within rounding of a "
+           f"bf16 session's", before == after and close)
+
+
+def g_googlenet():
+    """GoogLeNet: g_googlenet_layers, the node in an fp8 session, a native-only training step, googlenet against
+    torchvision and graph replay."""
+    g_googlenet_layers()
+    _inception_fp8_session()
+    _native_step("googlenet")
+    _zoo_vs_torchvision("googlenet", 16)
+    _replay("googlenet", 32)
+
+
+def g_mnasnet():
+    """MNASNet: a native-only training step of each width, mnasnet1_0 against torchvision and graph replay."""
+    for name in ("mnasnet0_5", "mnasnet0_75", "mnasnet1_0", "mnasnet1_3"):
+        _native_step(name)
+    _zoo_vs_torchvision("mnasnet1_0", 16)
+    _replay("mnasnet1_0", 32)
+
+
+def g_mnasnet_layers():
+    """A native-only training step of each MNASNet width (the layer kernels under the current conv-kernel settings)."""
+    for name in ("mnasnet0_5", "mnasnet0_75", "mnasnet1_0", "mnasnet1_3"):
+        _native_step(name)
 
 
 def run_group(name):
