@@ -104,37 +104,45 @@ def imagenet_synthetic_remote(c, node_count=None, epochs=1, no_cuda=False, batch
             int(node_count or _max_nodes()), "synthetic_images_remote", no_cuda)
 
 
-@task
-def imagenet_images_local(c, epochs=1, no_cuda=False):
+def _augment_extra(augment):
+    return ["--augment", str(augment)] if augment and augment != "host" else []
+
+
+_AUGMENT_HELP = {"augment": "host (default; PIL in the loader workers) or device (one GPU kernel after the copy)"}
+
+
+@task(help=_AUGMENT_HELP)
+def imagenet_images_local(c, epochs=1, no_cuda=False, augment="host"):
     """ImageNet trainer on $DATA/train and $DATA/validation, one rank."""
     data = _env()["DATA"]
-    _submit(_IMAGENET, _imagenet_argv(epochs, not no_cuda, os.path.join(data, "train"), os.path.join(data, "validation")),
-            1, "real_images_local", no_cuda)
+    _submit(_IMAGENET, _imagenet_argv(epochs, not no_cuda, os.path.join(data, "train"), os.path.join(data, "validation"),
+                                      _augment_extra(augment)), 1, "real_images_local", no_cuda)
 
 
-@task
-def imagenet_images_remote(c, node_count=None, epochs=1, no_cuda=False):
+@task(help=_AUGMENT_HELP)
+def imagenet_images_remote(c, node_count=None, epochs=1, no_cuda=False, augment="host"):
     """ImageNet trainer on the datastore's train/validation folders, --node-count ranks."""
     store = _datastore_path()
-    _submit(_IMAGENET, _imagenet_argv(epochs, not no_cuda, os.path.join(store, "train"), os.path.join(store, "validation")),
-            int(node_count or _max_nodes()), "real_images_remote", no_cuda)
+    _submit(_IMAGENET, _imagenet_argv(epochs, not no_cuda, os.path.join(store, "train"), os.path.join(store, "validation"),
+                                      _augment_extra(augment)), int(node_count or _max_nodes()), "real_images_remote",
+            no_cuda)
 
 
-@task
-def imagenet_records_local(c, epochs=1, no_cuda=False):
+@task(help=_AUGMENT_HELP)
+def imagenet_records_local(c, epochs=1, no_cuda=False, augment="host"):
     """ImageNet trainer on the record shards under $DATA/records (reference: tf-imagenet ... tfrecords), one rank."""
     rec = os.path.join(_env()["DATA"], "records")
     _submit(_IMAGENET, _imagenet_argv(epochs, not no_cuda, os.path.join(rec, "train"), os.path.join(rec, "validation"),
-                                      ["--data_type", "records"]), 1, "records_local", no_cuda)
+                                      ["--data_type", "records", *_augment_extra(augment)]), 1, "records_local", no_cuda)
 
 
-@task
-def imagenet_records_remote(c, node_count=None, epochs=1, no_cuda=False):
+@task(help=_AUGMENT_HELP)
+def imagenet_records_remote(c, node_count=None, epochs=1, no_cuda=False, augment="host"):
     """ImageNet trainer on the datastore's record shards, --node-count ranks (file-level sharding across ranks)."""
     rec = os.path.join(_datastore_path(), "records")
     _submit(_IMAGENET, _imagenet_argv(epochs, not no_cuda, os.path.join(rec, "train"), os.path.join(rec, "validation"),
-                                      ["--data_type", "records"]), int(node_count or _max_nodes()), "records_remote",
-            no_cuda)
+                                      ["--data_type", "records", *_augment_extra(augment)]),
+            int(node_count or _max_nodes()), "records_remote", no_cuda)
 
 
 # ------------------------------------------------------------------ pytorch-hvd (orphan in the reference; wired here)
@@ -150,11 +158,12 @@ def hvd_synthetic_remote(c, node_count=None, epochs=1, batch_size=32, no_cuda=Fa
     _submit(_HVD, argv, int(node_count or _max_nodes()), "hvd_synthetic_remote", no_cuda)
 
 
-@task
-def hvd_images_remote(c, node_count=None, epochs=90, batch_size=32, no_cuda=False):
+@task(help=_AUGMENT_HELP)
+def hvd_images_remote(c, node_count=None, epochs=90, batch_size=32, no_cuda=False, augment="host"):
     store = _datastore_path()
     argv = ["--epochs", str(epochs), "--batch-size", str(batch_size), "--train-dir", os.path.join(store, "train"),
             "--val-dir", os.path.join(store, "validation")] + (["--no-cuda"] if no_cuda else [])
+    argv += _augment_extra(augment)
     _submit(_HVD, argv, int(node_count or _max_nodes()), "hvd_images_remote", no_cuda)
 
 

@@ -688,6 +688,10 @@ PYBIND11_MODULE(_C, m) {
     check(ddl::launch_adaptive_avgpool_bwd(P<const __nv_bfloat16>(dy), P<__nv_bfloat16>(dx), N, H, W, C, Pq, Q, sms,
                                            S(stream)), "adaptive_avgpool_bwd");
   });
+  m.def("resized_crop", [](ptr_t src, ptr_t desc, ptr_t out, int B, int Sz, ptr_t mean, ptr_t stdv, ptr_t stream) {
+    check(ddl::launch_resized_crop(P<const uint8_t>(src), P<const double>(desc), P<__nv_bfloat16>(out), B, Sz,
+                                   P<const float>(mean), P<const float>(stdv), S(stream)), "resized_crop");
+  });
   m.def("transpose_rows", [](ptr_t in, ptr_t out, int N, int A, int B, int sms, ptr_t stream) {
     check(ddl::launch_transpose_rows(P<const __nv_bfloat16>(in), P<__nv_bfloat16>(out), N, A, B, sms, S(stream)),
           "transpose_rows");

@@ -474,6 +474,13 @@ cudaError_t launch_adaptive_avgpool_bwd(const __nv_bfloat16* dy, __nv_bfloat16* 
 cudaError_t launch_transpose_rows(const __nv_bfloat16* in, __nv_bfloat16* out, int N, int A, int B, int sms,
                                   cudaStream_t stream);
 
+// ---- Device-side image augmentation (augment.cu) -------------------------------------------------------
+// B ragged uint8 HWC3 regions in one buffer, desc [B][8] float64 = (byte offset, Hr, Wr, sy, sx, oy, ox, flip) ->
+// bf16 NHWC4 [B][S][S][4]: antialiased bilinear resample of each region, flip of the output column, (v/255 - mean)/std,
+// channel 3 = 0.  The caller checks every descriptor against the buffer.
+cudaError_t launch_resized_crop(const uint8_t* src, const double* desc, __nv_bfloat16* out, int B, int S,
+                                const float* mean, const float* stdv, cudaStream_t stream);
+
 // ---- FP8 operand preparation (fp8.cu) ----------------------------------------------------------------
 cudaError_t launch_fp8_quantize(const __nv_bfloat16* x, uint8_t* out, int64_t n, Fp8Slot* slot, bool e5m2, int sms,
                                 cudaStream_t stream);

@@ -133,14 +133,15 @@ class RecordLoader:
     (``TensorFlow_imagenet/tensorflow_imagenet.py:110-151``).  Here ``RecordDataset`` does the file-level sharding
     (rank r reads shards r, r+size, ...; DataLoader workers split those again), ``set_epoch`` reseeds the shard order,
     and ``len()`` is the number of batches EVERY rank runs (the minimum over ranks, so collectives stay in step).
+    ``augment``: ``host`` or ``device`` (``data/images.py``).
     """
 
     def __init__(self, directory: str, split: str, batch_size: int, train: bool, size: int = 224, num_workers: int = 4,
-                 rank: int = 0, world: int = 1, normalize_on_host: bool = True, seed: int = 0):
-        from .images import build_transforms
+                 rank: int = 0, world: int = 1, normalize_on_host: bool = True, seed: int = 0, augment: str = "host"):
+        from .images import worker_transform
 
-        self.dataset = RecordDataset(directory, split, rank, world, build_transforms(train, size, normalize_on_host),
-                                     shuffle_seed=seed if train else None)
+        transform, collate = worker_transform(train, size, augment, normalize_on_host)
+        self.dataset = RecordDataset(directory, split, rank, world, transform, shuffle_seed=seed if train else None)
         all_files = sorted(os.path.join(directory, f) for f in os.listdir(directory)
                            if f.startswith(split + "-") and f.endswith(".rec"))
         if not all_files:
@@ -152,7 +153,8 @@ class RecordLoader:
         self.batch_size, self.train, self._seed = batch_size, train, seed
         workers = min(num_workers, max(1, len(self.dataset.files)))
         self._loader = torch.utils.data.DataLoader(self.dataset, batch_size=batch_size, num_workers=workers,
-                                                   pin_memory=torch.cuda.is_available(), drop_last=False)
+                                                   pin_memory=torch.cuda.is_available(), drop_last=False,
+                                                   collate_fn=collate)
         self._batches = -(-self.per_rank // batch_size) if self.per_rank else 0
 
     def set_epoch(self, epoch: int) -> None:

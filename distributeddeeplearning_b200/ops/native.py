@@ -2106,6 +2106,46 @@ def u8_nhwc_to_nhwc4(x_u8: torch.Tensor, mean: Optional[torch.Tensor] = None, st
     return out
 
 
+def check_resized_crop_desc(desc: torch.Tensor, nbytes: int, size: int) -> None:
+    """Raise ValueError unless every row of the float64 [B, 8] descriptor (offset, Hr, Wr, sy, sx, oy, ox, flip) names a
+    region inside an ``nbytes`` buffer and gives every one of the ``size`` output rows and columns at least one tap."""
+    if desc.dtype != torch.float64 or desc.dim() != 2 or desc.shape[1] != 8 or desc.device.type != "cpu":
+        raise ValueError("resized_crop: the descriptor must be a float64 [B, 8] tensor on the host")
+    if not 1 <= desc.shape[0] <= 65535 or not 1 <= size <= 4096:
+        raise ValueError(f"resized_crop: batch {desc.shape[0]} or size {size} out of range")
+    off, hr, wr, sy, sx, oy, ox, flip = desc.unbind(1)
+    ints = torch.stack([off, hr, wr, oy, ox, flip])
+    if not (torch.isfinite(desc).all() and (ints == ints.trunc()).all()):
+        raise ValueError("resized_crop: non-integer or non-finite descriptor entry")
+    bad = (off < 0) | (hr < 1) | (wr < 1) | (off + hr * wr * 3 > nbytes) | ~((flip == 0) | (flip == 1))
+    for s, o, n in ((sy, oy, hr), (sx, ox, wr)):
+        support = torch.where(s >= 1, s, torch.ones_like(s))
+        last = s * (o + size - 0.5)                    # center of the last output index: its first tap must be inside
+        bad |= (s <= 0) | (o < 0) | (last + support >= 2 ** 30) | ((last - support + 0.5).trunc() >= n)
+    if bool(bad.any()):
+        i = int(bad.nonzero()[0, 0])
+        raise ValueError(f"resized_crop: descriptor {i} {desc[i].tolist()} does not fit a {nbytes}-byte buffer "
+                         f"at output size {size}")
+
+
+def resized_crop(data: torch.Tensor, desc: torch.Tensor, size: int, mean: torch.Tensor, std: torch.Tensor):
+    """Packed uint8 regions (CUDA, 1-D) + host float64 descriptor [B, 8] -> bf16 NHWC4 [B, size, size] activations:
+    the antialiased bilinear resized crop, flip and (v/255 - mean)/std of every image (csrc/ops/augment.cu)."""
+    if data.dtype != torch.uint8 or data.dim() != 1 or not data.is_cuda or not data.is_contiguous():
+        raise ValueError("resized_crop: data must be a contiguous 1-D CUDA uint8 tensor")
+    for t in (mean, std):
+        if t.dtype != torch.float32 or t.numel() != 3 or t.device != data.device or not t.is_contiguous():
+            raise ValueError("resized_crop: mean and std must be 3 contiguous fp32 values on the data's device")
+    size = int(size)
+    check_resized_crop_desc(desc, data.numel(), size)
+    C = _C()
+    B = desc.shape[0]
+    d = desc.to(data.device, non_blocking=True)
+    out = empty_act(B, 4, size, size, data.device)
+    C.resized_crop(data.data_ptr(), d.data_ptr(), out.data_ptr(), B, size, mean.data_ptr(), std.data_ptr(), _stream())
+    return out
+
+
 def dgrad_supports_add(kernel: Tuple[int, int], stride: int) -> bool:
     """Whether conv_dgrad can fold ``+ add`` into its epilogue for this geometry without leaving the fast path
     (the stride-2 phase decomposition writes each output phase from a different launch, so it cannot)."""

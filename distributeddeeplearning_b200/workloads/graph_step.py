@@ -32,7 +32,11 @@ def model_has_dropout(model: torch.nn.Module) -> bool:
 class GraphedStep:
     """``fn(*inputs) -> tensor | tuple of tensors`` replayed from a CUDA graph for inputs of the captured shapes."""
 
-    def __init__(self, fn: Callable, optimizer, log: Optional[Callable[[str], None]] = None):
+    def __init__(self, fn: Callable, optimizer, log: Optional[Callable[[str], None]] = None,
+                 capture_error_mode: str = "global"):
+        """``capture_error_mode``: torch's mode for the capture.  ``thread_local`` for callers whose DataLoader runs a
+        pin-memory thread: that thread allocates pinned buffers (``cudaHostAlloc``) while the step is captured, which
+        the default ``global`` mode makes fail as an unsafe call from another thread (DESIGN.md 4.1)."""
         def stepped(*inputs):
             out = fn(*inputs)
             ops.advance_dropout_step()          # part of the captured step: replays draw fresh dropout masks
@@ -44,6 +48,7 @@ class GraphedStep:
         self.static_out = None
         self.launches = 0
         self.failed = False
+        self.capture_error_mode = capture_error_mode
 
     @staticmethod
     def applicable(model: torch.nn.Module, optimizer, example: torch.Tensor) -> bool:
@@ -63,7 +68,7 @@ class GraphedStep:
         graph = torch.cuda.CUDAGraph()
         before = _ext.launch_count()
         try:
-            with torch.cuda.graph(graph):
+            with torch.cuda.graph(graph, capture_error_mode=self.capture_error_mode):
                 native.begin_capture_scratch(self.static_in[0].device)
                 self.static_out = self.fn(*self.static_in)
         except Exception as e:  # stay eager, say why

@@ -50,6 +50,9 @@ def build_parser():
     p.add_argument("--num-workers", type=int, default=4)
     p.add_argument("--precision", choices=["bf16", "fp8"], default="bf16",
                    help="tensor-core operand format of the forward / data-gradient convolutions (ops/fp8.py)")
+    p.add_argument("--augment", choices=["host", "device"], default="host",
+                   help="where the crop, resize, flip and normalisation of real images run: the loader workers (PIL) "
+                        "or one GPU kernel after the copy (data/images.py)")
     p.add_argument("--no-cuda-graph", action="store_true", default=False,
                    help="launch every kernel of the training step eagerly instead of replaying a captured CUDA graph")
     return p
@@ -78,6 +81,10 @@ def main(argv=None) -> int:
 
         fp8.enable(True)
     args.cuda = not args.no_cuda and torch.cuda.is_available()
+    if args.augment == "device" and args.train_dir is None:
+        raise ValueError("--augment device needs real data (--train-dir)")
+    if args.augment == "device" and not args.cuda:
+        raise ValueError("--augment device needs CUDA (the augmentation kernel runs on the GPU)")
     if not args.cuda:
         os.environ["DDL_NO_CUDA"] = "1"
     dist.init()
@@ -107,14 +114,17 @@ def main(argv=None) -> int:
             train_sampler = get_sampler(ds)
             train_loader = torch.utils.data.DataLoader(ds, batch_size=args.batch_size, sampler=train_sampler)
     else:
-        from ..data.images import DeviceNormalizer, image_folder_loader
+        from ..data.images import DeviceAugment, DeviceNormalizer, image_folder_loader
 
         train_loader, train_sampler = image_folder_loader(args.train_dir, args.batch_size, True, size,
-                                                          args.num_workers, device_normalize=args.cuda)
+                                                          args.num_workers, device_normalize=args.cuda,
+                                                          augment=args.augment)
         prepare = DeviceNormalizer(device) if args.cuda else None
+        if args.augment == "device":
+            prepare = DeviceAugment(device, size)
         if args.val_dir:
             val_loader, _ = image_folder_loader(args.val_dir, args.val_batch_size, False, size, args.num_workers,
-                                                device_normalize=args.cuda)
+                                                device_normalize=args.cuda, augment=args.augment)
     if args.cuda:
         net.cuda()
     # Horovod: scale learning rate by the number of GPUs
@@ -174,7 +184,7 @@ def main(argv=None) -> int:
 
                     graph_state["step"] = train_step
                     if not args.no_cuda_graph and GraphedStep.applicable(net, optimizer, data):
-                        g = GraphedStep(train_step, optimizer)
+                        g = GraphedStep(train_step, optimizer, capture_error_mode="thread_local")   # loader pin thread
                         if g.capture((data, target), warmup=2):
                             graph_state["step"] = g
                 l, a = graph_state["step"](data, target)

@@ -110,7 +110,7 @@ def train(train_loader, model, criterion, optimizer, base_lr, warmup_epochs, epo
             fn = _train_step_fn(model, criterion, optimizer)
             graph["step"] = fn
             if GraphedStep.applicable(model, optimizer, data):
-                g = GraphedStep(fn, optimizer, logger.info)
+                g = GraphedStep(fn, optimizer, logger.info, capture_error_mode="thread_local")   # loader pin thread
                 if g.capture((data, target), warmup=2):
                     graph["step"] = g
                     logger.info("training step captured into a CUDA graph (%d kernels per replay)" % g.launches)
@@ -157,7 +157,7 @@ def validate(val_loader, model, criterion, device, classes, prepare=None):
 
 def main(training_data_path=None, validation_data_path=None, use_gpu=False, save_filepath=None, model="resnet50",
          epochs=_EPOCHS, batch_size=_BATCHSIZE, fp16_allreduce=False, base_lr=0.0125, warmup_epochs=5,
-         num_workers=5, host_data=False, cuda_graph=True, data_type=None, precision="bf16"):
+         num_workers=5, host_data=False, cuda_graph=True, data_type=None, precision="bf16", augment="host"):
     """``cuda_graph``: on a GPU with the fused engine, replay the training step from a captured CUDA graph (the
     reference's default batch of 64 per GPU is launch-bound: ~340 kernels per ResNet-50 step).
     ``data_type``: ``synthetic`` | ``images`` (class folders) | ``records`` / ``tfrecords`` (sharded record files
@@ -166,12 +166,24 @@ def main(training_data_path=None, validation_data_path=None, use_gpu=False, save
     synthetic without a training path, images with one.
     ``precision``: ``bf16`` (default) or ``fp8`` — e4m3 / e5m2 tensor-core operands for the forward and data-gradient
     convolutions (``ops/fp8.py``; the analogue of the reference's ``--use_fp16``,
-    ``TensorFlow_benchmark/tensorflow_benchmark.py:51``)."""
+    ``TensorFlow_benchmark/tensorflow_benchmark.py:51``).
+    ``augment``: ``host`` (default; the reference's PIL crop / resize / flip in the loader workers) or ``device`` (the
+    workers decode and cut the crop box; resize, flip and normalisation run in one kernel, ``data/images.py``)."""
     logger = logging.getLogger(__name__)
     epochs = int(epochs)
     cuda_graph = _str_to_bool(cuda_graph) if isinstance(cuda_graph, str) else bool(cuda_graph)
     use_gpu = _str_to_bool(use_gpu) if isinstance(use_gpu, str) else bool(use_gpu)
     use_gpu = use_gpu and torch.cuda.is_available()
+    augment = str(augment).lower()
+    data_type = (data_type or ("synthetic" if training_data_path is None else "images")).lower()
+    if data_type == "tfrecords":
+        data_type = "records"
+    if augment not in ("host", "device"):
+        raise ValueError(f"augment must be host or device, got {augment!r}")
+    if augment == "device" and data_type == "synthetic":
+        raise ValueError("--augment device needs real data (--data_type images or records)")
+    if augment == "device" and not use_gpu:
+        raise ValueError("--augment device needs --use_gpu True (the augmentation kernel runs on the GPU)")
     if not use_gpu:
         os.environ["DDL_NO_CUDA"] = "1"
     dist.init()
@@ -210,9 +222,6 @@ def main(training_data_path=None, validation_data_path=None, use_gpu=False, save
     classes = getattr(net, "num_classes", 1000)
     prepare = None
     val_loader = None
-    data_type = (data_type or ("synthetic" if training_data_path is None else "images")).lower()
-    if data_type == "tfrecords":
-        data_type = "records"
     if data_type not in ("synthetic", "images", "records"):
         raise ValueError(f"data_type must be synthetic, images or records, got {data_type!r}")
     if data_type != "synthetic" and training_data_path is None:
@@ -228,31 +237,31 @@ def main(training_data_path=None, validation_data_path=None, use_gpu=False, save
             train_loader = torch.utils.data.DataLoader(ds, batch_size=batch_size, sampler=train_sampler,
                                                        num_workers=num_workers if use_gpu else 0, pin_memory=use_gpu)
     elif data_type == "records":
-        from ..data.images import DeviceNormalizer
+        from ..data.images import DeviceAugment, DeviceNormalizer
         from ..data.records import RecordLoader
 
         logger.info("Setting up record loaders")
         logger.info(f"Loading training shards from {training_data_path}")
         train_loader = RecordLoader(training_data_path, "train", batch_size, True, size, num_workers, rank, world,
-                                    normalize_on_host=not use_gpu, seed=_SEED)
+                                    normalize_on_host=not use_gpu, seed=_SEED, augment=augment)
         train_sampler = train_loader
-        prepare = DeviceNormalizer(device) if use_gpu else None
+        prepare = DeviceAugment(device, size) if augment == "device" else DeviceNormalizer(device) if use_gpu else None
         if validation_data_path is not None:
             logger.info(f"Loading validation shards from {validation_data_path}")
             val_loader = RecordLoader(validation_data_path, "validation", batch_size, False, size, num_workers, rank,
-                                      world, normalize_on_host=not use_gpu)
+                                      world, normalize_on_host=not use_gpu, augment=augment)
     else:
-        from ..data.images import DeviceNormalizer, image_folder_loader
+        from ..data.images import DeviceAugment, DeviceNormalizer, image_folder_loader
 
         logger.info("Setting up loaders")
         logger.info(f"Loading training from {training_data_path}")
         train_loader, train_sampler = image_folder_loader(training_data_path, batch_size, True, size, num_workers,
-                                                          device_normalize=use_gpu)
-        prepare = DeviceNormalizer(device) if use_gpu else None
+                                                          device_normalize=use_gpu, augment=augment)
+        prepare = DeviceAugment(device, size) if augment == "device" else DeviceNormalizer(device) if use_gpu else None
         if validation_data_path is not None:
             logger.info(f"Loading validation from {validation_data_path}")
             val_loader, _ = image_folder_loader(validation_data_path, batch_size, False, size, num_workers,
-                                                device_normalize=use_gpu)
+                                                device_normalize=use_gpu, augment=augment)
 
     logger.info("Loading model")
     if use_gpu:

@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "shufflenet", "googlenet", "mnasnet", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "shufflenet", "googlenet", "mnasnet", "augment", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -6032,6 +6032,120 @@ def g_mnasnet_layers():
     """A native-only training step of each MNASNet width (the layer kernels under the current conv-kernel settings)."""
     for name in ("mnasnet0_5", "mnasnet0_75", "mnasnet1_0", "mnasnet1_3"):
         _native_step(name)
+
+
+def _augment_case(name, packed, size, nv, mean, std, ref_images):
+    """resized_crop on one packed batch against its float64 twin.  Tolerance: the kernel sums in fp32 and rounds to
+    bf16, so each value may differ from the twin by one bf16 ulp of the twin's magnitude (rounding plus fp32 error
+    that moves a value across a rounding boundary), plus 1e-4 for values near 0."""
+    import torch
+
+    data = packed.data.cuda()
+    o = nv.resized_crop(data, packed.desc, size, mean, std)
+    o2 = nv.resized_crop(data, packed.desc, size, mean, std)
+    torch.cuda.synchronize()
+    twin = ref_images.resized_crop_reference(packed.data, packed.desc, size, ref_images.RGB_MEAN, ref_images.RGB_SD)
+    got = o[:, :3].double().cpu()
+    ulp = torch.exp2(torch.floor(torch.log2(twin.abs().clamp(min=2.0 ** -20))) - 7)
+    bound = ulp + 1e-4
+    err = (got - twin).abs()
+    ok = bool((err <= bound).all()) and bool(torch.isfinite(got).all())
+    zero = bool((o[:, 3] == 0).all())
+    same = torch.equal(o, o2)
+    print(f"[{'ok' if ok else 'FAIL'}] resized_crop {name:46s} max_abs={err.max().item():.3e} "
+          f"worst/bound={(err / bound).max().item():.3f}", flush=True)
+    print(f"[{'ok' if zero and same else 'FAIL'}] resized_crop {name:46s} channel 3 == 0: {zero}; two runs bitwise "
+          f"equal: {same}", flush=True)
+    RESULTS.extend([ok, zero and same])
+    return o
+
+
+def g_augment():
+    """Device augmentation (csrc/ops/augment.cu, data/images.py augment="device"): the kernel against its float64 twin
+    at wide / tall / tiny / huge images and every input size, train and validation descriptors, a mixed batch of 256
+    ImageNet-like crops, a 1x1 region, S = 600 from 4000 x 3000, both flips; and a loader batch of the device path
+    against the host PIL path."""
+    import numpy as np
+    import torch
+    from PIL import Image
+
+    from augment_bench import make_folder
+    from distributeddeeplearning_b200.data import images
+    from distributeddeeplearning_b200.ops import native as nv
+
+    dev = torch.device("cuda")
+    mean = torch.tensor(images.RGB_MEAN, dtype=torch.float32, device=dev)
+    std = torch.tensor(images.RGB_SD, dtype=torch.float32, device=dev)
+
+    def photo(w, h, seed):
+        rng = np.random.default_rng(seed)
+        y, x = np.mgrid[0:h, 0:w].astype(np.float32)
+        a = (127 + 60 * np.sin(x / (7.0 + seed % 11)) + 50 * np.cos(y / 23.0))[..., None]
+        return Image.fromarray(np.clip(a + rng.normal(0, 25, (h, w, 3)), 0, 255).astype(np.uint8))
+
+    def pack(samples):
+        return images.collate_regions([(s, 0) for s in samples])[0]
+
+    shapes = [("wide", 800, 200), ("tall", 375, 500), ("tiny", 120, 90), ("huge", 2000, 1500), ("imagenet", 500, 375)]
+    for label, w, h in shapes:
+        img = photo(w, h, w + h)
+        for size in (224, 299, 384, 480, 600):
+            for train in (True, False):
+                torch.manual_seed(size)
+                samples = [images.DeviceAugmentTransform(train, size)(img) for _ in range(4 if train else 1)]
+                _augment_case(f"{label} {w}x{h} S={size} {'train' if train else 'val'}", pack(samples), size, nv, mean,
+                              std, images)
+    # a mixed batch of 256 ImageNet-like crops (sizes as augment_bench's folder), both flips among them
+    rng = np.random.default_rng(1)
+    torch.manual_seed(2)
+    samples = []
+    for k in range(256):
+        short = int(rng.integers(333, 501)) if k % 10 else int(rng.integers(800, 1201))
+        ar = (4 / 3, 3 / 4, 1.0)[k % 3]
+        w, h = (int(short * ar), short) if ar >= 1 else (short, int(short / ar))
+        samples.append(images.DeviceAugmentTransform(True, 224)(photo(w, h, k)))
+    flips = {d[6] for _, d in samples}
+    RESULTS.append(flips == {0, 1})
+    _augment_case("mixed batch 256 ImageNet-like train crops", pack(samples), 224, nv, mean, std, images)
+    # a 1x1 region: every output pixel is that pixel
+    px = np.array([[[200, 100, 30]]], dtype=np.uint8)
+    o = _augment_case("1x1 region S=224", pack([(px, (1, 1, 1 / 224, 1 / 224, 0, 0, 0))]), 224, nv, mean, std, images)
+    RESULTS.append(bool((o[0, :3] == o[0, :3, :1, :1]).all()))
+    # S = 600 from 4000 x 3000 (train crop and validation)
+    big = photo(4000, 3000, 5)
+    torch.manual_seed(3)
+    _augment_case("4000x3000 S=600 train", pack([images.DeviceAugmentTransform(True, 600)(big)]), 600, nv, mean, std,
+                  images)
+    _augment_case("4000x3000 S=600 val", pack([images.DeviceAugmentTransform(False, 600)(big)]), 600, nv, mean, std,
+                  images)
+    # both flips of one region: the outputs mirror bit for bit
+    reg = np.asarray(photo(500, 375, 9))
+    o = _augment_case("flip 0 / 1 of one region", pack([(reg, (375, 500, 375 / 224, 500 / 224, 0, 0, f)) for f in (0, 1)]),
+                      224, nv, mean, std, images)
+    mirror = torch.equal(o[0].flip(-1), o[1])
+    print(f"[{'ok' if mirror else 'FAIL'}] resized_crop flip mirrors the unflipped output bit for bit", flush=True)
+    RESULTS.append(mirror)
+    # a loader batch: device path against the host PIL path, same seed (PIL differs from the exact filter by up to one
+    # uint8 level, i.e. 1/255/std after normalisation, plus bf16 rounding of the kernel's output)
+    import tempfile
+
+    with tempfile.TemporaryDirectory() as tmp:
+        root = make_folder(os.path.join(tmp, "train"), 64)
+        got = {}
+        for augment in ("host", "device"):
+            torch.manual_seed(4)
+            loader, _ = images.image_folder_loader(root, 32, True, 224, 2, device_normalize=False, augment=augment)
+            got[augment] = next(iter(loader))
+        (hx, hy), (dx, dy) = got["host"], got["device"]
+        o = images.DeviceAugment(dev, 224)(dx.to(dev, non_blocking=True))[:, :3].double().cpu()
+        sd = torch.tensor(images.RGB_SD, dtype=torch.float64).view(1, 3, 1, 1)
+        ref = hx.double()
+        bound = 1.0001 / 255 / sd + torch.exp2(torch.floor(torch.log2(ref.abs().clamp(min=2.0 ** -20))) - 7) + 1e-4
+        err = (o - ref).abs()
+        ok = torch.equal(hy, dy) and bool((err <= bound).all())
+        print(f"[{'ok' if ok else 'FAIL'}] loader batch 32: device path vs host PIL path max_abs={err.max().item():.3e} "
+              f"worst/bound={(err / bound).max().item():.3f} labels equal: {torch.equal(hy, dy)}", flush=True)
+        RESULTS.append(ok)
 
 
 def run_group(name):
