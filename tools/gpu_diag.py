@@ -15,7 +15,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "shufflenet", "googlenet", "mnasnet", "augment", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "linear", "bn", "sgd", "model"]
+GROUPS = ["fp8", "benchshape", "block", "grouped", "depthwise", "mobilenet", "mobilenet_v3", "efficientnet", "efficientnet_v2", "convnext", "vit", "swin", "swin_v2", "maxvit", "regnet", "shufflenet", "googlenet", "mnasnet", "augment", "classic", "elementwise", "zoo", "graph", "zoograd", "gemm", "conv_generic", "conv_fwd", "conv_dgrad", "conv_wgrad", "wgrad", "linear", "bn", "sgd", "model"]
 RESULTS = []
 WORST = {}          # tensor kind -> worst ratio to its budget (report_abs(..., kind=))
 
@@ -590,6 +590,316 @@ def g_linear():
         gw = torch.zeros(N, K, device=dev)
         nv.linear_wgrad(x, dy, gw)
         report(f"linear wgrad B{B} K{K} N{N}", gw, dy[:, :N].float().t() @ x.float(), 2e-2)
+
+
+# ------------------------------------------------------------------------------------------------
+# weight gradients element-wise against float64 (group `wgrad`)
+# ------------------------------------------------------------------------------------------------
+# Both wgrad operands are bf16, so every product dy * x is exact in fp32 and the only error of conv_wgrad_kernel is fp32
+# summation: within a split (wgmma accumulator) and in each split's red.add into the running gradient.  Per element the
+# check is
+#     |got - (G0 + ref)| <= WGRAD_C * sqrt(S2) + splits * 2^-24 * (|G0| + |ref|),      S2 = sum_m (dy_m * x_m)^2
+# where G0 is what grad_w held before the call (the kernels accumulate) and the second term is one fp32 rounding of the
+# running value per split.  A K-block of 64 pixel rows that goes missing moves an element by a sum of 64 of its M
+# products: rms sqrt(64 / M) * sqrt(S2), which at the largest M checked (the 7x7 stem at batch 256, M = 3.2 M) is
+# 2^-7.8 * sqrt(S2).  With WGRAD_C <= 2^-10 that is 4.6 bounds, so most of the elements of such a case fail (a normal
+# variable stays within 1 / 4.6 of its sigma 17 % of the time); a whole missing split (>= 1 / 264 of the rows) is
+# 16 bounds or more.  Measured on an H100 SXM (80 GB HBM3, 700 W limit), the summation error grows with the K-blocks one
+# split chains in the wgmma accumulator: at most 2^-12.6 * sqrt(S2) (448 K-blocks in one split, 128-wide tile sweep),
+# 2^-13.7 at 224, over all three configurations of the group.  WGRAD_C = 2^-10 leaves 6x margin over the worst.
+WGRAD_C = 2.0 ** -10
+WGRAD_LONG = 12                # K-blocks per split a long-chain case must reach (a 4-stage ring wrapping 3 times)
+WGRAD_LOG = []                 # (tiles, total_kb, splits) of every nv._wgrad_splits call while the group runs
+_CANARY = 4096                 # floats of canary before and after the gradient slot
+
+
+def _wgrad_ref64(x, dy, kernel, stride, pad, dil=1, groups=1, squares=False, chunk=64):
+    """float64 weight gradient sum_m dy[m][co] * x_tap[m][c] of a convolution in the KRSC layout of the kernels'
+    gradient, [Cout, R, S, Cin / groups]: per filter tap (r, s) and group one float64 matmul dy_flat^T @ x_tap, x_tap
+    a strided view of the zero-padded NHWC input.  The batch goes in chunks of at most ``chunk`` images, fewer where
+    that keeps each float64 copy under 2^27 elements (1 GB).  ``squares``: the same sum over (dy * x)^2, i.e. of the
+    operands squared in float64.  ``pad`` is an int or (pad_h, pad_w); any device."""
+    import torch
+    import torch.nn.functional as F
+
+    R, S = kernel
+    ph, pw = (pad, pad) if isinstance(pad, int) else pad
+    N, Cin, H, W = x.shape
+    _, Cout, P, Q = dy.shape
+    cg, og = Cin // groups, Cout // groups
+    per_image = max(Cin * (H + 2 * ph) * (W + 2 * pw), Cout * P * Q)
+    chunk = max(1, min(chunk, (1 << 27) // per_image))
+    out = torch.zeros(Cout, R, S, cg, dtype=torch.float64, device=x.device)
+    for n0 in range(0, N, chunk):
+        xc = x[n0:n0 + chunk].permute(0, 2, 3, 1).double()
+        d = dy[n0:n0 + chunk].permute(0, 2, 3, 1).double().reshape(-1, Cout)
+        if squares:
+            xc, d = xc * xc, d * d
+        xp = F.pad(xc, (0, 0, pw, pw, ph, ph))                 # [n, H + 2 ph, W + 2 pw, Cin]
+        for r in range(R):
+            for s in range(S):
+                h0, w0 = r * dil, s * dil
+                xt = xp[:, h0:h0 + stride * (P - 1) + 1:stride, w0:w0 + stride * (Q - 1) + 1:stride].reshape(-1, Cin)
+                for g in range(groups):
+                    out[g * og:(g + 1) * og, r, s] += d[:, g * og:(g + 1) * og].t() @ xt[:, g * cg:(g + 1) * cg]
+    return out
+
+
+def _wgrad_geometry(total_kb, splits, force_stages=0, tma_fed=True):
+    """(splits, K-blocks per split, K-blocks of the last split, ring stages) that launch_conv_wgrad derives from the
+    requested split count (csrc/ops/conv_gemm.cu; the forced depth applies to the TMA-fed modes only)."""
+    sp = max(1, min(splits, total_kb))
+    kbps = -(-total_kb // sp)
+    sp = -(-total_kb // kbps)
+    stages = force_stages if (tma_fed and 0 < force_stages <= 4) else 4
+    stages = min(stages, kbps)
+    if kbps > stages and stages < (2 if tma_fed else 4):
+        stages = 2 if tma_fed else 4
+    return sp, kbps, total_kb - (sp - 1) * kbps, max(1, stages)
+
+
+def _one_kb_last(total_kb):
+    """The smallest requested split count (>= 3) whose last split is one K-block long after a longer one, or None."""
+    for req in range(3, total_kb + 1):
+        sp, kbps, last, _ = _wgrad_geometry(total_kb, req)
+        if last == 1 and kbps > 1:
+            return req
+    return None
+
+
+def _wgrad_mode(nv, cin, kernel, stride, pad, groups, hw):
+    """Operand mode conv_wgrad picks (ops/native.py): GEMM (1x1), tile (TMA windows), gather (cp.async) or a stem."""
+    if cin <= 4:
+        return "stem TMA" if nv.stem_tma_geometry(hw[0], hw[1], kernel, stride, pad) is not None else "stem gather"
+    if groups == 1 and tuple(kernel) == (1, 1) and stride == 1 and tuple(pad) == (0, 0):
+        return "GEMM"
+    if nv.USE_TILE_TMA and (stride == 1 or (stride == 2 and nv.USE_TILE_S2)):
+        return "tile"
+    return "gather"
+
+
+def _canaried(g0):
+    """(buffer, slot): a copy of g0 in the interior of a larger fp32 buffer whose head and tail are canaries: NaN (a
+    plain store shows) alternating with -0.0 (a red.add of anything but -0.0 shows, since -0 + +0 = +0)."""
+    import torch
+
+    n = g0.numel()
+    pat = torch.tensor([float("nan"), -0.0], device=g0.device).repeat(_CANARY // 2)
+    buf = torch.empty(n + 2 * _CANARY, device=g0.device)
+    buf[:_CANARY], buf[_CANARY + n:] = pat, pat
+    buf[_CANARY:_CANARY + n] = g0.reshape(-1)
+    return buf, buf[_CANARY:_CANARY + n]
+
+
+def _canaries_intact(buf):
+    import torch
+
+    pat = torch.tensor([float("nan"), -0.0], device=buf.device).repeat(_CANARY // 2).view(torch.int32)
+    bits = buf.view(torch.int32)
+    return torch.equal(bits[:_CANARY], pat) and torch.equal(bits[-_CANARY:], pat)
+
+
+def _wgrad_check(name, got, g0, ref, s2, splits, kind, pad_only=False):
+    """The element-wise bound above (all tensors [Cout, R, S, Cin / groups]); elements whose S2 is 0 (taps that only
+    ever see padding) must come back as G0 bit for bit.  ``pad_only``: the case exists for such taps and fails without
+    them.  Returns the worst ratio to the bound."""
+    import math
+
+    import torch
+
+    got, want = got.double(), g0 + ref
+    err = (got - want).abs()
+    bound = WGRAD_C * s2.sqrt() + splits * 2.0 ** -24 * (g0.abs() + ref.abs())
+    bound = torch.where(bound > 0, bound, torch.full_like(bound, 1e-300))
+    bad = int((err > bound).sum().item())
+    worst = float((err / bound).max().item())
+    finite = bool(torch.isfinite(got).all().item())
+    zero = s2 == 0
+    nzero = int(zero.sum().item())
+    exact = bool((got[zero] == g0[zero]).all().item())
+    ok = bad == 0 and finite and exact and (nzero > 0 or not pad_only)
+    WORST[kind] = max(WORST.get(kind, 0.0), worst)
+    print(f"[{'ok' if ok else 'FAIL'}] {name:58s} violations={bad}/{got.numel()} worst={worst:.3f}x of "
+          f"(2^{math.log2(WGRAD_C):g}*sqrt(S2) + {splits}*2^-24*(|G0|+|ref|)); padding-only taps: {nzero} elements"
+          f"{', == G0' if exact else ', NOT G0'}" + ("" if finite else " NONFINITE"), flush=True)
+    RESULTS.append(ok)
+    return worst
+
+
+def _wgrad_case(label, x, dy, kernel, stride, pad, groups=1, linear=False, want=None, force_stages=0, pad_only=False,
+                ref=None):
+    """One conv_wgrad (or linear_wgrad) call onto a random G0 in a canaried slot, checked against float64, with its
+    launch geometry from WGRAD_LOG.  ``want(geometry)``: (ok, what) the geometry must satisfy (default: a long chain);
+    ``ref``: (ref, S2) of the same operands from an earlier call (required for ``linear``).  Returns (ref, S2)."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    R, S = kernel
+    if ref is None:
+        xr = x[:, :3] if x.shape[1] == 4 else x               # an NHWC4 stem image: channel 3 is zero padding
+        ref = (_wgrad_ref64(xr, dy, kernel, stride, pad, 1, groups),
+               _wgrad_ref64(xr, dy, kernel, stride, pad, 1, groups, squares=True))
+    r64, s2 = ref
+    Cout, _, _, cg = r64.shape
+    g0 = (torch.randn(r64.shape, device=r64.device, dtype=torch.float64) * r64.pow(2).mean().sqrt()).float().double()
+    buf, slot = _canaried(g0)
+    del WGRAD_LOG[:]
+    if linear:
+        nv.linear_wgrad(x, dy, slot.view(Cout, cg))
+    else:
+        gw = slot.view(Cout, R, S, cg).permute(0, 3, 1, 2)          # [Cout, Cin / groups, R, S] channels_last
+        nv.conv_wgrad(x, dy, gw, kernel, stride, pad, groups=groups)
+    torch.cuda.synchronize()
+    got = slot.view(Cout, R, S, cg)
+    mode = "GEMM" if linear else _wgrad_mode(nv, x.shape[1], kernel, stride, pad, groups, x.shape[2:])
+    tma_fed = mode in ("GEMM", "tile", "stem TMA")
+    swap = groups > 1 or (os.environ.get("DDL_WGRAD_SWAP", "1") != "0" and 0 < Cout % 128 <= 64)
+    tiles, total_kb, req = WGRAD_LOG[-1] if len(WGRAD_LOG) == 1 else (0, 0, 0)
+    geo = _wgrad_geometry(total_kb, req, force_stages, tma_fed) if total_kb else (0, 0, 0, 0)
+    sp, kbps, last, stages = geo
+    kind = f"wgrad {'stem' if mode.startswith('stem') else mode}{' grouped' if groups > 1 else ''}" + \
+           (" swapped" if swap and groups == 1 else "")
+    _wgrad_check(f"wgrad {label}", got, g0, r64, s2, sp, kind, pad_only)
+    ok = _canaries_intact(buf)
+    RESULTS.append(ok)
+    print(f"[{'ok' if ok else 'FAIL'}]    canaries around grad_w {'intact' if ok else 'OVERWRITTEN'}", flush=True)
+    if want is None:
+        want = lambda g: (g[1] >= WGRAD_LONG, f">= {WGRAD_LONG} K-blocks per split")
+    good, what = want(geo)
+    good = good and len(WGRAD_LOG) == 1
+    RESULTS.append(good)
+    print(f"[{'ok' if good else 'FAIL'}]    {mode}, {'64' if swap else '128'}-channel tiles: {tiles} tiles x {sp} splits, "
+          f"{kbps} K-blocks per split (last {last}) of {total_kb}, {stages} stages (wants {what})", flush=True)
+    return ref
+
+
+def _resnet50_conv_shapes():
+    """Distinct (Cin, Cout, (R, S), stride, H) of the ResNet-50 (v1.5) bottleneck convolutions at 224."""
+    from distributeddeeplearning_b200.models import resnet
+
+    m = resnet.resnet50()
+    out, hw = [], 56
+    for layer in (m.layer1, m.layer2, m.layer3, m.layer4):
+        for blk in layer:
+            s = blk.conv2.stride
+            convs = [(blk.conv1, hw), (blk.conv2, hw), (blk.conv3, hw // s)]
+            if blk.downsample is not None:
+                convs.append((blk.downsample[0], hw))
+            for c, h in convs:
+                key = (c.in_channels, c.out_channels, tuple(c.kernel_size), c.stride, h)
+                if key not in out:
+                    out.append(key)
+            hw //= s
+    return out
+
+
+def g_wgrad():
+    """conv_wgrad / linear_wgrad element-wise against float64 (bound above) at training scale, onto a random G0 in a
+    canaried slot: every ResNet-50 shape, the stem in both modes and the FC at batch 256; every operand mode and tile
+    shape with long split-K chains (channel tails, swapped and 128-wide tiles, stride 3, 1x7 / 7x1, three kinds of
+    group width); taps that only see padding; and a sweep of split counts and forced ring depths."""
+    import torch
+
+    from distributeddeeplearning_b200.ops import native as nv
+
+    t0 = time.time()
+    torch.manual_seed(0)
+    dev = "cuda"
+    policy = nv._wgrad_splits
+
+    def logged(pick):
+        def f(tiles, total_kb, dev_index):
+            s = pick(tiles, total_kb, dev_index)
+            WGRAD_LOG.append((tiles, total_kb, s))
+            return s
+        return f
+
+    def act(n, c, h, w_=None):
+        return cl(bf(torch.randn(n, c, h, h if w_ is None else w_, device=dev)))
+
+    def conv(label, n, ci, h, co, kernel, stride, pad, groups=1, **kw):
+        R, S = kernel
+        P, Q = (h + 2 * pad[0] - R) // stride + 1, (h + 2 * pad[1] - S) // stride + 1
+        _wgrad_case(f"{label} n{n} {ci}x{h}->{co} {R}x{S}/{stride} p{pad[0]},{pad[1]}"
+                    + (f" g{groups}" if groups > 1 else ""), act(n, ci, h), act(n, co, P, Q), kernel, stride, pad,
+                    groups, **kw)
+
+    nv._wgrad_splits = logged(policy)
+    stem_tma0 = nv.USE_STEM_TMA
+    try:
+        # ---- ResNet-50 at batch 256: every bottleneck shape, the stem in both of its modes, the FC
+        for ci, co, k, s, h in _resnet50_conv_shapes():
+            conv("resnet50", 256, ci, h, co, k, s, (k[0] // 2, k[1] // 2))
+        img = torch.randn(256, 3, 224, 224, device=dev)
+        x4 = nv.nchw_to_nhwc4(img)
+        dy = act(256, 64, 112)
+        ref = None
+        for tma in ((True, False) if stem_tma0 else (False,)):
+            nv.USE_STEM_TMA = tma
+            ref = _wgrad_case(f"resnet50 stem 7x7/2 224 n256 ({'TMA' if tma else 'gather'})", x4, dy, (7, 7), 2,
+                              (3, 3), ref=ref)
+        nv.USE_STEM_TMA = stem_tma0
+        del img, x4, dy
+        xf, dyf = bf(torch.randn(256, 2048, device=dev)), bf(torch.randn(256, 1024, device=dev))
+        xr, dyr = xf.view(*xf.shape, 1, 1), dyf[:, :1000].reshape(-1, 1000, 1, 1)
+        ref = (_wgrad_ref64(xr, dyr, (1, 1), 1, 0), _wgrad_ref64(xr, dyr, (1, 1), 1, 0, squares=True))
+        # dy's 24 padding columns hold values too: grad_w += dy[:, :1000]^T x reads none of them
+        _wgrad_case("resnet50 fc 2048->1000 n256 (linear_wgrad)", xf, dyf, (1, 1), 1, 0, linear=True, ref=ref,
+                    want=lambda g: (True, "the FC's own geometry"))
+        # ---- operand modes and tile shapes at long chains
+        conv("channels 24 (GEMM)", 64, 24, 56, 144, (1, 1), 1, (0, 0))
+        conv("channels 96, Cout 96 < 128", 128, 96, 28, 96, (3, 3), 1, (1, 1))
+        conv("channels 160, Cout % 128 = 32", 256, 160, 28, 160, (3, 3), 2, (1, 1))
+        conv("Cout % 128 = 64", 128, 192, 28, 192, (1, 1), 1, (0, 0))
+        conv("Cout 1000 (128-wide tail)", 256, 512, 13, 1000, (1, 1), 1, (0, 0))
+        conv("stride 3", 128, 64, 56, 64, (3, 3), 3, (1, 1))
+        conv("stride 3, channels 160", 256, 160, 28, 160, (3, 3), 3, (1, 1))
+        conv("1x7", 256, 160, 17, 160, (1, 7), 1, (0, 3))
+        conv("7x1", 256, 160, 17, 192, (7, 1), 1, (3, 0))
+        conv("grouped cg 4 (ResNeXt-50 32x4d)", 256, 128, 56, 128, (3, 3), 1, (1, 1), groups=32)
+        conv("grouped cg 4, stride 2", 256, 256, 56, 256, (3, 3), 2, (1, 1), groups=64)
+        conv("grouped cg 64", 256, 1024, 14, 1024, (3, 3), 1, (1, 1), groups=16)
+        conv("grouped cg 112 (RegNet)", 128, 448, 28, 448, (3, 3), 1, (1, 1), groups=4)
+        conv("grouped cg 120 (RegNet), stride 2", 64, 240, 56, 240, (3, 3), 2, (1, 1), groups=2)
+        # ---- taps that only see padding (1x1 map; first row / column of taps of a 3x3/2 on 2x2) and a 2x2 map
+        short = lambda g: (True, "any")
+        conv("padding taps 1x1 map", 256, 256, 1, 256, (3, 3), 1, (1, 1), want=short, pad_only=True)
+        conv("2x2 map", 256, 256, 2, 256, (3, 3), 1, (1, 1), want=short)
+        conv("padding taps 2x2 map", 256, 256, 2, 256, (3, 3), 2, (1, 1), want=short, pad_only=True)
+        # ---- split geometry: requested split counts, then forced 2- and 3-stage rings (13 K-blocks per split)
+        C = nv._C()
+        for label, n, ci, h, co, k, p in (("swapped GEMM", 64, 256, 14, 64, (1, 1), (0, 0)),
+                                          ("128-wide tile", 32, 128, 28, 128, (3, 3), (1, 1))):
+            x, dy = act(n, ci, h), act(n, co, h)
+            ref = None
+            sweeps = [("1 split", lambda t: 1, lambda g: (g[0] == 1, "1 split")),
+                      ("2 splits", lambda t: 2, lambda g: (g[0] == 2, "2 splits")),
+                      ("3 splits", lambda t: 3, lambda g: (g[0] == 3, "3 splits")),
+                      ("one-K-block last split", _one_kb_last, lambda g: (g[2] == 1 and g[1] > 1, "last split 1")),
+                      ("total_kb - 1 splits", lambda t: t - 1, lambda g: (g[1] == 2, "2 K-blocks per split")),
+                      ("total_kb splits", lambda t: t, lambda g: (g[1] == 1, "1 K-block per split")),
+                      ("total_kb + 7 splits", lambda t: t + 7, lambda g: (g[1] == 1, "1 K-block per split"))]
+            for what, pick, want in sweeps:
+                nv._wgrad_splits = logged(lambda tiles, t, d, pick=pick: pick(t) or 1)
+                ref = _wgrad_case(f"sweep {label} n{n} {ci}x{h}->{co}: {what}", x, dy, k, 1, p, ref=ref, want=want)
+            for st in (2, 3):
+                tma_fed = _wgrad_mode(nv, ci, k, 1, p, 1, (h, h)) != "gather"
+                nv._wgrad_splits = logged(lambda tiles, t, d: -(-t // 13))
+                C.set_conv_force_stages(st)
+                try:
+                    ref = _wgrad_case(f"sweep {label} n{n} {ci}x{h}->{co}: {st} stages forced", x, dy, k, 1, p,
+                                      ref=ref, force_stages=st,
+                                      want=lambda g, st=st: (g[1] == 13 and g[3] == (st if tma_fed else 4),
+                                                             f"13 K-blocks per split, {st if tma_fed else 4} stages"))
+                finally:
+                    C.set_conv_force_stages(0)
+    finally:
+        nv._wgrad_splits = policy
+        nv.USE_STEM_TMA = stem_tma0
+    for kind, r in sorted(WORST.items()):
+        print(f"worst ratio to budget: {kind:24s} {r:.3f}x", flush=True)
+    print(f"wgrad group wall time {time.time() - t0:.1f} s", flush=True)
 
 
 def _unpack_mask(mask, numel):
